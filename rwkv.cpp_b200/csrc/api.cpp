@@ -580,7 +580,7 @@ bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, 
             p.Wt = tiled;
         }
         const bool use_tc = ok && gemm_tc_supported(p, T);
-        if (use_tc) ok = cudaMalloc(&act16, act16_bytes) == cudaSuccess && cudaMemset(act16, 0, GEMM_TC_COUNTER_BYTES) == cudaSuccess && gemm_tc_launch(b, di, 0, act16, act16_bytes) == cudaSuccess;
+        if (use_tc) ok = cudaMalloc(&act16, act16_bytes) == cudaSuccess && gemm_tc_launch(b, di, 0, act16, act16_bytes) == cudaSuccess;
         else ok = gemv_launch(b, di, 0) == cudaSuccess;
         ok = ok && cudaDeviceSynchronize() == cudaSuccess && cudaMemcpy(y, dy, sizeof(float) * M * T, cudaMemcpyDeviceToHost) == cudaSuccess;
         cudaFree(act16); cudaFree(tiled);

@@ -36,14 +36,6 @@ struct Scratch {      // carve-up of ctx->scratch for T tokens
 };
 
 constexpr int BATCH_TC_MIN = 16;
-// Smallest batch (in weights) that goes to the tensor cores in a pass of >= 32 tokens: 0 = every eligible batch. A tensor-core launch
-// has a fixed cost of tens of microseconds even for the 160 x 4096 LoRA matrix of a v6 layer, but the multi-column GEMV is worse for
-// such a matrix at T = 128 (32 column groups), and a 7B chunk measured slower with a 2^20 threshold than with none.
-// RWKV_B200_TC_MIN_WEIGHTS overrides (A/B aid).
-long long tc_min_weights() {
-    static const long long v = [] { const char * e = getenv("RWKV_B200_TC_MIN_WEIGHTS"); return e ? atoll(e) : 0ll; }();
-    return v;
-}
 
 struct Dims { size_t C, F, R; };
 
@@ -69,10 +61,9 @@ void segment_range(const Context * ctx, int seg, int & l0, int & l1) {
     // of the last group's are the two copies nothing can overlap, so those groups are small; a group may grow by about the ratio of
     // compute time to copy time per layer (about 1.7 at 7B) over its predecessor without starving the kernels, and shrink the same
     // way towards the end without queueing the downloads; a pipeline model with those two rates puts a 7B token closer to the
-    // kernels-alone time than eight even groups do. RWKV_B200_EVEN_SEGMENTS=1: the even split (A/B aid).
-    static const bool even = getenv("RWKV_B200_EVEN_SEGMENTS") != nullptr;
+    // kernels-alone time than eight even groups do.
     static const int cum32[9] = {0, 1, 3, 6, 11, 21, 27, 30, 32};
-    if (even || G != 8 || n < 16) {
+    if (G != 8 || n < 16) {
         l0 = m.layer_begin + (int) ((long long) n * (seg - 1) / G);
         l1 = m.layer_begin + (int) ((long long) n * seg / G);
         return;
@@ -117,19 +108,15 @@ struct Batch {
 };
 
 // ---- staged activation columns (act_stage.cuh) --------------------------------------------------------------------------------------
-// Single-token passes: the kernel that produces a GEMV's input vector (LayerNorm + mix, the v6 lerp, a WKV kernel) also writes
-// it in the layout the streaming GEMV keeps in shared memory, so the consumer copies ~5 KB instead of quantising 16 KB of fp32 on
-// its critical path. One slot per (producer, output); a slot serves every consumer whose weight type multiplies the same staged format.
-constexpr int XQ_SLOTS = 16;
-enum XqSlot { XQ_ATT_MIX = 0 /* .. 5 */, XQ_LERP = 6 /* .. 10 */, XQ_WKV = 11, XQ_FFN_MIX = 12 /* .. 13 */ };
+// Single-token passes: the kernel that produces a GEMV's input vector (the v6 lerp, a WKV kernel) also writes it in the layout
+// the streaming GEMV keeps in shared memory, so the consumer copies ~5 KB instead of quantising 16 KB of fp32 on its critical
+// path. One slot per (producer, output); a slot serves every consumer whose weight type multiplies the same staged format.
+constexpr int XQ_SLOTS = 6;
+enum XqSlot { XQ_LERP = 0 /* .. 4 */, XQ_WKV = 5 };
 
-bool handoff_enabled() {
-    static const bool on = getenv("RWKV_B200_NO_XQ") == nullptr && getenv("RWKV_B200_GENERIC_GEMV") == nullptr;
-    return on;
-}
 // The slot to fill for a consumer matrix W of this pass, or NULL when the pass / shape cannot use the hand-off.
 unsigned char * xq_slot(const Context * ctx, int T, int slot, const DevMatrix & W) {
-    if (!handoff_enabled() || T != 1 || ctx->batch_stride || !ctx->xq || !W.data || W.K % 32 != 0 || W.type == DT_F32 || act::stage_class(W.type) == act::SC_NONE) return nullptr;
+    if (T != 1 || ctx->batch_stride || !ctx->xq || !W.data || W.K % 32 != 0 || W.type == DT_F32 || act::stage_class(W.type) == act::SC_NONE) return nullptr;
     if (act::bytes_per_column(W.type, W.K) > ctx->xq_slot_bytes) return nullptr;
     return ctx->xq + (size_t) slot * ctx->xq_slot_bytes;
 }
@@ -144,22 +131,19 @@ void xq_bind(GemvProblem & p, const unsigned char * q, int q_type) {
 
 // Passes of >= 32 tokens send every problem the tensor-core kernel can take (any weight type but F32, K % 64 == 0) to
 // gemm_tc.cu; the rest (and all shorter passes) use the batch-invariant GEMV, so serial == sequence stays bit-exact
-// wherever the reference's tests compare states.
+// wherever the reference's tests compare states. Every eligible problem goes, however small: a tensor-core launch has a fixed cost
+// of tens of microseconds even for the 160 x 4096 LoRA matrix of a v6 layer, but the multi-column GEMV is worse for such a matrix
+// at T = 128 (32 column groups), and a 7B chunk measured slower with a 2^20-weight threshold than with none.
 bool launch_batch(Context * ctx, GemvBatch & b) {
     // tensor cores: chunks of >= 32 tokens; batch contexts (one token of each of B sequences: nothing to stay bit-identical with
-    // across pass sizes) from 16 sequences on, where the multi-column SIMT consumer is instruction-bound (DESIGN.md 6.2)
+    // across pass sizes) from 16 sequences on, where the multi-column SIMT consumer is instruction-bound
     if ((b.T >= 32 || (ctx->batch_n > 0 && b.T >= BATCH_TC_MIN)) && ctx->use_tensor_cores && ctx->act16) {
         GemvBatch tcb, rest;
         memset(&tcb, 0, sizeof(tcb)); memset(&rest, 0, sizeof(rest));
         tcb.T = rest.T = b.T;
-        long long tc_weights = 0;
         for (int i = 0; i < b.n; i++) {
-            if (gemm_tc_supported(b.p[i], b.T)) { tcb.p[tcb.n++] = b.p[i]; tc_weights += (long long) b.p[i].M * b.p[i].K; }
+            if (gemm_tc_supported(b.p[i], b.T)) tcb.p[tcb.n++] = b.p[i];
             else rest.p[rest.n++] = b.p[i];
-        }
-        if (tc_weights < tc_min_weights()) {
-            for (int i = 0; i < tcb.n; i++) rest.p[rest.n++] = tcb.p[i];
-            tcb.n = 0;
         }
         if (tcb.n) CUDA_OK(ctx, gemm_tc_launch(tcb, ctx->model->dev, ctx->stream, ctx->act16, ctx->act16_bytes));
         if (rest.n) CUDA_OK(ctx, gemv_launch(rest, ctx->model->dev, ctx->stream));
@@ -185,6 +169,18 @@ bool run_batch(Context * ctx, Batch & batch) {
 
 // The three stages that touch the recurrent state: a batch context (one token of each of batch_n sequences) uses the kernels of
 // batch.cu, where column t works on sequence t's state; everything else is identical for both kinds of context.
+// LayerNorm + token shift + mix in front of a batch of GEMVs is a launch of its own (ln_mix_kernel). Four variations were built,
+// measured at 7B Q5_1 and removed:
+// (a) fused into the CONSUMING GEMV, every CTA recomputing the LayerNorm in its prologue: a third slower per token;
+// (b) as the tail job of the PRODUCING GEMV (att.output / ffn.value), run by the CTA that draws the last ticket: a quarter slower
+//     -- every CTA pays a device-wide fence + ticket before it may retire, and the one CTA left behind does
+//     the LayerNorm of 4096 channels with 256 threads where this kernel uses 1024 and has its parameter loads in flight before the
+//     dependency wait;
+// (c) ln_mix_kernel emitting the staged columns of its consumers (act_stage.cuh, as the lerp and WKV kernels do): it adds more to
+//     every launch of the single-CTA, latency-bound kernel than it takes out of the consumer: 3 % slower per token;
+// (d) for passes of >= 32 tokens, ln_mix_kernel writing the fp16 GEMM operands of its consumers itself, so that two of the six
+//     convert_f16 launches of a v6 layer disappear: 1 % per 7B chunk, and the tail of the state went NaN in the shift-state-3e5
+//     robustness test of the 64-channel fixture (not understood). 1 % was not worth an unexplained failure.
 cudaError_t do_ln_mix(Context * ctx, const LnMixParams & lp) {
     return ctx->batch_stride ? launch_ln_mix_batch(lp, ctx->batch_stride, ctx->stream) : launch_ln_mix(lp, ctx->stream);
 }
@@ -193,23 +189,6 @@ cudaError_t do_wkv6(Context * ctx, const Wkv6Params & wp) {
 }
 cudaError_t do_wkv4(Context * ctx, const Wkv4Params & wp) {
     return ctx->batch_stride ? launch_wkv4_batch(wp, ctx->batch_stride, ctx->stream) : launch_wkv4(wp, ctx->stream);
-}
-
-// LayerNorm + token shift + mix in front of a batch of GEMVs: its own launch (ln_mix_kernel); *staged = the mixed vectors also left
-// as staged columns (never, today). Three variations were built, measured at 7B Q5_1 and removed in round 2:
-// (a) fused into the CONSUMING GEMV, every CTA recomputing the LayerNorm in its prologue: a third slower per token;
-// (b) as the tail job of the PRODUCING GEMV (att.output / ffn.value), run by the CTA that draws the last ticket: a quarter slower
-//     -- every CTA pays a device-wide fence + ticket before it may retire, and the one CTA left behind does
-//     the LayerNorm of 4096 channels with 256 threads where this kernel uses 1024 and has its parameter loads in flight before the
-//     dependency wait;
-// (c) ln_mix_kernel emitting the staged columns of its consumers: 3 % slower.
-// And for passes of >= 32 tokens: (d) ln_mix_kernel writing the fp16 GEMM operands of its consumers itself, so that two of the six
-//     convert_f16 launches of a v6 layer disappear: 1 % per 7B chunk, and the tail of the state went NaN in the shift-state-3e5
-//     robustness test of the 64-channel fixture (not understood). 1 % was not worth an unexplained failure: not kept.
-bool ln_mix_then(Context * ctx, const LnMixParams & lp, bool * staged) {
-    *staged = false;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
-    return true;
 }
 
 // LayerNorm + mix parameters of the channel-mixing block (rwkv_ffn_v4_v5 :484-511, rwkv_ffn_v6 :513-531, rwkv_ffn_v7 :533-543).
@@ -229,8 +208,6 @@ LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
         lp.coef[0] = L.ffn_time_mix_k.data; lp.out[0] = s.mix[0];
         lp.coef[1] = L.ffn_time_mix_r.data; lp.out[1] = s.mix[1];
     }
-    lp.q_out[0] = xq_slot(ctx, T, XQ_FFN_MIX, L.ffn_key); lp.q_type[0] = L.ffn_key.type;
-    if (m.arch_major != 7) { lp.q_out[1] = xq_slot(ctx, T, XQ_FFN_MIX + 1, L.ffn_receptance); lp.q_type[1] = L.ffn_receptance.type; }
     return lp;
 }
 
@@ -238,13 +215,11 @@ LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
 bool ffn(Context * ctx, const Layer & L, const Scratch & s, int T, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
+    CUDA_OK(ctx, do_ln_mix(ctx, lp));
     {
         Batch b(T);
-        GemvProblem & pk = b.add(L.ffn_key, s.mix[0], s.ffn_k, EPI_RELU_SQR);
-        GemvProblem * pr = (m.arch_major != 7) ? &b.add(L.ffn_receptance, s.mix[1], s.ffn_r, EPI_SIGMOID) : nullptr;
-        bool staged = false;
-        if (!ln_mix_then(ctx, lp, &staged)) return false;
-        if (staged) { xq_bind(pk, lp.q_out[0], lp.q_type[0]); if (pr) xq_bind(*pr, lp.q_out[1], lp.q_type[1]); }
+        b.add(L.ffn_key, s.mix[0], s.ffn_k, EPI_RELU_SQR);
+        if (m.arch_major != 7) b.add(L.ffn_receptance, s.mix[1], s.ffn_r, EPI_SIGMOID);
         if (!run_batch(ctx, b)) return false;
     }
     {
@@ -266,23 +241,19 @@ bool att_output(Context * ctx, const Layer & L, const Scratch & s, int T, const 
     return run_batch(ctx, b);
 }
 
-// LayerNorm + mix parameters of the time-mixing block of layer `layer`, per architecture (:94-97, :306-311, :400-413), with the staged
-// columns of the consumers of each mixed vector.
-LnMixParams att_ln(const Context * ctx, const Layer & L, int layer, const Scratch & s, int T, const float * st_in, float * st_out) {
+// LayerNorm + mix parameters of the time-mixing block, per architecture (:94-97, :306-311, :400-413).
+LnMixParams att_ln(const Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     LnMixParams lp{};
     lp.x = s.x; lp.ln_w = L.ln1_w.data; lp.ln_b = L.ln1_b.data;
     lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = T;
-    const DevMatrix * cons[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};      // first consumer of out[j]
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 6;
         for (int j = 0; j < 6; j++) { lp.coef[j] = L.att_x_rwkvag.data + (size_t) j * C; lp.out[j] = s.mix[j]; }   // r w k v a g
-        cons[0] = &L.att_receptance; cons[1] = &L.att_w1; cons[2] = &L.att_key; cons[3] = &L.att_value; cons[4] = &L.att_a1; cons[5] = &L.att_g1;
     } else if (m.arch_major == 6) {
         lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.att_maa_x.data; lp.out[0] = s.mix[0];
         lp.out_xx = s.xx; lp.out_sx = s.sx;
-        cons[0] = &L.att_maa_w1;
     } else {
         const bool v52 = m.arch_major == 5 && m.arch_minor >= 2;
         lp.formula = 0; lp.n_out = v52 ? 4 : 3;
@@ -290,22 +261,17 @@ LnMixParams att_ln(const Context * ctx, const Layer & L, int layer, const Scratc
         lp.coef[1] = L.att_time_mix_v.data; lp.out[1] = s.mix[1];
         lp.coef[2] = L.att_time_mix_r.data; lp.out[2] = s.mix[2];
         if (v52) { lp.coef[3] = L.att_time_mix_g.data; lp.out[3] = s.mix[3]; }
-        cons[0] = &L.att_key; cons[1] = &L.att_value; cons[2] = &L.att_receptance; cons[3] = &L.att_gate;
     }
-    (void) layer;
-    for (int j = 0; j < lp.n_out; j++) if (cons[j]) { lp.q_out[j] = xq_slot(ctx, T, XQ_ATT_MIX + j, *cons[j]); lp.q_type[j] = cons[j]->type; }
     return lp;
 }
 
 bool att_v4(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
     const int C = ctx->model->n_embed;
+    CUDA_OK(ctx, do_ln_mix(ctx, lp));
     Batch b(T);
-    GemvProblem & pr = b.add(L.att_receptance, s.mix[2], s.r, EPI_SIGMOID);
-    GemvProblem & pk = b.add(L.att_key, s.mix[0], s.k);
-    GemvProblem & pv = b.add(L.att_value, s.mix[1], s.v);
-    bool staged = false;
-    if (!ln_mix_then(ctx, lp, &staged)) return false;
-    if (staged) { xq_bind(pr, lp.q_out[2], lp.q_type[2]); xq_bind(pk, lp.q_out[0], lp.q_type[0]); xq_bind(pv, lp.q_out[1], lp.q_type[1]); }
+    b.add(L.att_receptance, s.mix[2], s.r, EPI_SIGMOID);
+    b.add(L.att_key, s.mix[0], s.k);
+    b.add(L.att_value, s.mix[1], s.v);
     if (!run_batch(ctx, b)) return false;
     Wkv4Params wp{};
     wp.k = s.k; wp.v = s.v; wp.r = s.r;
@@ -322,17 +288,12 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     const bool v52 = m.arch_minor >= 2;
+    CUDA_OK(ctx, do_ln_mix(ctx, lp));
     Batch b(T);
-    GemvProblem & pr = b.add(L.att_receptance, s.mix[2], s.r);
-    GemvProblem & pk = b.add(L.att_key, s.mix[0], s.k);
-    GemvProblem & pv = b.add(L.att_value, s.mix[1], s.v);
-    GemvProblem * pg = v52 ? &b.add(L.att_gate, s.mix[3], s.g, EPI_SILU) : nullptr;
-    bool staged = false;
-    if (!ln_mix_then(ctx, lp, &staged)) return false;
-    if (staged) {
-        xq_bind(pr, lp.q_out[2], lp.q_type[2]); xq_bind(pk, lp.q_out[0], lp.q_type[0]); xq_bind(pv, lp.q_out[1], lp.q_type[1]);
-        if (pg) xq_bind(*pg, lp.q_out[3], lp.q_type[3]);
-    }
+    b.add(L.att_receptance, s.mix[2], s.r);
+    b.add(L.att_key, s.mix[0], s.k);
+    b.add(L.att_value, s.mix[1], s.v);
+    if (v52) b.add(L.att_gate, s.mix[3], s.g, EPI_SILU);
     if (!run_batch(ctx, b)) return false;
     Wkv6Params wp{};
     wp.r = s.r; wp.k = s.k; wp.v = s.v;
@@ -351,12 +312,10 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
 bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
+    CUDA_OK(ctx, do_ln_mix(ctx, lp));
     {   // :313-321  tanh(W1 . xxx)
         Batch b(T);
-        GemvProblem & p1 = b.add(L.att_maa_w1, s.mix[0], s.lora[0], EPI_TANH);
-        bool staged = false;
-        if (!ln_mix_then(ctx, lp, &staged)) return false;
-        if (staged) xq_bind(p1, lp.q_out[0], lp.q_type[0]);
+        b.add(L.att_maa_w1, s.mix[0], s.lora[0], EPI_TANH);
         if (!run_batch(ctx, b)) return false;
     }
     V6LerpParams vp{};   // :323-346
@@ -403,16 +362,16 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Scratch & s, int T,
     const int C = m.n_embed;
     const bool first = layer == 0;
     float * v_dst = first ? s.v_first : s.v;
-    {   // :415-432, 439, 447 -- first halves of the LoRA pairs. The staged column of a mix output was written for its first consumer;
-        // att_v1 shares x_v with att_value only if both multiply the same staged format (in quantised files the LoRA matrices stay fp16)
+    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    {   // :415-432, 439, 447 -- first halves of the LoRA pairs
         Batch b(T);
-        GemvProblem * ps[7] = {&b.add(L.att_receptance, s.mix[0], s.r), &b.add(L.att_key, s.mix[2], s.k), &b.add(L.att_value, s.mix[3], v_dst),
-                               &b.add(L.att_w1, s.mix[1], s.lora[0], EPI_TANH), &b.add(L.att_a1, s.mix[4], s.lora[1]), &b.add(L.att_g1, s.mix[5], s.lora[2], EPI_SIGMOID),
-                               first ? nullptr : &b.add(L.att_v1, s.mix[3], s.lora[3])};
-        const int src[7] = {0, 2, 3, 1, 4, 5, 3};      // which mix output each problem reads
-        bool staged = false;
-        if (!ln_mix_then(ctx, lp, &staged)) return false;
-        if (staged) for (int i = 0; i < 7; i++) if (ps[i]) xq_bind(*ps[i], lp.q_out[src[i]], lp.q_type[src[i]]);
+        b.add(L.att_receptance, s.mix[0], s.r);
+        b.add(L.att_key, s.mix[2], s.k);
+        b.add(L.att_value, s.mix[3], v_dst);
+        b.add(L.att_w1, s.mix[1], s.lora[0], EPI_TANH);
+        b.add(L.att_a1, s.mix[4], s.lora[1]);
+        b.add(L.att_g1, s.mix[5], s.lora[2], EPI_SIGMOID);
+        if (!first) b.add(L.att_v1, s.mix[3], s.lora[3]);
         if (!run_batch(ctx, b)) return false;
     }
     {   // second halves
@@ -465,7 +424,6 @@ bool ensure_capacity(Context * ctx, int T) {
         const size_t kmax = d.F > d.C ? d.F : d.C;
         ctx->act16_bytes = gemm_tc_workspace_bytes(cap, (size_t) GEMV_MAX_PROBLEMS * (kmax * (size_t) ((cap + 15) / 16 * 16) + 128));
         e = cudaMalloc(&ctx->act16, ctx->act16_bytes);
-        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->act16, 0, GEMM_TC_COUNTER_BYTES, ctx->stream);      // split-K tile counters
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate fp16 staging: %s", cudaGetErrorString(e));
     }
     ctx->scratch_floats = n;
@@ -491,7 +449,7 @@ bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
         const Layer & L = m.layers[i];
         const float * st_in = ctx->state_a + (size_t) i * per_layer;
         float * st_out = ctx->state_b + (size_t) i * per_layer;
-        const LnMixParams alp = att_ln(ctx, L, i, s, T, st_in, st_out), flp = ffn_ln(ctx, L, s, T, st_in, st_out);
+        const LnMixParams alp = att_ln(ctx, L, s, T, st_in, st_out), flp = ffn_ln(ctx, L, s, T, st_in, st_out);
         bool ok;
         switch (m.arch_major) {
             case 7: ok = att_v7(ctx, L, i, s, T, st_in, st_out, alp); break;
@@ -619,9 +577,7 @@ Context * create_context(Model * model, ErrorSink sink, int batch_n) {
     { const char * e = getenv("RWKV_B200_OVERLAP"); ctx->overlap_copies = e ? atoi(e) != 0 : OVERLAP_DEFAULT; }
     {   // layer groups of the overlapped host-state path: at least 4 layers each, at most MAX_SEGMENTS groups
         const int n = model->layer_end - model->layer_begin;
-        int g = n / 4;
-        if (const char * e = getenv("RWKV_B200_SEGMENTS")) g = atoi(e);
-        ctx->n_segments = g < 1 ? 1 : (g > Context::MAX_SEGMENTS ? Context::MAX_SEGMENTS : (g > n ? n : g));
+        ctx->n_segments = std::clamp(n / 4, 1, Context::MAX_SEGMENTS);
     }
     const size_t n = model->state_len();
     const size_t seqs = batch_n > 0 ? (size_t) batch_n : 1;

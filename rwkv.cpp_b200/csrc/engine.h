@@ -147,11 +147,6 @@ bool eval_host_chunks(Context * ctx, const uint32_t * tokens, size_t T, size_t c
 // into ctx->logits. Asynchronous except for the token upload.
 bool forward(Context * ctx, const uint32_t * tokens, size_t T, bool want_logits);
 
-// One pipeline stage: the resident layers [layer_begin, layer_end) for T <= MAX_TOKENS_PER_PASS tokens. The first stage
-// embeds `tokens`, the others start from `hidden_in`; every stage but the last leaves its result in `hidden_out`
-// (device pointers, stage_hidden_len(T) floats); the last one computes the logits when asked. `stream` (may be NULL = the
-// context's own) is the CUDA stream everything is enqueued on, so the hand-off can be ordered against NCCL sends and
-// receives without host synchronisation.
 // Batch contexts: state of sequence `seq` <- host state (NULL = fresh) / -> host; one token of every sequence; logits of `seq`.
 bool batch_set_state(Context * ctx, int seq, const float * state_in);
 bool batch_get_state(Context * ctx, int seq, float * state_out);
@@ -164,6 +159,10 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
 
 size_t stage_hidden_len(const Model & m, size_t T);
 
+// One pipeline stage: the resident layers [layer_begin, layer_end) for T <= MAX_TOKENS_PER_PASS tokens. The first stage
+// embeds `tokens`, the others start from `hidden_in`; every stage but the last leaves its result in `hidden_out`
+// (device pointers, stage_hidden_len(T) floats); the last one computes the logits when asked. `stream` (may be NULL = the
+// context's own) is the CUDA stream everything is enqueued on.
 bool stage_forward(Context * ctx, const uint32_t * tokens, size_t T, const float * hidden_in, float * hidden_out, bool want_logits, cudaStream_t stream);
 // The same with the hand-off done by peer-memory kernels on the stream (kernels/pipe.cu): receive from the previous stage's
 // stores (unless this stage embeds tokens), run the resident layers, store into the next stage's mailbox (unless this is the last).

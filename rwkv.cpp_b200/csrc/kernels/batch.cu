@@ -121,7 +121,6 @@ cudaError_t launch_ln_mix_batch(const LnMixParams & p_in, long long seq_stride, 
     LnMixParams p = p_in;
     if (p.C > 256 * steps::LN_MAXCH) return cudaErrorInvalidValue;
     p.trace = trace_slot("ln_mix_batch");
-    g_kernel_launches++;
     return launch_pdl(ln_mix_batch_kernel, dim3(p.T), dim3(BATCH_THREADS), 0, s, p, seq_stride);
 }
 
@@ -130,7 +129,6 @@ cudaError_t launch_wkv6_batch(const Wkv6Params & w, long long seq_stride, cudaSt
     k.r = w.r; k.k = w.k; k.v = w.v; k.td = w.td; k.tf = w.tf; k.state_in = w.state_in; k.lnx_w = w.lnx_w; k.lnx_b = w.lnx_b; k.g = w.g;
     k.state_out = w.state_out; k.y = w.y; k.eps = w.eps; k.td_per_token = w.td_per_token; k.per_head_scalars = w.per_head_scalars; k.H = w.H; k.S = w.S;
     TraceRec * trace = trace_slot("wkv6_batch");
-    g_kernel_launches++;
     const dim3 grid(w.H, w.T), block(BATCH_THREADS);
     const int C = w.H * w.S;
     switch (w.S) {
@@ -146,7 +144,6 @@ cudaError_t launch_wkv4_batch(const Wkv4Params & p_in, long long seq_stride, cud
     Wkv4Params p = p_in;
     p.trace = trace_slot("wkv4_batch");
     const int threads = 128;
-    g_kernel_launches++;
     return launch_pdl(wkv4_batch_kernel, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p, seq_stride);
 }
 

@@ -30,7 +30,6 @@
 #include "quant_decode.cuh"
 
 #include <cuda_fp16.h>
-#include <cstdlib>
 #include <cstring>
 
 namespace rwkv {
@@ -366,7 +365,6 @@ template <int TYPE> __device__ __forceinline__ void block_to_half(const BlockReg
 struct TcBatch {
     int n, T, npad;                  // problems, tokens, tokens padded to a multiple of 16
     int stages;                     // ring depth, 2 .. MAX_STAGES
-    int stagger;                     // 1: every CTA starts its K range at a different step (RWKV_B200_TC_STAGGER=0 turns it off)
     const __half * act16[GEMV_MAX_PROBLEMS];   // canonical-layout fp16 activations per problem (convert_f16_kernel)
     const float * colscale[GEMV_MAX_PROBLEMS]; // [npad] power-of-two factor per token that the epilogue multiplies back in
     GemvProblem p[GEMV_MAX_PROBLEMS];          // first_cta / n_cta: CTA range of the problem = splits x tiles
@@ -421,7 +419,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_tc_kernel(const TcBatch batch
             // pull the same 16-32 KB out of the same few L2 slices at the same moment (microseconds per K-step however the weights
             // arrive). So CTA (tile, split) starts at K-step `rot` of its range and wraps around: at any moment the CTAs read different
             // blocks. The accumulation order of a tile is then a function of its tile index: fixed from run to run.
-            const int rot = batch.stagger ? (int) (((unsigned) tile * 29u + (unsigned) split * 11u) % (unsigned) n) : 0;
+            const int rot = (int) (((unsigned) tile * 29u + (unsigned) split * 11u) % (unsigned) n);
             auto kstep = [&](int it) { const int k = it + rot; return k >= n ? k - n : k; };
             const int pre = n < nst ? n : nst;
             for (int i = 0; i < pre; i++) {
@@ -658,21 +656,20 @@ bool gemm_tc_supported(const GemvProblem & p, int T) {
            (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.Wt) & 15) == 0;
 }
 
-// Workspace layout (gemm_tc_workspace_bytes): [reserved header][fp16 operands + per-token scales of the batch's distinct inputs].
+// Workspace layout (gemm_tc_workspace_bytes): the fp16 operands + per-token scales of the batch's distinct inputs, each part starting
+// on a 256-byte boundary.
 size_t gemm_tc_workspace_bytes(int T, size_t operand_halves) {
     const size_t npad = (size_t) (T + 15) / 16 * 16;
-    return GEMM_TC_COUNTER_BYTES + GEMM_TC_PARTIAL_BYTES + operand_halves * 2 + (size_t) GEMV_MAX_PROBLEMS * (npad * 4 + 512);
+    return operand_halves * 2 + (size_t) GEMV_MAX_PROBLEMS * (npad * 4 + 512);
 }
 
 cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes) {
-    if (workspace_bytes < GEMM_TC_COUNTER_BYTES + GEMM_TC_PARTIAL_BYTES) return cudaErrorMemoryAllocation;
     tc::TcBatch tb;
     memset(&tb, 0, sizeof(tb));
     tb.n = batch.n; tb.T = batch.T;
     tb.npad = (batch.T + 15) / 16 * 16;
 
-    uint8_t * scratch = reinterpret_cast<uint8_t *>(workspace) + GEMM_TC_COUNTER_BYTES + GEMM_TC_PARTIAL_BYTES;
-    const size_t scratch_bytes = workspace_bytes - GEMM_TC_COUNTER_BYTES - GEMM_TC_PARTIAL_BYTES;
+    uint8_t * scratch = reinterpret_cast<uint8_t *>(workspace);
     size_t used = 0;
     tc::ConvertBatch cvt;
     memset(&cvt, 0, sizeof(cvt));
@@ -687,7 +684,7 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
         for (int j = 0; j < i; j++)
             if (batch.p[j].x == p.x && batch.p[j].K == p.K && batch.p[j].ldx == p.ldx && (batch.p[j].type != DT_F16) == (quant != 0)) shared = share_of[j];
         if (shared < 0) {
-            if (used + need > scratch_bytes) return cudaErrorMemoryAllocation;
+            if (used + need > workspace_bytes) return cudaErrorMemoryAllocation;
             shared = cvt.n;
             cvt.x[cvt.n] = p.x; cvt.ldx[cvt.n] = p.ldx; cvt.K[cvt.n] = p.K; cvt.quant[cvt.n] = quant;
             cvt.out[cvt.n] = reinterpret_cast<__half *>(scratch + used);
@@ -702,12 +699,10 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     // ---- work decomposition: one CTA per (row tile, K-split). Every CTA streams its share of the weights from HBM, so what matters
     // is that close to all SMs have a CTA: launches with few tiles (4096-row matrices: 32; LoRA: 1-2) are cut along K over clusters
     // of c = 2 / 4 / 8 CTAs (a problem is cut c ways or not at all: the cluster size is one per launch).
-    static const int force_split = [] { const char * e = getenv("RWKV_B200_TC_SPLITK"); return e ? atoi(e) : -1; }();
     int total = 0;
     for (int i = 0; i < batch.n; i++) { tb.tiles[i] = (batch.p[i].M + tc::TILE_M - 1) / tc::TILE_M; total += tb.tiles[i]; }
     const int sms = dev.num_sms > 0 ? dev.num_sms : 132;
-    int want = total * 4 < sms * 3 ? sms / total : 1;      // below 75 % of the SMs: split, but never into a second wave
-    if (force_split >= 0) want = force_split < 1 ? 1 : force_split;
+    const int want = total * 4 < sms * 3 ? sms / total : 1;      // below 75 % of the SMs: split, but never into a second wave
     int cluster = 1;
     while (cluster * 2 <= want && cluster < 8) cluster *= 2;
     bool any_split = false;
@@ -732,7 +727,6 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     }
     {   // every distinct input of the batch -> fp16 canonical layout, one launch: one CTA per (token column, input)
         cvt.trace = trace_slot("convert_f16");
-        g_kernel_launches++;
         cudaError_t e = launch_pdl(tc::convert_f16_kernel, dim3(tb.npad, cvt.n), dim3(tc::CVT_THREADS), 0, stream, cvt);
         if (e != cudaSuccess) return e;
     }
@@ -743,8 +737,6 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     if (nst > tc::MAX_STAGES) nst = tc::MAX_STAGES;
     if (nst < 2) return cudaErrorInvalidValue;
     tb.stages = nst;
-    static const int stagger = [] { const char * e = getenv("RWKV_B200_TC_STAGGER"); return e ? atoi(e) : 1; }();
-    tb.stagger = stagger;
     const size_t smem = (size_t) nst * stage_bytes;
     if (smem < (size_t) tb.npad * tc::PARK_LD * sizeof(float)) return cudaErrorInvalidValue;     // the parked accumulator
     // one instantiation per padded token count (the wgmma N and the accumulator registers are compile-time)
@@ -761,28 +753,7 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     const cudaError_t ae = once[ki].run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem_budget); });
     if (ae != cudaSuccess) return ae;
     tb.trace = trace_slot("gemm_tc");
-    g_kernel_launches++;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned) next);
-    cfg.blockDim = dim3(tc::THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (cluster > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = (unsigned) cluster; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-        na++;
-    }
-    if (g_use_pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        na++;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = (unsigned) na;
-    prefer_max_shared_carveout(reinterpret_cast<const void *>(kernel));
-    return cudaLaunchKernelEx(&cfg, kernel, tb);
+    return launch_pdl((unsigned) cluster, kernel, dim3((unsigned) next), dim3(tc::THREADS), smem, stream, tb);
 }
 
 }  // namespace rwkv

@@ -17,7 +17,6 @@
 #include "quant_decode.cuh"
 
 #include <cuda_fp16.h>
-#include <cstdlib>
 #include <mutex>
 #include <set>
 #include <utility>
@@ -296,7 +295,6 @@ cudaError_t launch_nc(const GemvBatch & batch, int grid, size_t smem, int max_op
     static PerDeviceOnce once;                // the shared-memory opt-in is per device
     const cudaError_t ae = once.run([&] { return cudaFuncSetAttribute(gemv_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_optin - 1024); });
     if (ae != cudaSuccess) return ae;
-    g_kernel_launches++;
     return launch_pdl(gemv_kernel<NC>, dim3(grid), dim3(GEMV_THREADS), smem, stream, batch);
 }
 
@@ -316,8 +314,6 @@ __global__ void qh5_to_device_kernel(uint8_t * W, long long pitch, int M, int nb
 }  // namespace
 
 void prefer_max_shared_carveout(const void * kernel) {
-    static const bool on = [] { const char * e = getenv("RWKV_B200_CARVEOUT"); return !e || atoi(e) != 0; }();
-    if (!on) return;
     static std::mutex mu;
     static std::set<std::pair<int, const void *>> done;
     int dev = 0;
@@ -339,13 +335,8 @@ cudaError_t weights_to_device_layout(void * W, long long pitch, int type, int M,
 
 cudaError_t gemv_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream) {
     if (batch.n <= 0 || batch.T <= 0) return cudaSuccess;
-    static const bool force_generic = getenv("RWKV_B200_GENERIC_GEMV") != nullptr;
-    static const bool no_pdl = getenv("RWKV_B200_NO_PDL") != nullptr;
-    if (no_pdl) g_use_pdl = false;
-    if (!force_generic) {
-        cudaError_t e = gemv_tma_launch(batch, dev, stream);
-        if (e != cudaErrorNotSupported) return e;
-    }
+    const cudaError_t e = gemv_tma_launch(batch, dev, stream);
+    if (e != cudaErrorNotSupported) return e;
     return gemv_generic_launch(batch, dev, stream);
 }
 

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <atomic>
 #include <cstdint>
+#include <utility>
 
 namespace rwkv {
 
@@ -87,38 +88,47 @@ bool gemm_tc_supported(const GemvProblem & p, int T);
 bool gemm_tc_eligible(int type, int K);
 size_t gemm_tc_tiled_bytes(int type, int M, int K);
 cudaError_t gemm_tc_repack(const void * W, long long pitch, int type, int M, int K, void * dst, cudaStream_t stream);
-// workspace: gemm_tc_workspace_bytes(T, sum over the batch's distinct inputs of round16(T) * K) bytes of device memory whose first
-// GEMM_TC_COUNTER_BYTES were zeroed once after the allocation (split-K tile counters; every launch leaves them zero again).
-constexpr size_t GEMM_TC_COUNTER_BYTES = 4096;
-constexpr size_t GEMM_TC_PARTIAL_BYTES = 0;                      // (K-splits are reduced through distributed shared memory: no global partials)
+// workspace: gemm_tc_workspace_bytes(T, sum over the batch's distinct inputs of round16(T) * K) bytes of device memory, 256-byte aligned
+// (what cudaMalloc returns).
 size_t gemm_tc_workspace_bytes(int T, size_t operand_halves);
 cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes);
-
-// Programmatic dependent launch for every kernel of the eval path (RWKV_B200_NO_PDL=1 turns it off).
-extern bool g_use_pdl;
 
 // Every kernel of the eval path asks for the SAME L1 / shared-memory split (all shared): an SM can only change its carve-out when it is
 // idle, so a stream that alternates between 113-225 KB weight-streaming kernels and small glue kernels with the default (L1-heavy)
 // preference makes every kernel boundary wait for the SMs to drain instead of overlapping through programmatic dependent launch.
-// Once per (device, kernel); RWKV_B200_CARVEOUT=0 leaves the driver's default (A/B aid).
+// Once per (device, kernel).
 void prefer_max_shared_carveout(const void * kernel);
 
-// Launch with the PDL attribute: the kernel may start while its predecessor in the stream is still running; it must
-// execute griddepcontrol.wait before touching anything the predecessor writes.
+// Per-launch count of kernels this module has enqueued (bench.py reports it as gpu_launches).
+extern std::atomic<unsigned long long> g_kernel_launches;
+
+// Launches every kernel of the eval path, and counts it: with the PDL attribute (the kernel may start while its predecessor in the
+// stream is still running; it must execute griddepcontrol.wait before touching anything the predecessor writes), the carve-out
+// preference above and, when cluster > 1, thread-block clusters of that many CTAs along x.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args &&... args) {
+inline cudaError_t launch_pdl(unsigned cluster, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args &&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.numAttrs = 1;
+    if (cluster > 1) {
+        attr[1].id = cudaLaunchAttributeClusterDimension;
+        attr[1].val.clusterDim.x = cluster; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
+        cfg.numAttrs = 2;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
     prefer_max_shared_carveout(reinterpret_cast<const void *>(kernel));
+    g_kernel_launches++;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args &&... args) {
+    return launch_pdl(1u, kernel, grid, block, smem, stream, std::forward<Args>(args)...);
 }
 #if defined(__CUDACC__)
 // First statement of every non-GEMV kernel: let the successor start (it will prefetch its weights), then wait for the
@@ -137,9 +147,6 @@ __device__ __forceinline__ void pdl_prologue() {
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 #endif
-
-// Per-launch count of kernels this module has enqueued (bench.py reports it as gpu_launches).
-extern std::atomic<unsigned long long> g_kernel_launches;
 
 // One-time per-device function attribute (dynamic shared-memory opt-in): several host threads may launch concurrently.
 struct PerDeviceOnce {

@@ -21,8 +21,6 @@
 #include "gemv_tma_device.cuh"
 #include "act_stage.cuh"
 
-#include <cstdlib>
-
 namespace rwkv {
 namespace tma {
 
@@ -31,7 +29,7 @@ namespace tma {
 // (248 KB) of which a launch runs ~1 500 scattered ones; ncu attributes 34 % of the warp stall cycles of a 12 MB launch, and 50-64 %
 // of the LoRA launches', to instruction fetch. A per-format instantiation is ~2 000
 // instructions, contiguous.
-template <int NC, bool STAGE_V2 = false, int ONLY = -1, bool HAS_LN = true>
+template <int NC, int ONLY = -1, bool HAS_LN = true>
 __global__ void __launch_bounds__(THREADS, 2) gemv_tma_kernel(const GemvBatch batch) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ Shared sh;
@@ -98,7 +96,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tma_kernel(const GemvBatch ba
             int4 * dst = reinterpret_cast<int4 *>(act);
             for (int i = threadIdx.x; i < (int) (colb / 16); i += CONSUMER_THREADS) dst[i] = __ldcg(src + i);
         } else {
-            for (int c = 0; c < nc; c++) stage_column<4, STAGE_V2, ONLY, HAS_LN>(P, c0 + c, act + c * colb, sh.red_d);
+            for (int c = 0; c < nc; c++) stage_column<4, NC == 1, ONLY, HAS_LN>(P, c0 + c, act + c * colb, sh.red_d);
         }
         consumer_barrier();
         trace_mark(batch.trace, 1);
@@ -137,8 +135,6 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tma_kernel(const GemvBatch ba
 
 }  // namespace tma
 
-bool g_use_pdl = true;
-
 // ---- host side: shape planning + launch ----------------------------------------------------------------
 namespace {
 
@@ -166,44 +162,26 @@ bool plan_wk(GemvProblem & p) {
     return false;
 }
 
-template <int NC, bool STAGE_V2 = false, int ONLY = -1, bool HAS_LN = true>
+template <int NC, int ONLY = -1, bool HAS_LN = true>
 cudaError_t launch_tma_nc(const GemvBatch & batch, int grid, size_t smem, cudaStream_t stream) {
-    if constexpr (NC == 1 && !STAGE_V2 && ONLY < 0) {
-        // single-column launches stage their activation column one thread per 32-element block (gemv_tma_device.cuh: stage_column
-        // PER_BLOCK; bit-identical bytes, faster per 7B token); RWKV_B200_STAGE_V2=0 selects the 8-lanes-per-block variant
-        static const bool stage_v2 = [] { const char * e = getenv("RWKV_B200_STAGE_V2"); return !e || atoi(e) != 0; }();
-        if (stage_v2) {
-            // ... and run the instantiation of their weight format when the launch has only one (RWKV_B200_GEMV_PER_TYPE=0: never)
-            static const bool per_type = [] { const char * e = getenv("RWKV_B200_GEMV_PER_TYPE"); return !e || atoi(e) != 0; }();
-            int only = batch.p[0].type;
-            for (int i = 1; i < batch.n; i++) if (batch.p[i].type != only) only = -1;
-            bool has_ln = false;
-            for (int i = 0; i < batch.n; i++) has_ln = has_ln || batch.p[i].pro == PRO_LAYERNORM;
-#define RWKV_PER_TYPE(T_) case T_: return has_ln ? launch_tma_nc<1, true, T_, true>(batch, grid, smem, stream) : launch_tma_nc<1, true, T_, false>(batch, grid, smem, stream);
-            if (per_type) switch (only) {
-                RWKV_PER_TYPE(DT_Q4_0) RWKV_PER_TYPE(DT_Q4_1) RWKV_PER_TYPE(DT_Q5_0) RWKV_PER_TYPE(DT_Q5_1) RWKV_PER_TYPE(DT_Q8_0) RWKV_PER_TYPE(DT_F16) RWKV_PER_TYPE(DT_F32)
-                default: break;
-            }
-#undef RWKV_PER_TYPE
-            return launch_tma_nc<1, true>(batch, grid, smem, stream);
-        }
-    }
     static PerDeviceOnce once;                // the shared-memory opt-in is per device
-    const cudaError_t ae = once.run([&] { return cudaFuncSetAttribute(tma::gemv_tma_kernel<NC, STAGE_V2, ONLY, HAS_LN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma::CTA_SMEM_BUDGET); });
+    const cudaError_t ae = once.run([&] { return cudaFuncSetAttribute(tma::gemv_tma_kernel<NC, ONLY, HAS_LN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma::CTA_SMEM_BUDGET); });
     if (ae != cudaSuccess) return ae;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned) grid);
-    cfg.blockDim = dim3(tma::THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
-    g_kernel_launches++;
-    prefer_max_shared_carveout(reinterpret_cast<const void *>(tma::gemv_tma_kernel<NC, STAGE_V2, ONLY, HAS_LN>));
-    return cudaLaunchKernelEx(&cfg, tma::gemv_tma_kernel<NC, STAGE_V2, ONLY, HAS_LN>, batch);
+    return launch_pdl(tma::gemv_tma_kernel<NC, ONLY, HAS_LN>, dim3((unsigned) grid), dim3(tma::THREADS), smem, stream, batch);
+}
+
+// Single-column launches run the instantiation of their weight format when every problem of the launch has the same one.
+cudaError_t launch_tma_single(const GemvBatch & batch, int grid, size_t smem, cudaStream_t stream) {
+    int only = batch.p[0].type;
+    for (int i = 1; i < batch.n; i++) if (batch.p[i].type != only) only = -1;
+    bool has_ln = false;
+    for (int i = 0; i < batch.n; i++) has_ln = has_ln || batch.p[i].pro == PRO_LAYERNORM;
+#define RWKV_PER_TYPE(T_) case T_: return has_ln ? launch_tma_nc<1, T_, true>(batch, grid, smem, stream) : launch_tma_nc<1, T_, false>(batch, grid, smem, stream);
+    switch (only) {
+        RWKV_PER_TYPE(DT_Q4_0) RWKV_PER_TYPE(DT_Q4_1) RWKV_PER_TYPE(DT_Q5_0) RWKV_PER_TYPE(DT_Q5_1) RWKV_PER_TYPE(DT_Q8_0) RWKV_PER_TYPE(DT_F16) RWKV_PER_TYPE(DT_F32)
+        default: return launch_tma_nc<1>(batch, grid, smem, stream);
+    }
+#undef RWKV_PER_TYPE
 }
 
 }  // namespace
@@ -249,22 +227,6 @@ static int assign_tiles_and_ctas(GemvBatch & batch, int total_ctas, long long st
     return next;
 }
 
-bool gemv_tma_plan(GemvBatch & batch, int total_ctas, long long stage_bytes, size_t * max_col_bytes) {
-    using namespace tma;
-    size_t max_col = 0;
-    for (int i = 0; i < batch.n; i++) {
-        GemvProblem & p = batch.p[i];
-        if (!plan_wk(p)) return false;
-        if ((long long) (CONSUMER_WARPS / p.wk) * p.pitch > stage_bytes) return false;   // not even one row per warp row-slot fits a stage
-        const size_t cb = act_bytes_per_column(p.type, p.K);
-        if (cb > max_col) max_col = cb;
-    }
-    if (batch.n > total_ctas) return false;
-    assign_tiles_and_ctas(batch, total_ctas, stage_bytes);
-    if (max_col_bytes) *max_col_bytes = max_col;
-    return true;
-}
-
 // Returns cudaErrorNotSupported when some problem of the batch does not fit the streaming kernel
 // (the caller then uses the generic kernel for the whole batch).
 cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream) {
@@ -295,7 +257,7 @@ cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStrea
     switch (nc) {
         case 4: return launch_tma_nc<4>(batch, next, smem, stream);
         case 2: return launch_tma_nc<2>(batch, next, smem, stream);
-        default: return launch_tma_nc<1>(batch, next, smem, stream);
+        default: return launch_tma_single(batch, next, smem, stream);
     }
 }
 

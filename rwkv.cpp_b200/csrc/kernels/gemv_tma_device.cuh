@@ -184,9 +184,9 @@ template <int TYPE> __device__ __forceinline__ void load_unit(const uint8_t * ro
 // would multiply with (ggml-cpu.c:253-311 `vec_dot_type`): Q8_0 / Q8_1 blocks for quantised weights (x86 flavour of
 // quantize_row_q8_0 / q8_1, ggml-cpu-quants.c:781-846, 1085-1160; one thread per 32-element block), fp16 for F16
 // weights, fp32 for F32 weights. PRO_LAYERNORM applies rwkv_layer_norm (rwkv_operators.inc:93-97) on the fly.
-// PER_BLOCK (experimental, RWKV_B200_STAGE_V2=1): one thread quantises a whole 32-element block instead of 8 lanes sharing it --
+// PER_BLOCK (single-column launches): one thread quantises a whole 32-element block instead of 8 lanes sharing it --
 // the two IEEE divisions, the scale and the sums once per 32 elements instead of once per 4, no shuffles; ~4x fewer instructions for
-// a stage that is instruction-bound (DESIGN.md 6.3). The staged bytes are identical: the maximum and the integer sum of a block do
+// a stage that is instruction-bound. The staged bytes are identical: the maximum and the integer sum of a block do
 // not depend on the order they are taken in.
 // TYPE_HINT: the weight type when the whole launch has one (a compile-time constant: the other formats' code is not generated), else -1.
 // HAS_LN = false: the launch has no PRO_LAYERNORM problem (every launch but the head): the LayerNorm code, ~1 500 of the 4 200

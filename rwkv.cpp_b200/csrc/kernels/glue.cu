@@ -1,7 +1,7 @@
 // Embedding gather + ln0, LayerNorm + token shift + mixing, and the v6 data-dependent lerp.
 // These are the small fp32 element-wise stages between the GEMVs; each is one launch over [C, T].
 #include "ops.h"
-#include "gemv.h"          // g_kernel_launches
+#include "gemv.h"          // launch_pdl
 #include "../formats.h"
 #include "act_stage.cuh"
 
@@ -148,9 +148,6 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
         xb[i] = (t > 0) ? __fadd_rn(__fmul_rn(__fmul_rn(xb[i], scale_b), lw[i]), lb[i]) : pv[i];          // LN(x[:, t-1]) or the carry
     }
     const size_t o0 = (size_t) t * C + tid;
-    // (Emitting the mixed vectors as staged columns here as well -- act_stage.cuh, as the lerp and WKV kernels do -- was measured: it
-    // adds more to every launch of this single-CTA, latency-bound kernel than it takes out of the consumer: 3 % slower per 7B token.
-    // Not kept: its consumers quantise the column themselves.)
     if constexpr (PRE) {
 #pragma unroll
         for (int j = 0; j < PRE_N; j++) {
@@ -363,14 +360,12 @@ __global__ void __launch_bounds__(LERP_THREADS) v6_lerp_kernel(const V6LerpParam
 
 cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch, const int * tokens, int T, int C,
                              const float * ln_w, const float * ln_b, float * x, cudaStream_t s) {
-    g_kernel_launches++;
     return launch_pdl(embed_ln0_kernel, dim3(T), dim3(GLUE_THREADS), (size_t) C * sizeof(float), s, reinterpret_cast<const uint8_t *>(emb), emb_type, emb_pitch, tokens, C, ln_w, ln_b, x);
 }
 
 cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s) {
     LnMixParams p = p_in;
     p.trace = trace_slot("ln_mix");
-    g_kernel_launches++;
     const int per = (p.C + LN_THREADS - 1) / LN_THREADS;
 #define RWKV_LN(PER_) return p.n_out > 3 ? launch_pdl(ln_mix_kernel<PER_, 6>, dim3(p.T), dim3(LN_THREADS), 0, s, p) : launch_pdl(ln_mix_kernel<PER_, 3>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
     if (per <= 1) { RWKV_LN(1) }
@@ -387,10 +382,8 @@ cudaError_t launch_v6_lerp(const V6LerpParams & p_in, cudaStream_t s) {
     p.trace = trace_slot("v6_lerp");
     if (p.T < LERP_MIN_TOKENS) {
         dim3 grid((p.C + 31) / 32, p.T);
-        g_kernel_launches++;
         return launch_pdl(v6_lerp_decode_kernel, grid, dim3(GLUE_THREADS), (size_t) 5 * p.mix * sizeof(float), s, p);
     }
-    g_kernel_launches++;
     const int tile = (p.T >= 32 && (size_t) 32 * p.mix * sizeof(float) <= 48 * 1024) ? 32 : 8;      // which tile a token falls into does not touch its arithmetic
     const size_t smem = (size_t) tile * p.mix * sizeof(float);
     if (smem > 48 * 1024) return cudaErrorInvalidValue;

@@ -29,10 +29,6 @@ struct LnMixParams {
     float * out[6];           // [C, T] each
     float * out_xx;           // optional [C, T]: LN(x)
     float * out_sx;           // optional [C, T]: prev - xx
-    // T == 1, C % 32 == 0 only: out_j additionally as the staged column (act_stage.cuh) of a consumer with weight type q_type[j]
-    // (NULL: not wanted); the batch kernel ignores these
-    unsigned char * q_out[6];
-    int q_type[6];
 };
 cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s);
 

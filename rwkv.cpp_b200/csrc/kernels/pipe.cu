@@ -82,7 +82,6 @@ cudaError_t launch_pipe_recv(PipeBox * mine, PipeBox * prev, unsigned long long 
 }
 
 cudaError_t launch_pipe_send(PipeBox * mine, PipeBox * next, unsigned long long * counters, size_t slot_floats, float * x, size_t nx, float * v, size_t nv, cudaStream_t s) {
-    g_kernel_launches++;
     return launch_pdl(pipe_kernel<true>, dim3(PIPE_CTAS), dim3(PIPE_THREADS), 0, s, mine, next, counters, slot_floats, x, nx, v, nv, trace_slot("pipe_send"));
 }
 

@@ -160,7 +160,6 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const SamplePara
 
 cudaError_t launch_sample(const SampleParams & p, cudaStream_t s) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64) return cudaErrorInvalidValue;
-    g_kernel_launches++;
     const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
     if (per <= 1) return launch_pdl(sample_kernel<1>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
     if (per <= 4) return launch_pdl(sample_kernel<4>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);

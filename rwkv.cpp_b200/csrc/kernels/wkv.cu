@@ -2,7 +2,7 @@
 // gating that follows it in the reference graph. The recurrent state stays in registers for the
 // whole chunk; one CTA per head (v5+), one thread per state column (v5/v6) or row (v7).
 #include "ops.h"
-#include "gemv.h"   // g_kernel_launches
+#include "gemv.h"   // launch_pdl
 #include "act_stage.cuh"
 #include "../formats.h"
 
@@ -368,7 +368,6 @@ cudaError_t launch_wkv4(const Wkv4Params & p_in, cudaStream_t s) {
     Wkv4Params p = p_in;
     p.trace = trace_slot("wkv4");
     const int threads = 128;
-    g_kernel_launches++;
     return launch_pdl(wkv4_kernel, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p);
 }
 
@@ -385,7 +384,6 @@ cudaError_t launch_wkv4(const Wkv4Params & p_in, cudaStream_t s) {
 cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
     Wkv6Params p = p_in;
     p.trace = trace_slot("wkv6");
-    g_kernel_launches++;
     switch (p.S) {
         case 8: return launch_pdl(wkv6_kernel<8>, dim3(p.H), dim3(Wkv6Layout<8>::BLOCK), 0, s, p);
         case 16: return launch_pdl(wkv6_kernel<16>, dim3(p.H), dim3(Wkv6Layout<16>::BLOCK), 0, s, p);
@@ -399,7 +397,6 @@ cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
 cudaError_t launch_wkv7(const Wkv7Params & p_in, cudaStream_t s) {
     Wkv7Params p = p_in;
     p.trace = trace_slot("wkv7");
-    g_kernel_launches++;
     const long long none = 0;
     RWKV_DISPATCH_HEAD_SIZE(p.S, wkv7_kernel, p, s, dim3(p.H), none)
 }
@@ -408,7 +405,6 @@ cudaError_t launch_wkv7(const Wkv7Params & p_in, cudaStream_t s) {
 cudaError_t launch_wkv7_batch(const Wkv7Params & p_in, long long seq_stride, cudaStream_t s) {
     Wkv7Params p = p_in;
     p.trace = trace_slot("wkv7_batch");
-    g_kernel_launches++;
     RWKV_DISPATCH_HEAD_SIZE(p.S, wkv7_kernel, p, s, dim3(p.H, p.T), seq_stride)
 }
 

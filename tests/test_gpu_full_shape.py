@@ -96,7 +96,7 @@ def test_decode_matches_reference(lib, synth, golden, name):
 @pytest.mark.parametrize("name", [n for n in CASES if n in ("rwkv4-169m:Q5_1", "rwkv5-1b5:Q4_0", "rwkv6-7b:Q5_1")])
 def test_chunked_prefill_matches_reference(lib, synth, golden, name):
     """One rwkv_eval_sequence_in_chunks call (chunk = 128: BASELINE.json config 2 and the headline prefill) == the compiled
-    reference; the >= 32-token passes run the tcgen05 kernel. With the tensor cores off the same call must equal serial
+    reference; the >= 32-token passes run the wgmma kernel. With the tensor cores off the same call must equal serial
     evaluation bit for bit (the reference's own contract, tests/test_eval_sequence_in_chunks.c:54)."""
     ctx = lib.rwkv_init_from_file(synth(name), 1, 0)
     try:

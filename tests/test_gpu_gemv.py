@@ -108,8 +108,8 @@ def q8_block_values(x):
 def test_tensor_core_gemm_matches_fp16_reference(lib, fmt, shape, T):
     """wgmma prefill kernel (csrc/kernels/gemm_tc.cu), used for passes of >= 32 tokens: weights exactly as stored (rounded once to
     fp16), the B operand = fp16(x) for F16 weights and fp16 of the reference's Q8 block values (d * q) for quantised weights, fp32
-    accumulation -- compared with that computation done in float64. The shapes cover the cluster / multicast decomposition
-    (>= 16 row tiles), stand-in CTAs (tile counts that are no multiple of 4), K-splits (few tiles, long K) and ragged M / T."""
+    accumulation -- compared with that computation done in float64. The shapes cover launches with enough row tiles to run without a
+    K-split, K-splits over thread-block clusters of 2 / 4 / 8 CTAs (few tiles, long K) and ragged M / T."""
     M, K = shape
     rng = np.random.default_rng(M + K + T)
     tid, raw = make_weights(fmt, M, K, rng)
@@ -127,7 +127,7 @@ def test_tensor_core_gemm_matches_fp16_reference(lib, fmt, shape, T):
 
 
 def test_tensor_core_gemm_is_deterministic_and_scales_large_columns(lib):
-    """K-split partial tiles are added in split order by the last-arriving CTA: the same launch twice gives the same bits. A column
+    """The K-splits of a tile are summed in cluster rank order through distributed shared memory: the same launch twice gives the same bits. A column
     whose values exceed the fp16 range carries a power-of-two scale through the GEMM and comes out finite and accurate."""
     M, K, T = 160, 4096, 64          # 2 row tiles, 64 K-steps: cut along K
     rng = np.random.default_rng(77)
