@@ -13,6 +13,7 @@
 #include "../../include/rwkv.h"
 #include "../../include/rwkv_b200.h"
 #include "engine.h"
+#include "kernels/act_stage.cuh"
 #include "kernels/ops.h"
 #include "quantizer.h"
 
@@ -28,6 +29,73 @@ static int default_device() {
     const char * e = getenv("RWKV_B200_DEVICE");
     return e ? atoi(e) : 0;
 }
+
+namespace {
+
+// Device copies of a kernel test hook's host buffers. Inputs are copied in; outputs get a guard region of RWKV_B200_GUARD floats
+// after their end, are filled with 0xFF bytes (NaN) before the launch and copied back whole, guard included. NULL host pointers stay
+// NULL on the device.
+struct HookBuffers {
+    struct Out { void * dev; void * host; size_t bytes; };
+    std::vector<void *> allocs;
+    std::vector<Out> outs;
+    bool ok = true;
+
+    void * alloc(size_t bytes) {
+        void * d = nullptr;
+        if (ok) ok = cudaMalloc(&d, bytes) == cudaSuccess;
+        if (ok) allocs.push_back(d);
+        return ok ? d : nullptr;
+    }
+    template <class T> const T * in(const T * host, size_t n) {
+        if (!host) return nullptr;
+        void * d = alloc(n * sizeof(T));
+        if (ok) ok = cudaMemcpy(d, host, n * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
+        return static_cast<const T *>(d);
+    }
+    template <class T> T * out(T * host, size_t n) {
+        if (!host) return nullptr;
+        const size_t bytes = n * sizeof(T) + RWKV_B200_GUARD * sizeof(float);
+        void * d = alloc(bytes);
+        if (ok) ok = cudaMemset(d, 0xFF, bytes) == cudaSuccess;
+        if (ok) outs.push_back(Out{d, host, bytes});
+        return static_cast<T *>(d);
+    }
+    // After the launch: wait for it and return every output to the host. The launch error, if any, is what gets reported.
+    bool finish(cudaError_t launch) {
+        ok = ok && launch == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
+        for (const Out & o : outs)
+            if (ok) ok = cudaMemcpy(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost) == cudaSuccess;
+        return ok;
+    }
+    ~HookBuffers() { for (void * d : allocs) cudaFree(d); }
+};
+
+// The device every test hook runs on; false (and the flags set) without one.
+bool hook_device(ErrorSink sink) {
+    int dev = default_device(), n_dev = 0;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceCount(&n_dev) == cudaSuccess && dev < n_dev && cudaSetDevice(dev) == cudaSuccess,
+               "No usable CUDA device; this engine has no CPU execution path");
+    return true;
+}
+
+// Shape of a state or activation set: n_seq = 0 -> one, else n_seq sequences seq_stride floats apart, each per_seq floats long.
+bool seq_layout_ok(int n_seq, long long seq_stride, int T, size_t per_seq) {
+    return n_seq == 0 || (n_seq > 0 && T == 1 && seq_stride >= (long long) per_seq);
+}
+size_t seq_floats(int n_seq, long long seq_stride, size_t per_seq) {
+    return n_seq > 0 ? (size_t) (n_seq - 1) * (size_t) seq_stride + per_seq : per_seq;
+}
+
+// A staged column may be requested only where the kernels emit one: single-token, single-sequence passes in which every emitting
+// warp is whole and owns whole 32-blocks of the vector. `unit` is what one warp-aligned group of threads covers: the whole vector
+// for the v4 WKV and the lerp (one thread per channel), one head (S) for the v5/6/7 WKV (act::warp_emit_block uses full-warp
+// reductions, and with S % 32 != 0 a block would straddle two heads' CTAs).
+bool staged_ok(const unsigned char * q_out, int q_type, int T, int n_seq, int unit) {
+    return !q_out || (T == 1 && n_seq == 0 && unit % 32 == 0 && act::stage_class(q_type) != act::SC_NONE);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -588,6 +656,147 @@ bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, 
     cudaError_t e = cudaGetLastError();
     cudaFree(dW); cudaFree(dx); cudaFree(dy);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "matvec failed on the device: %s", cudaGetErrorString(e));
+    return true;
+}
+
+// ---- kernel test hooks (include/rwkv_b200.h): one launcher each, on host buffers ----
+
+bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, int n_vocab, const int * tokens, int T, int C,
+                              const float * ln_w, const float * ln_b, float * x) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    bool args = emb && tokens && ln_w && ln_b && x && T > 0 && C > 0 && n_vocab > 0 && (emb_type == DT_F32 || emb_type == DT_F16) &&
+                emb_pitch >= (size_t) C * (emb_type == DT_F32 ? 4 : 2) && emb_pitch % (emb_type == DT_F32 ? 4 : 2) == 0;   // rows are read as elements
+    for (int t = 0; args && t < T; t++) args = tokens[t] >= 0 && tokens[t] < n_vocab;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid embed_ln0 arguments");
+    if (!hook_device(sink)) return false;
+    HookBuffers b;
+    const void * d_emb = b.in(static_cast<const uint8_t *>(emb), (size_t) n_vocab * emb_pitch);
+    const int * d_tok = b.in(tokens, T);
+    const float * d_w = b.in(ln_w, C), * d_b = b.in(ln_b, C);
+    float * d_x = b.out(x, (size_t) C * T);
+    const cudaError_t e = b.ok ? launch_embed_ln0(d_emb, emb_type, (long long) emb_pitch, d_tok, T, C, d_w, d_b, d_x, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "embed_ln0 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_ln_mix(const struct rwkv_b200_ln_mix_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    bool args = a && a->x && a->ln_w && a->ln_b && a->state_in && a->state_out && a->C > 0 && a->T > 0 && (a->formula == 0 || a->formula == 1) &&
+                a->n_out >= 1 && a->n_out <= 6 && seq_layout_ok(a->n_seq, a->seq_stride, a->T, (size_t) a->C);
+    for (int j = 0; args && j < a->n_out; j++) args = a->coef[j] && a->out[j];
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid ln_mix arguments");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C, cols = a->n_seq > 0 ? (size_t) a->n_seq : (size_t) a->T, st = seq_floats(a->n_seq, a->seq_stride, C);
+    HookBuffers b;
+    LnMixParams p{};
+    p.x = b.in(a->x, C * cols); p.ln_w = b.in(a->ln_w, C); p.ln_b = b.in(a->ln_b, C);
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.C = a->C; p.T = (int) cols; p.formula = a->formula; p.n_out = a->n_out;
+    for (int j = 0; j < a->n_out; j++) { p.coef[j] = b.in(a->coef[j], C); p.out[j] = b.out(a->out[j], C * cols); }
+    p.out_xx = b.out(a->out_xx, C * cols); p.out_sx = b.out(a->out_sx, C * cols);
+    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_ln_mix_batch(p, a->seq_stride, 0) : launch_ln_mix(p, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ln_mix failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_v6_lerp(const struct rwkv_b200_v6_lerp_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    bool args = a && a->w2 && a->z && a->xx && a->sx && a->C > 0 && a->T > 0 && a->mix > 0;
+    int n_q = 0;
+    for (int j = 0; args && j < 5; j++) {
+        args = a->maa[j] && a->out[j] && staged_ok(a->q_out[j], a->q_type[j], a->T, 0, a->C);
+        n_q += a->q_out[j] != nullptr;
+    }
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args && (n_q == 0 || n_q == 5), "Invalid v6_lerp arguments (staged columns: all five or none)");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C, T = (size_t) a->T, mix = (size_t) a->mix;
+    HookBuffers b;
+    V6LerpParams p{};
+    p.w2 = b.in(a->w2, 5 * C * mix); p.z = b.in(a->z, 5 * mix * T); p.xx = b.in(a->xx, C * T); p.sx = b.in(a->sx, C * T);
+    for (int j = 0; j < 5; j++) {
+        p.maa[j] = b.in(a->maa[j], C); p.out[j] = b.out(a->out[j], C * T);
+        p.q_out[j] = a->q_out[j] ? b.out(a->q_out[j], act::bytes_per_column(a->q_type[j], a->C)) : nullptr;
+        p.q_type[j] = a->q_type[j];
+    }
+    p.C = a->C; p.T = a->T; p.mix = a->mix;
+    const cudaError_t e = b.ok ? launch_v6_lerp(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "v6_lerp failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv4(const struct rwkv_b200_wkv4_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const bool args = a && a->k && a->v && a->r && a->time_first && a->time_decay && a->aa_in && a->bb_in && a->pp_in && a->aa_out && a->bb_out && a->pp_out && a->y &&
+                      a->C > 0 && a->T > 0 && seq_layout_ok(a->n_seq, a->seq_stride, a->T, (size_t) a->C) && staged_ok(a->q_out, a->q_type, a->T, a->n_seq, a->C);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid wkv4 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C, cols = a->n_seq > 0 ? (size_t) a->n_seq : (size_t) a->T, st = seq_floats(a->n_seq, a->seq_stride, C);
+    HookBuffers b;
+    Wkv4Params p{};
+    p.k = b.in(a->k, C * cols); p.v = b.in(a->v, C * cols); p.r = b.in(a->r, C * cols);
+    p.time_first = b.in(a->time_first, C); p.time_decay = b.in(a->time_decay, C);
+    p.aa_in = b.in(a->aa_in, st); p.bb_in = b.in(a->bb_in, st); p.pp_in = b.in(a->pp_in, st);
+    p.aa_out = b.out(a->aa_out, st); p.bb_out = b.out(a->bb_out, st); p.pp_out = b.out(a->pp_out, st);
+    p.y = b.out(a->y, C * cols);
+    p.C = a->C; p.T = (int) cols;
+    p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, a->C)) : nullptr; p.q_type = a->q_type;
+    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv4_batch(p, a->seq_stride, 0) : launch_wkv4(p, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv4 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv6(const struct rwkv_b200_wkv6_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const size_t C = a ? (size_t) a->H * (size_t) a->S : 0, SS = a ? C * (size_t) a->S : 0;
+    const bool args = a && a->r && a->k && a->v && a->td && a->tf && a->state_in && a->state_out && a->lnx_w && a->lnx_b && a->y && a->H > 0 && a->S > 0 && a->T > 0 &&
+                      !(a->td_per_token && a->per_head_scalars) && seq_layout_ok(a->n_seq, a->seq_stride, a->T, SS) &&
+                      a->seq_stride % 4 == 0 &&          // the batch kernel moves the state in float4s from state + seq * seq_stride
+                      staged_ok(a->q_out, a->q_type, a->T, a->n_seq, a->S);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid wkv6 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t cols = a->n_seq > 0 ? (size_t) a->n_seq : (size_t) a->T, st = seq_floats(a->n_seq, a->seq_stride, SS);
+    HookBuffers b;
+    Wkv6Params p{};
+    p.r = b.in(a->r, C * cols); p.k = b.in(a->k, C * cols); p.v = b.in(a->v, C * cols);
+    p.td = b.in(a->td, a->td_per_token ? C * cols : a->per_head_scalars ? (size_t) a->H : C);
+    p.tf = b.in(a->tf, a->per_head_scalars ? (size_t) a->H : C);
+    p.td_per_token = a->td_per_token; p.per_head_scalars = a->per_head_scalars;
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C); p.g = b.in(a->g, C * cols);
+    p.y = b.out(a->y, C * cols);
+    p.eps = a->eps; p.H = a->H; p.S = a->S; p.T = (int) cols;
+    p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
+    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv6_batch(p, a->seq_stride, 0) : launch_wkv6(p, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv6 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const size_t C = a ? (size_t) a->H * (size_t) a->S : 0, SS = a ? C * (size_t) a->S : 0;
+    const bool args = a && a->r && a->w && a->k && a->v && a->a && a->g && (!a->vgate || a->v_first) && a->k_k && a->k_a && a->r_k && a->lnx_w && a->lnx_b &&
+                      a->state_in && a->state_out && a->y && a->H > 0 && a->S > 0 && a->T > 0 && seq_layout_ok(a->n_seq, a->seq_stride, a->T, SS) &&
+                      staged_ok(a->q_out, a->q_type, a->T, a->n_seq, a->S);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid wkv7 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t cols = a->n_seq > 0 ? (size_t) a->n_seq : (size_t) a->T, st = seq_floats(a->n_seq, a->seq_stride, SS), n = C * cols;
+    HookBuffers b;
+    Wkv7Params p{};
+    p.r = b.in(a->r, n); p.w = b.in(a->w, n); p.k = b.in(a->k, n); p.v = b.in(a->v, n); p.a = b.in(a->a, n); p.g = b.in(a->g, n);
+    p.vgate = b.in(a->vgate, n); p.v_first = a->vgate ? b.in(a->v_first, n) : nullptr; p.v_out = b.out(a->v_out, n);
+    p.k_k = b.in(a->k_k, C); p.k_a = b.in(a->k_a, C); p.r_k = b.in(a->r_k, C); p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C);
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.y = b.out(a->y, n);
+    p.H = a->H; p.S = a->S; p.T = (int) cols;
+    p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
+    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv7_batch(p, a->seq_stride, 0) : launch_wkv7(p, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

@@ -1,7 +1,7 @@
-// Single-token building blocks shared by the persistent decode kernel (decode_persistent.cu) and the batched multi-sequence
-// kernels (batch.cu): LayerNorm statistics and one WKV5/6 step, restated from glue.cu / wkv.cu for T = 1 with the same per-element
-// operations and reduction trees, so their results are bit-identical to the per-launch kernels'. All of them are written for a
-// group of exactly 256 threads that synchronises with tma::consumer_barrier() (named barrier 1).
+// Single-token building blocks of the batched multi-sequence kernels (batch.cu): LayerNorm statistics and one WKV5/6 step,
+// restated from glue.cu / wkv.cu for T = 1 with the same per-element operations and reduction trees, so their results are
+// bit-identical to the per-launch kernels' (tests/test_gpu_kernels.py checks it). All of them are written for a group of exactly
+// 256 threads that synchronises with tma::consumer_barrier() (named barrier 1).
 #pragma once
 #include "gemv_tma_device.cuh"
 

@@ -1,0 +1,193 @@
+"""ctypes bindings of the kernel test hooks (rwkv_b200_test_* in include/rwkv_b200.h). Activations go in and come out as numpy
+[dim, T] arrays; every output comes back with the guard region the hook returns, so a test can tell a value the kernel never wrote
+(still NaN from the 0xFF fill) and a write past the end (a guard byte that is no longer 0xFF) from a wrong value."""
+import ctypes
+
+import numpy as np
+
+from kernel_ref import staged_bytes
+
+GUARD = 64            # RWKV_B200_GUARD: floats after the end of every output
+GUARD_BYTES = 4 * GUARD
+VP = ctypes.c_void_p
+F6, P5, I5 = VP * 6, VP * 5, ctypes.c_int * 5
+
+
+class LnMixArgs(ctypes.Structure):
+    _fields_ = [("x", VP), ("ln_w", VP), ("ln_b", VP), ("state_in", VP), ("state_out", VP), ("C", ctypes.c_int), ("T", ctypes.c_int),
+                ("formula", ctypes.c_int), ("n_out", ctypes.c_int), ("coef", F6), ("out", F6), ("out_xx", VP), ("out_sx", VP),
+                ("n_seq", ctypes.c_int), ("seq_stride", ctypes.c_longlong)]
+
+
+class V6LerpArgs(ctypes.Structure):
+    _fields_ = [("w2", VP), ("z", VP), ("xx", VP), ("sx", VP), ("maa", P5), ("out", P5), ("C", ctypes.c_int), ("T", ctypes.c_int),
+                ("mix", ctypes.c_int), ("q_out", P5), ("q_type", I5)]
+
+
+class Wkv4Args(ctypes.Structure):
+    _fields_ = [("k", VP), ("v", VP), ("r", VP), ("time_first", VP), ("time_decay", VP), ("aa_in", VP), ("bb_in", VP), ("pp_in", VP),
+                ("aa_out", VP), ("bb_out", VP), ("pp_out", VP), ("y", VP), ("C", ctypes.c_int), ("T", ctypes.c_int), ("q_out", VP),
+                ("q_type", ctypes.c_int), ("n_seq", ctypes.c_int), ("seq_stride", ctypes.c_longlong)]
+
+
+class Wkv6Args(ctypes.Structure):
+    _fields_ = [("r", VP), ("k", VP), ("v", VP), ("td", VP), ("tf", VP), ("td_per_token", ctypes.c_int), ("per_head_scalars", ctypes.c_int),
+                ("state_in", VP), ("state_out", VP), ("lnx_w", VP), ("lnx_b", VP), ("g", VP), ("y", VP), ("eps", ctypes.c_float),
+                ("H", ctypes.c_int), ("S", ctypes.c_int), ("T", ctypes.c_int), ("q_out", VP), ("q_type", ctypes.c_int),
+                ("n_seq", ctypes.c_int), ("seq_stride", ctypes.c_longlong)]
+
+
+class Wkv7Args(ctypes.Structure):
+    _fields_ = [("r", VP), ("w", VP), ("k", VP), ("v", VP), ("a", VP), ("g", VP), ("vgate", VP), ("v_first", VP), ("v_out", VP),
+                ("k_k", VP), ("k_a", VP), ("r_k", VP), ("lnx_w", VP), ("lnx_b", VP), ("state_in", VP), ("state_out", VP), ("y", VP),
+                ("H", ctypes.c_int), ("S", ctypes.c_int), ("T", ctypes.c_int), ("q_out", VP), ("q_type", ctypes.c_int),
+                ("n_seq", ctypes.c_int), ("seq_stride", ctypes.c_longlong)]
+
+
+class HookError(RuntimeError):
+    def __init__(self, flags):
+        super().__init__("kernel hook failed, error flags 0x%x" % flags)
+        self.flags = flags
+
+
+class Out:
+    """A host output buffer of n elements plus the guard region (GUARD_BYTES bytes)."""
+
+    def __init__(self, n, dtype=np.float32):
+        self.n = n
+        self.buf = np.zeros(n + GUARD_BYTES // np.dtype(dtype).itemsize, dtype)
+
+    @property
+    def ptr(self):
+        return self.buf.ctypes.data
+
+    @property
+    def value(self):
+        return self.buf[:self.n]
+
+    def cols(self, C):
+        """The value as a [C, T] array."""
+        return self.value.reshape(-1, C).T
+
+    def guard_intact(self):
+        return bool((self.buf[self.n:].view(np.uint8) == 0xFF).all())
+
+
+class Inputs:
+    """Keeps the contiguous float32 copies of the inputs alive for the duration of a call."""
+
+    def __init__(self):
+        self.keep = []
+
+    def __call__(self, a, columns=False):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a.T if columns else a, np.float32)    # [C, T] -> column t contiguous
+        self.keep.append(a)
+        return a.ctypes.data
+
+
+def _call(lib, fn, args):
+    if not fn(ctypes.byref(args)):
+        raise HookError(lib.rwkv_get_last_error(None))
+
+
+def embed_ln0(lib, emb, tokens, w, b):
+    """emb: [n_vocab, C] float32 or float16 table. Returns Out of C*T floats."""
+    n_vocab, C = emb.shape
+    emb = np.ascontiguousarray(emb)
+    tok = np.ascontiguousarray(tokens, np.int32)
+    w, b = np.ascontiguousarray(w, np.float32), np.ascontiguousarray(b, np.float32)
+    x = Out(C * tok.size)
+    ok = lib.library.rwkv_b200_test_embed_ln0(VP(emb.ctypes.data), ctypes.c_int(0 if emb.dtype == np.float32 else 1), ctypes.c_size_t(emb.strides[0]),
+                                              ctypes.c_int(n_vocab), VP(tok.ctypes.data), ctypes.c_int(tok.size), ctypes.c_int(C), VP(w.ctypes.data),
+                                              VP(b.ctypes.data), VP(x.ptr))
+    if not ok:
+        raise HookError(lib.rwkv_get_last_error(None))
+    return x
+
+
+def ln_mix(lib, x, w, b, state_in, coefs, formula, n_seq=0, seq_stride=0, xx=True, sx=True):
+    """x: [C, T] (or [C, n_seq] with n_seq > 0, state_in then holding n_seq states seq_stride floats apart).
+    Returns dict of Out: out0.., xx, sx, state."""
+    C, cols = x.shape
+    i = Inputs()
+    a = LnMixArgs(x=i(x, True), ln_w=i(w), ln_b=i(b), state_in=i(state_in), C=C, T=1 if n_seq else cols, formula=formula, n_out=len(coefs),
+                  n_seq=n_seq, seq_stride=seq_stride)
+    o = {"state": Out(state_in.size)}
+    a.state_out = o["state"].ptr
+    for j, m in enumerate(coefs):
+        o["out%d" % j] = Out(C * cols)
+        a.coef[j], a.out[j] = i(m), o["out%d" % j].ptr
+    if xx:
+        o["xx"] = Out(C * cols)
+        a.out_xx = o["xx"].ptr
+    if sx:
+        o["sx"] = Out(C * cols)
+        a.out_sx = o["sx"].ptr
+    _call(lib, lib.library.rwkv_b200_test_ln_mix, a)
+    return o
+
+
+def v6_lerp(lib, w2, z, xx, sx, maa, q_types=None):
+    """w2: [5, C, mix]; z: [5*mix, T]; maa: [5, C]. Returns dict of Out: out0..out4 and q0..q4 when q_types is given."""
+    _, C, mix = w2.shape
+    T = z.shape[1]
+    i = Inputs()
+    a = V6LerpArgs(w2=i(w2), z=i(z, True), xx=i(xx, True), sx=i(sx, True), C=C, T=T, mix=mix)
+    o = {}
+    for j in range(5):
+        o["out%d" % j] = Out(C * T)
+        a.maa[j], a.out[j] = i(maa[j]), o["out%d" % j].ptr
+        if q_types is not None:
+            o["q%d" % j] = Out(staged_bytes(q_types[j], C), np.uint8)
+            a.q_out[j], a.q_type[j] = o["q%d" % j].ptr, q_types[j]
+    _call(lib, lib.library.rwkv_b200_test_v6_lerp, a)
+    return o
+
+
+def _staged(o, a, q_type, K):
+    if q_type is not None:
+        o["q"] = Out(staged_bytes(q_type, K), np.uint8)
+        a.q_out, a.q_type = o["q"].ptr, q_type
+
+
+def wkv4(lib, k, v, r, tf, td, aa, bb, pp, n_seq=0, seq_stride=0, q_type=None):
+    C, cols = k.shape
+    i = Inputs()
+    a = Wkv4Args(k=i(k, True), v=i(v, True), r=i(r, True), time_first=i(tf), time_decay=i(td), aa_in=i(aa), bb_in=i(bb), pp_in=i(pp), C=C,
+                 T=1 if n_seq else cols, n_seq=n_seq, seq_stride=seq_stride)
+    o = {"aa": Out(aa.size), "bb": Out(bb.size), "pp": Out(pp.size), "y": Out(C * cols)}
+    a.aa_out, a.bb_out, a.pp_out, a.y = o["aa"].ptr, o["bb"].ptr, o["pp"].ptr, o["y"].ptr
+    _staged(o, a, q_type, C)
+    _call(lib, lib.library.rwkv_b200_test_wkv4, a)
+    return o
+
+
+def wkv6(lib, r, k, v, td, tf, state, lnx_w, lnx_b, g, eps, H, S, td_per_token, per_head, n_seq=0, seq_stride=0, q_type=None):
+    C, cols = r.shape
+    i = Inputs()
+    a = Wkv6Args(r=i(r, True), k=i(k, True), v=i(v, True), td=i(td, td_per_token), tf=i(tf), td_per_token=int(td_per_token),
+                 per_head_scalars=int(per_head), state_in=i(state), lnx_w=i(lnx_w), lnx_b=i(lnx_b), g=i(g, True), eps=eps, H=H, S=S,
+                 T=1 if n_seq else cols, n_seq=n_seq, seq_stride=seq_stride)
+    o = {"state": Out(state.size), "y": Out(C * cols)}
+    a.state_out, a.y = o["state"].ptr, o["y"].ptr
+    _staged(o, a, q_type, C)
+    _call(lib, lib.library.rwkv_b200_test_wkv6, a)
+    return o
+
+
+def wkv7(lib, r, w, k, v, aa, g, vgate, v_first, k_k, k_a, r_k, lnx_w, lnx_b, state, H, S, v_out=True, n_seq=0, seq_stride=0, q_type=None):
+    C, cols = r.shape
+    i = Inputs()
+    a = Wkv7Args(r=i(r, True), w=i(w, True), k=i(k, True), v=i(v, True), a=i(aa, True), g=i(g, True), vgate=i(vgate, True),
+                 v_first=i(v_first, True), k_k=i(k_k), k_a=i(k_a), r_k=i(r_k), lnx_w=i(lnx_w), lnx_b=i(lnx_b), state_in=i(state),
+                 H=H, S=S, T=1 if n_seq else cols, n_seq=n_seq, seq_stride=seq_stride)
+    o = {"state": Out(state.size), "y": Out(C * cols)}
+    a.state_out, a.y = o["state"].ptr, o["y"].ptr
+    if v_out:
+        o["v"] = Out(C * cols)
+        a.v_out = o["v"].ptr
+    _staged(o, a, q_type, C)
+    _call(lib, lib.library.rwkv_b200_test_wkv7, a)
+    return o

@@ -124,6 +124,50 @@ def test_no_cpu_fallback(lib):
     assert not ok
 
 
+def test_kernel_hooks_reject_invalid_arguments(lib):
+    """The kernel test hooks check their arguments before they touch a device: staged columns only for single-token, single-sequence
+    passes in which whole warps emit whole 32-blocks (head size a multiple of 32 for the v5/6/7 WKV, not just n_embed) and for a
+    weight type that has a stage class, batch passes of one token with non-overlapping states (and float4-aligned ones for the v5/6
+    batch kernel), known formulas, tokens inside the table, embedding rows aligned to their element type, the lerp's staged columns
+    all or none."""
+    import kernel_hooks as kh
+    f = lambda *shape: np.ones(shape, np.float32)
+    Q = gf.TYPE_IDS["Q5_0"]
+    cases = [
+        lambda: kh.wkv6(lib, f(64, 2), f(64, 2), f(64, 2), f(64, 2), f(64), f(64 * 64), f(64), f(64), None, 1e-5, 1, 64, True, False, q_type=Q),
+        lambda: kh.wkv6(lib, f(16, 1), f(16, 1), f(16, 1), f(16, 1), f(16), f(2 * 8 * 8), f(16), f(16), None, 1e-5, 2, 8, True, False, q_type=Q),
+        lambda: kh.wkv6(lib, f(64, 2), f(64, 2), f(64, 2), f(64, 2), f(64), f(2 * 64 * 64), f(64), f(64), None, 1e-5, 1, 64, True, False, n_seq=2,
+                        seq_stride=100),
+        # n_embed 32 is whole 32-blocks, but heads of 8 are not: a block would span four CTAs, each a quarter of a warp
+        lambda: kh.wkv6(lib, f(32, 1), f(32, 1), f(32, 1), f(32, 1), f(32), f(4 * 8 * 8), f(32), f(32), None, 1e-5, 4, 8, True, False, q_type=Q),
+        lambda: kh.wkv7(lib, *[f(32, 1)] * 6, None, None, *[f(32)] * 5, f(4 * 8 * 8), 4, 8, q_type=Q),
+        lambda: kh.wkv7(lib, *[f(64, 1)] * 6, None, None, *[f(64)] * 5, f(4 * 16 * 16), 4, 16, q_type=Q),
+        lambda: kh.wkv6(lib, f(64, 2), f(64, 2), f(64, 2), f(64, 2), f(64), f(64 * 64 + 4098), f(64), f(64), None, 1e-5, 1, 64, True, False, n_seq=2,
+                        seq_stride=4098),                                                                     # not a multiple of 4
+        lambda: kh.wkv4(lib, f(64, 1), f(64, 1), f(64, 1), f(64), f(64), f(64), f(64), f(64), q_type=5),      # removed format Q4_2
+        lambda: kh.ln_mix(lib, f(64, 2), f(64), f(64), f(64 + 64), [f(64)], 0, n_seq=2, seq_stride=32),
+        lambda: kh.ln_mix(lib, f(64, 1), f(64), f(64), f(64), [f(64)], 2),
+        lambda: kh.embed_ln0(lib, np.ones((4, 64), np.float32), [0, 4], f(64), f(64)),
+    ]
+    for i, call in enumerate(cases):
+        with pytest.raises(kh.HookError) as e:
+            call()
+        assert e.value.flags == ERR["ARGS"], i
+    emb, one = np.ones(4 * 66, np.float32), np.ones(64, np.float32)      # F32 rows 258 bytes apart
+    tok = np.zeros(1, np.int32)
+    assert not lib.library.rwkv_b200_test_embed_ln0(ctypes.c_void_p(emb.ctypes.data), 0, ctypes.c_size_t(258), 3, ctypes.c_void_p(tok.ctypes.data), 1, 64,
+                                                    ctypes.c_void_p(one.ctypes.data), ctypes.c_void_p(one.ctypes.data), ctypes.c_void_p(emb.ctypes.data))
+    assert lib.rwkv_get_last_error(None) == ERR["ARGS"]
+    a = kh.V6LerpArgs(C=64, T=1, mix=32)          # staged columns for two of the five outputs
+    buf = np.zeros(4096, np.float32)
+    a.w2 = a.z = a.xx = a.sx = buf.ctypes.data
+    for j in range(5):
+        a.maa[j] = a.out[j] = buf.ctypes.data
+    a.q_out[0] = a.q_out[1] = buf.ctypes.data
+    assert not lib.library.rwkv_b200_test_v6_lerp(ctypes.byref(a))
+    assert lib.rwkv_get_last_error(None) == ERR["ARGS"]
+
+
 @pytest.mark.parametrize("fmt", QUANT_FORMATS)
 def test_quantizer_bit_exact_vs_oracle(lib, fmt, tmp_path):
     """rwkv_quantize_model_file (rwkv_quantize.inc:16-171) vs the numpy restatement of quantize_row_*_ref, tensor by tensor."""
