@@ -255,6 +255,46 @@ struct rwkv_b200_wkv7_args {
 };
 RWKV_API bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a);
 
+/* A batch of up to 8 matrix problems y_i[M_i, T] = epi_i(W_i . pro_i(x[input_i])) launched the way the eval path launches them
+ * (csrc/kernels/gemv.h). Weights go up through the model loader's code (row pitch, zeroed row padding, device layout, and the
+ * tile-major tensor-core copy when `tiled` is set). Problems whose `input` index is the same share one device input, as the
+ * mixed inputs of a layer do. epi: 0 none, 1 sigmoid, 2 silu, 3 tanh, 4 relu^2, 5 res + v, 6 res + gate * v, 7 exp(-exp(v + bias)),
+ * 8 sigmoid(v + bias), 9 exp(-0.606531 * sigmoid(v + bias)); res / gate [M, T], bias [M]. pro 1: LayerNorm of the input (ln_w,
+ * ln_b [K], eps 1e-5). y_aliases_res: the device y starts as a copy of res and is also the residual the kernel reads (x += ...).
+ * xq: the input's column already staged for this problem's weight type (csrc/kernels/act_stage.cuh layout), T = 1 only.
+ * Outputs need RWKV_B200_GUARD floats of room after their end, as for the hooks above.
+ * path: */
+#define RWKV_B200_GEMV_ENGINE 0            /* single-sequence context: tensor cores for T >= 32, the rest through the GEMV */
+#define RWKV_B200_GEMV_ENGINE_BATCH_CTX 1  /* batch context: tensor cores from T >= 16 */
+#define RWKV_B200_GEMV_STREAMING 2         /* the TMA streaming GEMV only (CTX | UNSUPPORTED if a shape does not fit it) */
+#define RWKV_B200_GEMV_GENERIC 3           /* the generic GEMV only */
+#define RWKV_B200_GEMV_TENSOR_CORES 4      /* the tensor-core GEMM only (CTX | UNSUPPORTED unless every problem can take it) */
+struct rwkv_b200_gemv_problem {
+    int type, K, M;
+    const void * weights;                  /* M rows in the file layout of `type`, unpadded */
+    int tiled;
+    int input;                             /* 0 .. 7: which x[] */
+    int epi, pro;
+    const float * res, * gate, * bias, * ln_w, * ln_b;
+    const unsigned char * xq;
+    int y_aliases_res;
+    float * y;
+};
+/* One kernel launch: family 0 streaming GEMV, 1 generic GEMV, 2 tensor-core GEMM, 3 fp16 operand conversion, 4 tensor-core weight
+ * expansion (of the upload). nc: columns per group (streaming, generic) or distinct inputs (conversion); only: the streaming
+ * kernel's single weight type (-1: mixed) or the expanded type; has_ln: the streaming kernel's LayerNorm code; npad: tokens padded
+ * to 16; cluster: CTAs per cluster of the GEMM. */
+struct rwkv_b200_gemv_launch { int family, nc, only, has_ln, npad, cluster; };
+struct rwkv_b200_gemv_batch_args {
+    int T, n, path;
+    const float * x[8];                    /* [K, T] column-major, K of the problems that read it */
+    struct rwkv_b200_gemv_problem p[8];
+    struct rwkv_b200_gemv_launch * launches;   /* optional record, max_launches entries; *n_launches = entries written */
+    int max_launches;
+    int * n_launches;
+};
+RWKV_API bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -61,6 +61,12 @@ struct HookBuffers {
         if (ok) outs.push_back(Out{d, host, bytes});
         return static_cast<T *>(d);
     }
+    // An output that starts as a copy of `init` (a buffer the kernel updates in place); guard and return as for out().
+    template <class T> T * inout(const T * init, T * host, size_t n) {
+        T * d = out(host, n);
+        if (ok && d) ok = cudaMemcpy(d, init, n * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
+        return d;
+    }
     // After the launch: wait for it and return every output to the host. The launch error, if any, is what gets reported.
     bool finish(cudaError_t launch) {
         ok = ok && launch == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
@@ -622,39 +628,26 @@ bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, 
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, dev);
     DeviceInfo di{dev, prop.multiProcessorCount, (int) prop.sharedMemPerBlockOptin};
-    const size_t row_bytes = tensor_nbytes(data_type, (uint64_t) K, 1, 1);
-    size_t unit_bytes = row_bytes;
-    if (data_type == DT_Q4_0 || data_type == DT_Q5_0 || data_type == DT_Q8_0) unit_bytes = (size_t) ((K / 32 + 1) / 2 * 2) * dtype_block_bytes(data_type);
-    const size_t pitch = (unit_bytes + 15) / 16 * 16;
-    uint8_t * dW = nullptr; float * dx = nullptr, * dy = nullptr;
-    bool ok = cudaMalloc((void **) &dW, pitch * M + 256) == cudaSuccess && cudaMalloc((void **) &dx, sizeof(float) * K * T) == cudaSuccess &&
-              cudaMalloc((void **) &dy, sizeof(float) * M * T) == cudaSuccess;
-    ok = ok && cudaMemset(dW, 0, pitch * M + 256) == cudaSuccess &&
-         cudaMemcpy2D(dW, pitch, weights, row_bytes, row_bytes, M, cudaMemcpyHostToDevice) == cudaSuccess &&
-         cudaMemcpy(dx, x, sizeof(float) * K * T, cudaMemcpyHostToDevice) == cudaSuccess &&
-         weights_to_device_layout(dW, (long long) pitch, data_type, M, K, 0) == cudaSuccess;       // what the model loader does after an upload
+    // passes of >= 32 tokens go through the tensor-core kernel, which streams the tile-major copy of the matrix
+    const bool tiled = T >= 32 && gemm_tc_eligible(data_type, K) && !getenv("RWKV_B200_NO_TC");
+    const size_t ws_bytes = gemm_tc_batch_workspace_bytes(T, (size_t) K);
+    uint8_t * dW = nullptr, * dWt = nullptr; float * dx = nullptr, * dy = nullptr; void * ws = nullptr;
+    bool ok = cudaMalloc((void **) &dW, (size_t) matrix_pitch(data_type, (uint64_t) K) * M + 256) == cudaSuccess && cudaMalloc((void **) &dx, sizeof(float) * K * T) == cudaSuccess &&
+              cudaMalloc((void **) &dy, sizeof(float) * M * T) == cudaSuccess && cudaMemcpy(dx, x, sizeof(float) * K * T, cudaMemcpyHostToDevice) == cudaSuccess &&
+              (!tiled || (cudaMalloc((void **) &dWt, gemm_tc_tiled_bytes(data_type, M, K)) == cudaSuccess && cudaMalloc(&ws, ws_bytes) == cudaSuccess)) &&
+              upload_matrix(weights, data_type, M, K, dW, dWt) == cudaSuccess;
     if (ok) {
         GemvBatch b;
         memset(&b, 0, sizeof(b));
         b.n = 1; b.T = T;
         GemvProblem & p = b.p[0];
-        p.W = dW; p.pitch = (long long) pitch; p.type = data_type; p.K = K; p.M = M;
+        p.W = dW; p.Wt = dWt; p.pitch = matrix_pitch(data_type, (uint64_t) K); p.type = data_type; p.K = K; p.M = M;
         p.x = dx; p.ldx = K; p.y = dy; p.ldy = M; p.epi = epilogue; p.pro = PRO_NONE;
-        void * act16 = nullptr, * tiled = nullptr;
-        const size_t act16_bytes = gemm_tc_workspace_bytes(T, (size_t) ((T + 15) / 16 * 16) * K + 128);
-        // passes of >= 32 tokens go through the tensor-core kernel, which streams the tile-major copy of the matrix
-        if (T >= 32 && gemm_tc_eligible(data_type, K) && !getenv("RWKV_B200_NO_TC")) {
-            ok = cudaMalloc(&tiled, gemm_tc_tiled_bytes(data_type, M, K)) == cudaSuccess && gemm_tc_repack(dW, (long long) pitch, data_type, M, K, tiled, 0) == cudaSuccess;
-            p.Wt = tiled;
-        }
-        const bool use_tc = ok && gemm_tc_supported(p, T);
-        if (use_tc) ok = cudaMalloc(&act16, act16_bytes) == cudaSuccess && gemm_tc_launch(b, di, 0, act16, act16_bytes) == cudaSuccess;
-        else ok = gemv_launch(b, di, 0) == cudaSuccess;
-        ok = ok && cudaDeviceSynchronize() == cudaSuccess && cudaMemcpy(y, dy, sizeof(float) * M * T, cudaMemcpyDeviceToHost) == cudaSuccess;
-        cudaFree(act16); cudaFree(tiled);
+        ok = gemv_route(b, di, 0, ws, ws_bytes, 32) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess &&
+             cudaMemcpy(y, dy, sizeof(float) * M * T, cudaMemcpyDeviceToHost) == cudaSuccess;
     }
     cudaError_t e = cudaGetLastError();
-    cudaFree(dW); cudaFree(dx); cudaFree(dy);
+    cudaFree(dW); cudaFree(dWt); cudaFree(dx); cudaFree(dy); cudaFree(ws);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "matvec failed on the device: %s", cudaGetErrorString(e));
     return true;
 }
@@ -797,6 +790,95 @@ bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a) {
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
     const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv7_batch(p, a->seq_stride, 0) : launch_wkv7(p, 0);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    bool args = a && a->T >= 1 && a->T <= 256 && a->n >= 1 && a->n <= GEMV_MAX_PROBLEMS && a->path >= RWKV_B200_GEMV_ENGINE &&
+                a->path <= RWKV_B200_GEMV_TENSOR_CORES && (!a->launches || (a->n_launches && a->max_launches >= 0));
+    int input_K[GEMV_MAX_PROBLEMS] = {};
+    for (int i = 0; args && i < a->n; i++) {
+        const rwkv_b200_gemv_problem & q = a->p[i];
+        const bool ln = q.pro == PRO_LAYERNORM, res_epi = q.epi == EPI_ADD || q.epi == EPI_MUL_ADD, bias_epi = q.epi >= EPI_BIAS_EXPNEGEXP;
+        args = q.weights && q.y && dtype_supported(q.type) && q.K > 0 && q.M > 0 && q.K % dtype_block_elems(q.type) == 0 &&
+               q.input >= 0 && q.input < GEMV_MAX_PROBLEMS && a->x[q.input] && (input_K[q.input] == 0 || input_K[q.input] == q.K) &&
+               q.epi >= EPI_NONE && q.epi <= EPI_BIAS_W7 && (q.pro == PRO_NONE || ln) &&
+               !q.res == !res_epi && !q.gate == (q.epi != EPI_MUL_ADD) && !q.bias == !bias_epi && (!q.y_aliases_res || q.res) &&
+               !q.ln_w == !ln && !q.ln_b == !ln &&
+               (!q.xq || (a->T == 1 && act::stage_class(q.type) != act::SC_NONE)) &&   // the streaming kernel reads xq of single-token launches only
+               (!q.tiled || gemm_tc_eligible(q.type, q.K));
+        if (args) input_K[q.input] = q.K;
+    }
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid gemv_batch arguments");
+    if (!hook_device(sink)) return false;
+    cudaDeviceProp prop;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceProperties(&prop, default_device()) == cudaSuccess, "cudaGetDeviceProperties failed");
+    const DeviceInfo di{default_device(), prop.multiProcessorCount, (int) prop.sharedMemPerBlockOptin};
+    LaunchLog log{};
+    struct LogScope {
+        explicit LogScope(LaunchLog * l) { g_launch_log = l; }
+        ~LogScope() { g_launch_log = nullptr; }
+    } scope(a->launches ? &log : nullptr);      // from the upload on: the tensor-core weight expansion is recorded too
+    HookBuffers b;
+    const size_t T = (size_t) a->T;
+    const float * dx[GEMV_MAX_PROBLEMS] = {};
+    size_t k_max = 0;
+    for (int j = 0; j < GEMV_MAX_PROBLEMS; j++) {
+        if (input_K[j]) dx[j] = b.in(a->x[j], (size_t) input_K[j] * T);
+        if ((size_t) input_K[j] > k_max) k_max = (size_t) input_K[j];
+    }
+    GemvBatch batch;
+    memset(&batch, 0, sizeof(batch));
+    batch.n = a->n; batch.T = a->T;
+    bool tc_ok = true;
+    for (int i = 0; i < a->n; i++) {
+        const rwkv_b200_gemv_problem & q = a->p[i];
+        GemvProblem & p = batch.p[i];
+        const size_t MT = (size_t) q.M * T;
+        p.type = q.type; p.K = q.K; p.M = q.M;
+        p.pitch = matrix_pitch(q.type, (uint64_t) q.K);
+        uint8_t * W = static_cast<uint8_t *>(b.alloc((size_t) q.M * (size_t) p.pitch + 256));
+        uint8_t * Wt = q.tiled ? static_cast<uint8_t *>(b.alloc(gemm_tc_tiled_bytes(q.type, q.M, q.K))) : nullptr;
+        if (b.ok) b.ok = upload_matrix(q.weights, q.type, q.M, q.K, W, Wt) == cudaSuccess;
+        p.W = W; p.Wt = Wt;
+        p.x = dx[q.input]; p.ldx = q.K;
+        p.y = q.y_aliases_res ? b.inout(q.res, q.y, MT) : b.out(q.y, MT); p.ldy = q.M;
+        p.res = q.y_aliases_res ? p.y : b.in(q.res, MT); p.ldres = q.M;
+        p.gate = b.in(q.gate, MT); p.ldgate = q.M;
+        p.bias = b.in(q.bias, (size_t) q.M);
+        p.ln_w = b.in(q.ln_w, (size_t) q.K); p.ln_b = b.in(q.ln_b, (size_t) q.K);
+        p.xq = q.xq ? b.in(q.xq, act::bytes_per_column(q.type, q.K)) : nullptr;
+        p.epi = q.epi; p.pro = q.pro;
+        tc_ok = tc_ok && gemm_tc_supported(p, a->T);
+    }
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, a->path != RWKV_B200_GEMV_TENSOR_CORES || !b.ok || tc_ok,
+               "A problem of the batch cannot take the tensor-core path");
+    void * ws = nullptr;
+    size_t ws_bytes = 0;
+    if (a->path == RWKV_B200_GEMV_ENGINE || a->path == RWKV_B200_GEMV_ENGINE_BATCH_CTX || a->path == RWKV_B200_GEMV_TENSOR_CORES) {
+        ws_bytes = gemm_tc_batch_workspace_bytes(a->T, k_max);      // as the engine sizes its workspace (ensure_capacity)
+        ws = b.alloc(ws_bytes);
+    }
+    cudaError_t e = cudaSuccess;
+    if (b.ok) {
+        switch (a->path) {
+            case RWKV_B200_GEMV_STREAMING: e = gemv_tma_launch(batch, di, 0); break;
+            case RWKV_B200_GEMV_GENERIC: e = gemv_generic_launch(batch, di, 0); break;
+            case RWKV_B200_GEMV_TENSOR_CORES: e = gemm_tc_launch(batch, di, 0, ws, ws_bytes); break;
+            default: e = gemv_route(batch, di, 0, ws, ws_bytes, a->path == RWKV_B200_GEMV_ENGINE ? 32 : 16); break;
+        }
+    }
+    if (a->launches) {
+        const int n = log.n < a->max_launches ? log.n : a->max_launches;
+        for (int i = 0; i < n; i++) {
+            const LaunchRec & r = log.rec[i];
+            a->launches[i] = rwkv_b200_gemv_launch{r.family, r.nc, r.only, r.has_ln, r.npad, r.cluster};
+        }
+        *a->n_launches = n;
+    }
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "gemv_batch failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

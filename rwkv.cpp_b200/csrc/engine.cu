@@ -137,19 +137,8 @@ void xq_bind(GemvProblem & p, const unsigned char * q, int q_type) {
 bool launch_batch(Context * ctx, GemvBatch & b) {
     // tensor cores: chunks of >= 32 tokens; batch contexts (one token of each of B sequences: nothing to stay bit-identical with
     // across pass sizes) from 16 sequences on, where the multi-column SIMT consumer is instruction-bound
-    if ((b.T >= 32 || (ctx->batch_n > 0 && b.T >= BATCH_TC_MIN)) && ctx->use_tensor_cores && ctx->act16) {
-        GemvBatch tcb, rest;
-        memset(&tcb, 0, sizeof(tcb)); memset(&rest, 0, sizeof(rest));
-        tcb.T = rest.T = b.T;
-        for (int i = 0; i < b.n; i++) {
-            if (gemm_tc_supported(b.p[i], b.T)) tcb.p[tcb.n++] = b.p[i];
-            else rest.p[rest.n++] = b.p[i];
-        }
-        if (tcb.n) CUDA_OK(ctx, gemm_tc_launch(tcb, ctx->model->dev, ctx->stream, ctx->act16, ctx->act16_bytes));
-        if (rest.n) CUDA_OK(ctx, gemv_launch(rest, ctx->model->dev, ctx->stream));
-        return true;
-    }
-    CUDA_OK(ctx, gemv_launch(b, ctx->model->dev, ctx->stream));
+    void * ws = ctx->use_tensor_cores ? ctx->act16 : nullptr;
+    CUDA_OK(ctx, gemv_route(b, ctx->model->dev, ctx->stream, ws, ctx->act16_bytes, ctx->batch_n > 0 ? BATCH_TC_MIN : 32));
     return true;
 }
 
@@ -422,7 +411,7 @@ bool ensure_capacity(Context * ctx, int T) {
     if (cap >= BATCH_TC_MIN) {   // fp16 staging for the tensor-core path: up to 8 distinct inputs of max(C, F) x round16(cap)
         Dims d = model_dims(m);
         const size_t kmax = d.F > d.C ? d.F : d.C;
-        ctx->act16_bytes = gemm_tc_workspace_bytes(cap, (size_t) GEMV_MAX_PROBLEMS * (kmax * (size_t) ((cap + 15) / 16 * 16) + 128));
+        ctx->act16_bytes = gemm_tc_batch_workspace_bytes(cap, kmax);
         e = cudaMalloc(&ctx->act16, ctx->act16_bytes);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate fp16 staging: %s", cudaGetErrorString(e));
     }

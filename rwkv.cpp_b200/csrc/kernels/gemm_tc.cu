@@ -639,6 +639,7 @@ cudaError_t gemm_tc_repack(const void * W, long long pitch, int type, int M, int
     const dim3 grid((unsigned) nsteps, (unsigned) ntiles);
     const uint8_t * src = reinterpret_cast<const uint8_t *>(W);
     uint4 * out = reinterpret_cast<uint4 *>(dst);
+    log_launch(LF_EXPAND, 0, type, 0, 0, 0);
     switch (type) {
         case DT_Q4_0: tc::tc_expand_kernel<DT_Q4_0><<<grid, tc::TILE_M, 0, stream>>>(src, pitch, M, nsteps, out); break;
         case DT_Q4_1: tc::tc_expand_kernel<DT_Q4_1><<<grid, tc::TILE_M, 0, stream>>>(src, pitch, M, nsteps, out); break;
@@ -651,8 +652,9 @@ cudaError_t gemm_tc_repack(const void * W, long long pitch, int type, int M, int
     return cudaGetLastError();
 }
 
+// convert_f16_kernel applies no LayerNorm: a problem with a prologue takes the GEMV.
 bool gemm_tc_supported(const GemvProblem & p, int T) {
-    return T >= 16 && T <= tc::MAX_N && p.Wt != nullptr && gemm_tc_eligible(p.type, p.K) && (p.ldx % 4) == 0 &&
+    return T >= 16 && T <= tc::MAX_N && p.Wt != nullptr && p.pro == PRO_NONE && gemm_tc_eligible(p.type, p.K) && (p.ldx % 4) == 0 &&
            (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.Wt) & 15) == 0;
 }
 
@@ -727,6 +729,7 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     }
     {   // every distinct input of the batch -> fp16 canonical layout, one launch: one CTA per (token column, input)
         cvt.trace = trace_slot("convert_f16");
+        log_launch(LF_CONVERT, cvt.n, 0, 0, tb.npad, 0);
         cudaError_t e = launch_pdl(tc::convert_f16_kernel, dim3(tb.npad, cvt.n), dim3(tc::CVT_THREADS), 0, stream, cvt);
         if (e != cudaSuccess) return e;
     }
@@ -753,6 +756,7 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
     const cudaError_t ae = once[ki].run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem_budget); });
     if (ae != cudaSuccess) return ae;
     tb.trace = trace_slot("gemm_tc");
+    log_launch(LF_TENSOR_CORES, 0, 0, 0, tb.npad, cluster);
     return launch_pdl((unsigned) cluster, kernel, dim3((unsigned) next), dim3(tc::THREADS), smem, stream, tb);
 }
 

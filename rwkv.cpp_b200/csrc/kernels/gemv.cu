@@ -17,6 +17,7 @@
 #include "quant_decode.cuh"
 
 #include <cuda_fp16.h>
+#include <cstring>
 #include <mutex>
 #include <set>
 #include <utility>
@@ -27,6 +28,7 @@ std::atomic<unsigned long long> g_kernel_launches{0};
 thread_local TraceRec * g_trace_base = nullptr;
 thread_local int g_trace_next = 0;
 thread_local const char * g_trace_names[1024];
+thread_local LaunchLog * g_launch_log = nullptr;
 
 namespace {
 
@@ -295,6 +297,7 @@ cudaError_t launch_nc(const GemvBatch & batch, int grid, size_t smem, int max_op
     static PerDeviceOnce once;                // the shared-memory opt-in is per device
     const cudaError_t ae = once.run([&] { return cudaFuncSetAttribute(gemv_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_optin - 1024); });
     if (ae != cudaSuccess) return ae;
+    log_launch(LF_GENERIC, NC, -1, 0, 0, 0);
     return launch_pdl(gemv_kernel<NC>, dim3(grid), dim3(GEMV_THREADS), smem, stream, batch);
 }
 
@@ -338,6 +341,22 @@ cudaError_t gemv_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t 
     const cudaError_t e = gemv_tma_launch(batch, dev, stream);
     if (e != cudaErrorNotSupported) return e;
     return gemv_generic_launch(batch, dev, stream);
+}
+
+cudaError_t gemv_route(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes, int tc_min_T) {
+    if (!workspace || batch.T < tc_min_T) return gemv_launch(batch, dev, stream);
+    GemvBatch tcb, rest;
+    memset(&tcb, 0, sizeof(tcb)); memset(&rest, 0, sizeof(rest));
+    tcb.T = rest.T = batch.T;
+    for (int i = 0; i < batch.n; i++) {
+        if (gemm_tc_supported(batch.p[i], batch.T)) tcb.p[tcb.n++] = batch.p[i];
+        else rest.p[rest.n++] = batch.p[i];
+    }
+    if (tcb.n) {
+        const cudaError_t e = gemm_tc_launch(tcb, dev, stream, workspace, workspace_bytes);
+        if (e != cudaSuccess) return e;
+    }
+    return rest.n ? gemv_launch(rest, dev, stream) : cudaSuccess;
 }
 
 cudaError_t gemv_generic_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream) {

@@ -73,6 +73,9 @@ struct DeviceInfo { int device; int num_sms; int max_smem_optin; };
 // Uses the TMA streaming kernel (gemv_tma.cu) whenever every problem's shape fits it, else the generic
 // direct-load kernel (gemv.cu); the choice depends on the problem shapes only, never on T.
 cudaError_t gemv_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);
+// The eval path's routing of a batch: with a tensor-core workspace and T >= tc_min_T, the problems gemm_tc_supported accepts go to one
+// gemm_tc_launch and the rest to gemv_launch; otherwise the whole batch goes to gemv_launch. workspace may be NULL (no tensor cores).
+cudaError_t gemv_route(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes, int tc_min_T);
 cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);      // cudaErrorNotSupported if a shape does not fit
 cudaError_t gemv_generic_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);
 
@@ -91,6 +94,10 @@ cudaError_t gemm_tc_repack(const void * W, long long pitch, int type, int M, int
 // workspace: gemm_tc_workspace_bytes(T, sum over the batch's distinct inputs of round16(T) * K) bytes of device memory, 256-byte aligned
 // (what cudaMalloc returns).
 size_t gemm_tc_workspace_bytes(int T, size_t operand_halves);
+// Enough for any batch of T tokens whose inputs have at most k_max rows (GEMV_MAX_PROBLEMS distinct inputs).
+inline size_t gemm_tc_batch_workspace_bytes(int T, size_t k_max) {
+    return gemm_tc_workspace_bytes(T, (size_t) GEMV_MAX_PROBLEMS * (k_max * (size_t) ((T + 15) / 16 * 16) + 128));
+}
 cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes);
 
 // Every kernel of the eval path asks for the SAME L1 / shared-memory split (all shared): an SM can only change its carve-out when it is
@@ -101,6 +108,25 @@ void prefer_max_shared_carveout(const void * kernel);
 
 // Per-launch count of kernels this module has enqueued (bench.py reports it as gpu_launches).
 extern std::atomic<unsigned long long> g_kernel_launches;
+
+// Which instantiation of the matrix kernels a launch ran, recorded while a log is attached to the calling thread (the GEMV test hook
+// attaches one, so its tests can assert the kernel they reached instead of assuming it). Fields that do not apply to a family are 0,
+// except `only`, -1 where a kernel serves every format.
+enum LaunchFamily : int { LF_STREAMING = 0, LF_GENERIC = 1, LF_TENSOR_CORES = 2, LF_CONVERT = 3, LF_EXPAND = 4 };
+struct LaunchRec {
+    int family;
+    int nc;        // streaming / generic: columns per group (NC); convert: distinct inputs
+    int only;      // streaming: ONLY (-1 = mixed formats); expand: the weight type
+    int has_ln;    // streaming: HAS_LN
+    int npad;      // tensor cores / convert: tokens padded to 16
+    int cluster;   // tensor cores: CTAs per cluster
+};
+struct LaunchLog { static constexpr int CAP = 32; LaunchRec rec[CAP]; int n; };
+extern thread_local LaunchLog * g_launch_log;
+inline void log_launch(int family, int nc, int only, int has_ln, int npad, int cluster) {
+    LaunchLog * l = g_launch_log;
+    if (l && l->n < LaunchLog::CAP) l->rec[l->n++] = LaunchRec{family, nc, only, has_ln, npad, cluster};
+}
 
 // Launches every kernel of the eval path, and counts it: with the PDL attribute (the kernel may start while its predecessor in the
 // stream is still running; it must execute griddepcontrol.wait before touching anything the predecessor writes), the carve-out

@@ -167,6 +167,7 @@ cudaError_t launch_tma_nc(const GemvBatch & batch, int grid, size_t smem, cudaSt
     static PerDeviceOnce once;                // the shared-memory opt-in is per device
     const cudaError_t ae = once.run([&] { return cudaFuncSetAttribute(tma::gemv_tma_kernel<NC, ONLY, HAS_LN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma::CTA_SMEM_BUDGET); });
     if (ae != cudaSuccess) return ae;
+    log_launch(LF_STREAMING, NC, ONLY, HAS_LN, 0, 0);
     return launch_pdl(tma::gemv_tma_kernel<NC, ONLY, HAS_LN>, dim3((unsigned) grid), dim3(tma::THREADS), smem, stream, batch);
 }
 

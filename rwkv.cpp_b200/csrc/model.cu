@@ -38,16 +38,6 @@ struct Request {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-inline long long matrix_pitch(int type, uint64_t K) {
-    // whole 4-byte-aligned units (pairs of blocks for the 2-byte-aligned formats), then 16-byte rows
-    size_t bytes = tensor_nbytes(type, K, 1, 1);
-    if (type == DT_Q4_0 || type == DT_Q5_0 || type == DT_Q8_0) {
-        uint64_t nblk = K / 32;
-        bytes = (size_t) ((nblk + 1) / 2 * 2) * dtype_block_bytes(type);
-    }
-    return (long long) align_up(bytes, 16);
-}
-
 // Host dequantisation of a whole tensor to fp32 (only for element-wise parameters that someone
 // stored in a narrower type; dequantize_row_q*, ggml-quants.c:255-363).
 void widen_to_f32(int type, const uint8_t * src, size_t n, float * dst) {
@@ -87,6 +77,33 @@ void widen_to_f32(int type, const uint8_t * src, size_t n, float * dst) {
 }
 
 }  // namespace
+
+long long matrix_pitch(int type, uint64_t K) {
+    size_t bytes = tensor_nbytes(type, K, 1, 1);
+    if (type == DT_Q4_0 || type == DT_Q5_0 || type == DT_Q8_0) {
+        uint64_t nblk = K / 32;
+        bytes = (size_t) ((nblk + 1) / 2 * 2) * dtype_block_bytes(type);
+    }
+    return (long long) align_up(bytes, 16);
+}
+
+cudaError_t upload_matrix(const void * host, int type, int M, int K, uint8_t * dst, uint8_t * tiled) {
+    const long long pitch = matrix_pitch(type, (uint64_t) K);
+    const size_t row_bytes = tensor_nbytes(type, (uint64_t) K, 1, 1);
+    cudaError_t ce;
+    if ((size_t) pitch == row_bytes) {
+        ce = cudaMemcpy(dst, host, row_bytes * (size_t) M, cudaMemcpyHostToDevice);
+    } else {
+        ce = cudaMemset(dst, 0, (size_t) M * (size_t) pitch);
+        if (ce == cudaSuccess) ce = cudaMemcpy2D(dst, (size_t) pitch, host, row_bytes, row_bytes, (size_t) M, cudaMemcpyHostToDevice);
+    }
+    if (ce == cudaSuccess) ce = weights_to_device_layout(dst, pitch, type, M, K, 0);      // Q5 fifth-bit words -> device order
+    if (ce == cudaSuccess && tiled) {
+        ce = gemm_tc_repack(dst, pitch, type, M, K, tiled, 0);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(0);     // the caller may reuse the host buffer
+    }
+    return ce;
+}
 
 Model * load_model(const char * path, int device, int layer_begin, int layer_end, ErrorSink sink) {
     ModelFile mf;
@@ -319,17 +336,9 @@ Model * load_model(const char * path, int device, int layer_begin, int layer_end
             d.pitch = matrix_pitch(d.type, t.ne[0]);
             d.data = dst;
             const size_t row_bytes = tensor_nbytes(d.type, t.ne[0], 1, 1);
-            if ((size_t) d.pitch == row_bytes) {
-                ce = cudaMemcpy(dst, staging.get(), t.nbytes, cudaMemcpyHostToDevice);
-            } else {
-                ce = cudaMemset(dst, 0, (size_t) d.M * (size_t) d.pitch);
-                if (ce == cudaSuccess) ce = cudaMemcpy2D(dst, (size_t) d.pitch, staging.get(), row_bytes, row_bytes, (size_t) d.M, cudaMemcpyHostToDevice);
-            }
-            if (ce == cudaSuccess) ce = weights_to_device_layout(dst, d.pitch, d.type, d.M, d.K, 0);      // Q5 fifth-bit words -> device order
-            if (ce == cudaSuccess && r.tiled_bytes) {
-                uint8_t * td = m.arena + r.tiled_offset;
-                ce = gemm_tc_repack(dst, d.pitch, d.type, d.M, d.K, td, 0);
-                if (ce == cudaSuccess) ce = cudaStreamSynchronize(0);     // the staging buffer is reused by the next tensor
+            uint8_t * td = r.tiled_bytes ? m.arena + r.tiled_offset : nullptr;
+            ce = upload_matrix(staging.get(), d.type, d.M, d.K, dst, td);
+            if (td) {
                 d.tiled = td;
                 m.tiled_bytes += r.tiled_bytes;
             }

@@ -95,4 +95,11 @@ struct Model {
 // recording the failure in `sink` (same categories/codes as rwkv_model_loading.inc:288-419).
 Model * load_model(const char * path, int device, int layer_begin, int layer_end, ErrorSink sink);
 
+// Device row pitch of a matrix: whole 4-byte-aligned units (pairs of blocks for the 2-byte-aligned formats), then 16-byte rows.
+long long matrix_pitch(int type, uint64_t K);
+// Uploads M rows of K elements in the file layout of `type` to dst (M * matrix_pitch bytes; the padding of every row is zeroed) and
+// brings them into the device layout (weights_to_device_layout). When tiled is not NULL (gemm_tc_tiled_bytes of room) it also writes
+// the tile-major copy the tensor-core path streams. The host buffer may be reused when it returns.
+cudaError_t upload_matrix(const void * host, int type, int M, int K, uint8_t * dst, uint8_t * tiled);
+
 }  // namespace rwkv

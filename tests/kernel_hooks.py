@@ -191,3 +191,54 @@ def wkv7(lib, r, w, k, v, aa, g, vgate, v_first, k_k, k_a, r_k, lnx_w, lnx_b, st
     _staged(o, a, q_type, C)
     _call(lib, lib.library.rwkv_b200_test_wkv7, a)
     return o
+
+
+class GemvProblem(ctypes.Structure):
+    _fields_ = [("type", ctypes.c_int), ("K", ctypes.c_int), ("M", ctypes.c_int), ("weights", VP), ("tiled", ctypes.c_int), ("input", ctypes.c_int),
+                ("epi", ctypes.c_int), ("pro", ctypes.c_int), ("res", VP), ("gate", VP), ("bias", VP), ("ln_w", VP), ("ln_b", VP), ("xq", VP),
+                ("y_aliases_res", ctypes.c_int), ("y", VP)]
+
+
+class GemvLaunch(ctypes.Structure):
+    _fields_ = [(f, ctypes.c_int) for f in ("family", "nc", "only", "has_ln", "npad", "cluster")]
+
+
+class GemvBatchArgs(ctypes.Structure):
+    _fields_ = [("T", ctypes.c_int), ("n", ctypes.c_int), ("path", ctypes.c_int), ("x", VP * 8), ("p", GemvProblem * 8),
+                ("launches", ctypes.POINTER(GemvLaunch)), ("max_launches", ctypes.c_int), ("n_launches", ctypes.POINTER(ctypes.c_int))]
+
+
+GEMV_PATHS = {"engine": 0, "engine_batch_ctx": 1, "streaming": 2, "generic": 3, "tensor_cores": 4}
+LAUNCH_FAMILIES = ("streaming", "generic", "tensor_cores", "convert", "expand")
+
+
+def gemv_batch(lib, T, problems, xs, path="engine"):
+    """rwkv_b200_test_gemv_batch. problems: dicts with type, K, M, raw (file-layout bytes), input (index into xs) and optionally
+    tiled, epi, pro, res / gate ([M, T]), bias ([M]), ln_w / ln_b ([K]), xq (staged bytes), alias (y aliases res). xs: [K, T] arrays.
+    Returns (one Out of M*T floats per problem, the launches as (family, nc, only, has_ln, npad, cluster) tuples)."""
+    i = Inputs()
+    a = GemvBatchArgs(T=T, n=len(problems), path=GEMV_PATHS[path])
+    for j, x in enumerate(xs):
+        a.x[j] = i(x, True)
+    outs = []
+    for j, p in enumerate(problems):
+        raw = np.ascontiguousarray(p["raw"])
+        i.keep.append(raw)
+        q = a.p[j]
+        q.type, q.K, q.M, q.weights = p["type"], p["K"], p["M"], raw.ctypes.data
+        q.tiled, q.input, q.epi, q.pro = int(p.get("tiled", 0)), p.get("input", 0), p.get("epi", 0), p.get("pro", 0)
+        q.res, q.gate = i(p.get("res"), True), i(p.get("gate"), True)
+        q.bias, q.ln_w, q.ln_b = i(p.get("bias")), i(p.get("ln_w")), i(p.get("ln_b"))
+        if p.get("xq") is not None:
+            xq = np.ascontiguousarray(p["xq"], np.uint8)
+            i.keep.append(xq)
+            q.xq = xq.ctypes.data
+        q.y_aliases_res = int(p.get("alias", 0))
+        outs.append(Out(p["M"] * T))
+        q.y = outs[-1].ptr
+    rec = (GemvLaunch * 32)()
+    n_rec = ctypes.c_int(0)
+    a.launches, a.max_launches, a.n_launches = rec, 32, ctypes.pointer(n_rec)
+    _call(lib, lib.library.rwkv_b200_test_gemv_batch, a)
+    launches = [(LAUNCH_FAMILIES[r.family], r.nc, r.only, r.has_ln, r.npad, r.cluster) for r in rec[:n_rec.value]]
+    return outs, launches

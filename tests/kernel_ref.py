@@ -10,18 +10,20 @@ import numpy as np
 import ggml_file as gf
 import rwkv_oracle as ro
 
+F64 = np.float64
 
-def bar(r64, r32):
-    """How far a kernel output may land from the float64 result r64: four times the distance of the float32 restatement r32, but
-    at least 1e-6 of the output's largest magnitude. For [dim, T] activations each token column has its own bar, so one
+
+def bar(r64, r32, factor=4):
+    """How far a kernel output may land from the float64 result r64: `factor` (four) times the distance of the float32 restatement
+    r32, but at least 1e-6 of the output's largest magnitude. For [dim, T] activations each token column has its own bar, so one
     ill-conditioned column (a constant one, say, whose variance fp32 cannot resolve) does not widen the bar of the others."""
     r64, r32 = np.asarray(r64, np.float64), np.asarray(r32, np.float64)
-    return np.maximum(4 * np.abs(r32 - r64).max(axis=0), max(1e-6 * np.abs(r64).max(), 1e-30))
+    return np.maximum(factor * np.abs(r32 - r64).max(axis=0), max(1e-6 * np.abs(r64).max(), 1e-30))
 
 
-def error_over_bar(x, r64, r32):
+def error_over_bar(x, r64, r32, factor=4):
     """The largest ratio of |x - r64| to the bar over the output's columns."""
-    return float((np.abs(np.asarray(x, np.float64) - np.asarray(r64, np.float64)).max(axis=0) / bar(r64, r32)).max())
+    return float((np.abs(np.asarray(x, np.float64) - np.asarray(r64, np.float64)).max(axis=0) / bar(r64, r32, factor)).max())
 
 
 def norm(x, eps, dt):
@@ -206,3 +208,228 @@ def staged_column(y, q_type, fill=0xFF, guard=0):
         o = nunits * UB * 32 + (bi * nunits + u) * 8
         out[o:o + 8] = np.frombuffer(np.array([d[blk], s[blk]], "<f4").tobytes(), np.uint8)
     return out
+
+
+# ---- matrix kernels (csrc/kernels/gemv.cu, gemv_tma.cu, gemm_tc.cu) ----------------------------------------------------
+# y[M, T] = epi(W[M, K] . pro(x[K, T])). The decode GEMV multiplies the reference's own operands (ggml-cpu.c:253-311 vec_dot_type);
+# the tensor-core GEMM multiplies fp16 roundings of them. Both restatements take the exact operand values and accumulate in `dt`.
+
+EPI_NONE, EPI_SIGMOID, EPI_SILU, EPI_TANH, EPI_RELU_SQR, EPI_ADD, EPI_MUL_ADD, EPI_BIAS_EXPNEGEXP, EPI_BIAS_SIGMOID, EPI_BIAS_W7 = range(10)
+RES_EPIS, BIAS_EPIS = (EPI_ADD, EPI_MUL_ADD), (EPI_BIAS_EXPNEGEXP, EPI_BIAS_SIGMOID, EPI_BIAS_W7)
+ROW_CHUNK = 4096          # rows restated at a time: bounds the memory of a 65536-row head
+
+
+def weight_operands(w_type, raw, M, K):
+    """The stored weights: dense [M, K] values for F32 / F16, else the blocks (q - offset [M, K/32, 32], d [M, K/32], m or None)
+    of dequantize_row_q* (ggml-quants.c:255-363; ro.unpack_blocks)."""
+    if w_type in (TYPE_F32, TYPE_F16):
+        return ro.dequantize(w_type, raw, M * K).reshape(M, K)
+    q, d, m, off = ro.unpack_blocks(w_type, raw, M * K)
+    nb = K // 32
+    return (q - off).reshape(M, nb, 32), d.reshape(M, nb), None if m is None else m.reshape(M, nb)
+
+
+def act_operands(w_type, x, bug=None):
+    """The activation operands the decode GEMV multiplies with weights of w_type, from the fp32 values x [K, T]: x for F32 (in the
+    dtype given), fp16(x) for F16, else Q8 blocks (q [K/32, 32, T], d = fp16(amax / 127), s) as quantize_row_q8_0 / q8_1 make them
+    (ggml-cpu-quants.c:781-846, 1085-1160; ro.quantize_activations). s is sum(q) for the *_0 formats (it folds their offset) and
+    fp16(d32 * sum(q)) for Q4_1 / Q5_1: the block minimum multiplies the ROUNDED s."""
+    if w_type == TYPE_F32:
+        return x
+    if w_type == TYPE_F16:
+        return np.asarray(x, np.float32).astype(np.float16)
+    has_min = w_type in Q8_1_CONSUMERS
+    x32 = np.asarray(x, np.float32)
+    q, d, s = ro.quantize_activations(x32, with_sum=has_min)
+    if has_min and bug == "s_unrounded":
+        amax = np.abs(x32.reshape(q.shape)).max(axis=1)
+        s = (amax / np.float32(127)) * q.sum(axis=1).astype(np.float32)
+    if not has_min:
+        s = q.sum(axis=1).astype(np.float32)
+    return q, d, s
+
+
+def row_chunks(w_type, raw, M, K):
+    """(r0, r1, weight_operands of rows r0..r1) over the matrix, ROW_CHUNK rows at a time."""
+    elems, nbytes = gf.BLOCK[w_type]
+    row = K // elems * nbytes
+    raw = np.ascontiguousarray(raw).reshape(-1)
+    for r0 in range(0, M, ROW_CHUNK):
+        r1 = min(M, r0 + ROW_CHUNK)
+        yield r0, r1, weight_operands(w_type, raw[r0 * row:r1 * row], r1 - r0, K)
+
+
+def gemv_operands(w_type, raw, x, M, bug=None):
+    """(weight operands, activation operands) of the decode GEMV."""
+    return weight_operands(w_type, raw, M, x.shape[0]), act_operands(w_type, x, bug)
+
+
+def epilogue(v, epi, dt, res=None, gate=None, bias=None, bug=None):
+    """The fused epilogues of GemvEpilogue (csrc/kernels/gemv.h), per the reference's graph (rwkv_graph.inc:365-367, 417-430,
+    445-450, 667-679). v, res, gate: [M, T]; bias: [M]."""
+    if res is not None:
+        res = res.astype(dt)
+        if bug == "res_neighbour":
+            res = np.roll(res, 1, axis=0)
+    if gate is not None:
+        gate = gate.astype(dt)
+        if bug == "gate_prev_col":
+            gate = np.roll(gate, 1, axis=1)
+    if bias is not None:
+        bias = bias.astype(dt)[:, None]
+        if bug == "bias_next":
+            bias = np.roll(bias, -1, axis=0)
+    one = dt(1)
+    sig = lambda z: one / (one + np.exp(-z))
+    with np.errstate(over="ignore", under="ignore"):
+        if epi == EPI_SIGMOID:
+            return sig(v)
+        if epi == EPI_SILU:
+            return v / (one + np.exp(-v))
+        if epi == EPI_TANH:
+            return np.tanh(v)
+        if epi == EPI_RELU_SQR:
+            return np.maximum(v, dt(0)) ** 2
+        if epi == EPI_ADD:
+            return res + v
+        if epi == EPI_MUL_ADD:
+            return res + gate * v
+        if epi == EPI_BIAS_EXPNEGEXP:
+            return np.exp(-np.exp(v + bias))
+        if epi == EPI_BIAS_SIGMOID:
+            return sig(v + bias)
+        if epi == EPI_BIAS_W7:
+            return np.exp(sig(v + bias) * dt(-0.606531))
+    return v
+
+
+def prologue(x, ln, dt, bug=None):
+    """The head's LayerNorm prologue (PRO_LAYERNORM: rwkv_layer_norm, rwkv_operators.inc:93-97) or x itself. ln: (w, b) or None."""
+    if ln is None:
+        return np.asarray(x, np.float32)
+    w, b = ln
+    if bug == "ln_no_b":
+        b = np.zeros_like(b)
+    return layer_norm(x, w, b, dt, eps=1e-6 if bug == "ln_eps" else 1e-5)
+
+
+def gemv(w_type, raw, M, x, dt, epi=EPI_NONE, res=None, gate=None, bias=None, ln=None, bug=None):
+    """The decode GEMV (gemv_tma_kernel, gemv_kernel): sum over blocks of d_w d_a sum(q_w q_a) + m_w s_a (ggml-cpu-quants.c:2302-2316,
+    2594-2609, 2944-2963, 3318-3338, 3690-3698), fp16(x) . W for F16 (ggml-cpu.c:1463), plain for F32; then the epilogue. x: [K, T]
+    fp32; with `ln` the LayerNorm output in dt is what gets quantised (the tests choose ln_b so that fp32 and float64 give the same
+    operands). Accumulated in dt."""
+    xin = prologue(x, ln, dt, bug)
+    K, T = xin.shape
+    A = act_operands(w_type, xin.astype(dt) if w_type == TYPE_F32 else xin, bug)
+    y = np.empty((M, T), dt)
+    for r0, r1, W in row_chunks(w_type, raw, M, K):
+        if w_type in (TYPE_F32, TYPE_F16):
+            y[r0:r1] = W.astype(dt) @ A.astype(dt)
+            continue
+        qw, dw, mw = W
+        qa, da, sa = A
+        nb = qw.shape[1]
+        if bug == "drop_odd_block" and nb % 2:
+            nb -= 1
+        # exact integer block sums, [nb, rows, T]
+        isum = np.matmul(qw[:, :nb].transpose(1, 0, 2).astype(F64), qa[:nb].astype(F64))
+        part = (dw[:, :nb].T.astype(dt)[:, :, None] * da[:nb].astype(dt)[:, None, :]) * isum.astype(dt)
+        if mw is not None and bug != "drop_min":
+            part = part + mw[:, :nb].T.astype(dt)[:, :, None] * sa[:nb].astype(dt)[:, None, :]
+        y[r0:r1] = np.moveaxis(part, 0, -1).sum(axis=-1, dtype=dt)
+    return epilogue(y, epi, dt, res, gate, bias, bug)
+
+
+def tc_column_scale(x):
+    """e per token column (convert_f16_kernel): the column is multiplied by 2^-e before the fp16 rounding so that it stays inside the
+    fp16 range, e = exponent(column maximum) - 15 above 32768, else 0."""
+    cmax = np.abs(np.asarray(x, np.float32)).max(axis=0)
+    e = np.where((cmax > 32768) & (cmax <= 3.0e38), np.frexp(cmax)[1] - 15, 0)
+    return e.astype(np.int32)
+
+
+def tc_weights(w_type, W):
+    """A = fp16((q - offset) d + m) rounded ONCE (the kernel's __hfma2: the product and the sum are exact in float64, so float64 ->
+    float16 is that single rounding), or the stored fp16 weights. W: weight_operands of some rows."""
+    if w_type == TYPE_F16:
+        return W.astype(np.float16)
+    qw, dw, mw = W
+    a = qw.astype(F64) * dw.astype(F64)[:, :, None]
+    if mw is not None:
+        a = a + mw.astype(F64)[:, :, None]
+    return a.reshape(qw.shape[0], -1).astype(np.float16)
+
+
+def tc_activations(w_type, x):
+    """B = fp16(d q 2^-e) of the Q8 block values for quantised weights, fp16(x 2^-e) for F16 (convert_f16_kernel), and e [T]."""
+    e = tc_column_scale(x)
+    down = np.ldexp(np.float32(1), -e).astype(np.float32)
+    if w_type == TYPE_F16:
+        return (np.asarray(x, np.float32) * down).astype(np.float16), e
+    q, d, _ = ro.quantize_activations(np.asarray(x, np.float32), with_sum=False)
+    return (q.astype(np.float32) * (d * down)[:, None, :]).reshape(x.shape[0], -1).astype(np.float16), e
+
+
+def gemm_tc(w_type, raw, M, x, dt, epi=EPI_NONE, res=None, gate=None, bias=None, bug=None, ksplit=1):
+    """The tensor-core GEMM (gemm_tc_kernel): A . B accumulated in dt, times 2^e per column, then the epilogue. ksplit: the K-split
+    count of the launch, only used by the "drop_last_ksplit" bug."""
+    K = x.shape[0]
+    B, e = tc_activations(w_type, x)
+    k1 = K
+    if bug == "drop_last_ksplit" and ksplit > 1:
+        per = -(-(K // 64) // ksplit)
+        k1 = (ksplit - 1) * per * 64
+    y = np.empty((M, x.shape[1]), dt)
+    for r0, r1, W in row_chunks(w_type, raw, M, K):
+        y[r0:r1] = tc_weights(w_type, W)[:, :k1].astype(dt) @ B[:k1].astype(dt)
+    if bug == "drop_last_tile":
+        y[(M - 1) // 128 * 128:] = 0
+    if bug != "no_colscale":
+        y = y * np.ldexp(dt(1), e)[None, :].astype(dt)
+    return epilogue(y, epi, dt, res, gate, bias, bug)
+
+
+def _f16_tie_distance(v):
+    """Distance of |v| from the nearest half-way point between two fp16 values, in units of the fp16 spacing there."""
+    a = np.abs(np.asarray(v, F64))
+    h = a.astype(np.float16)
+    up = np.spacing(h).astype(F64)
+    down = (h - np.nextafter(h, np.float16(0))).astype(F64)
+    hd = h.astype(F64)
+    dist = np.minimum(np.abs(a - (hd + up / 2)), np.abs(a - (hd - down / 2)))
+    return dist / np.where(up > 0, up, 1.0)
+
+
+def ln_bias_away_from_roundings(x, ln_w, ln_b, w_type, rng, margin=1e-3, tie_margin=1e-2):
+    """ln_b nudged element by element until the float64 LayerNorm output of x gives the same operands as any faithful fp32 LayerNorm:
+    every Q8 value x 127 / amax at least `margin` (in units of q) away from a rint half-way point, and every block's amax / 127, every
+    Q8_1 s and every fp16 operand at least `tie_margin` of an fp16 spacing away from an fp16 tie. ln_b enters after the normalisation,
+    element by element, so moving ln_b[k] moves row k of the output and nothing else."""
+    b = np.asarray(ln_b, np.float32).copy()
+    if w_type == TYPE_F32:
+        return b
+    n = norm(x, 1e-5, F64) * np.asarray(ln_w, F64)[:, None]
+    K, T = n.shape
+    for _ in range(200):
+        y = n + b.astype(F64)[:, None]
+        if w_type == TYPE_F16:
+            bad = (_f16_tie_distance(y) < tie_margin).any(axis=1)
+            unit = np.abs(y).max(axis=1) * 2.0 ** -10 + 1e-8
+        else:
+            yb = y.reshape(K // 32, 32, T)
+            amax = np.abs(yb).max(axis=1)                                             # [nb, T]
+            qv = yb * 127 / np.where(amax > 0, amax, 1)[:, None, :]
+            bad_el = np.abs(qv - np.floor(qv) - 0.5) < margin
+            d32 = amax / 127
+            bad_blk = _f16_tie_distance(d32) < tie_margin
+            if w_type in Q8_1_CONSUMERS:
+                bad_blk |= _f16_tie_distance(d32 * np.rint(qv).sum(axis=1)) < tie_margin
+            # a bad block moves its largest element: that changes amax, d and s
+            arg = np.abs(yb).argmax(axis=1)                                           # [nb, T]
+            bad_el[np.nonzero(bad_blk)[0], arg[bad_blk], np.nonzero(bad_blk)[1]] = True
+            bad = bad_el.reshape(K, T).any(axis=1)
+            unit = np.repeat(amax.max(axis=1) / 127, 32)
+        if not bad.any():
+            return b
+        b[bad] += (rng.uniform(0.05, 0.95, bad.sum()) * unit[bad]).astype(np.float32)
+    raise AssertionError("could not move the LayerNorm output away from rounding boundaries")

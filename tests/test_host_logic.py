@@ -149,6 +149,32 @@ def test_kernel_hooks_reject_invalid_arguments(lib):
         lambda: kh.ln_mix(lib, f(64, 1), f(64), f(64), f(64), [f(64)], 2),
         lambda: kh.embed_ln0(lib, np.ones((4, 64), np.float32), [0, 4], f(64), f(64)),
     ]
+    # the GEMV batch hook: operands present exactly when the epilogue / prologue reads them, whole blocks, known inputs
+    Q51 = gf.TYPE_IDS["Q5_1"]
+    raw = np.zeros(64 * 24, np.uint8)
+
+    def gemv(T=1, xs=(f(64, 1),), path="engine", **kw):
+        p = dict(type=Q51, K=64, M=32, raw=raw)
+        p.update(kw)
+        probs = p.pop("_probs", [p])
+        return kh.gemv_batch(lib, T, probs, list(xs), path)
+    cases += [
+        lambda: gemv(T=2, xs=[f(64, 2)], xq=np.zeros(256, np.uint8)),          # staged input of a multi-token launch
+        lambda: gemv(epi=5),                                                    # EPI_ADD without a residual
+        lambda: gemv(res=f(32, 1)),                                             # a residual no epilogue reads
+        lambda: gemv(epi=6, res=f(32, 1)),                                      # EPI_MUL_ADD without a gate
+        lambda: gemv(epi=8),                                                    # a bias epilogue without a bias
+        lambda: gemv(epi=3, bias=f(32)),                                        # a bias no epilogue reads
+        lambda: gemv(alias=1),                                                  # y aliasing a residual that is not there
+        lambda: gemv(pro=1),                                                    # LayerNorm without its parameters
+        lambda: gemv(ln_w=f(64), ln_b=f(64)),                                   # LayerNorm parameters without the prologue
+        lambda: gemv(K=48, xs=[f(48, 1)]),                                      # K not a whole number of blocks
+        lambda: gemv(input=8),                                                  # input index out of range
+        lambda: gemv(input=1),                                                  # an input that was not given
+        lambda: gemv(_probs=[dict(type=Q51, K=64, M=32, raw=raw), dict(type=Q51, K=128, M=32, raw=np.zeros(128 * 24, np.uint8))]),  # one input, two K
+        lambda: gemv(type=gf.TYPE_IDS["FP32"], raw=np.zeros(64 * 32 * 4, np.uint8), tiled=1),    # a tiled copy of a type the tensor cores cannot take
+        lambda: gemv(path="tensor_cores", T=300, xs=[f(64, 300)]),              # more tokens than a pass holds
+    ]
     for i, call in enumerate(cases):
         with pytest.raises(kh.HookError) as e:
             call()

@@ -62,3 +62,84 @@ def test_lerp_coefficient_of_wrong_output_is_caught(T, mix, C):
     w2, z, xx, sx, maa = lerp_inputs(C, T, mix, rng_for("lerp", T, mix, C))
     r64, r32 = kr.v6_lerp(w2, z, xx, sx, maa, F64), kr.v6_lerp(w2, z, xx, sx, maa, F32)
     assert_caught(r64[2], r32[2], kr.v6_lerp(w2, z, xx, sx, maa, F64, bug="lerp_j")[2])
+
+
+# ---- the matrix kernels (tests/test_gpu_gemv.py) -----------------------------------------------------------------------------
+
+def matrix_case(fmt, M, K, T, epi=0, ln=False, tiled=False, seed=0):
+    import test_gpu_gemv as tg
+    rng = tg.rng_for("bars", fmt, M, K, T, epi, ln, seed)
+    xs = tg.inputs([K], T, rng, scale=0.05 if ln else 2.0)
+    p = tg.problem(fmt, M, K, T, rng, epi=epi, tiled=tiled)
+    if ln:
+        tg.with_layernorm(p, xs[0], rng)
+    return p, xs
+
+
+def assert_matrix_bug_caught(p, xs, bug, tc=False):
+    import test_gpu_gemv as tg
+    r64, r32 = tg.reference(p, xs, F64, tc), tg.reference(p, xs, F32, tc)
+    moved = kr.error_over_bar(tg.reference(p, xs, F64, tc, bug=bug), r64, r32, tg.TC_BAR_FACTOR if tc else 4)
+    assert moved > 10, (bug, moved)
+
+
+@pytest.mark.parametrize("fmt,M,K", [("Q5_1", 256, 4096), ("Q4_1", 4096, 160), ("Q4_1", 1000, 32)])
+def test_dropped_block_minimum_term_is_caught(fmt, M, K):
+    assert_matrix_bug_caught(*matrix_case(fmt, M, K, 1), "drop_min")
+
+
+@pytest.mark.parametrize("fmt,M,K,T", [("Q5_1", 256, 4096, 1), ("Q4_1", 1000, 32, 1), ("Q5_1", 300, 2048, 3)])
+def test_unrounded_activation_sum_is_caught(fmt, M, K, T):
+    assert_matrix_bug_caught(*matrix_case(fmt, M, K, T), "s_unrounded")
+
+
+@pytest.mark.parametrize("epi,tc", [(5, False), (6, False), (5, True), (6, True)])
+def test_residual_of_the_neighbouring_row_is_caught(epi, tc):
+    assert_matrix_bug_caught(*matrix_case("Q5_1", 300, 2048, 40 if tc else 1, epi, tiled=tc), "res_neighbour", tc)
+
+
+@pytest.mark.parametrize("tc", [False, True])
+def test_gate_of_the_previous_column_is_caught(tc):
+    assert_matrix_bug_caught(*matrix_case("Q4_0", 300, 1024, 40 if tc else 3, 6, tiled=tc), "gate_prev_col", tc)
+
+
+@pytest.mark.parametrize("epi", [7, 8, 9])
+@pytest.mark.parametrize("K,tc", [(64, False), (160, False), (256, True)])
+def test_bias_of_the_next_row_is_caught(epi, K, tc):
+    assert_matrix_bug_caught(*matrix_case("FP16" if tc else "Q5_1", 2048, K, 40 if tc else 1, epi, tiled=tc), "bias_next", tc)
+
+
+@pytest.mark.parametrize("case,bug", [(2, "ln_eps"), (4, "ln_eps"), (6, "ln_eps"), (0, "ln_no_b"), (2, "ln_no_b"), (4, "ln_no_b"), (6, "ln_no_b")])
+def test_layernorm_prologue_bugs_are_caught(case, bug):
+    """On the heads of tests/test_gpu_gemv.py: eps 1e-6 instead of 1e-5 on those whose inputs have a small variance (at unit variance
+    the difference is invisible), a dropped ln_b on unit-variance and small-variance ones."""
+    import test_gpu_gemv as tg
+    fmt, V, C, T, _, scale = tg.HEAD_CASES[case]
+    V = min(V, 4096)       # the same inputs; fewer rows keep this CPU test short
+    p, xs = tg.head_case(fmt, V, C, T, scale)
+    assert_matrix_bug_caught(dict(p, M=V, raw=p["raw"][:V * len(p["raw"]) // p["M"]]), xs, bug)
+
+
+def test_dropped_column_scale_is_caught():
+    p, xs = matrix_case("Q5_0", 256, 4096, 48, 5, tiled=True)
+    xs[0][:, 3] *= 3.0e5
+    assert_matrix_bug_caught(p, xs, "no_colscale", tc=True)
+
+
+@pytest.mark.parametrize("M", [300, 4096 + 1])
+def test_dropped_partial_row_tile_is_caught(M):
+    assert_matrix_bug_caught(*matrix_case("Q8_0", M, 256, 33, tiled=True), "drop_last_tile", tc=True)
+
+
+def test_dropped_last_k_split_is_caught():
+    """256 x 4096: two row tiles, each cut over a cluster of 8 CTAs (tests/test_gpu_gemv.py asserts the cut)."""
+    import test_gpu_gemv as tg
+    p, xs = matrix_case("Q5_0", 256, 4096, 64, tiled=True)
+    r64, r32 = (kr.gemm_tc(p["type"], p["raw"], p["M"], xs[0], dt) for dt in (F64, F32))
+    bugged = kr.gemm_tc(p["type"], p["raw"], p["M"], xs[0], F64, bug="drop_last_ksplit", ksplit=8)
+    assert kr.error_over_bar(bugged, r64, r32, tg.TC_BAR_FACTOR) > 10
+
+
+@pytest.mark.parametrize("fmt,K", [("Q4_0", 32), ("Q5_0", 96), ("Q8_0", 14336 + 32)])
+def test_dropped_odd_trailing_block_is_caught(fmt, K):
+    assert_matrix_bug_caught(*matrix_case(fmt, 128, K, 1), "drop_odd_block")
