@@ -165,16 +165,16 @@ RWKV_API int rwkv_b200_overlap_groups(const struct rwkv_context * ctx);
  * epilogue: 0 none, 1 sigmoid, 2 silu, 3 tanh, 4 relu^2. */
 RWKV_API bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, const float * x, float * y, int epilogue);
 
-/* Test hooks for the element-wise and recurrent kernels between the GEMVs (csrc/kernels/glue.cu, wkv.cu, batch.cu). Each runs
+/* Test hooks for the element-wise and recurrent kernels between the GEMVs (csrc/kernels/glue.cu, wkv.cu). Each runs
  * exactly the launcher the eval path calls, on host buffers: copy in, launch, synchronise, copy out. Activations are column-major
- * [dim, T] (column t = token t, contiguous). n_seq = 0 selects the T-token kernel; n_seq > 0 the batch kernel, which evaluates one
- * token of each of n_seq sequences (T must be 1, the activations have n_seq columns) on per-sequence states seq_stride floats apart.
+ * [dim, T] (column t = token t, contiguous). n_seq = 0 runs the kernel on T tokens of one sequence; n_seq > 0 runs it in batch mode,
+ * one token of each of n_seq sequences (T must be 1, the activations have n_seq columns) on per-sequence states seq_stride floats apart.
  * Every output (outputs, states, staged columns) must have room for RWKV_B200_GUARD floats (4 * RWKV_B200_GUARD bytes) after its
  * end: the device copy is filled with 0xFF bytes (NaN) before the launch, including that guard region, and returned whole, so a
  * value the kernel never wrote and a write past the end are both visible. Optional pointers may be NULL. Staged columns (q_out,
  * written for consumers of weight type q_type; layout in csrc/kernels/act_stage.cuh) are accepted for T = 1 and n_seq = 0 only,
  * and only where the kernel emits whole 32-element blocks from whole warps: n_embed a multiple of 32 for the v4 WKV and the lerp,
- * the head size a multiple of 32 for the v5/6/7 WKV. The v5/6 batch kernel needs seq_stride a multiple of 4, embed_ln0 an
+ * the head size a multiple of 32 for the v5/6/7 WKV. The v5/6 WKV needs seq_stride a multiple of 4, embed_ln0 an
  * emb_pitch that is a multiple of the element size. False with RWKV_ERROR_ARGS for invalid arguments, RWKV_ERROR_CTX | UNSUPPORTED
  * when the launcher refuses the shape or the device fails. */
 #define RWKV_B200_GUARD 64
@@ -183,7 +183,7 @@ RWKV_API bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * 
 RWKV_API bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, int n_vocab, const int * tokens, int T, int C,
                                        const float * ln_w, const float * ln_b, float * x);
 
-/* LayerNorm + token shift + mix (launch_ln_mix / launch_ln_mix_batch). formula 0: out_j = xx*m_j + (prev - prev*m_j);
+/* LayerNorm + token shift + mix (launch_ln_mix). formula 0: out_j = xx*m_j + (prev - prev*m_j);
  * formula 1: out_j = (prev - xx)*m_j + xx. state_in / state_out: the carried LN(x) of the previous token, [C] per sequence. */
 struct rwkv_b200_ln_mix_args {
     const float * x, * ln_w, * ln_b, * state_in;
@@ -209,7 +209,7 @@ struct rwkv_b200_v6_lerp_args {
 };
 RWKV_API bool rwkv_b200_test_v6_lerp(const struct rwkv_b200_v6_lerp_args * a);
 
-/* v4 WKV with the r* multiply (launch_wkv4 / launch_wkv4_batch). aa / bb / pp: [C] per sequence. */
+/* v4 WKV with the r* multiply (launch_wkv4). aa / bb / pp: [C] per sequence. */
 struct rwkv_b200_wkv4_args {
     const float * k, * v, * r, * time_first, * time_decay;
     const float * aa_in, * bb_in, * pp_in;
@@ -222,7 +222,7 @@ struct rwkv_b200_wkv4_args {
 };
 RWKV_API bool rwkv_b200_test_wkv4(const struct rwkv_b200_wkv4_args * a);
 
-/* v5 / v6 WKV + head norm + ln_x + gate (launch_wkv6 / launch_wkv6_batch). td: [C, T] when td_per_token, else [H] when
+/* v5 / v6 WKV + head norm + ln_x + gate (launch_wkv6). td: [C, T] when td_per_token, else [H] when
  * per_head_scalars, else [C]; tf: [H] when per_head_scalars, else [C]. State [H][S][S] per sequence. g optional. */
 struct rwkv_b200_wkv6_args {
     const float * r, * k, * v, * td, * tf;
@@ -240,7 +240,7 @@ struct rwkv_b200_wkv6_args {
 };
 RWKV_API bool rwkv_b200_test_wkv6(const struct rwkv_b200_wkv6_args * a);
 
-/* v7 WKV with kk / k / v corrections, head norm, ln_x, bonus and gate (launch_wkv7 / launch_wkv7_batch). vgate NULL = layer 0
+/* v7 WKV with kk / k / v corrections, head norm, ln_x, bonus and gate (launch_wkv7). vgate NULL = layer 0
  * (v_first ignored); v_out optional. State [H][S][S] per sequence. */
 struct rwkv_b200_wkv7_args {
     const float * r, * w, * k, * v, * a, * g, * vgate, * v_first;

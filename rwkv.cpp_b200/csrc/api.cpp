@@ -307,6 +307,18 @@ bool rwkv_b200_eval_resident(struct rwkv_context * ctx, const uint32_t * tokens,
     return true;
 }
 
+// Batch contexts accept the shapes tests/test_gpu_batch.py checks whole, sequence in a batch against sequence alone: n_embed up to
+// 4096, head sizes up to 64 (v7: 128). This is not a bound of the kernels, which take what a single-sequence context takes;
+// a wider range wants whole-context tests of its own.
+static bool batch_shape_supported(int arch_major, int n_embed, int head_size) {
+    if (n_embed > 4096) return false;
+    const bool head_upto_64 = head_size == 8 || head_size == 16 || head_size == 32 || head_size == 64;
+    if (arch_major == 4) return true;
+    if (arch_major == 5 || arch_major == 6) return head_upto_64;
+    if (arch_major == 7) return head_upto_64 || head_size == 128;
+    return false;
+}
+
 struct rwkv_context * rwkv_b200_batch_create(struct rwkv_context * ctx, size_t n_sequences) {
     if (!ctx) return nullptr;
     Context * c = C(ctx);
@@ -686,10 +698,10 @@ bool rwkv_b200_test_ln_mix(const struct rwkv_b200_ln_mix_args * a) {
     LnMixParams p{};
     p.x = b.in(a->x, C * cols); p.ln_w = b.in(a->ln_w, C); p.ln_b = b.in(a->ln_b, C);
     p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
-    p.C = a->C; p.T = (int) cols; p.formula = a->formula; p.n_out = a->n_out;
+    p.C = a->C; p.T = (int) cols; p.formula = a->formula; p.n_out = a->n_out; p.seq_stride = a->n_seq > 0 ? a->seq_stride : 0;
     for (int j = 0; j < a->n_out; j++) { p.coef[j] = b.in(a->coef[j], C); p.out[j] = b.out(a->out[j], C * cols); }
     p.out_xx = b.out(a->out_xx, C * cols); p.out_sx = b.out(a->out_sx, C * cols);
-    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_ln_mix_batch(p, a->seq_stride, 0) : launch_ln_mix(p, 0);
+    const cudaError_t e = b.ok ? launch_ln_mix(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ln_mix failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
@@ -735,9 +747,9 @@ bool rwkv_b200_test_wkv4(const struct rwkv_b200_wkv4_args * a) {
     p.aa_in = b.in(a->aa_in, st); p.bb_in = b.in(a->bb_in, st); p.pp_in = b.in(a->pp_in, st);
     p.aa_out = b.out(a->aa_out, st); p.bb_out = b.out(a->bb_out, st); p.pp_out = b.out(a->pp_out, st);
     p.y = b.out(a->y, C * cols);
-    p.C = a->C; p.T = (int) cols;
+    p.C = a->C; p.T = (int) cols; p.seq_stride = a->n_seq > 0 ? a->seq_stride : 0;
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, a->C)) : nullptr; p.q_type = a->q_type;
-    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv4_batch(p, a->seq_stride, 0) : launch_wkv4(p, 0);
+    const cudaError_t e = b.ok ? launch_wkv4(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv4 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
@@ -748,7 +760,7 @@ bool rwkv_b200_test_wkv6(const struct rwkv_b200_wkv6_args * a) {
     const size_t C = a ? (size_t) a->H * (size_t) a->S : 0, SS = a ? C * (size_t) a->S : 0;
     const bool args = a && a->r && a->k && a->v && a->td && a->tf && a->state_in && a->state_out && a->lnx_w && a->lnx_b && a->y && a->H > 0 && a->S > 0 && a->T > 0 &&
                       !(a->td_per_token && a->per_head_scalars) && seq_layout_ok(a->n_seq, a->seq_stride, a->T, SS) &&
-                      a->seq_stride % 4 == 0 &&          // the batch kernel moves the state in float4s from state + seq * seq_stride
+                      a->seq_stride % 4 == 0 &&          // wkv6_kernel moves the state in float4s from state + seq * seq_stride
                       staged_ok(a->q_out, a->q_type, a->T, a->n_seq, a->S);
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid wkv6 arguments");
     if (!hook_device(sink)) return false;
@@ -762,9 +774,9 @@ bool rwkv_b200_test_wkv6(const struct rwkv_b200_wkv6_args * a) {
     p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
     p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C); p.g = b.in(a->g, C * cols);
     p.y = b.out(a->y, C * cols);
-    p.eps = a->eps; p.H = a->H; p.S = a->S; p.T = (int) cols;
+    p.eps = a->eps; p.H = a->H; p.S = a->S; p.T = (int) cols; p.seq_stride = a->n_seq > 0 ? a->seq_stride : 0;
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
-    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv6_batch(p, a->seq_stride, 0) : launch_wkv6(p, 0);
+    const cudaError_t e = b.ok ? launch_wkv6(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv6 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
@@ -786,9 +798,9 @@ bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a) {
     p.k_k = b.in(a->k_k, C); p.k_a = b.in(a->k_a, C); p.r_k = b.in(a->r_k, C); p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C);
     p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
     p.y = b.out(a->y, n);
-    p.H = a->H; p.S = a->S; p.T = (int) cols;
+    p.H = a->H; p.S = a->S; p.T = (int) cols; p.seq_stride = a->n_seq > 0 ? a->seq_stride : 0;
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
-    const cudaError_t e = !b.ok ? cudaSuccess : a->n_seq > 0 ? launch_wkv7_batch(p, a->seq_stride, 0) : launch_wkv7(p, 0);
+    const cudaError_t e = b.ok ? launch_wkv7(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }

@@ -156,8 +156,8 @@ bool run_batch(Context * ctx, Batch & batch) {
     return true;
 }
 
-// The three stages that touch the recurrent state: a batch context (one token of each of batch_n sequences) uses the kernels of
-// batch.cu, where column t works on sequence t's state; everything else is identical for both kinds of context.
+// The stages that touch the recurrent state pass seq_stride = batch_stride: in a batch context (one token of each of batch_n
+// sequences) their kernels work on sequence t's state for column t; everything else is identical for both kinds of context.
 // LayerNorm + token shift + mix in front of a batch of GEMVs is a launch of its own (ln_mix_kernel). Four variations were built,
 // measured at 7B Q5_1 and removed:
 // (a) fused into the CONSUMING GEMV, every CTA recomputing the LayerNorm in its prologue: a third slower per token;
@@ -170,22 +170,13 @@ bool run_batch(Context * ctx, Batch & batch) {
 // (d) for passes of >= 32 tokens, ln_mix_kernel writing the fp16 GEMM operands of its consumers itself, so that two of the six
 //     convert_f16 launches of a v6 layer disappear: 1 % per 7B chunk, and the tail of the state went NaN in the shift-state-3e5
 //     robustness test of the 64-channel fixture (not understood). 1 % was not worth an unexplained failure.
-cudaError_t do_ln_mix(Context * ctx, const LnMixParams & lp) {
-    return ctx->batch_stride ? launch_ln_mix_batch(lp, ctx->batch_stride, ctx->stream) : launch_ln_mix(lp, ctx->stream);
-}
-cudaError_t do_wkv6(Context * ctx, const Wkv6Params & wp) {
-    return ctx->batch_stride ? launch_wkv6_batch(wp, ctx->batch_stride, ctx->stream) : launch_wkv6(wp, ctx->stream);
-}
-cudaError_t do_wkv4(Context * ctx, const Wkv4Params & wp) {
-    return ctx->batch_stride ? launch_wkv4_batch(wp, ctx->batch_stride, ctx->stream) : launch_wkv4(wp, ctx->stream);
-}
 
 // LayerNorm + mix parameters of the channel-mixing block (rwkv_ffn_v4_v5 :484-511, rwkv_ffn_v6 :513-531, rwkv_ffn_v7 :533-543).
 LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out) {
     const Model & m = *ctx->model;
     LnMixParams lp{};
     lp.x = s.x; lp.ln_w = L.ln2_w.data; lp.ln_b = L.ln2_b.data;
-    lp.state_in = st_in; lp.state_out = st_out; lp.C = m.n_embed; lp.T = T;
+    lp.state_in = st_in; lp.state_out = st_out; lp.C = m.n_embed; lp.T = T; lp.seq_stride = ctx->batch_stride;
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.ffn_x_k.data; lp.out[0] = s.mix[0];
     } else if (m.arch_major == 6) {
@@ -204,7 +195,7 @@ LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
 bool ffn(Context * ctx, const Layer & L, const Scratch & s, int T, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
     {
         Batch b(T);
         b.add(L.ffn_key, s.mix[0], s.ffn_k, EPI_RELU_SQR);
@@ -236,7 +227,7 @@ LnMixParams att_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
     const int C = m.n_embed;
     LnMixParams lp{};
     lp.x = s.x; lp.ln_w = L.ln1_w.data; lp.ln_b = L.ln1_b.data;
-    lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = T;
+    lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = T; lp.seq_stride = ctx->batch_stride;
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 6;
         for (int j = 0; j < 6; j++) { lp.coef[j] = L.att_x_rwkvag.data + (size_t) j * C; lp.out[j] = s.mix[j]; }   // r w k v a g
@@ -256,7 +247,7 @@ LnMixParams att_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
 
 bool att_v4(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
     const int C = ctx->model->n_embed;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
     Batch b(T);
     b.add(L.att_receptance, s.mix[2], s.r, EPI_SIGMOID);
     b.add(L.att_key, s.mix[0], s.k);
@@ -267,9 +258,9 @@ bool att_v4(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     wp.time_first = L.att_time_first.data; wp.time_decay = L.att_time_decay.data;
     wp.aa_in = st_in + 2 * C; wp.bb_in = st_in + 3 * C; wp.pp_in = st_in + 4 * C;
     wp.aa_out = st_out + 2 * C; wp.bb_out = st_out + 3 * C; wp.pp_out = st_out + 4 * C;
-    wp.y = s.y; wp.C = C; wp.T = T;
+    wp.y = s.y; wp.C = C; wp.T = T; wp.seq_stride = ctx->batch_stride;
     wp.q_out = (C % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, do_wkv4(ctx, wp));
+    CUDA_OK(ctx, launch_wkv4(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
 }
 
@@ -277,7 +268,7 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     const bool v52 = m.arch_minor >= 2;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
     Batch b(T);
     b.add(L.att_receptance, s.mix[2], s.r);
     b.add(L.att_key, s.mix[0], s.k);
@@ -292,16 +283,16 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.g = v52 ? s.g : nullptr;
-    wp.y = s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T;
+    wp.y = s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, do_wkv6(ctx, wp));
+    CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
 }
 
 bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
     {   // :313-321  tanh(W1 . xxx)
         Batch b(T);
         b.add(L.att_maa_w1, s.mix[0], s.lora[0], EPI_TANH);
@@ -340,9 +331,9 @@ bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     wp.td = s.w; wp.td_per_token = 1; wp.tf = L.att_time_faaaa.data; wp.per_head_scalars = 0;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
-    wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T;
+    wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, do_wkv6(ctx, wp));
+    CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
 }
 
@@ -351,7 +342,7 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Scratch & s, int T,
     const int C = m.n_embed;
     const bool first = layer == 0;
     float * v_dst = first ? s.v_first : s.v;
-    CUDA_OK(ctx, do_ln_mix(ctx, lp));
+    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
     {   // :415-432, 439, 447 -- first halves of the LoRA pairs
         Batch b(T);
         b.add(L.att_receptance, s.mix[0], s.r);
@@ -377,9 +368,9 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Scratch & s, int T,
     wp.k_k = L.att_k_k.data; wp.k_a = L.att_k_a.data; wp.r_k = L.att_r_k.data;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
-    wp.y = s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = T;
+    wp.y = s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, ctx->batch_stride ? launch_wkv7_batch(wp, ctx->batch_stride, ctx->stream) : launch_wkv7(wp, ctx->stream));
+    CUDA_OK(ctx, launch_wkv7(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
 }
 

@@ -89,7 +89,7 @@ struct Context {
     const float * hidden_in = nullptr;
     float * hidden_out = nullptr;
 
-    // Batched multi-sequence decode (kernels/batch.cu, rwkv_b200_batch_*): batch_n > 0 makes this a batch context whose state
+    // Batched multi-sequence decode (rwkv_b200_batch_*): batch_n > 0 makes this a batch context whose state
     // buffers hold batch_n states back to back (batch_stride = state_len floats apart) and whose logits buffer holds batch_n columns;
     // every pass evaluates exactly one token of each sequence.
     int batch_n = 0;

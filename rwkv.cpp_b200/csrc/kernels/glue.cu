@@ -80,7 +80,9 @@ __device__ __forceinline__ double block_sum_ln(double v, double * slots) {
 // cost of a run-once kernel). Statistics as ggml_compute_forward_norm_f32 (ggml-cpu.c:6906-6925, sums in double).
 // PRE_N: how many of the mix-coefficient vectors are requested before the dependency wait (3 for blocks with up to three mixed
 // vectors -- every v6 block --, 6 for v4 / v5.2 / v7 time mixing: a few spilled registers there against one HBM round trip per vector).
-template <int PER, int PRE_N>
+// BATCH (seq_stride > 0): block t is the one token of sequence t. Its previous LN(x) is always that sequence's carry, never
+// column t - 1, and it always writes the sequence's new carry.
+template <int PER, int PRE_N, bool BATCH>
 __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p) {
     __shared__ double slots[4][LN_WARPS];
     trace_begin(p.trace);
@@ -97,7 +99,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
             const bool live = c < C;
             lw[i] = live ? p.ln_w[c] : 0.f;
             lb[i] = live ? p.ln_b[c] : 0.f;
-            pv[i] = (live && t == 0) ? p.state_in[c] : 0.f;   // written by the previous token's pass: safe before the wait
+            pv[i] = (live && (BATCH || t == 0)) ? p.state_in[BATCH ? t * p.seq_stride + c : c] : 0.f;   // written by the previous token's pass: safe before the wait
         }
     };
     if constexpr (EARLY) load_ln();
@@ -123,12 +125,12 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
         const int c = tid + i * LN_THREADS;
         const bool live = c < C;
         xa[i] = live ? p.x[(size_t) t * C + c] : 0.f;
-        xb[i] = (live && t > 0) ? p.x[(size_t) (t - 1) * C + c] : 0.f;
+        xb[i] = (live && !BATCH && t > 0) ? p.x[(size_t) (t - 1) * C + c] : 0.f;
         sa += (double) xa[i];
         sb += (double) xb[i];
     }
     const float mean_a = (float) (block_sum_ln(sa, slots[0]) / C);
-    const float mean_b = (t > 0) ? (float) (block_sum_ln(sb, slots[1]) / C) : 0.f;
+    const float mean_b = (!BATCH && t > 0) ? (float) (block_sum_ln(sb, slots[1]) / C) : 0.f;
     double va = 0, vb = 0;
 #pragma unroll
     for (int i = 0; i < PER; i++) {
@@ -139,13 +141,13 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
         vb += (double) (xb[i] * xb[i]);
     }
     const float scale_a = 1.0f / sqrtf((float) (block_sum_ln(va, slots[2]) / C) + 1e-5f);
-    const float scale_b = (t > 0) ? 1.0f / sqrtf((float) (block_sum_ln(vb, slots[3]) / C) + 1e-5f) : 0.f;
+    const float scale_b = (!BATCH && t > 0) ? 1.0f / sqrtf((float) (block_sum_ln(vb, slots[3]) / C) + 1e-5f) : 0.f;
     if constexpr (!EARLY) load_ln();
     // normalised current / previous token, in place
 #pragma unroll
     for (int i = 0; i < PER; i++) {
         xa[i] = __fadd_rn(__fmul_rn(__fmul_rn(xa[i], scale_a), lw[i]), lb[i]);                            // LN(x[:, t])
-        xb[i] = (t > 0) ? __fadd_rn(__fmul_rn(__fmul_rn(xb[i], scale_b), lw[i]), lb[i]) : pv[i];          // LN(x[:, t-1]) or the carry
+        xb[i] = (!BATCH && t > 0) ? __fadd_rn(__fmul_rn(__fmul_rn(xb[i], scale_b), lw[i]), lb[i]) : pv[i];   // LN(x[:, t-1]) or the carry
     }
     const size_t o0 = (size_t) t * C + tid;
     if constexpr (PRE) {
@@ -186,7 +188,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
         if (c >= C) continue;
         if (p.out_sx) p.out_sx[o0 + i * LN_THREADS] = __fsub_rn(xb[i], xa[i]);
         if (p.out_xx) p.out_xx[o0 + i * LN_THREADS] = xa[i];
-        if (t == p.T - 1) p.state_out[c] = xa[i];
+        if (BATCH || t == p.T - 1) p.state_out[BATCH ? t * p.seq_stride + c : c] = xa[i];
     }
     trace_end(p.trace);
 }
@@ -363,11 +365,19 @@ cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch
     return launch_pdl(embed_ln0_kernel, dim3(T), dim3(GLUE_THREADS), (size_t) C * sizeof(float), s, reinterpret_cast<const uint8_t *>(emb), emb_type, emb_pitch, tokens, C, ln_w, ln_b, x);
 }
 
+// Grid row t is token t, or sequence t in batch mode. The single-sequence instantiation comes first: with the batch one first,
+// nvcc emitted different code for the untouched v6_lerp_kernel<8, 16> of this file.
+template <int PER, int PRE_N>
+cudaError_t launch_ln_mix_kernel(const LnMixParams & p, cudaStream_t s) {
+    return !p.seq_stride ? launch_pdl(ln_mix_kernel<PER, PRE_N, false>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
+                         : launch_pdl(ln_mix_kernel<PER, PRE_N, true>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
+}
+
 cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s) {
     LnMixParams p = p_in;
     p.trace = trace_slot("ln_mix");
     const int per = (p.C + LN_THREADS - 1) / LN_THREADS;
-#define RWKV_LN(PER_) return p.n_out > 3 ? launch_pdl(ln_mix_kernel<PER_, 6>, dim3(p.T), dim3(LN_THREADS), 0, s, p) : launch_pdl(ln_mix_kernel<PER_, 3>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
+#define RWKV_LN(PER_) return p.n_out > 3 ? launch_ln_mix_kernel<PER_, 6>(p, s) : launch_ln_mix_kernel<PER_, 3>(p, s);
     if (per <= 1) { RWKV_LN(1) }
     if (per <= 2) { RWKV_LN(2) }
     if (per <= 4) { RWKV_LN(4) }

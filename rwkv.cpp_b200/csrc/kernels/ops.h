@@ -1,6 +1,11 @@
 // Launchers for the non-GEMV kernels of the RWKV eval path: embedding gather + ln0, LayerNorm +
 // token shift + mixing, the v6 data-dependent lerp, and the WKV4/5/6/7 recurrences with their
 // per-head normalisation and gating fused in. All activations are fp32, column-major [dim, T].
+//
+// The four stages that carry recurrent state (LayerNorm + mix, WKV4, WKV5/6, WKV7) also serve batch contexts, which evaluate one
+// token of each of several sequences per pass. Their seq_stride selects the mode: 0 means T tokens of one sequence; > 0 means T
+// sequences of one token each, column t working on the state of sequence t, which lives t * seq_stride floats after the state
+// pointers (sequence 0's). Both modes run the same arithmetic, so a sequence gives the same bits in a batch as alone.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -29,6 +34,7 @@ struct LnMixParams {
     float * out[6];           // [C, T] each
     float * out_xx;           // optional [C, T]: LN(x)
     float * out_sx;           // optional [C, T]: prev - xx
+    long long seq_stride = 0;
 };
 cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s);
 
@@ -57,6 +63,7 @@ struct Wkv4Params {
     float * y;                        // [C, T] = r * wkv
     int C, T;
     unsigned char * q_out; int q_type;  // T == 1, C % 32 == 0 only: y as a staged column (act_stage.cuh)
+    long long seq_stride = 0;
 };
 cudaError_t launch_wkv4(const Wkv4Params & p, cudaStream_t s);
 
@@ -76,6 +83,7 @@ struct Wkv6Params {
     float eps;                        // 1e-5 (v5) or 64e-5 (v6)
     int H, S, T;
     unsigned char * q_out; int q_type;  // T == 1, S % 32 == 0 only: y as a staged column (act_stage.cuh)
+    long long seq_stride = 0;         // a multiple of 4: the state moves in float4s
 };
 cudaError_t launch_wkv6(const Wkv6Params & p, cudaStream_t s);
 
@@ -95,16 +103,9 @@ struct Wkv7Params {
     float * y;                        // [C, T]
     int H, S, T;
     unsigned char * q_out; int q_type;  // T == 1, S % 32 == 0 only: y as a staged column (act_stage.cuh)
+    long long seq_stride = 0;
 };
 cudaError_t launch_wkv7(const Wkv7Params & p, cudaStream_t s);
-
-// Batched multi-sequence decode (batch.cu): the same stages with column t working on the recurrent state of sequence t, which
-// lives seq_stride floats after sequence t-1's (p.T = number of sequences; state pointers are sequence 0's).
-bool batch_shape_supported(int arch_major, int n_embed, int head_size);
-cudaError_t launch_ln_mix_batch(const LnMixParams & p, long long seq_stride, cudaStream_t s);
-cudaError_t launch_wkv6_batch(const Wkv6Params & p, long long seq_stride, cudaStream_t s);
-cudaError_t launch_wkv4_batch(const Wkv4Params & p, long long seq_stride, cudaStream_t s);
-cudaError_t launch_wkv7_batch(const Wkv7Params & p, long long seq_stride, cudaStream_t s);
 
 // Layer-pipeline hand-off over peer memory (pipe.cu). A PipeBox sits at the start of every stage's mailbox allocation, followed by
 // PIPE_SLOTS data areas of slot_floats floats each.

@@ -14,15 +14,19 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 // v4: rwkv_att_wkv_v4 (rwkv_graph.inc:119-161). One thread per channel, sequential over tokens.
 // Every ggml node is its own rounding, so no FMA contraction here.
+// BATCH (seq_stride > 0): one token, column blockIdx.y, on the state of sequence blockIdx.y.
 // ---------------------------------------------------------------------------------------------
+template <bool BATCH>
 __global__ void wkv4_kernel(const Wkv4Params p) {
     trace_begin(p.trace);
     pdl_prologue();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= p.C) return;
-    float aa = p.aa_in[c], bb = p.bb_in[c], pp = p.pp_in[c];
+    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
+    const int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
+    float aa = p.aa_in[so + c], bb = p.bb_in[so + c], pp = p.pp_in[so + c];
     const float tf = p.time_first[c], td = p.time_decay[c];
-    for (int t = 0; t < p.T; t++) {
+    for (int t = t_begin; t < t_end; t++) {
         const size_t o = (size_t) t * p.C + c;
         const float k = p.k[o], v = p.v[o];
         float ww = __fadd_rn(tf, k);
@@ -41,7 +45,7 @@ __global__ void wkv4_kernel(const Wkv4Params p) {
         p.y[o] = yv;
         if (p.q_out) act::warp_emit_block(act::StagedOut{p.q_out, p.q_type, p.C}, c >> 5, yv);      // T == 1, C % 32 == 0: whole warps only
     }
-    p.aa_out[c] = aa; p.bb_out[c] = bb; p.pp_out[c] = pp;
+    p.aa_out[so + c] = aa; p.bb_out[so + c] = bb; p.pp_out[so + c] = pp;
     trace_end(p.trace);
 }
 
@@ -101,7 +105,8 @@ template <int S> struct Wkv6Layout {
 __device__ __forceinline__ void wkv_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void wkv_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-template <int S>
+// BATCH (seq_stride > 0): the block walks ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
+template <int S, bool BATCH>
 __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Params p) {
     using LY = Wkv6Layout<S>;
     constexpr int TB = WKV6_TB, NOCT = LY::NOCT, NT = LY::NT, WORK = LY::WORK, BLOCK = LY::BLOCK, NNW = LY::NORM_WARPS, CPL = (S + 31) / 32;
@@ -112,19 +117,21 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int h = blockIdx.x, tid = threadIdx.x, C = p.H * S;
+    const int col0 = BATCH ? blockIdx.y : 0;      // column of the block's first token
+    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
     const bool is_norm = tid >= WORK;
     const bool worker = tid < NT;
     const int oct = worker ? tid % NOCT : 0, jg = worker ? tid / NOCT : 0;
     const int i0 = oct * 8, j0 = jg * 4;
     const int lane = tid & 31;
-    const int nchunks = (p.T + TB - 1) / TB;
+    const int nchunks = BATCH ? 1 : (p.T + TB - 1) / TB;
     // the recurrent state (written by the previous token's pass) and the parameters do not depend on the previous
     // kernel: pull them in before the programmatic-dependency wait
     float st[8][4];
     if (!is_norm) {
 #pragma unroll
         for (int ii = 0; ii < 8; ii++) {
-            const float4 v = *reinterpret_cast<const float4 *>(p.state_in + ((size_t) h * S + i0 + ii) * S + j0);
+            const float4 v = *reinterpret_cast<const float4 *>(p.state_in + so + ((size_t) h * S + i0 + ii) * S + j0);
             st[ii][0] = v.x; st[ii][1] = v.y; st[ii][2] = v.z; st[ii][3] = v.w;
         }
     }
@@ -147,11 +154,11 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         // the recurrence walks a chunk's tokens serially with the state in registers and no barrier inside the chunk.
         auto stage = [&](int c) {
             Wkv6Chunk<S> & B = buf[c & 1];
-            const int t0 = c * TB, nt = min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
             constexpr int PER_ROW = S / 4;
             for (int idx = tid; idx < nt * PER_ROW; idx += WORK) {
                 const int tt = idx / PER_ROW, f = (idx % PER_ROW) * 4;
-                const size_t o = (size_t) (t0 + tt) * C + h * S + f;
+                const size_t o = (size_t) (col0 + t0 + tt) * C + h * S + f;
                 wkv_cp16(&B.k[tt][f], p.k + o);
                 wkv_cp16(&B.r[tt][f], p.r + o);
                 wkv_cp16(&B.v[tt][f], p.v + o);
@@ -160,7 +167,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         };
         // trace marks of CTA 0 (cycles, stored as start + cycles): [0] waiting for the staged chunk, [1] the recurrence,
         // [2] waiting for the normalising warps to hand an output buffer back
-        const bool acct = p.trace != nullptr && blockIdx.x == 0 && tid == 0;
+        const bool acct = p.trace != nullptr && blockIdx.x == 0 && (!BATCH || blockIdx.y == 0) && tid == 0;
         long long a0 = 0, a1 = 0, a2 = 0, tq = acct ? clock64() : 0;
         auto tick = [&](long long & a) { if (acct) { const long long now = clock64(); a += now - tq; tq = now; } };
         float tfr[8];     // time_first of my key rows
@@ -178,7 +185,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
             tick(a2);
             const Wkv6Chunk<S> & B = buf[c & 1];
             float (* yb)[S] = ybuf[c & 1];
-            const int t0 = c * TB, nt = min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
             // recurrence (kv = v_j*k_i;  y_j += (kv*tf_i + S_ij) * r_i;  S_ij = S_ij*td_i + kv), 8 + 8 + 8 + 4 operands per token from
             // shared memory
             float kk[8], rr[8], dv[8], vv[4];
@@ -224,7 +231,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         if (worker) {
 #pragma unroll
             for (int ii = 0; ii < 8; ii++)
-                *reinterpret_cast<float4 *>(p.state_out + ((size_t) h * S + i0 + ii) * S + j0) = make_float4(st[ii][0], st[ii][1], st[ii][2], st[ii][3]);
+                *reinterpret_cast<float4 *>(p.state_out + so + ((size_t) h * S + i0 + ii) * S + j0) = make_float4(st[ii][0], st[ii][1], st[ii][2], st[ii][3]);
         }
         if (acct) {
             p.trace->mark[0] = p.trace->start + (unsigned long long) a0;
@@ -238,7 +245,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         const int nwarp = (tid - WORK) >> 5;
         constexpr int PER = (TB + NNW - 1) / NNW;        // tokens of a chunk per normalising warp
         for (int c = 0; c < nchunks; c++) {
-            const int t0 = c * TB, nt = min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
             // the gate values of my tokens: requested before the wait for the chunk, so their latency hides behind the recurrence
             float gg[PER][CPL];
 #pragma unroll
@@ -247,7 +254,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
 #pragma unroll
                 for (int i = 0; i < CPL; i++) {
                     const int col = lane + 32 * i;
-                    gg[u][i] = (p.g && tt < nt && col < S) ? p.g[(size_t) (t0 + tt) * C + h * S + col] : 0.f;
+                    gg[u][i] = (p.g && tt < nt && col < S) ? p.g[(size_t) (col0 + t0 + tt) * C + h * S + col] : 0.f;
                 }
             }
             wkv_bar_sync(BAR_FULL + (c & 1), BLOCK);
@@ -272,7 +279,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
                 const float mean = (float) mean_d;
                 const float var = (float) fmax(s2 * INV_S - mean_d * mean_d, 0.0);
                 const float rstd = 1.0f / sqrtf(var + p.eps);
-                const size_t o = (size_t) (t0 + tt) * C + h * S;
+                const size_t o = (size_t) (col0 + t0 + tt) * C + h * S;
 #pragma unroll
                 for (int i = 0; i < CPL; i++) {
                     const int col = lane + 32 * i;
@@ -295,16 +302,15 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
 // v7: rwkv_att_v7 (rwkv_graph.inc:432-479) around rwkv_wkv_v7_impl (rwkv_operators_wkv_v7.inc:63-101).
 // Thread i owns state row S[i][.] (value index i, key index j).
 // ---------------------------------------------------------------------------------------------
-// seq_stride > 0 (batch contexts, grid = heads x sequences): the block handles ONE token, column blockIdx.y, on the state of sequence
-// blockIdx.y, which lives seq_stride floats after sequence 0's.
-template <int S>
-__global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p, const long long seq_stride) {
+// BATCH (seq_stride > 0): the block handles ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
+template <int S, bool BATCH>
+__global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
     __shared__ float sr[S], sw[S], sk[S], sa[S], sb[S], red[S];
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int h = blockIdx.x, i = threadIdx.x, C = p.H * S, c = h * S + i;
-    const long long so = seq_stride ? (long long) blockIdx.y * seq_stride : 0;
-    const int t_begin = seq_stride ? (int) blockIdx.y : 0, t_end = seq_stride ? (int) blockIdx.y + 1 : p.T;
+    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
+    const int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
     float st[S];
 #pragma unroll
     for (int j = 0; j < S; j++) st[j] = p.state_in[so + ((size_t) h * S + i) * S + j];
@@ -364,48 +370,51 @@ __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p, const long 
 
 }  // namespace
 
+// Grid row y is sequence y in batch mode (seq_stride > 0); one sequence has a single row.
 cudaError_t launch_wkv4(const Wkv4Params & p_in, cudaStream_t s) {
     Wkv4Params p = p_in;
     p.trace = trace_slot("wkv4");
     const int threads = 128;
-    return launch_pdl(wkv4_kernel, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p);
+    return !p.seq_stride ? launch_pdl(wkv4_kernel<false>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
+                         : launch_pdl(wkv4_kernel<true>, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p);
 }
 
-#define RWKV_DISPATCH_HEAD_SIZE(S_, KERNEL, PARAMS, STREAM, GRID, STRIDE)                              \
-    switch (S_) {                                                                        \
-        case 8: return launch_pdl(KERNEL<8>, GRID, dim3(8), 0, STREAM, PARAMS, STRIDE);         \
-        case 16: return launch_pdl(KERNEL<16>, GRID, dim3(16), 0, STREAM, PARAMS, STRIDE);      \
-        case 32: return launch_pdl(KERNEL<32>, GRID, dim3(32), 0, STREAM, PARAMS, STRIDE);      \
-        case 64: return launch_pdl(KERNEL<64>, GRID, dim3(64), 0, STREAM, PARAMS, STRIDE);      \
-        case 128: return launch_pdl(KERNEL<128>, GRID, dim3(128), 0, STREAM, PARAMS, STRIDE);   \
-        default: return cudaErrorInvalidValue;                                           \
-    }
+template <int S>
+cudaError_t launch_wkv6_kernel(const Wkv6Params & p, cudaStream_t s) {
+    return !p.seq_stride ? launch_pdl(wkv6_kernel<S, false>, dim3(p.H), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
+                         : launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
+}
 
 cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
     Wkv6Params p = p_in;
     p.trace = trace_slot("wkv6");
     switch (p.S) {
-        case 8: return launch_pdl(wkv6_kernel<8>, dim3(p.H), dim3(Wkv6Layout<8>::BLOCK), 0, s, p);
-        case 16: return launch_pdl(wkv6_kernel<16>, dim3(p.H), dim3(Wkv6Layout<16>::BLOCK), 0, s, p);
-        case 32: return launch_pdl(wkv6_kernel<32>, dim3(p.H), dim3(Wkv6Layout<32>::BLOCK), 0, s, p);
-        case 64: return launch_pdl(wkv6_kernel<64>, dim3(p.H), dim3(Wkv6Layout<64>::BLOCK), 0, s, p);
-        case 128: return launch_pdl(wkv6_kernel<128>, dim3(p.H), dim3(Wkv6Layout<128>::BLOCK), 0, s, p);
+        case 8: return launch_wkv6_kernel<8>(p, s);
+        case 16: return launch_wkv6_kernel<16>(p, s);
+        case 32: return launch_wkv6_kernel<32>(p, s);
+        case 64: return launch_wkv6_kernel<64>(p, s);
+        case 128: return launch_wkv6_kernel<128>(p, s);
         default: return cudaErrorInvalidValue;
     }
+}
+
+template <int S>
+cudaError_t launch_wkv7_kernel(const Wkv7Params & p, cudaStream_t s) {
+    return !p.seq_stride ? launch_pdl(wkv7_kernel<S, false>, dim3(p.H), dim3(S), 0, s, p)
+                         : launch_pdl(wkv7_kernel<S, true>, dim3(p.H, p.T), dim3(S), 0, s, p);
 }
 
 cudaError_t launch_wkv7(const Wkv7Params & p_in, cudaStream_t s) {
     Wkv7Params p = p_in;
     p.trace = trace_slot("wkv7");
-    const long long none = 0;
-    RWKV_DISPATCH_HEAD_SIZE(p.S, wkv7_kernel, p, s, dim3(p.H), none)
-}
-
-// batch contexts: one token of each of p.T sequences, column t on the state of sequence t
-cudaError_t launch_wkv7_batch(const Wkv7Params & p_in, long long seq_stride, cudaStream_t s) {
-    Wkv7Params p = p_in;
-    p.trace = trace_slot("wkv7_batch");
-    RWKV_DISPATCH_HEAD_SIZE(p.S, wkv7_kernel, p, s, dim3(p.H, p.T), seq_stride)
+    switch (p.S) {
+        case 8: return launch_wkv7_kernel<8>(p, s);
+        case 16: return launch_wkv7_kernel<16>(p, s);
+        case 32: return launch_wkv7_kernel<32>(p, s);
+        case 64: return launch_wkv7_kernel<64>(p, s);
+        case 128: return launch_wkv7_kernel<128>(p, s);
+        default: return cudaErrorInvalidValue;
+    }
 }
 
 }  // namespace rwkv

@@ -1,4 +1,4 @@
-"""Plain restatements of the eval path's element-wise and recurrent kernels (csrc/kernels/glue.cu, wkv.cu, batch.cu), one function
+"""Plain restatements of the eval path's element-wise and recurrent kernels (csrc/kernels/glue.cu, wkv.cu), one function
 per operation, written from the reference's formulas and generic in the floating-point type: in float64 they give the truth, in
 float32 they show how far a faithful fp32 implementation lands from it on the same input. tests/test_gpu_kernels.py compares the
 kernels with both; tests/test_kernel_bars.py checks that plausible bugs move the results far beyond the bars derived from them.

@@ -1,6 +1,7 @@
-"""Batched multi-sequence decode (rwkv_b200_batch_*, csrc/kernels/batch.cu): B sequences advanced one token each per call must
-give, per sequence, exactly the bits of that sequence evaluated alone through rwkv_eval -- the weights are streamed once for the
-B tokens, nothing else may change."""
+"""Batched multi-sequence decode (rwkv_b200_batch_*: the LayerNorm-mix and WKV kernels of csrc/kernels/glue.cu and wkv.cu in
+batch mode): B sequences advanced one token each per call must give, per sequence, exactly the bits of that sequence evaluated
+alone through rwkv_eval -- the weights are streamed once for the B tokens, nothing else may change. batch_shape_supported (api.cpp)
+admits the model shapes these tests cover."""
 import ctypes
 
 import numpy as np

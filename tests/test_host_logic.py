@@ -128,7 +128,7 @@ def test_kernel_hooks_reject_invalid_arguments(lib):
     """The kernel test hooks check their arguments before they touch a device: staged columns only for single-token, single-sequence
     passes in which whole warps emit whole 32-blocks (head size a multiple of 32 for the v5/6/7 WKV, not just n_embed) and for a
     weight type that has a stage class, batch passes of one token with non-overlapping states (and float4-aligned ones for the v5/6
-    batch kernel), known formulas, tokens inside the table, embedding rows aligned to their element type, the lerp's staged columns
+    WKV), known formulas, tokens inside the table, embedding rows aligned to their element type, the lerp's staged columns
     all or none."""
     import kernel_hooks as kh
     f = lambda *shape: np.ones(shape, np.float32)
