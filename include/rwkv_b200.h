@@ -42,12 +42,14 @@ RWKV_API bool rwkv_b200_synchronize(struct rwkv_context * ctx);
  * context holds the recurrent states of n_sequences independent sequences in HBM and evaluates ONE token of EACH per call, so every
  * weight matrix is streamed once for n_sequences tokens (the fused dequantize-GEMV runs its multi-column path). Per sequence the
  * result is bit-identical to evaluating that sequence alone with rwkv_eval (below 32 sequences; from 32 on the tensor-core path
- * takes the layer matrices, with its own rounding of the activations). RWKV v4 / v5 / v6, n_embed <= 4096, head size <= 64.
+ * takes the layer matrices, with its own rounding of the activations). RWKV v4 / v5 / v6 / v7, n_embed <= 4096, head size <= 64
+ * (v7: 128).
  *   rwkv_b200_batch_create    : from any context of the model (shares its weights); free with rwkv_free; NULL on failure
  *   rwkv_b200_batch_set_state : state of one sequence <- state_in (host or device pointer, NULL = fresh state)
  *   rwkv_b200_batch_eval      : tokens[n_sequences], one per sequence; want_logits = run the head for every sequence
  *   rwkv_b200_batch_get_logits / rwkv_b200_batch_get_state : copy one sequence's logits / state out (host or device pointer)
- * rwkv_eval* and the resident / stage entry points refuse a batch context. */
+ * The next token of every sequence is drawn on the device by rwkv_b200_batch_sample / rwkv_b200_batch_eval_sample (below).
+ * rwkv_eval*, rwkv_b200_sample and the resident / stage entry points refuse a batch context. */
 RWKV_API struct rwkv_context * rwkv_b200_batch_create(struct rwkv_context * ctx, size_t n_sequences);
 RWKV_API bool rwkv_b200_batch_set_state(struct rwkv_context * batch, size_t sequence, const float * state_in);
 RWKV_API bool rwkv_b200_batch_get_state(struct rwkv_context * batch, size_t sequence, float * state_out);
@@ -69,6 +71,24 @@ RWKV_API bool rwkv_b200_eval_sample(struct rwkv_context * ctx, uint32_t token, f
  * prob_out (optional) receives the probability the chosen token had after top-p / temperature. */
 RWKV_API bool rwkv_b200_sample_logits(const float * logits, size_t n_vocab, float temperature, float top_p, double u, const uint32_t * bias_ids,
                                       const float * bias_values, size_t n_bias, uint32_t * token_out, float * prob_out);
+
+/* On-device sampling for a batch context: one kernel launch draws every sequence's next token and only n_sequences token ids cross
+ * PCIe. One draw per sequence from that sequence's logits of the most recent rwkv_b200_batch_eval that computed them; row b
+ * is exactly what rwkv_b200_sample draws from the same logits with temperature[b], top_p[b], u[b] and that row's bias.
+ * Arrays of n_sequences host values; bias_offsets (NULL = no bias) has n_sequences + 1 entries, starting at 0 and
+ * non-decreasing, and sequence b's bias is bias_ids / bias_values [bias_offsets[b], bias_offsets[b + 1]). */
+RWKV_API bool rwkv_b200_batch_sample(struct rwkv_context * batch, const float * temperature, const float * top_p, const double * u,
+                                     const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values,
+                                     uint32_t * tokens_out);
+/* rwkv_b200_batch_eval(tokens, true) + rwkv_b200_batch_sample without bias; arguments are checked before the pass. */
+RWKV_API bool rwkv_b200_batch_eval_sample(struct rwkv_context * batch, const uint32_t * tokens, const float * temperature,
+                                          const float * top_p, const double * u, uint32_t * tokens_out);
+/* Test hook: the batched kernel on n_rows x n_vocab host logits (row-major), no model needed; probs_out optional.
+ * 1 <= n_rows <= 256, n_vocab <= 65536. */
+RWKV_API bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows, size_t n_vocab, const float * temperature,
+                                            const float * top_p, const double * u, const uint32_t * bias_offsets,
+                                            const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out,
+                                            float * probs_out);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

@@ -403,6 +403,48 @@ bool rwkv_b200_eval_sample(struct rwkv_context * ctx, uint32_t token, float temp
     return sample_token(C(ctx), temperature, top_p, u, nullptr, nullptr, 0, next_token_out);
 }
 
+bool rwkv_b200_batch_sample(struct rwkv_context * batch, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets,
+                            const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out) {
+    C(batch)->last_error = RWKV_ERROR_NONE;
+    return batch_sample(C(batch), temperature, top_p, u, bias_offsets, bias_ids, bias_values, tokens_out);
+}
+
+bool rwkv_b200_batch_eval_sample(struct rwkv_context * batch, const uint32_t * tokens, const float * temperature, const float * top_p, const double * u,
+                                 uint32_t * tokens_out) {
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->batch_n > 0 && tokens, "Not a batch context or NULL tokens");
+    for (int i = 0; i < c->batch_n; i++)
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) c->model->n_vocab, "Token of sequence %d (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], c->model->n_vocab - 1);
+    return batch_eval_sample(c, tokens, temperature, top_p, u, tokens_out);
+}
+
+bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows, size_t n_vocab, const float * temperature, const float * top_p, const double * u,
+                                   const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out, float * probs_out) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, logits && n_rows > 0 && n_rows <= (size_t) SAMPLE_MAX_ROWS && n_vocab > 0 && n_vocab <= 65536,
+               "Invalid batch sampling arguments");
+    if (!check_sample_rows(sink, n_rows, n_vocab, temperature, top_p, u, bias_offsets, bias_ids, bias_values, tokens_out)) return false;
+    if (!hook_device(sink)) return false;
+    const size_t n_bias = bias_offsets ? bias_offsets[n_rows] : 0;
+    std::vector<SampleRow> rows(n_rows);
+    fill_sample_rows(rows.data(), n_rows, temperature, top_p, u, bias_offsets);
+    HookBuffers hb;     // the results are copied back at their exact size, without the guard region of HookBuffers::out
+    SampleBatchParams bp{};
+    bp.logits = hb.in(logits, n_rows * n_vocab); bp.n_vocab = (int) n_vocab; bp.n_rows = (int) n_rows;
+    bp.rows = hb.in(rows.data(), n_rows);
+    bp.bias_ids = n_bias ? hb.in(bias_ids, n_bias) : nullptr; bp.bias_values = n_bias ? hb.in(bias_values, n_bias) : nullptr;
+    bp.scratch = n_bias ? static_cast<float *>(hb.alloc(n_rows * n_vocab * sizeof(float))) : nullptr;
+    bp.token_out = static_cast<uint32_t *>(hb.alloc(n_rows * sizeof(uint32_t)));
+    bp.prob_out = probs_out ? static_cast<float *>(hb.alloc(n_rows * sizeof(float))) : nullptr;
+    const cudaError_t e = hb.ok ? launch_sample_batch(bp, 0) : cudaSuccess;
+    bool ok = hb.finish(e) && cudaMemcpy(tokens_out, bp.token_out, n_rows * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess;
+    if (ok && probs_out) ok = cudaMemcpy(probs_out, bp.prob_out, n_rows * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "batch sampling failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }
 
 bool rwkv_b200_stage_eval(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, const float * hidden_in, float * hidden_out, bool want_logits,

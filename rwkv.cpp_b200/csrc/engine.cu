@@ -621,6 +621,9 @@ void destroy_context(Context * ctx) {
     for (int i = 0; i < Context::MAX_SEGMENTS; i++) { if (ctx->seg_in[i]) cudaEventDestroy(ctx->seg_in[i]); if (ctx->seg_out[i]) cudaEventDestroy(ctx->seg_out[i]); }
     cudaFree(ctx->sample_token); cudaFree(ctx->sample_scratch); cudaFree(ctx->bias_ids); cudaFree(ctx->bias_values);
     if (ctx->sample_token_host) cudaFreeHost(ctx->sample_token_host);
+    cudaFree(ctx->sample_rows); cudaFree(ctx->sample_tokens);
+    if (ctx->sample_rows_host) cudaFreeHost(ctx->sample_rows_host);
+    if (ctx->sample_tokens_host) cudaFreeHost(ctx->sample_tokens_host);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
     if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
@@ -931,6 +934,26 @@ bool batch_get_logits(Context * ctx, int seq, float * logits_out) {
     return true;
 }
 
+namespace {
+
+// Device copy of a logit bias list (the buffers grow as needed) and the scratch of scratch_floats floats the biased logits go to.
+bool upload_bias(Context * ctx, const uint32_t * bias_ids, const float * bias_values, size_t n_bias, size_t scratch_floats) {
+    if (!ctx->sample_scratch) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_scratch), scratch_floats * sizeof(float)));
+    if (n_bias > ctx->bias_capacity) {
+        CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+        cudaFree(ctx->bias_ids); cudaFree(ctx->bias_values);
+        ctx->bias_ids = nullptr; ctx->bias_values = nullptr; ctx->bias_capacity = 0;
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_ids), n_bias * sizeof(uint32_t)));
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_values), n_bias * sizeof(float)));
+        ctx->bias_capacity = n_bias;
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_ids, bias_ids, n_bias * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_values, bias_values, n_bias * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    return true;
+}
+
+}  // namespace
+
 bool sample_token(Context * ctx, float temperature, float top_p, double u, const uint32_t * bias_ids, const float * bias_values, size_t n_bias, uint32_t * token_out) {
     const Model & m = *ctx->model;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, token_out != nullptr, "token_out is NULL");
@@ -948,19 +971,7 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
     }
     for (size_t i = 0; i < n_bias; i++)
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, bias_ids[i] < (uint32_t) m.n_vocab, "logit bias id %u is out of range", bias_ids[i]);
-    if (n_bias > 0) {
-        if (!ctx->sample_scratch) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_scratch), (size_t) m.n_vocab * sizeof(float)));
-        if (n_bias > ctx->bias_capacity) {
-            CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-            cudaFree(ctx->bias_ids); cudaFree(ctx->bias_values);
-            ctx->bias_ids = nullptr; ctx->bias_values = nullptr; ctx->bias_capacity = 0;
-            CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_ids), n_bias * sizeof(uint32_t)));
-            CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_values), n_bias * sizeof(float)));
-            ctx->bias_capacity = n_bias;
-        }
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_ids, bias_ids, n_bias * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_values, bias_values, n_bias * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    }
+    if (n_bias > 0 && !upload_bias(ctx, bias_ids, bias_values, n_bias, (size_t) m.n_vocab)) return false;
     SampleParams sp{};
     sp.logits = ctx->logits; sp.n_vocab = m.n_vocab; sp.temperature = temperature; sp.top_p = top_p; sp.u = u;
     sp.bias_ids = ctx->bias_ids; sp.bias_values = ctx->bias_values; sp.n_bias = (int) n_bias;
@@ -970,6 +981,70 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     *token_out = ctx->sample_token_host[0];
     return true;
+}
+
+static_assert(SAMPLE_MAX_ROWS == MAX_TOKENS_PER_PASS, "the batched sampling launch takes a row per sequence of the largest batch");
+
+bool check_sample_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const float * temperature, const float * top_p, const double * u,
+                       const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values, const uint32_t * tokens_out) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, temperature && top_p && u && tokens_out, "NULL temperature, top_p, u or tokens_out");
+    for (size_t b = 0; b < n_rows; b++) {     // sampling.py:20-23, as sample_token checks its one row
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, temperature[b] >= 0.0f, "temperature of row %zu must be >= 0", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, top_p[b] >= 0.0f && top_p[b] <= 1.0f, "top_p of row %zu must be in [0, 1]", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, u[b] >= 0.0 && u[b] < 1.0, "u of row %zu must be in [0, 1)", b);
+    }
+    if (!bias_offsets) return true;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, bias_offsets[0] == 0, "bias_offsets must start at 0");
+    for (size_t b = 0; b < n_rows; b++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, bias_offsets[b + 1] >= bias_offsets[b], "bias_offsets decrease after row %zu", b);
+    const size_t n_bias = bias_offsets[n_rows];
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_bias <= (size_t) INT32_MAX, "More than 2^31 - 1 logit bias entries");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_bias == 0 || (bias_ids && bias_values), "logit bias arrays are NULL");
+    for (size_t i = 0; i < n_bias; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, bias_ids[i] < n_vocab, "logit bias id %u is out of range", bias_ids[i]);
+    return true;
+}
+
+void fill_sample_rows(SampleRow * rows, size_t n_rows, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets) {
+    for (size_t b = 0; b < n_rows; b++)
+        rows[b] = SampleRow{temperature[b], top_p[b], u[b], bias_offsets ? (int) bias_offsets[b] : 0, bias_offsets ? (int) bias_offsets[b + 1] : 0};
+}
+
+bool batch_sample(Context * ctx, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets,
+                  const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out) {
+    const Model & m = *ctx->model;
+    const int B = ctx->batch_n;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, B > 0, "Not a batch context");
+    if (!check_sample_rows(ctx->sink(), B, m.n_vocab, temperature, top_p, u, bias_offsets, bias_ids, bias_values, tokens_out)) return false;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last batch evaluation skipped the head");
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.n_vocab <= 65536, "On-device sampling supports n_vocab <= 65536");
+    const size_t n_bias = bias_offsets ? bias_offsets[B] : 0;
+    CUDA_OK(ctx, cudaSetDevice(m.dev.device));
+    if (!ctx->sample_rows) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_rows), (size_t) B * sizeof(SampleRow)));
+    if (!ctx->sample_rows_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_rows_host), (size_t) B * sizeof(SampleRow)));
+    if (!ctx->sample_tokens) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_tokens), (size_t) B * sizeof(uint32_t)));
+    if (!ctx->sample_tokens_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_tokens_host), (size_t) B * sizeof(uint32_t)));
+    if (n_bias > 0 && !upload_bias(ctx, bias_ids, bias_values, n_bias, (size_t) B * m.n_vocab)) return false;
+    // every call ends with a stream synchronisation, so the previous copy out of the pinned rows has completed
+    fill_sample_rows(ctx->sample_rows_host, B, temperature, top_p, u, bias_offsets);
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_rows, ctx->sample_rows_host, (size_t) B * sizeof(SampleRow), cudaMemcpyHostToDevice, ctx->stream));
+    SampleBatchParams bp{};
+    bp.logits = ctx->logits; bp.n_vocab = m.n_vocab; bp.n_rows = B; bp.rows = ctx->sample_rows;
+    bp.bias_ids = n_bias ? ctx->bias_ids : nullptr; bp.bias_values = n_bias ? ctx->bias_values : nullptr;
+    bp.scratch = n_bias ? ctx->sample_scratch : nullptr; bp.token_out = ctx->sample_tokens; bp.prob_out = nullptr;
+    CUDA_OK(ctx, launch_sample_batch(bp, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_tokens_host, ctx->sample_tokens, (size_t) B * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    memcpy(tokens_out, ctx->sample_tokens_host, (size_t) B * sizeof(uint32_t));
+    return true;
+}
+
+bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * temperature, const float * top_p, const double * u, uint32_t * tokens_out) {
+    const Model & m = *ctx->model;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->batch_n > 0, "Not a batch context");
+    if (!check_sample_rows(ctx->sink(), ctx->batch_n, m.n_vocab, temperature, top_p, u, nullptr, nullptr, nullptr, tokens_out)) return false;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.n_vocab <= 65536, "On-device sampling supports n_vocab <= 65536");
+    return batch_eval(ctx, tokens, true) && batch_sample(ctx, temperature, top_p, u, nullptr, nullptr, nullptr, tokens_out);
 }
 
 bool pipe_ensure_box(Context * ctx) {

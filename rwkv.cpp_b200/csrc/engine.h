@@ -23,6 +23,7 @@ struct PipeGroup {
     std::atomic<int> refs{0};
 };
 
+struct SampleRow;                       // per-sequence sampling parameters (kernels/ops.h)
 struct CopyPool;                        // helper threads of the pageable-buffer bounce path (engine.cu)
 void destroy_copy_pool(CopyPool * p);
 
@@ -99,8 +100,11 @@ struct Context {
     bool logits_valid = false;       // ctx->logits holds the head output of the most recent pass
     uint32_t * sample_token = nullptr;   // device
     uint32_t * sample_token_host = nullptr;   // pinned
-    float * sample_scratch = nullptr;    // [n_vocab] device
-    uint32_t * bias_ids = nullptr; float * bias_values = nullptr; size_t bias_capacity = 0;   // device
+    float * sample_scratch = nullptr;    // [n_vocab] device ([batch_n, n_vocab] in a batch context)
+    uint32_t * bias_ids = nullptr; float * bias_values = nullptr; size_t bias_capacity = 0;   // device (a batch: all rows' lists back to back)
+    // ... and in a batch context the per-sequence parameters and results, [batch_n] each, allocated on the first batch_sample
+    SampleRow * sample_rows = nullptr, * sample_rows_host = nullptr;          // device / pinned
+    uint32_t * sample_tokens = nullptr, * sample_tokens_host = nullptr;       // device / pinned
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -156,6 +160,23 @@ bool batch_get_logits(Context * ctx, int seq, float * logits_out);
 // Samples the next token from ctx->logits on the device (reference python/sampling.py:10-52 with the caller's uniform number u in
 // [0, 1) in place of numpy's RandomState draw); only the token id is copied back. Requires a preceding pass that computed logits.
 bool sample_token(Context * ctx, float temperature, float top_p, double u, const uint32_t * bias_ids, const float * bias_values, size_t n_bias, uint32_t * token_out);
+
+// The arguments of a draw for each of n_rows rows (batch_sample, the batched kernel's test hook): non-NULL arrays, every row's
+// temperature, top_p and u in range, and, with bias_offsets, offsets from 0 that never decrease and bias ids below n_vocab.
+bool check_sample_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const float * temperature, const float * top_p, const double * u,
+                       const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values, const uint32_t * tokens_out);
+// rows[b] <- row b's parameters and its bias range (empty without bias_offsets); the arguments passed check_sample_rows.
+void fill_sample_rows(SampleRow * rows, size_t n_rows, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets);
+
+// Batch contexts: one draw per sequence from its column of ctx->logits, row b exactly what sample_token draws from the same logits
+// with temperature[b], top_p[b], u[b] and bias entries [bias_offsets[b], bias_offsets[b + 1]) of bias_ids / bias_values
+// (bias_offsets NULL = no bias; else batch_n + 1 entries from 0, non-decreasing). Checks every argument before it enqueues anything,
+// then one launch; only the batch_n token ids are copied back. Synchronises.
+bool batch_sample(Context * ctx, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets,
+                  const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out);
+// batch_eval(tokens, want_logits = true) + batch_sample without bias. The sampling arguments are checked before the pass, so a
+// rejected call leaves every sequence's state as it was.
+bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * temperature, const float * top_p, const double * u, uint32_t * tokens_out);
 
 size_t stage_hidden_len(const Model & m, size_t T);
 

@@ -135,4 +135,25 @@ struct SampleParams {
 };
 cudaError_t launch_sample(const SampleParams & p, cudaStream_t s);
 
+// The same draw for each row of a [n_rows, n_vocab] block of logits (a batch context's head output), one CTA per row. Row b uses
+// logits + b * n_vocab, rows[b] and bias entries [rows[b].bias_begin, rows[b].bias_end) of bias_ids / bias_values, and, when it has a
+// bias, scratch + b * n_vocab; it writes token_out[b] and, if prob_out, prob_out[b]. Each row gives the bits of launch_sample on it.
+struct SampleRow {
+    float temperature, top_p;
+    double u;
+    int bias_begin, bias_end;
+};
+constexpr int SAMPLE_MAX_ROWS = 256;  // MAX_TOKENS_PER_PASS: the sequences of the largest batch context
+struct SampleBatchParams {
+    const float * logits;             // [n_rows, n_vocab] device
+    int n_vocab, n_rows;
+    const SampleRow * rows;           // [n_rows] device
+    const uint32_t * bias_ids;        // device, concatenated bias lists of all rows, or NULL when no row has one
+    const float * bias_values;
+    float * scratch;                  // [n_rows, n_vocab] device, or NULL when no row has a bias
+    uint32_t * token_out;             // [n_rows] device
+    float * prob_out;                 // optional [n_rows] device
+};
+cudaError_t launch_sample_batch(const SampleBatchParams & p, cudaStream_t s);
+
 }  // namespace rwkv

@@ -8,6 +8,9 @@
 // The top-p cutoff -- the value of the sorted probabilities at the first index whose running sum exceeds top_p (:42-45) -- is found
 // without sorting: it is the largest value v for which sum(p[p >= v]) > top_p, located by bisection on the float bit pattern
 // (31 masked block sums over registers).
+//
+// The batched launch runs one such CTA per row of a [n_rows, n_vocab] logits block (a batch context's head output), each row with
+// its own parameters and bias; both kernels call the same sample_row body.
 #include "ops.h"
 #include "gemv.h"
 
@@ -41,12 +44,13 @@ __device__ float block_max_f(float v, float * slots) {
     return r;
 }
 
+// The whole draw for one row of logits, shared by the single-row and the batched kernel so that a row of a batch gives the bits of
+// a single launch. `p` is that row's view: its logits, parameters, bias, scratch and result words.
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const SampleParams p) {
+__device__ __forceinline__ void sample_row(const SampleParams & p) {
     __shared__ double dslots[SAMPLE_WARPS];
     __shared__ float fslots[SAMPLE_WARPS];
     __shared__ int first_flagged;
-    pdl_prologue();
     const int tid = threadIdx.x, V = p.n_vocab, base = tid * PER;
     const float * src = p.logits;
     if (p.n_bias > 0) {     // logits + bias through the scratch copy (a dict has no duplicate ids, :30-33)
@@ -156,6 +160,27 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const SamplePara
     }
 }
 
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(const SampleParams p) {
+    pdl_prologue();
+    sample_row<PER>(p);
+}
+
+// CTA b draws row b: logits + b * n_vocab with rows[b]'s parameters and bias entries [bias_begin, bias_end), scratch slice b.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS) batch_sample_kernel(const SampleBatchParams bp) {
+    pdl_prologue();
+    const int b = blockIdx.x;
+    const SampleRow r = bp.rows[b];
+    const size_t off = (size_t) b * bp.n_vocab;
+    SampleParams p;
+    p.logits = bp.logits + off; p.n_vocab = bp.n_vocab;
+    p.temperature = r.temperature; p.top_p = r.top_p; p.u = r.u;
+    p.bias_ids = bp.bias_ids + r.bias_begin; p.bias_values = bp.bias_values + r.bias_begin; p.n_bias = r.bias_end - r.bias_begin;
+    p.scratch = bp.scratch ? bp.scratch + off : nullptr; p.token_out = bp.token_out + b; p.prob_out = bp.prob_out ? bp.prob_out + b : nullptr;
+    sample_row<PER>(p);
+}
+
 }  // namespace
 
 cudaError_t launch_sample(const SampleParams & p, cudaStream_t s) {
@@ -166,6 +191,17 @@ cudaError_t launch_sample(const SampleParams & p, cudaStream_t s) {
     if (per <= 16) return launch_pdl(sample_kernel<16>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
     if (per <= 50) return launch_pdl(sample_kernel<50>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
     return launch_pdl(sample_kernel<64>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
+}
+
+cudaError_t launch_sample_batch(const SampleBatchParams & p, cudaStream_t s) {
+    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    const dim3 grid(p.n_rows);
+    if (per <= 1) return launch_pdl(batch_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 4) return launch_pdl(batch_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 16) return launch_pdl(batch_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 50) return launch_pdl(batch_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return launch_pdl(batch_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
 }
 
 }  // namespace rwkv

@@ -158,6 +158,14 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_sample_logits.restype = ctypes.c_bool
         lib.rwkv_b200_eval_sample.argtypes = [vp, ctypes.c_uint32, ctypes.c_float, ctypes.c_float, ctypes.c_double, P_U32]
         lib.rwkv_b200_eval_sample.restype = ctypes.c_bool
+        P_DOUBLE = ctypes.POINTER(ctypes.c_double)
+        lib.rwkv_b200_batch_sample.argtypes = [vp, P_FLOAT, P_FLOAT, P_DOUBLE, P_U32, P_U32, P_FLOAT, P_U32]
+        lib.rwkv_b200_batch_sample.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_eval_sample.argtypes = [vp, P_U32, P_FLOAT, P_FLOAT, P_DOUBLE, P_U32]
+        lib.rwkv_b200_batch_eval_sample.restype = ctypes.c_bool
+        lib.rwkv_b200_sample_logits_batch.argtypes = [P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, P_FLOAT, P_FLOAT, P_DOUBLE, P_U32, P_U32, P_FLOAT,
+                                                      P_U32, P_FLOAT]
+        lib.rwkv_b200_sample_logits_batch.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
