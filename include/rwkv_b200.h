@@ -135,7 +135,9 @@ RWKV_API bool rwkv_b200_pipe_eval(struct rwkv_context * ctx, const uint32_t * to
 RWKV_API float rwkv_b200_last_device_ms(const struct rwkv_context * ctx);     /* CUDA-event time of the last pass */
 RWKV_API uint64_t rwkv_b200_kernel_launch_count(void);                         /* kernels enqueued by this process */
 RWKV_API uint64_t rwkv_b200_bytes_per_token(const struct rwkv_context * ctx, bool with_logits);
-/* The part of that byte model the fused dequantize-GEMV kernel streams: every layer matrix (+ the head), at file precision. */
+/* The part of that byte model the GEMV launches of the context's decode pass stream: every layer matrix (+ the head), at file
+ * precision -- except, in a single-sequence context, the v6 LoRA matrices maa_w1 / decay_w2 of the layers whose single-token pass folds
+ * them into the LayerNorm-mix and WKV launches (rwkv_b200_v6_lora_fold_supported). */
 RWKV_API uint64_t rwkv_b200_gemv_bytes_per_token(const struct rwkv_context * ctx, bool with_logits);
 /* Times `n_steps` back-to-back resident passes of `tokens_per_step` tokens each (after `warmup_steps` untimed ones)
  * with CUDA events on the context's own stream. `tokens` holds (warmup_steps + n_steps) * tokens_per_step ids.
@@ -314,6 +316,41 @@ struct rwkv_b200_gemv_batch_args {
     int * n_launches;
 };
 RWKV_API bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a);
+
+/* The v6 fold of single-token passes of single-sequence contexts: does a layer of this shape run maa_w1 (5 * mix rows of n_embed, type
+ * w1_type) inside the LayerNorm-mix launch and decay_w2 (n_embed rows of `decay`, type w2_type) inside the WKV launch? Shapes only, no
+ * device. Otherwise the layer runs the two GEMV launches. */
+RWKV_API bool rwkv_b200_v6_lora_fold_supported(int n_embed, int head_size, int w1_type, int mix, int w2_type, int decay);
+
+/* The two folded kernels on host buffers. Arguments outside what rwkv_b200_v6_lora_fold_supported admits are rejected (ARGS) before any
+ * device is touched. Weights are in the file layout of their type, unpadded.
+ * v6 prologue (launch_v6_prologue): ln_mix of one token, formula 1, one mix vector `coef` (state_out, out_xx, out_sx [C]), then
+ * y1[M1] = tanh(W1 . mix), W1 [M1, C]; equal to rwkv_b200_test_ln_mix followed by rwkv_b200_test_gemv_batch (epi 3) on its out0. */
+struct rwkv_b200_v6_prologue_args {
+    const float * x, * ln_w, * ln_b, * state_in, * coef;
+    float * state_out, * out_xx, * out_sx;
+    const void * w1;
+    int w1_type, M1;
+    float * y1;
+    int C;
+};
+RWKV_API bool rwkv_b200_test_v6_prologue(const struct rwkv_b200_v6_prologue_args * a);
+/* wkv6 of one token of one sequence with head size 64 whose decay is exp(-exp(W2 . lora1 + td_bias)), W2 [C, K2]: equal to
+ * rwkv_b200_test_gemv_batch (epi 7) followed by rwkv_b200_test_wkv6 with td_per_token. Other fields as in rwkv_b200_wkv6_args. */
+struct rwkv_b200_wkv6_decay_args {
+    const float * r, * k, * v, * tf, * state_in;
+    float * state_out;
+    const float * lnx_w, * lnx_b, * g;
+    float * y;
+    float eps;
+    int H;
+    const void * w2;
+    int w2_type, K2;
+    const float * lora1, * td_bias;
+    unsigned char * q_out;
+    int q_type;
+};
+RWKV_API bool rwkv_b200_test_wkv6_decay(const struct rwkv_b200_wkv6_decay_args * a);
 
 #if defined(__cplusplus)
 }

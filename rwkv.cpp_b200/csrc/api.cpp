@@ -568,7 +568,9 @@ uint64_t rwkv_b200_kernel_launch_count(void) { return g_kernel_launches; }
 
 uint64_t rwkv_b200_gemv_bytes_per_token(const struct rwkv_context * ctx, bool with_logits) {
     const Model & m = *C(ctx)->model;
-    return (uint64_t) (m.gemv_bytes_per_token - (with_logits ? 0 : m.head_matrix_bytes));
+    // the decode pass of a single-sequence context folds v6 LoRA matrices into other kernels; a batch context streams them all
+    const size_t folded = C(ctx)->batch_n ? 0 : v6_folded_gemv_bytes(m);
+    return (uint64_t) (m.gemv_bytes_per_token - (with_logits ? 0 : m.head_matrix_bytes) - folded);
 }
 
 uint64_t rwkv_b200_bytes_per_token(const struct rwkv_context * ctx, bool with_logits) {
@@ -844,6 +846,70 @@ bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a) {
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
     const cudaError_t e = b.ok ? launch_wkv7(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+static GemvProblem fold_problem(int type, int K, int M, int epi) {
+    GemvProblem p{};
+    p.type = type; p.K = K; p.M = M; p.epi = epi; p.ldx = K; p.ldy = M;
+    p.pitch = dtype_supported(type) && K > 0 && K % dtype_block_elems(type) == 0 ? matrix_pitch(type, (uint64_t) K) : 0;
+    return p;
+}
+
+bool rwkv_b200_v6_lora_fold_supported(int n_embed, int head_size, int w1_type, int mix, int w2_type, int decay) {
+    if (mix < 1 || decay < 1) return false;
+    GemvProblem w1 = fold_problem(w1_type, n_embed, 5 * mix, EPI_TANH), dw2 = fold_problem(w2_type, decay, n_embed, EPI_BIAS_EXPNEGEXP);
+    return v6_lora_fold_shapes(n_embed, head_size, w1, dw2);
+}
+
+bool rwkv_b200_test_v6_prologue(const struct rwkv_b200_v6_prologue_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    GemvProblem w1 = fold_problem(a ? a->w1_type : -1, a ? a->C : 0, a ? a->M1 : 0, EPI_TANH);
+    const bool args = a && a->x && a->ln_w && a->ln_b && a->state_in && a->coef && a->state_out && a->out_xx && a->out_sx && a->w1 && a->y1 &&
+                      a->M1 > 0 && v6_prologue_fits(a->C, w1);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid v6_prologue arguments");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C;
+    HookBuffers b;
+    LnMixParams p{};
+    p.x = b.in(a->x, C); p.ln_w = b.in(a->ln_w, C); p.ln_b = b.in(a->ln_b, C);
+    p.state_in = b.in(a->state_in, C); p.state_out = b.out(a->state_out, C);
+    p.C = a->C; p.T = 1; p.formula = 1; p.n_out = 1; p.coef[0] = b.in(a->coef, C);
+    p.out_xx = b.out(a->out_xx, C); p.out_sx = b.out(a->out_sx, C);
+    uint8_t * W = static_cast<uint8_t *>(b.alloc((size_t) a->M1 * (size_t) w1.pitch + 256));
+    if (b.ok) b.ok = upload_matrix(a->w1, a->w1_type, a->M1, a->C, W, nullptr) == cudaSuccess;
+    w1.W = W; w1.y = b.out(a->y1, (size_t) a->M1);
+    const cudaError_t e = b.ok ? launch_v6_prologue(p, w1, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "v6_prologue failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv6_decay(const struct rwkv_b200_wkv6_decay_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const int C = a ? a->H * 64 : 0;
+    GemvProblem dw2 = fold_problem(a ? a->w2_type : -1, a ? a->K2 : 0, C, EPI_BIAS_EXPNEGEXP);
+    const bool args = a && a->r && a->k && a->v && a->tf && a->state_in && a->state_out && a->lnx_w && a->lnx_b && a->y && a->w2 && a->lora1 &&
+                      a->td_bias && a->H > 0 && a->H <= 4096 / 64 && wkv6_decay_fits(C, 64, dw2) && staged_ok(a->q_out, a->q_type, 1, 0, 64);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid wkv6_decay arguments");
+    if (!hook_device(sink)) return false;
+    const size_t Cs = (size_t) C;
+    HookBuffers b;
+    Wkv6Params p{};
+    p.r = b.in(a->r, Cs); p.k = b.in(a->k, Cs); p.v = b.in(a->v, Cs); p.tf = b.in(a->tf, Cs);
+    p.td = nullptr; p.td_per_token = 0; p.per_head_scalars = 0;
+    p.state_in = b.in(a->state_in, Cs * 64); p.state_out = b.out(a->state_out, Cs * 64);
+    p.lnx_w = b.in(a->lnx_w, Cs); p.lnx_b = b.in(a->lnx_b, Cs); p.g = b.in(a->g, Cs);
+    p.y = b.out(a->y, Cs);
+    p.eps = a->eps; p.H = a->H; p.S = 64; p.T = 1;
+    p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, C)) : nullptr; p.q_type = a->q_type;
+    uint8_t * W = static_cast<uint8_t *>(b.alloc(Cs * (size_t) dw2.pitch + 256));
+    if (b.ok) b.ok = upload_matrix(a->w2, a->w2_type, C, a->K2, W, nullptr) == cudaSuccess;
+    dw2.W = W; dw2.x = b.in(a->lora1, (size_t) a->K2); dw2.bias = b.in(a->td_bias, Cs);
+    p.dw2 = dw2;
+    const cudaError_t e = b.ok ? launch_wkv6(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv6_decay failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

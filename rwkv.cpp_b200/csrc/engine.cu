@@ -289,12 +289,64 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     return att_output(ctx, L, s, T, wp.q_out);
 }
 
+}  // namespace
+
+bool v6_prologue_fits(int C, GemvProblem & w1) {
+    if (C < 1 || C > 4096 || w1.K != C || w1.M < 1 || !dtype_supported(w1.type) || w1.K % dtype_block_elems(w1.type)) return false;
+    return gemv_tma_plan(w1) && w1.wk == 1 && v6_prologue_smem_bytes(w1, C) <= V6_PROLOGUE_MAX_SMEM;
+}
+
+bool wkv6_decay_fits(int C, int S, GemvProblem & dw2) {
+    // dw2.K <= 128: lora1 is staged by stage_column, whose F16 / F32 loops give element k to thread k with a stride of 256, run by the
+    // 192 threads of the WKV block -- elements 192..255 of a stride would be skipped, so K must stay below 192
+    if (S != 64 || C < S || C % S || dw2.M != C || dw2.K < 32 || dw2.K > 128 || !dtype_supported(dw2.type) || dw2.K % dtype_block_elems(dw2.type)) return false;
+    return gemv_tma_plan(dw2) && dw2.wk == 1 && wkv6_decay_smem_bytes(dw2) <= WKV6_DECAY_MAX_SMEM;
+}
+
+bool v6_lora_fold_shapes(int C, int S, GemvProblem & w1, GemvProblem & dw2) {
+    return v6_prologue_fits(C, w1) && wkv6_decay_fits(C, S, dw2);
+}
+
+bool v6_lora_fold(const Layer & L, int C, int S, GemvProblem & w1, GemvProblem & dw2) {
+    if (!L.att_maa_w1.data || !L.att_decay_w2.data) return false;
+    auto problem = [](const DevMatrix & W, int epi) {
+        GemvProblem p{};
+        p.W = W.data; p.Wt = W.tiled; p.pitch = W.pitch; p.type = W.type; p.K = W.K; p.M = W.M;
+        p.ldx = W.K; p.ldy = W.M; p.epi = epi; p.pro = PRO_NONE;
+        return p;
+    };
+    w1 = problem(L.att_maa_w1, EPI_TANH);
+    dw2 = problem(L.att_decay_w2, EPI_BIAS_EXPNEGEXP);
+    return v6_lora_fold_shapes(C, S, w1, dw2);
+}
+
+size_t v6_folded_gemv_bytes(const Model & m) {
+    if (m.arch_major != 6) return 0;
+    size_t n = 0;
+    for (int i = m.layer_begin; i < m.layer_end; i++) {
+        const Layer & L = m.layers[i];
+        GemvProblem w1, dw2;
+        if (v6_lora_fold(L, m.n_embed, m.head_size, w1, dw2))
+            n += tensor_nbytes(w1.type, (uint64_t) w1.K, (uint64_t) w1.M, 1) + tensor_nbytes(dw2.type, (uint64_t) dw2.K, (uint64_t) dw2.M, 1);
+    }
+    return n;
+}
+
+namespace {
+
 bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
-    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
-    {   // :313-321  tanh(W1 . xxx)
-        Batch b(T);
+    // single-token passes of one sequence: maa_w1 folded into the LayerNorm-mix launch and decay_w2 into the WKV launch
+    GemvProblem w1{}, dw2{};
+    const bool fold = T == 1 && !ctx->batch_stride && v6_lora_fold(L, m.n_embed, m.head_size, w1, dw2);
+    if (fold) {
+        w1.x = s.mix[0]; w1.y = s.lora[0];
+        dw2.x = s.lora[1]; dw2.bias = L.att_time_decay.data;     // dw2's output is the WKV kernel's decay row in shared memory
+        CUDA_OK(ctx, launch_v6_prologue(lp, w1, ctx->stream));
+    } else {
+        CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
+        Batch b(T);   // :313-321  tanh(W1 . xxx)
         b.add(L.att_maa_w1, s.mix[0], s.lora[0], EPI_TANH);
         if (!run_batch(ctx, b)) return false;
     }
@@ -320,7 +372,7 @@ bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
         xq_bind(b.add(L.att_decay_w1, s.mix[1], s.lora[1], EPI_TANH), vp.q_out[0], vp.q_type[0]);
         if (!run_batch(ctx, b)) return false;
     }
-    {   // :357-367  w = exp(-exp(Wd2 . tanh(..) + time_decay))
+    if (!fold) {   // :357-367  w = exp(-exp(Wd2 . tanh(..) + time_decay))
         Batch b(T);
         GemvProblem & p = b.add(L.att_decay_w2, s.lora[1], s.w, EPI_BIAS_EXPNEGEXP);
         p.bias = L.att_time_decay.data;
@@ -328,7 +380,8 @@ bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     }
     Wkv6Params wp{};   // :370-382
     wp.r = s.r; wp.k = s.k; wp.v = s.v;
-    wp.td = s.w; wp.td_per_token = 1; wp.tf = L.att_time_faaaa.data; wp.per_head_scalars = 0;
+    wp.td = fold ? nullptr : s.w; wp.td_per_token = fold ? 0 : 1; wp.tf = L.att_time_faaaa.data; wp.per_head_scalars = 0;
+    if (fold) wp.dw2 = dw2;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;

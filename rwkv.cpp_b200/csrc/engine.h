@@ -180,6 +180,20 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 
 size_t stage_hidden_len(const Model & m, size_t T);
 
+// Single-token passes of a single-sequence v6 context fold the two LoRA matrices that stream almost nothing into their neighbours:
+// maa_w1 into the LayerNorm-mix launch (launch_v6_prologue), decay_w2 into the WKV launch (Wkv6Params::dw2). This is the one
+// predicate that decides it, from shapes alone: head size 64, n_embed <= 4096, both matrices planned by the streaming GEMV with one
+// warp per row (WK == 1) and their rows fitting the shared memory of the two kernels. On true, w1 and dw2 hold the matrices' problems
+// (weights, plan, epilogue) without activation pointers.
+bool v6_lora_fold_shapes(int C, int S, GemvProblem & w1, GemvProblem & dw2);
+// Its two halves, also the argument checks of the fused kernels' test hooks: maa_w1 (w1) for launch_v6_prologue, decay_w2 (dw2) for
+// launch_wkv6 with Wkv6Params::dw2 set. Both fill the plan (wk, g) of the problem they are given.
+bool v6_prologue_fits(int C, GemvProblem & w1);
+bool wkv6_decay_fits(int C, int S, GemvProblem & dw2);
+bool v6_lora_fold(const Layer & L, int C, int S, GemvProblem & w1, GemvProblem & dw2);
+// GEMV-streamed weight bytes of one token that the fold takes out of the GEMV launches (maa_w1 + decay_w2 of the folded layers).
+size_t v6_folded_gemv_bytes(const Model & m);
+
 // One pipeline stage: the resident layers [layer_begin, layer_end) for T <= MAX_TOKENS_PER_PASS tokens. The first stage
 // embeds `tokens`, the others start from `hidden_in`; every stage but the last leaves its result in `hidden_out`
 // (device pointers, stage_hidden_len(T) floats); the last one computes the logits when asked. `stream` (may be NULL = the

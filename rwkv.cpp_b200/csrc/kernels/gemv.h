@@ -77,6 +77,8 @@ cudaError_t gemv_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t 
 // gemm_tc_launch and the rest to gemv_launch; otherwise the whole batch goes to gemv_launch. workspace may be NULL (no tensor cores).
 cudaError_t gemv_route(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream, void * workspace, size_t workspace_bytes, int tc_min_T);
 cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);      // cudaErrorNotSupported if a shape does not fit
+// The streaming kernel's row plan of p (p.wk, p.g), a function of (type, K, pitch) alone; false if the shape needs the generic kernel.
+bool gemv_tma_plan(GemvProblem & p);
 cudaError_t gemv_generic_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);
 
 // Brings a freshly uploaded matrix (file bytes, rows `pitch` bytes apart) into the device layout of quant_decode.cuh, in place: the

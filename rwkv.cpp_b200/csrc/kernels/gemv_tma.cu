@@ -162,6 +162,12 @@ bool plan_wk(GemvProblem & p) {
     return false;
 }
 
+}  // namespace
+
+bool gemv_tma_plan(GemvProblem & p) { return plan_wk(p); }
+
+namespace {
+
 template <int NC, int ONLY = -1, bool HAS_LN = true>
 cudaError_t launch_tma_nc(const GemvBatch & batch, int grid, size_t smem, cudaStream_t stream) {
     static PerDeviceOnce once;                // the shared-memory opt-in is per device

@@ -354,6 +354,100 @@ __device__ __forceinline__ float group_sum(float v, int G) {
     return v;
 }
 
+// One row's lane partials for NC activation columns in shared memory (colb bytes apart), the lane map's order: lane `sub` of
+// warp slice `wk` takes items wk * per + sub, + G, ... (quantised types: units, each block in order). acc[] starts at 0 and is
+// summed by group_sum, then across the WK warps of the row in warp order. The streaming GEMV and the fused v6 LoRA kernels
+// (glue.cu, wkv.cu) all compute a row through this function, so their bits agree.
+template <int TYPE, int NC>
+__device__ __forceinline__ void row_partial(const uint8_t * wrow, const uint8_t * act, size_t colb, int nc, int K, const LaneMap & m, float (&acc)[NC]) {
+#pragma unroll
+    for (int c = 0; c < NC; c++) acc[c] = 0.f;
+    if constexpr (TYPE == DT_F32) {
+        const int n4 = K / 4, per = (n4 + m.WK - 1) / m.WK, end = min(n4, (m.wk + 1) * per);
+        for (int i = m.wk * per + m.sub; i < end; i += m.G) {
+            const float4 wv = reinterpret_cast<const float4 *>(wrow)[i];
+#pragma unroll
+            for (int c = 0; c < NC; c++) if (c < nc) {
+                const float4 xv = reinterpret_cast<const float4 *>(act + c * colb)[i];
+                acc[c] = __fmaf_rn(wv.x, xv.x, acc[c]); acc[c] = __fmaf_rn(wv.y, xv.y, acc[c]);
+                acc[c] = __fmaf_rn(wv.z, xv.z, acc[c]); acc[c] = __fmaf_rn(wv.w, xv.w, acc[c]);
+            }
+        }
+        if (m.wk == m.WK - 1) for (int k = n4 * 4 + m.sub; k < K; k += m.G) {
+            const float wf = reinterpret_cast<const float *>(wrow)[k];
+#pragma unroll
+            for (int c = 0; c < NC; c++) if (c < nc) acc[c] = __fmaf_rn(wf, reinterpret_cast<const float *>(act + c * colb)[k], acc[c]);
+        }
+    } else if constexpr (TYPE == DT_F16) {
+        const int n8 = K / 8, per = (n8 + m.WK - 1) / m.WK, end = min(n8, (m.wk + 1) * per);
+        for (int i = m.wk * per + m.sub; i < end; i += m.G) {
+            const uint4 wv = reinterpret_cast<const uint4 *>(wrow)[i];
+            const __half2 * wh = reinterpret_cast<const __half2 *>(&wv);
+#pragma unroll
+            for (int c = 0; c < NC; c++) if (c < nc) {
+                const uint4 xv = reinterpret_cast<const uint4 *>(act + c * colb)[i];
+                const __half2 * xh = reinterpret_cast<const __half2 *>(&xv);
+#pragma unroll
+                for (int q = 0; q < 4; q++) {
+                    const float2 wf = __half22float2(wh[q]), xf = __half22float2(xh[q]);
+                    acc[c] = __fmaf_rn(wf.x, xf.x, acc[c]);
+                    acc[c] = __fmaf_rn(wf.y, xf.y, acc[c]);
+                }
+            }
+        }
+        if (m.wk == m.WK - 1) for (int k = n8 * 8 + m.sub; k < K; k += m.G) {
+            const float wf = __half2float(reinterpret_cast<const __half *>(wrow)[k]);
+#pragma unroll
+            for (int c = 0; c < NC; c++) if (c < nc) acc[c] = __fmaf_rn(wf, __half2float(reinterpret_cast<const __half *>(act + c * colb)[k]), acc[c]);
+        }
+    } else {
+        using TR = QTraits<TYPE>;
+        constexpr int UB = TR::UNIT_BLOCKS, UW = TR::UNIT_WORDS;
+        const int nblk = K / 32, nunits = (nblk + UB - 1) / UB;
+        const int upw = (nunits + m.WK - 1) / m.WK, u_end = min(nunits, (m.wk + 1) * upw);
+        // same block order per lane as consume_quant_regs: u = wk*upw + sub + G j, bi = 0..UB-1
+        for (int u = m.wk * upw + m.sub; u < u_end; u += m.G) {
+            uint32_t w[UW];
+            load_unit<TYPE>(wrow, u, w);
+#pragma unroll
+            for (int bi = 0; bi < UB; bi++) {
+                if (u * UB + bi < nblk) {
+                    BlockQ bq;
+                    decode_block<TYPE>(w, bi, bq);
+#pragma unroll
+                    for (int c = 0; c < NC; c++) if (c < nc) {
+                        const uint8_t * col = act + c * colb;
+                        const int4 lo = *act_q_ptr<UB>(col, nunits, u, bi, 0), hi = *act_q_ptr<UB>(col, nunits, u, bi, 1);
+                        const int a8[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+                        acc[c] = block_dot<TYPE>(bq, a8, *act_s_ptr<UB>(col, nunits, u, bi), acc[c]);
+                    }
+                }
+            }
+        }
+    }
+}
+
+// Rows [0, n_rows) of P starting at row0, held in shared memory (P.pitch bytes apart), against one activation column staged by
+// stage_column, for a problem whose plan has WK == 1 (gemv_tma_plan): the CTA's warps take row groups of 32 / G rows in turn,
+// and out[r] = epilogue(row row0 + r). Used by kernels that fold a small GEMV into themselves; blockDim.x is a multiple of 32.
+template <int TYPE>
+__device__ __forceinline__ void rows_dot(const GemvProblem & P, const uint8_t * rows, int n_rows, int row0, const uint8_t * act, float * out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    LaneMap m;
+    m.G = P.g; m.RPS = 32 / m.G; m.sub = lane & (m.G - 1); m.rs = lane / m.G;
+    m.WK = 1; m.WR = nwarps; m.wk = 0; m.wr = warp;
+    for (int rb = warp * m.RPS; rb < n_rows; rb += nwarps * m.RPS) {
+        const int r = rb + m.rs;
+        const bool store = r < n_rows && m.sub == 0;
+        EpiOperands e; e.a = 0.f; e.b = 0.f;
+        if (store) e = prefetch_epilogue(P, row0 + r, 0);
+        float acc[1];
+        row_partial<TYPE, 1>(rows + (size_t) min(r, n_rows - 1) * (size_t) P.pitch, act, 0, 1, P.K, m, acc);
+        const float v = group_sum(acc[0], m.G);
+        if (store) out[r] = apply_epilogue(P, v, e.a, e.b);
+    }
+}
+
 // ---- consumer: quantised weights, one column, activations in registers (the decode hot path) ------------------
 template <int TYPE, bool GUARD = false>
 __device__ void consume_quant_regs(Shared & sh, uint8_t * ring, uint32_t stage_bytes, const uint8_t * act, int c0, float * red, int it0, int my_tiles,
@@ -476,71 +570,7 @@ __device__ void consume_smem(Shared & sh, uint8_t * ring, uint32_t stage_bytes, 
                 if (m.WK == 1 && m.sub == 0 && live_row && c < nc) e[c] = prefetch_epilogue(P, row0 + r, c0 + c);
             }
             float acc[NC];
-#pragma unroll
-            for (int c = 0; c < NC; c++) acc[c] = 0.f;
-            if constexpr (TYPE == DT_F32) {
-                const int n4 = K / 4, per = (n4 + m.WK - 1) / m.WK, end = min(n4, (m.wk + 1) * per);
-                for (int i = m.wk * per + m.sub; i < end; i += m.G) {
-                    const float4 wv = reinterpret_cast<const float4 *>(wrow)[i];
-#pragma unroll
-                    for (int c = 0; c < NC; c++) if (c < nc) {
-                        const float4 xv = reinterpret_cast<const float4 *>(act + c * colb)[i];
-                        acc[c] = __fmaf_rn(wv.x, xv.x, acc[c]); acc[c] = __fmaf_rn(wv.y, xv.y, acc[c]);
-                        acc[c] = __fmaf_rn(wv.z, xv.z, acc[c]); acc[c] = __fmaf_rn(wv.w, xv.w, acc[c]);
-                    }
-                }
-                if (m.wk == m.WK - 1) for (int k = n4 * 4 + m.sub; k < K; k += m.G) {
-                    const float wf = reinterpret_cast<const float *>(wrow)[k];
-#pragma unroll
-                    for (int c = 0; c < NC; c++) if (c < nc) acc[c] = __fmaf_rn(wf, reinterpret_cast<const float *>(act + c * colb)[k], acc[c]);
-                }
-            } else if constexpr (TYPE == DT_F16) {
-                const int n8 = K / 8, per = (n8 + m.WK - 1) / m.WK, end = min(n8, (m.wk + 1) * per);
-                for (int i = m.wk * per + m.sub; i < end; i += m.G) {
-                    const uint4 wv = reinterpret_cast<const uint4 *>(wrow)[i];
-                    const __half2 * wh = reinterpret_cast<const __half2 *>(&wv);
-#pragma unroll
-                    for (int c = 0; c < NC; c++) if (c < nc) {
-                        const uint4 xv = reinterpret_cast<const uint4 *>(act + c * colb)[i];
-                        const __half2 * xh = reinterpret_cast<const __half2 *>(&xv);
-#pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            const float2 wf = __half22float2(wh[q]), xf = __half22float2(xh[q]);
-                            acc[c] = __fmaf_rn(wf.x, xf.x, acc[c]);
-                            acc[c] = __fmaf_rn(wf.y, xf.y, acc[c]);
-                        }
-                    }
-                }
-                if (m.wk == m.WK - 1) for (int k = n8 * 8 + m.sub; k < K; k += m.G) {
-                    const float wf = __half2float(reinterpret_cast<const __half *>(wrow)[k]);
-#pragma unroll
-                    for (int c = 0; c < NC; c++) if (c < nc) acc[c] = __fmaf_rn(wf, __half2float(reinterpret_cast<const __half *>(act + c * colb)[k]), acc[c]);
-                }
-            } else {
-                using TR = QTraits<TYPE>;
-                constexpr int UB = TR::UNIT_BLOCKS, UW = TR::UNIT_WORDS;
-                const int nblk = K / 32, nunits = (nblk + UB - 1) / UB;
-                const int upw = (nunits + m.WK - 1) / m.WK, u_end = min(nunits, (m.wk + 1) * upw);
-                // same block order per lane as consume_quant_regs: u = wk*upw + sub + G j, bi = 0..UB-1
-                for (int u = m.wk * upw + m.sub; u < u_end; u += m.G) {
-                    uint32_t w[UW];
-                    load_unit<TYPE>(wrow, u, w);
-#pragma unroll
-                    for (int bi = 0; bi < UB; bi++) {
-                        if (u * UB + bi < nblk) {
-                            BlockQ bq;
-                            decode_block<TYPE>(w, bi, bq);
-#pragma unroll
-                            for (int c = 0; c < NC; c++) if (c < nc) {
-                                const uint8_t * col = act + c * colb;
-                                const int4 lo = *act_q_ptr<UB>(col, nunits, u, bi, 0), hi = *act_q_ptr<UB>(col, nunits, u, bi, 1);
-                                const int a8[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-                                acc[c] = block_dot<TYPE>(bq, a8, *act_s_ptr<UB>(col, nunits, u, bi), acc[c]);
-                            }
-                        }
-                    }
-                }
-            }
+            row_partial<TYPE, NC>(wrow, act, colb, nc, K, m, acc);
 #pragma unroll
             for (int c = 0; c < NC; c++) {
                 const float v = group_sum(acc[c], m.G);

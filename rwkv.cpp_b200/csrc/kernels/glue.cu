@@ -4,6 +4,7 @@
 #include "gemv.h"          // launch_pdl
 #include "../formats.h"
 #include "act_stage.cuh"
+#include "gemv_tma_device.cuh"   // stage_column / rows_dot of the v6 prologue
 
 #include <cuda_fp16.h>
 
@@ -82,12 +83,11 @@ __device__ __forceinline__ double block_sum_ln(double v, double * slots) {
 // vectors -- every v6 block --, 6 for v4 / v5.2 / v7 time mixing: a few spilled registers there against one HBM round trip per vector).
 // BATCH (seq_stride > 0): block t is the one token of sequence t. Its previous LN(x) is always that sequence's carry, never
 // column t - 1, and it always writes the sequence's new carry.
+// The body is shared with v6_prologue_kernel: token t of the launch; out0, if not NULL, takes the place of p.out[0] (t == 0);
+// write_carry = false skips out_sx, out_xx and state_out.
 template <int PER, int PRE_N, bool BATCH>
-__global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p) {
-    __shared__ double slots[4][LN_WARPS];
-    trace_begin(p.trace);
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    const int C = p.C, t = blockIdx.x, tid = threadIdx.x;
+__device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float * out0, bool write_carry, double (&slots)[4][LN_WARPS]) {
+    const int C = p.C, tid = threadIdx.x;
     // LayerNorm weights and the carry are loaded before the wait where registers allow it (PER <= 8); at PER = 16 holding them
     // across the statistics spills past the stack budget, so they are read where they are used
     constexpr bool EARLY = PER <= 8;
@@ -154,7 +154,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
 #pragma unroll
         for (int j = 0; j < PRE_N; j++) {
             if (j >= p.n_out) break;
-            float * out = p.out[j];
+            float * out = (out0 && j == 0) ? out0 : p.out[j];
 #pragma unroll
             for (int i = 0; i < PER; i++) {
                 const int c = tid + i * LN_THREADS;
@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
 #pragma unroll 1
         for (int j = PRE ? PRE_N : 0; j < p.n_out; j++) {     // rolled: kernel parameters are indexable in the constant bank
             const float * coef = p.coef[j];
-            float * out = p.out[j];
+            float * out = (out0 && j == 0) ? out0 : p.out[j];
 #pragma unroll
             for (int i = 0; i < PER; i++) {
                 const int c = tid + i * LN_THREADS;
@@ -182,6 +182,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
             }
         }
     }
+    if (!write_carry) return;
 #pragma unroll
     for (int i = 0; i < PER; i++) {
         const int c = tid + i * LN_THREADS;
@@ -190,6 +191,44 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
         if (p.out_xx) p.out_xx[o0 + i * LN_THREADS] = xa[i];
         if (BATCH || t == p.T - 1) p.state_out[BATCH ? t * p.seq_stride + c : c] = xa[i];
     }
+}
+
+template <int PER, int PRE_N, bool BATCH>
+__global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p) {
+    __shared__ double slots[4][LN_WARPS];
+    trace_begin(p.trace);
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    ln_mix_body<PER, PRE_N, BATCH>(p, blockIdx.x, nullptr, true, slots);
+    trace_end(p.trace);
+}
+
+// ln_mix + the first v6 LoRA matrix of a single-token pass (launch_v6_prologue). CTA b computes rows [8b, 8b + 8) of W1 = w1.W, whose
+// bytes it copies to shared memory before the dependency wait; after it, the LayerNorm and mix[0] of ln_mix_body (into shared
+// memory), mix[0] staged as the streaming GEMV stages a column (TYPE = w1.type), and rows_dot.
+template <int PER, int TYPE>
+__global__ void __launch_bounds__(LN_THREADS) v6_prologue_kernel(const LnMixParams p, const GemvProblem w1) {
+    extern __shared__ __align__(16) uint8_t v6p_smem[];       // [V6_PROLOGUE_ROWS rows of W1][mix[0]: C floats][staged mix[0]]
+    __shared__ double slots[4][LN_WARPS];
+    trace_begin(p.trace);
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    const int row0 = blockIdx.x * V6_PROLOGUE_ROWS, rows = min(V6_PROLOGUE_ROWS, w1.M - row0);
+    const int bytes = rows * (int) w1.pitch;
+    const uint8_t * src = reinterpret_cast<const uint8_t *>(w1.W) + (size_t) row0 * w1.pitch;
+    for (int i = threadIdx.x * 16; i < bytes; i += LN_THREADS * 16)
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((uint32_t) __cvta_generic_to_shared(v6p_smem + i)), "l"(src + i) : "memory");
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    float * mix = reinterpret_cast<float *>(v6p_smem + (size_t) V6_PROLOGUE_ROWS * w1.pitch);
+    uint8_t * act = reinterpret_cast<uint8_t *>(mix) + (((size_t) p.C * sizeof(float) + 15) & ~(size_t) 15);
+    ln_mix_body<PER, 3, false>(p, 0, mix, blockIdx.x == 0, slots);
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncthreads();
+    GemvProblem P = w1;
+    P.x = mix;
+    // the 8-lanes-per-block staging, not the GEMV's one-thread-per-block form: that one holds 16 float4 per thread, more than the 64
+    // registers a 1024-thread CTA leaves (it spilled). Both write the same bytes (stage_column).
+    if (threadIdx.x < tma::CONSUMER_THREADS) tma::stage_column<4, false, TYPE, false>(P, 0, act, nullptr);
+    __syncthreads();
+    tma::rows_dot<TYPE>(P, v6p_smem, rows, row0, act, w1.y + row0);
     trace_end(p.trace);
 }
 
@@ -385,6 +424,46 @@ cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s) {
     if (per <= 16) { RWKV_LN(16) }
 #undef RWKV_LN
     return cudaErrorInvalidValue;   // n_embed > 16384
+}
+
+size_t v6_prologue_smem_bytes(const GemvProblem & w1, int C) {
+    return (size_t) V6_PROLOGUE_ROWS * (size_t) w1.pitch + (((size_t) C * sizeof(float) + 15) & ~(size_t) 15) + tma::act_bytes_per_column(w1.type, w1.K);
+}
+
+template <int PER, int TYPE>
+static cudaError_t launch_v6_prologue_kernel(const LnMixParams & p, const GemvProblem & w1, cudaStream_t s) {
+    static PerDeviceOnce once;
+    const cudaError_t e = once.run([&] { return cudaFuncSetAttribute(v6_prologue_kernel<PER, TYPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, V6_PROLOGUE_MAX_SMEM); });
+    if (e != cudaSuccess) return e;
+    return launch_pdl(v6_prologue_kernel<PER, TYPE>, dim3((w1.M + V6_PROLOGUE_ROWS - 1) / V6_PROLOGUE_ROWS), dim3(LN_THREADS), v6_prologue_smem_bytes(w1, p.C), s, p, w1);
+}
+
+// Only the (PER, type) pairs a one-warp-per-row plan admits are compiled: F32 rows up to n_embed 896 (PER 1), F16 up to 1792 (PER <= 2).
+template <int PER>
+static cudaError_t launch_v6_prologue_per(const LnMixParams & p, const GemvProblem & w1, cudaStream_t s) {
+    switch (w1.type) {
+        case DT_Q4_0: return launch_v6_prologue_kernel<PER, DT_Q4_0>(p, w1, s);
+        case DT_Q4_1: return launch_v6_prologue_kernel<PER, DT_Q4_1>(p, w1, s);
+        case DT_Q5_0: return launch_v6_prologue_kernel<PER, DT_Q5_0>(p, w1, s);
+        case DT_Q5_1: return launch_v6_prologue_kernel<PER, DT_Q5_1>(p, w1, s);
+        case DT_Q8_0: return launch_v6_prologue_kernel<PER, DT_Q8_0>(p, w1, s);
+        case DT_F16: if constexpr (PER <= 2) return launch_v6_prologue_kernel<PER, DT_F16>(p, w1, s); else return cudaErrorInvalidValue;
+        case DT_F32: if constexpr (PER == 1) return launch_v6_prologue_kernel<PER, DT_F32>(p, w1, s); else return cudaErrorInvalidValue;
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+// v6_lora_fold has checked the shape (C <= 4096, a WK == 1 plan, the shared memory); these checks only keep a wrong call from launching.
+cudaError_t launch_v6_prologue(const LnMixParams & p_in, const GemvProblem & w1, cudaStream_t s) {
+    LnMixParams p = p_in;
+    p.trace = trace_slot("v6_prologue");
+    if (p.T != 1 || p.seq_stride || p.n_out != 1 || p.formula != 1 || w1.K != p.C || w1.wk != 1 || v6_prologue_smem_bytes(w1, p.C) > V6_PROLOGUE_MAX_SMEM)
+        return cudaErrorInvalidValue;
+    const int per = (p.C + LN_THREADS - 1) / LN_THREADS;
+    if (per <= 1) return launch_v6_prologue_per<1>(p, w1, s);
+    if (per <= 2) return launch_v6_prologue_per<2>(p, w1, s);
+    if (per <= 4) return launch_v6_prologue_per<4>(p, w1, s);
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_v6_lerp(const V6LerpParams & p_in, cudaStream_t s) {

@@ -38,6 +38,15 @@ struct LnMixParams {
 };
 cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s);
 
+// v6 time-mixing prologue of a single-token pass, ln_mix (one token, n_out == 1) and the first LoRA matrix in one launch:
+// w1.y = tanh(W1 . mix[0]) with w1 = {maa_w1, EPI_TANH} planned by gemv_tma_plan. Every CTA runs the LayerNorm of ln_mix_kernel on
+// all channels, CTA 0 alone writes out_xx / out_sx / state_out, and each CTA computes V6_PROLOGUE_ROWS rows of W1 from a staged
+// copy of mix[0]. p.out[0] is not written. The bits equal launch_ln_mix followed by the GEMV.
+constexpr int V6_PROLOGUE_ROWS = 8;
+constexpr size_t V6_PROLOGUE_MAX_SMEM = 96 * 1024;
+size_t v6_prologue_smem_bytes(const GemvProblem & w1, int C);
+cudaError_t launch_v6_prologue(const LnMixParams & p, const GemvProblem & w1, cudaStream_t s);
+
 // v6 data-dependent lerp (rwkv_graph.inc:323-346): for j in {w,k,v,r,g}
 //   m_j[c,t] = sum_i W2[j][c][i] * z[j*mix + i, t];   out_j = (m_j + maa_j[c]) * sx + xx
 struct V6LerpParams {
@@ -84,8 +93,14 @@ struct Wkv6Params {
     int H, S, T;
     unsigned char * q_out; int q_type;  // T == 1, S % 32 == 0 only: y as a staged column (act_stage.cuh)
     long long seq_stride = 0;         // a multiple of 4: the state moves in float4s
+    // v6 single-token passes with dw2.W set (v6_lora_fold): the decay is computed here, w = exp(-exp(Wd2 . lora1 + time_decay)) with
+    // dw2 = {decay_w2, x = lora1, bias = time_decay, EPI_BIAS_EXPNEGEXP} planned by gemv_tma_plan, instead of read from td.
+    GemvProblem dw2 = {};
 };
 cudaError_t launch_wkv6(const Wkv6Params & p, cudaStream_t s);
+// Dynamic shared memory of a wkv6 launch that computes the decay (head size 64): the head's rows of dw2 and the staged lora1.
+constexpr size_t WKV6_DECAY_MAX_SMEM = 96 * 1024;
+size_t wkv6_decay_smem_bytes(const GemvProblem & dw2);
 
 // v7 (rwkv_att_v7, rwkv_graph.inc:432-479 + rwkv_wkv_v7_impl, rwkv_operators_wkv_v7.inc:37-106):
 // kk/l2norm, k and v corrections, the recurrence, per-head norm, ln_x, the r*k*r_k bonus and the gate.

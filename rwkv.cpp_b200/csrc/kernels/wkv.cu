@@ -4,6 +4,7 @@
 #include "ops.h"
 #include "gemv.h"   // launch_pdl
 #include "act_stage.cuh"
+#include "gemv_tma_device.cuh"   // row_partial / rows_dot, stage_column: the decay LoRA folded into wkv6_kernel
 #include "../formats.h"
 
 #include <cuda_fp16.h>
@@ -106,7 +107,10 @@ __device__ __forceinline__ void wkv_bar_sync(int id, int count) { asm volatile("
 __device__ __forceinline__ void wkv_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // BATCH (seq_stride > 0): the block walks ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
-template <int S, bool BATCH>
+// DW2 >= 0 (v6, one token of one sequence): the decay of the head's S channels is the last LoRA GEMV, p.dw2 with weights of type DW2,
+// computed here: its S rows are copied to shared memory before the dependency wait, lora1 is staged after it as the streaming GEMV
+// stages a column, and rows_dot writes exp(-exp(..)) straight into the decay row the recurrence reads.
+template <int S, bool BATCH, int DW2 = -1>
 __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Params p) {
     using LY = Wkv6Layout<S>;
     constexpr int TB = WKV6_TB, NOCT = LY::NOCT, NT = LY::NT, WORK = LY::WORK, BLOCK = LY::BLOCK, NNW = LY::NORM_WARPS, CPL = (S + 31) / 32;
@@ -135,9 +139,16 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
             st[ii][0] = v.x; st[ii][1] = v.y; st[ii][2] = v.z; st[ii][3] = v.w;
         }
     }
+    extern __shared__ __align__(16) uint8_t wkv_dw2_smem[];      // DW2 >= 0: [S rows of dw2][staged lora1]
+    if constexpr (DW2 >= 0) {
+        const int bytes = S * (int) p.dw2.pitch;
+        const uint8_t * src = reinterpret_cast<const uint8_t *>(p.dw2.W) + (size_t) h * bytes;
+        for (int i = tid * 16; i < bytes; i += BLOCK * 16) wkv_cp16(wkv_dw2_smem + i, src + i);
+        wkv_cp_commit();
+    }
     for (int i = tid; i < S; i += BLOCK) {
         sf[i] = p.per_head_scalars ? p.tf[h] : p.tf[h * S + i];
-        sdc[i] = p.td_per_token ? 0.f : (p.per_head_scalars ? p.td[h] : p.td[h * S + i]);
+        if constexpr (DW2 < 0) sdc[i] = p.td_per_token ? 0.f : (p.per_head_scalars ? p.td[h] : p.td[h * S + i]);
     }
     float lw[CPL], lb[CPL];
 #pragma unroll
@@ -147,6 +158,24 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         lb[i] = (is_norm && col < S) ? p.lnx_b[h * S + col] : 0.f;
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    if constexpr (DW2 >= 0) {
+        // the token's k / r / v rows (chunk 0, which the workers' stage(0) copies on the other paths) are requested first: their L2
+        // round trip overlaps the one of lora1 and the decay rows instead of following it
+        for (int f = tid * 4; f < S && tid < WORK; f += WORK * 4) {
+            const size_t o = (size_t) h * S + f;
+            wkv_cp16(&buf[0].k[0][f], p.k + o);
+            wkv_cp16(&buf[0].r[0][f], p.r + o);
+            wkv_cp16(&buf[0].v[0][f], p.v + o);
+        }
+        wkv_cp_commit();
+        uint8_t * act = wkv_dw2_smem + (size_t) S * p.dw2.pitch;
+        // stage_column's F16 / F32 loops take element k on thread k (stride 256): with 192 threads that needs dw2.K <= 192
+        // (v6_lora_fold_shapes: K <= 128); quantised columns use one thread per 32-element block
+        if (tid < tma::CONSUMER_THREADS) tma::stage_column<4, true, DW2, false>(p.dw2, 0, act, nullptr);
+        wkv_cp_wait<0>();
+        __syncthreads();
+        tma::rows_dot<DW2>(p.dw2, wkv_dw2_smem, S, h * S, act, sdc);
+    }
     __syncthreads();                                   // sf / sdc
 
     if (!is_norm) {
@@ -173,7 +202,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         float tfr[8];     // time_first of my key rows
 #pragma unroll
         for (int ii = 0; ii < 8; ii++) tfr[ii] = sf[i0 + ii];
-        stage(0);
+        if constexpr (DW2 < 0) stage(0);               // DW2 >= 0: already on its way
         wkv_cp_commit();
         for (int c = 0; c < nchunks; c++) {
             wkv_cp_wait<0>();
@@ -385,9 +414,35 @@ cudaError_t launch_wkv6_kernel(const Wkv6Params & p, cudaStream_t s) {
                          : launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
 }
 
+template <int DW2>
+cudaError_t launch_wkv6_decay(const Wkv6Params & p, cudaStream_t s) {
+    static PerDeviceOnce once;
+    const size_t smem = wkv6_decay_smem_bytes(p.dw2);
+    const cudaError_t e = once.run([&] { return cudaFuncSetAttribute(wkv6_kernel<64, false, DW2>, cudaFuncAttributeMaxDynamicSharedMemorySize, WKV6_DECAY_MAX_SMEM); });
+    if (e != cudaSuccess) return e;
+    return launch_pdl(wkv6_kernel<64, false, DW2>, dim3(p.H), dim3(Wkv6Layout<64>::BLOCK), smem, s, p);
+}
+
+size_t wkv6_decay_smem_bytes(const GemvProblem & dw2) {
+    return (size_t) 64 * (size_t) dw2.pitch + tma::act_bytes_per_column(dw2.type, dw2.K);
+}
+
 cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
     Wkv6Params p = p_in;
     p.trace = trace_slot("wkv6");
+    if (p.dw2.W) {      // v6_lora_fold has checked the shape: S == 64, one token of one sequence, a WK == 1 plan
+        if (p.S != 64 || p.T != 1 || p.seq_stride || wkv6_decay_smem_bytes(p.dw2) > WKV6_DECAY_MAX_SMEM) return cudaErrorInvalidValue;
+        switch (p.dw2.type) {
+            case DT_Q4_0: return launch_wkv6_decay<DT_Q4_0>(p, s);
+            case DT_Q4_1: return launch_wkv6_decay<DT_Q4_1>(p, s);
+            case DT_Q5_0: return launch_wkv6_decay<DT_Q5_0>(p, s);
+            case DT_Q5_1: return launch_wkv6_decay<DT_Q5_1>(p, s);
+            case DT_Q8_0: return launch_wkv6_decay<DT_Q8_0>(p, s);
+            case DT_F16: return launch_wkv6_decay<DT_F16>(p, s);
+            case DT_F32: return launch_wkv6_decay<DT_F32>(p, s);
+            default: return cudaErrorInvalidValue;
+        }
+    }
     switch (p.S) {
         case 8: return launch_wkv6_kernel<8>(p, s);
         case 16: return launch_wkv6_kernel<16>(p, s);

@@ -80,6 +80,8 @@ class RWKVSharedLibrary:
         # additive API
         lib.rwkv_b200_inspect_file.argtypes = [ctypes.c_char_p, ctypes.POINTER(FileInfo)]
         lib.rwkv_b200_inspect_file.restype = ctypes.c_bool
+        lib.rwkv_b200_v6_lora_fold_supported.argtypes = [ctypes.c_int] * 6
+        lib.rwkv_b200_v6_lora_fold_supported.restype = ctypes.c_bool
         lib.rwkv_b200_init_from_file_ex.argtypes = [ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
         lib.rwkv_b200_init_from_file_ex.restype = vp
         lib.rwkv_b200_state_load.argtypes = [vp, P_FLOAT]
