@@ -47,13 +47,25 @@ RWKV_API bool rwkv_b200_synchronize(struct rwkv_context * ctx);
  *   rwkv_b200_batch_create    : from any context of the model (shares its weights); free with rwkv_free; NULL on failure
  *   rwkv_b200_batch_set_state : state of one sequence <- state_in (host or device pointer, NULL = fresh state)
  *   rwkv_b200_batch_eval      : tokens[n_sequences], one per sequence; want_logits = run the head for every sequence
+ *   rwkv_b200_batch_eval_ragged : continuous batching -- sequence b advances counts[b] tokens (a prompt, one decode token, or none)
+ *                                 in the same single pass over the weights
  *   rwkv_b200_batch_get_logits / rwkv_b200_batch_get_state : copy one sequence's logits / state out (host or device pointer)
  * The next token of every sequence is drawn on the device by rwkv_b200_batch_sample / rwkv_b200_batch_eval_sample (below).
- * rwkv_eval*, rwkv_b200_sample and the resident / stage entry points refuse a batch context. */
+ * A batch context's logits start as zeros. rwkv_eval*, rwkv_b200_sample and the resident / stage entry points refuse a batch context. */
 RWKV_API struct rwkv_context * rwkv_b200_batch_create(struct rwkv_context * ctx, size_t n_sequences);
 RWKV_API bool rwkv_b200_batch_set_state(struct rwkv_context * batch, size_t sequence, const float * state_in);
 RWKV_API bool rwkv_b200_batch_get_state(struct rwkv_context * batch, size_t sequence, float * state_out);
 RWKV_API bool rwkv_b200_batch_eval(struct rwkv_context * batch, const uint32_t * tokens, bool want_logits);
+/* Ragged pass of a batch context: sequence b advances counts[b] tokens (0 = the sequence is left exactly as it is), all in one pass
+ * over the weights. tokens holds the sequences' tokens back to back in sequence order (sum of counts entries);
+ * 1 <= sum of counts <= 256. want_logits: the logits column of every sequence with counts[b] > 0 receives the logits of its last
+ * token; the other columns keep what they held. Longer prompts are fed over several calls; the states stay resident in between.
+ * Every argument is checked before anything is enqueued, so a rejected call changes no state and no logits column: a context that is
+ * not a batch context gives RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED; NULL arrays, a sum of 0 or above 256 and a token >= n_vocab give
+ * RWKV_ERROR_ARGS. Per sequence the result is bit-identical to feeding its tokens to a single-sequence context one at a time while the
+ * sum stays below 16, and with rwkv_b200_set_tensor_cores(batch, false) at any sum. rwkv_b200_batch_sample / get_logits / get_state
+ * work after it unchanged; an idle sequence's row draws from the column it still holds. */
+RWKV_API bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits);
 RWKV_API bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out);
 RWKV_API size_t rwkv_b200_batch_size(const struct rwkv_context * ctx);   /* 0 for an ordinary context */
 
@@ -276,6 +288,15 @@ struct rwkv_b200_wkv7_args {
     long long seq_stride;
 };
 RWKV_API bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a);
+
+/* The same four kernels in ragged mode (the mode of rwkv_b200_batch_eval_ragged): sequence s advances counts[s] tokens, its columns
+ * back to back in sequence order, on its state seq_stride floats after sequence s - 1's. The struct's T is the sum of the counts (the
+ * activations' columns), its n_seq equals n_seq (1 .. 256), its seq_stride is at least one sequence's state; no staged columns.
+ * A sequence with no tokens is not touched: its state_out slice keeps the 0xFF fill. */
+RWKV_API bool rwkv_b200_test_ln_mix_ragged(const struct rwkv_b200_ln_mix_args * a, const uint32_t * counts, size_t n_seq);
+RWKV_API bool rwkv_b200_test_wkv4_ragged(const struct rwkv_b200_wkv4_args * a, const uint32_t * counts, size_t n_seq);
+RWKV_API bool rwkv_b200_test_wkv6_ragged(const struct rwkv_b200_wkv6_args * a, const uint32_t * counts, size_t n_seq);
+RWKV_API bool rwkv_b200_test_wkv7_ragged(const struct rwkv_b200_wkv7_args * a, const uint32_t * counts, size_t n_seq);
 
 /* A batch of up to 8 matrix problems y_i[M_i, T] = epi_i(W_i . pro_i(x[input_i])) launched the way the eval path launches them
  * (csrc/kernels/gemv.h). Weights go up through the model loader's code (row pitch, zeroed row padding, device layout, and the

@@ -101,6 +101,25 @@ bool staged_ok(const unsigned char * q_out, int q_type, int T, int n_seq, int un
     return !q_out || (T == 1 && n_seq == 0 && unit % 32 == 0 && act::stage_class(q_type) != act::SC_NONE);
 }
 
+// Ragged hooks: counts[n_seq] with 1 <= n_seq <= MAX_TOKENS_PER_PASS, the struct's n_seq equal to n_seq, its T the sum of the counts
+// (the activations' columns), its seq_stride at least one sequence's state.
+bool ragged_ok(const uint32_t * counts, size_t n_seq, int a_n_seq, int T, long long seq_stride, size_t per_seq) {
+    if (!counts || n_seq < 1 || n_seq > (size_t) MAX_TOKENS_PER_PASS || a_n_seq != (int) n_seq || T < 1 || seq_stride < (long long) per_seq) return false;
+    size_t sum = 0;
+    for (size_t s = 0; s < n_seq; s++) sum += counts[s];
+    return sum == (size_t) T;
+}
+// The device map of a ragged launch: column offsets [n_seq + 1] and the sequence of every column.
+struct RaggedMap {
+    std::vector<int> off, col_seq;
+    RaggedMap(const uint32_t * counts, size_t n_seq) : off(n_seq + 1, 0) {
+        for (size_t s = 0; s < n_seq; s++) {
+            off[s + 1] = off[s] + (int) counts[s];
+            col_seq.insert(col_seq.end(), counts[s], (int) s);
+        }
+    }
+};
+
 }  // namespace
 
 extern "C" {
@@ -355,6 +374,11 @@ bool rwkv_b200_batch_eval(struct rwkv_context * batch, const uint32_t * tokens, 
     for (int i = 0; i < c->batch_n; i++)
         RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) c->model->n_vocab, "Token of sequence %d (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], c->model->n_vocab - 1);
     return batch_eval(c, tokens, want_logits);
+}
+bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    return batch_eval_ragged(c, tokens, counts, want_logits);
 }
 bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
@@ -846,6 +870,103 @@ bool rwkv_b200_test_wkv7(const struct rwkv_b200_wkv7_args * a) {
     p.q_out = a->q_out ? b.out(a->q_out, act::bytes_per_column(a->q_type, (int) C)) : nullptr; p.q_type = a->q_type;
     const cudaError_t e = b.ok ? launch_wkv7(p, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_ln_mix_ragged(const struct rwkv_b200_ln_mix_args * a, const uint32_t * counts, size_t n_seq) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    bool args = a && a->x && a->ln_w && a->ln_b && a->state_in && a->state_out && a->C > 0 && (a->formula == 0 || a->formula == 1) &&
+                a->n_out >= 1 && a->n_out <= 6 && ragged_ok(counts, n_seq, a->n_seq, a->T, a->seq_stride, (size_t) a->C);
+    for (int j = 0; args && j < a->n_out; j++) args = a->coef[j] && a->out[j];
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid ragged ln_mix arguments");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C, cols = (size_t) a->T, st = seq_floats((int) n_seq, a->seq_stride, C);
+    const RaggedMap map(counts, n_seq);
+    HookBuffers b;
+    LnMixParams p{};
+    p.x = b.in(a->x, C * cols); p.ln_w = b.in(a->ln_w, C); p.ln_b = b.in(a->ln_b, C);
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.C = a->C; p.T = a->T; p.formula = a->formula; p.n_out = a->n_out; p.seq_stride = a->seq_stride;
+    p.seq_off = b.in(map.off.data(), map.off.size()); p.col_seq = b.in(map.col_seq.data(), map.col_seq.size());
+    for (int j = 0; j < a->n_out; j++) { p.coef[j] = b.in(a->coef[j], C); p.out[j] = b.out(a->out[j], C * cols); }
+    p.out_xx = b.out(a->out_xx, C * cols); p.out_sx = b.out(a->out_sx, C * cols);
+    const cudaError_t e = b.ok ? launch_ln_mix(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ragged ln_mix failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv4_ragged(const struct rwkv_b200_wkv4_args * a, const uint32_t * counts, size_t n_seq) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const bool args = a && a->k && a->v && a->r && a->time_first && a->time_decay && a->aa_in && a->bb_in && a->pp_in && a->aa_out && a->bb_out && a->pp_out && a->y &&
+                      a->C > 0 && !a->q_out && ragged_ok(counts, n_seq, a->n_seq, a->T, a->seq_stride, (size_t) a->C);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid ragged wkv4 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t C = (size_t) a->C, cols = (size_t) a->T, st = seq_floats((int) n_seq, a->seq_stride, C);
+    const RaggedMap map(counts, n_seq);
+    HookBuffers b;
+    Wkv4Params p{};
+    p.k = b.in(a->k, C * cols); p.v = b.in(a->v, C * cols); p.r = b.in(a->r, C * cols);
+    p.time_first = b.in(a->time_first, C); p.time_decay = b.in(a->time_decay, C);
+    p.aa_in = b.in(a->aa_in, st); p.bb_in = b.in(a->bb_in, st); p.pp_in = b.in(a->pp_in, st);
+    p.aa_out = b.out(a->aa_out, st); p.bb_out = b.out(a->bb_out, st); p.pp_out = b.out(a->pp_out, st);
+    p.y = b.out(a->y, C * cols);
+    p.C = a->C; p.T = a->T; p.seq_stride = a->seq_stride; p.q_out = nullptr; p.q_type = 0;
+    p.seq_off = b.in(map.off.data(), map.off.size()); p.n_seq = (int) n_seq;
+    const cudaError_t e = b.ok ? launch_wkv4(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ragged wkv4 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv6_ragged(const struct rwkv_b200_wkv6_args * a, const uint32_t * counts, size_t n_seq) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const size_t C = a ? (size_t) a->H * (size_t) a->S : 0, SS = a ? C * (size_t) a->S : 0;
+    const bool args = a && a->r && a->k && a->v && a->td && a->tf && a->state_in && a->state_out && a->lnx_w && a->lnx_b && a->y && a->H > 0 && a->S > 0 &&
+                      !(a->td_per_token && a->per_head_scalars) && !a->q_out && a->seq_stride % 4 == 0 &&
+                      ragged_ok(counts, n_seq, a->n_seq, a->T, a->seq_stride, SS);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid ragged wkv6 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t cols = (size_t) a->T, st = seq_floats((int) n_seq, a->seq_stride, SS);
+    const RaggedMap map(counts, n_seq);
+    HookBuffers b;
+    Wkv6Params p{};
+    p.r = b.in(a->r, C * cols); p.k = b.in(a->k, C * cols); p.v = b.in(a->v, C * cols);
+    p.td = b.in(a->td, a->td_per_token ? C * cols : a->per_head_scalars ? (size_t) a->H : C);
+    p.tf = b.in(a->tf, a->per_head_scalars ? (size_t) a->H : C);
+    p.td_per_token = a->td_per_token; p.per_head_scalars = a->per_head_scalars;
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C); p.g = b.in(a->g, C * cols);
+    p.y = b.out(a->y, C * cols);
+    p.eps = a->eps; p.H = a->H; p.S = a->S; p.T = a->T; p.seq_stride = a->seq_stride; p.q_out = nullptr; p.q_type = 0;
+    p.seq_off = b.in(map.off.data(), map.off.size()); p.n_seq = (int) n_seq;
+    const cudaError_t e = b.ok ? launch_wkv6(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ragged wkv6 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_wkv7_ragged(const struct rwkv_b200_wkv7_args * a, const uint32_t * counts, size_t n_seq) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const size_t C = a ? (size_t) a->H * (size_t) a->S : 0, SS = a ? C * (size_t) a->S : 0;
+    const bool args = a && a->r && a->w && a->k && a->v && a->a && a->g && (!a->vgate || a->v_first) && a->k_k && a->k_a && a->r_k && a->lnx_w && a->lnx_b &&
+                      a->state_in && a->state_out && a->y && a->H > 0 && a->S > 0 && !a->q_out && ragged_ok(counts, n_seq, a->n_seq, a->T, a->seq_stride, SS);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid ragged wkv7 arguments");
+    if (!hook_device(sink)) return false;
+    const size_t cols = (size_t) a->T, st = seq_floats((int) n_seq, a->seq_stride, SS), n = C * cols;
+    const RaggedMap map(counts, n_seq);
+    HookBuffers b;
+    Wkv7Params p{};
+    p.r = b.in(a->r, n); p.w = b.in(a->w, n); p.k = b.in(a->k, n); p.v = b.in(a->v, n); p.a = b.in(a->a, n); p.g = b.in(a->g, n);
+    p.vgate = b.in(a->vgate, n); p.v_first = a->vgate ? b.in(a->v_first, n) : nullptr; p.v_out = b.out(a->v_out, n);
+    p.k_k = b.in(a->k_k, C); p.k_a = b.in(a->k_a, C); p.r_k = b.in(a->r_k, C); p.lnx_w = b.in(a->lnx_w, C); p.lnx_b = b.in(a->lnx_b, C);
+    p.state_in = b.in(a->state_in, st); p.state_out = b.out(a->state_out, st);
+    p.y = b.out(a->y, n);
+    p.H = a->H; p.S = a->S; p.T = a->T; p.seq_stride = a->seq_stride; p.q_out = nullptr; p.q_type = 0;
+    p.seq_off = b.in(map.off.data(), map.off.size()); p.n_seq = (int) n_seq;
+    const cudaError_t e = b.ok ? launch_wkv7(p, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "ragged wkv7 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

@@ -5,6 +5,7 @@
 #include "engine.h"
 
 #include <algorithm>
+#include <cinttypes>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -177,6 +178,7 @@ LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
     LnMixParams lp{};
     lp.x = s.x; lp.ln_w = L.ln2_w.data; lp.ln_b = L.ln2_b.data;
     lp.state_in = st_in; lp.state_out = st_out; lp.C = m.n_embed; lp.T = T; lp.seq_stride = ctx->batch_stride;
+    lp.seq_off = ctx->pass_seq_off; lp.col_seq = ctx->pass_col_seq;
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.ffn_x_k.data; lp.out[0] = s.mix[0];
     } else if (m.arch_major == 6) {
@@ -228,6 +230,7 @@ LnMixParams att_ln(const Context * ctx, const Layer & L, const Scratch & s, int 
     LnMixParams lp{};
     lp.x = s.x; lp.ln_w = L.ln1_w.data; lp.ln_b = L.ln1_b.data;
     lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = T; lp.seq_stride = ctx->batch_stride;
+    lp.seq_off = ctx->pass_seq_off; lp.col_seq = ctx->pass_col_seq;
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 6;
         for (int j = 0; j < 6; j++) { lp.coef[j] = L.att_x_rwkvag.data + (size_t) j * C; lp.out[j] = s.mix[j]; }   // r w k v a g
@@ -258,7 +261,7 @@ bool att_v4(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     wp.time_first = L.att_time_first.data; wp.time_decay = L.att_time_decay.data;
     wp.aa_in = st_in + 2 * C; wp.bb_in = st_in + 3 * C; wp.pp_in = st_in + 4 * C;
     wp.aa_out = st_out + 2 * C; wp.bb_out = st_out + 3 * C; wp.pp_out = st_out + 4 * C;
-    wp.y = s.y; wp.C = C; wp.T = T; wp.seq_stride = ctx->batch_stride;
+    wp.y = s.y; wp.C = C; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (C % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
     CUDA_OK(ctx, launch_wkv4(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
@@ -283,7 +286,7 @@ bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.g = v52 ? s.g : nullptr;
-    wp.y = s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
+    wp.y = s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
     CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
@@ -384,7 +387,7 @@ bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const floa
     if (fold) wp.dw2 = dw2;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
-    wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
+    wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
     CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
@@ -421,7 +424,7 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Scratch & s, int T,
     wp.k_k = L.att_k_k.data; wp.k_a = L.att_k_a.data; wp.r_k = L.att_r_k.data;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
-    wp.y = s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride;
+    wp.y = s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
     CUDA_OK(ctx, launch_wkv7(wp, ctx->stream));
     return att_output(ctx, L, s, T, wp.q_out);
@@ -492,7 +495,16 @@ bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
         }
         if (!ok || !ffn(ctx, L, s, T, flp)) return false;
     }
-    if (want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
+    if (want_logits && l1 == m.n_layer && ctx->pass_seq_off) {
+        // ragged: the head on the last column of every advancing sequence, gathered; its columns go to those sequences' logits
+        const int n = ctx->pass_n_active;
+        CUDA_OK(ctx, launch_copy_columns(s.x, ctx->pass_head_col, ctx->head_x, nullptr, C, n, ctx->stream));
+        Batch b(n);
+        GemvProblem & p = b.add(m.head, ctx->head_x, ctx->head_y);
+        p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
+        if (!run_batch(ctx, b)) return false;
+        CUDA_OK(ctx, launch_copy_columns(ctx->head_y, nullptr, ctx->logits, ctx->pass_head_seq, m.n_vocab, n, ctx->stream));
+    } else if (want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
         Batch b(ctx->batch_n ? T : 1);
         GemvProblem & p = b.add(m.head, ctx->batch_n ? s.x : s.x + (size_t) (T - 1) * C, ctx->logits);
         p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
@@ -628,6 +640,8 @@ Context * create_context(Model * model, ErrorSink sink, int batch_n) {
         ctx->xq_slot_bytes = ((size_t) 2 * model->n_embed + 64 + 255) / 256 * 256;
         ok = cudaMalloc(reinterpret_cast<void **>(&ctx->xq), (size_t) XQ_SLOTS * ctx->xq_slot_bytes) == cudaSuccess;
     }
+    // a batch context's logits start as zeros: after ragged passes a column that was never computed is a uniform draw, not garbage
+    if (ok && batch_n > 0) ok = cudaMemset(ctx->logits, 0, seqs * (size_t) model->n_vocab * sizeof(float)) == cudaSuccess;
     if (ok) {
         std::vector<float> init(n);
         fill_init_state(*model, init.data());
@@ -661,8 +675,10 @@ void destroy_context(Context * ctx) {
     cudaFree(ctx->tokens); cudaFree(ctx->scratch); cudaFree(ctx->trace_buf); cudaFree(ctx->act16); cudaFree(ctx->xq);
     for (int i = 0; i < 2; i++) {
         if (ctx->tokens_host[i]) cudaFreeHost(ctx->tokens_host[i]);
+        if (ctx->ragged_host[i]) cudaFreeHost(ctx->ragged_host[i]);
         if (ctx->slot_free[i]) cudaEventDestroy(ctx->slot_free[i]);
     }
+    cudaFree(ctx->ragged_map); cudaFree(ctx->head_x); cudaFree(ctx->head_y);
     for (auto & g : ctx->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (ctx->copy_pool) destroy_copy_pool(ctx->copy_pool);
     if (ctx->bounce_in) { cudaFreeHost(ctx->bounce_in); cudaFreeHost(ctx->bounce_out); cudaFreeHost(ctx->bounce_logits); }
@@ -975,6 +991,63 @@ bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits) {
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->batch_n > 0 && tokens, "Not a batch context or NULL tokens");
     CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
     return forward_pass(ctx, tokens, ctx->batch_n, want_logits);
+}
+
+// Ints of one ragged map (Context::ragged_host): offsets [B + 1], column sequences [MAX_TOKENS_PER_PASS], head columns and sequences [B each].
+static size_t ragged_map_ints(int B) { return (size_t) 3 * B + 1 + MAX_TOKENS_PER_PASS; }
+
+bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ctx->batch_n > 0, "Not a batch context");
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, tokens && counts, "NULL tokens or counts");
+    const Model & m = *ctx->model;
+    const int B = ctx->batch_n;
+    size_t total = 0;
+    for (int b = 0; b < B; b++) total += counts[b];
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, total >= 1 && total <= (size_t) MAX_TOKENS_PER_PASS, "A ragged pass takes 1 .. %d tokens in all, not %zu", MAX_TOKENS_PER_PASS, total);
+    for (size_t i = 0; i < total; i++)
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) m.n_vocab, "Token at index %zu (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], m.n_vocab - 1);
+    CUDA_OK(ctx, cudaSetDevice(m.dev.device));
+    const size_t map_bytes = ragged_map_ints(B) * sizeof(int);
+    if (!ctx->ragged_map) {
+        for (int i = 0; i < 2; i++) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->ragged_host[i]), map_bytes));
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->head_x), (size_t) B * m.n_embed * sizeof(float)));
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->head_y), (size_t) B * m.n_vocab * sizeof(float)));
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->ragged_map), map_bytes));
+    }
+    const int T = (int) total;
+    if (!begin_pass(ctx, tokens, T)) return false;      // waits until the pass that last used this phase's slots has read them
+    const int phase = ctx->phase;
+    int * off = ctx->ragged_host[phase], * col_seq = off + B + 1, * head_col = col_seq + MAX_TOKENS_PER_PASS, * head_seq = head_col + B;
+    int n_active = 0;
+    off[0] = 0;
+    for (int b = 0; b < B; b++) {
+        off[b + 1] = off[b] + (int) counts[b];
+        for (int t = off[b]; t < off[b + 1]; t++) col_seq[t] = b;
+        if (counts[b]) { head_col[n_active] = off[b + 1] - 1; head_seq[n_active] = b; n_active++; }
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->ragged_map, off, map_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    // the state of every idle sequence (runs of them are contiguous) goes to state_b as it is: end_pass swaps the whole buffers
+    const size_t n = m.state_len();
+    for (int b = 0; b < B;) {
+        if (counts[b]) { b++; continue; }
+        int e = b;
+        while (e < B && !counts[e]) e++;
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_b + (size_t) b * n, ctx->state_a + (size_t) b * n, (size_t) (e - b) * n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+        b = e;
+    }
+    ctx->pass_seq_off = ctx->ragged_map;
+    ctx->pass_col_seq = ctx->ragged_map + B + 1;
+    ctx->pass_head_col = ctx->pass_col_seq + MAX_TOKENS_PER_PASS;
+    ctx->pass_head_seq = ctx->pass_head_col + B;
+    ctx->pass_n_active = n_active;
+    const bool ok = enqueue_pass(ctx, T, want_logits, phase, 0);     // never a graph: the map changes from call to call
+    ctx->pass_seq_off = ctx->pass_col_seq = ctx->pass_head_col = ctx->pass_head_seq = nullptr;
+    ctx->pass_n_active = 0;
+    if (!ok) return false;
+    const bool had_logits = ctx->logits_valid;
+    if (!end_pass(ctx, T, want_logits)) return false;
+    ctx->logits_valid = had_logits || want_logits;     // idle columns keep what they held
+    return true;
 }
 
 bool batch_get_logits(Context * ctx, int seq, float * logits_out) {

@@ -95,6 +95,16 @@ struct Context {
     // every pass evaluates exactly one token of each sequence.
     int batch_n = 0;
     long long batch_stride = 0;
+    // Ragged passes of a batch context (batch_eval_ragged), allocated on the first one. The host writes each pass's map into a pinned
+    // slot that follows the tokens_host / slot_free rule: column offsets [batch_n + 1], the sequence of every column
+    // [MAX_TOKENS_PER_PASS], then the last column and the index of every advancing sequence [batch_n each]; ragged_map is its device
+    // copy. The head runs on the gathered last columns (head_x [C, batch_n]) into head_y [n_vocab, batch_n].
+    int * ragged_host[2] = {nullptr, nullptr};
+    int * ragged_map = nullptr;
+    float * head_x = nullptr, * head_y = nullptr;
+    // while a ragged pass is being enqueued: its device map, and how many sequences advance (the head's columns)
+    const int * pass_seq_off = nullptr, * pass_col_seq = nullptr, * pass_head_col = nullptr, * pass_head_seq = nullptr;
+    int pass_n_active = 0;
 
     // On-device sampling (kernels/sampling.cu): result word, scratch for biased logits, device copy of the caller's logit bias.
     bool logits_valid = false;       // ctx->logits holds the head output of the most recent pass
@@ -156,6 +166,10 @@ bool batch_set_state(Context * ctx, int seq, const float * state_in);
 bool batch_get_state(Context * ctx, int seq, float * state_out);
 bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits);
 bool batch_get_logits(Context * ctx, int seq, float * logits_out);
+// Ragged pass: sequence b advances counts[b] tokens (tokens back to back in sequence order; 0 leaves it exactly as it was), all in one
+// pass over the weights. Checks every argument before it enqueues anything. want_logits: the logits column of every sequence with
+// counts[b] > 0 receives the logits of its last token, the other columns keep what they held. Never replays a CUDA graph.
+bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits);
 
 // Samples the next token from ctx->logits on the device (reference python/sampling.py:10-52 with the caller's uniform number u in
 // [0, 1) in place of numpy's RandomState draw); only the token id is copied back. Requires a preceding pass that computed logits.

@@ -81,13 +81,26 @@ __device__ __forceinline__ double block_sum_ln(double v, double * slots) {
 // cost of a run-once kernel). Statistics as ggml_compute_forward_norm_f32 (ggml-cpu.c:6906-6925, sums in double).
 // PRE_N: how many of the mix-coefficient vectors are requested before the dependency wait (3 for blocks with up to three mixed
 // vectors -- every v6 block --, 6 for v4 / v5.2 / v7 time mixing: a few spilled registers there against one HBM round trip per vector).
-// BATCH (seq_stride > 0): block t is the one token of sequence t. Its previous LN(x) is always that sequence's carry, never
+// MODE SEQ_BATCH: block t is the one token of sequence t. Its previous LN(x) is always that sequence's carry, never
 // column t - 1, and it always writes the sequence's new carry.
+// MODE SEQ_RAGGED: block t is a column of sequence s = col_seq[t]. Its previous LN(x) is the sequence's carry on the sequence's first
+// column and LN(x[:, t-1]) on the others; the sequence's last column writes its new carry.
 // The body is shared with v6_prologue_kernel: token t of the launch; out0, if not NULL, takes the place of p.out[0] (t == 0);
 // write_carry = false skips out_sx, out_xx and state_out.
-template <int PER, int PRE_N, bool BATCH>
+template <int PER, int PRE_N, int MODE>
 __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float * out0, bool write_carry, double (&slots)[4][LN_WARPS]) {
+    constexpr bool BATCH = MODE == SEQ_BATCH, RAGGED = MODE == SEQ_RAGGED;
     const int C = p.C, tid = threadIdx.x;
+    // ragged: the sequence's first and last column and its state's offset. The column map is written by the host: safe before the
+    // dependency wait. (The other modes keep their expressions below as they were: they are what their code was compiled from.)
+    int r_first = 0, r_last = 0;
+    long long r_so = 0;
+    if constexpr (RAGGED) {
+        const int s = p.col_seq[t];
+        r_first = p.seq_off[s];
+        r_last = p.seq_off[s + 1] - 1;
+        r_so = s * p.seq_stride;
+    }
     // LayerNorm weights and the carry are loaded before the wait where registers allow it (PER <= 8); at PER = 16 holding them
     // across the statistics spills past the stack budget, so they are read where they are used
     constexpr bool EARLY = PER <= 8;
@@ -99,7 +112,7 @@ __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float 
             const bool live = c < C;
             lw[i] = live ? p.ln_w[c] : 0.f;
             lb[i] = live ? p.ln_b[c] : 0.f;
-            pv[i] = (live && (BATCH || t == 0)) ? p.state_in[BATCH ? t * p.seq_stride + c : c] : 0.f;   // written by the previous token's pass: safe before the wait
+            pv[i] = (live && (BATCH || (RAGGED ? t == r_first : t == 0))) ? p.state_in[BATCH ? t * p.seq_stride + c : RAGGED ? r_so + c : c] : 0.f;   // written by the previous token's pass: safe before the wait
         }
     };
     if constexpr (EARLY) load_ln();
@@ -125,12 +138,12 @@ __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float 
         const int c = tid + i * LN_THREADS;
         const bool live = c < C;
         xa[i] = live ? p.x[(size_t) t * C + c] : 0.f;
-        xb[i] = (live && !BATCH && t > 0) ? p.x[(size_t) (t - 1) * C + c] : 0.f;
+        xb[i] = (live && !BATCH && (RAGGED ? t > r_first : t > 0)) ? p.x[(size_t) (t - 1) * C + c] : 0.f;
         sa += (double) xa[i];
         sb += (double) xb[i];
     }
     const float mean_a = (float) (block_sum_ln(sa, slots[0]) / C);
-    const float mean_b = (!BATCH && t > 0) ? (float) (block_sum_ln(sb, slots[1]) / C) : 0.f;
+    const float mean_b = (!BATCH && (RAGGED ? t > r_first : t > 0)) ? (float) (block_sum_ln(sb, slots[1]) / C) : 0.f;
     double va = 0, vb = 0;
 #pragma unroll
     for (int i = 0; i < PER; i++) {
@@ -141,13 +154,13 @@ __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float 
         vb += (double) (xb[i] * xb[i]);
     }
     const float scale_a = 1.0f / sqrtf((float) (block_sum_ln(va, slots[2]) / C) + 1e-5f);
-    const float scale_b = (!BATCH && t > 0) ? 1.0f / sqrtf((float) (block_sum_ln(vb, slots[3]) / C) + 1e-5f) : 0.f;
+    const float scale_b = (!BATCH && (RAGGED ? t > r_first : t > 0)) ? 1.0f / sqrtf((float) (block_sum_ln(vb, slots[3]) / C) + 1e-5f) : 0.f;
     if constexpr (!EARLY) load_ln();
     // normalised current / previous token, in place
 #pragma unroll
     for (int i = 0; i < PER; i++) {
         xa[i] = __fadd_rn(__fmul_rn(__fmul_rn(xa[i], scale_a), lw[i]), lb[i]);                            // LN(x[:, t])
-        xb[i] = (!BATCH && t > 0) ? __fadd_rn(__fmul_rn(__fmul_rn(xb[i], scale_b), lw[i]), lb[i]) : pv[i];   // LN(x[:, t-1]) or the carry
+        xb[i] = (!BATCH && (RAGGED ? t > r_first : t > 0)) ? __fadd_rn(__fmul_rn(__fmul_rn(xb[i], scale_b), lw[i]), lb[i]) : pv[i];   // LN(x[:, t-1]) or the carry
     }
     const size_t o0 = (size_t) t * C + tid;
     if constexpr (PRE) {
@@ -189,16 +202,16 @@ __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float 
         if (c >= C) continue;
         if (p.out_sx) p.out_sx[o0 + i * LN_THREADS] = __fsub_rn(xb[i], xa[i]);
         if (p.out_xx) p.out_xx[o0 + i * LN_THREADS] = xa[i];
-        if (BATCH || t == p.T - 1) p.state_out[BATCH ? t * p.seq_stride + c : c] = xa[i];
+        if (BATCH || (RAGGED ? t == r_last : t == p.T - 1)) p.state_out[BATCH ? t * p.seq_stride + c : RAGGED ? r_so + c : c] = xa[i];
     }
 }
 
-template <int PER, int PRE_N, bool BATCH>
+template <int PER, int PRE_N, int MODE>
 __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p) {
     __shared__ double slots[4][LN_WARPS];
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    ln_mix_body<PER, PRE_N, BATCH>(p, blockIdx.x, nullptr, true, slots);
+    ln_mix_body<PER, PRE_N, MODE>(p, blockIdx.x, nullptr, true, slots);
     trace_end(p.trace);
 }
 
@@ -219,7 +232,7 @@ __global__ void __launch_bounds__(LN_THREADS) v6_prologue_kernel(const LnMixPara
     asm volatile("cp.async.commit_group;" ::: "memory");
     float * mix = reinterpret_cast<float *>(v6p_smem + (size_t) V6_PROLOGUE_ROWS * w1.pitch);
     uint8_t * act = reinterpret_cast<uint8_t *>(mix) + (((size_t) p.C * sizeof(float) + 15) & ~(size_t) 15);
-    ln_mix_body<PER, 3, false>(p, 0, mix, blockIdx.x == 0, slots);
+    ln_mix_body<PER, 3, SEQ_ONE>(p, 0, mix, blockIdx.x == 0, slots);
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncthreads();
     GemvProblem P = w1;
@@ -404,12 +417,13 @@ cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch
     return launch_pdl(embed_ln0_kernel, dim3(T), dim3(GLUE_THREADS), (size_t) C * sizeof(float), s, reinterpret_cast<const uint8_t *>(emb), emb_type, emb_pitch, tokens, C, ln_w, ln_b, x);
 }
 
-// Grid row t is token t, or sequence t in batch mode. The single-sequence instantiation comes first: with the batch one first,
-// nvcc emitted different code for the untouched v6_lerp_kernel<8, 16> of this file.
+// Grid row t is token t, sequence t in batch mode, or column t in ragged mode. The single-sequence instantiation comes first: with
+// the batch one first, nvcc emitted different code for the untouched v6_lerp_kernel<8, 16> of this file. The ragged one comes last.
 template <int PER, int PRE_N>
 cudaError_t launch_ln_mix_kernel(const LnMixParams & p, cudaStream_t s) {
-    return !p.seq_stride ? launch_pdl(ln_mix_kernel<PER, PRE_N, false>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
-                         : launch_pdl(ln_mix_kernel<PER, PRE_N, true>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
+    return !p.seq_stride ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_ONE>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
+         : !p.seq_off    ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_BATCH>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
+                         : launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_RAGGED>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
 }
 
 cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s) {

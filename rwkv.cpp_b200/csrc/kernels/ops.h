@@ -6,6 +6,9 @@
 // token of each of several sequences per pass. Their seq_stride selects the mode: 0 means T tokens of one sequence; > 0 means T
 // sequences of one token each, column t working on the state of sequence t, which lives t * seq_stride floats after the state
 // pointers (sequence 0's). Both modes run the same arithmetic, so a sequence gives the same bits in a batch as alone.
+// A third, ragged mode (seq_off set, seq_stride > 0) lies between them: sequence s advances seq_off[s + 1] - seq_off[s] tokens, its
+// columns [seq_off[s], seq_off[s + 1]) back to back in the pass, on the state s * seq_stride floats on; T is the sum of the counts.
+// A sequence without columns is not touched. seq_off (and LnMixParams::col_seq) are written by the host before the pass.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -13,6 +16,9 @@
 #include "gemv.h"   // TraceRec
 
 namespace rwkv {
+
+// The MODE template argument of the state-carrying kernels: T tokens of one sequence, one token of each of T sequences, ragged.
+constexpr int SEQ_ONE = 0, SEQ_BATCH = 1, SEQ_RAGGED = 2;
 
 // x[:, t] = LN(emb[tokens[t]]; ln0)     (rwkv_graph.inc:655-658, 787-790)
 cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch, const int * tokens, int T, int C,
@@ -35,6 +41,8 @@ struct LnMixParams {
     float * out_xx;           // optional [C, T]: LN(x)
     float * out_sx;           // optional [C, T]: prev - xx
     long long seq_stride = 0;
+    const int * seq_off = nullptr;   // ragged mode: [n_seq + 1] column offsets of the sequences
+    const int * col_seq = nullptr;   // ragged mode: [T] the sequence of each column
 };
 cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s);
 
@@ -73,6 +81,7 @@ struct Wkv4Params {
     int C, T;
     unsigned char * q_out; int q_type;  // T == 1, C % 32 == 0 only: y as a staged column (act_stage.cuh)
     long long seq_stride = 0;
+    const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
 };
 cudaError_t launch_wkv4(const Wkv4Params & p, cudaStream_t s);
 
@@ -96,6 +105,7 @@ struct Wkv6Params {
     // v6 single-token passes with dw2.W set (v6_lora_fold): the decay is computed here, w = exp(-exp(Wd2 . lora1 + time_decay)) with
     // dw2 = {decay_w2, x = lora1, bias = time_decay, EPI_BIAS_EXPNEGEXP} planned by gemv_tma_plan, instead of read from td.
     GemvProblem dw2 = {};
+    const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
 };
 cudaError_t launch_wkv6(const Wkv6Params & p, cudaStream_t s);
 // Dynamic shared memory of a wkv6 launch that computes the decay (head size 64): the head's rows of dw2 and the staged lora1.
@@ -119,8 +129,13 @@ struct Wkv7Params {
     int H, S, T;
     unsigned char * q_out; int q_type;  // T == 1, S % 32 == 0 only: y as a staged column (act_stage.cuh)
     long long seq_stride = 0;
+    const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
 };
 cudaError_t launch_wkv7(const Wkv7Params & p, cudaStream_t s);
+
+// dst[:, dst_col[j]] = src[:, src_col[j]] for j < n, columns of `rows` floats (columns.cu); a NULL map stands for column j. The
+// ragged pass of a batch context gathers the last column of every advancing sequence for the head and scatters the head's output.
+cudaError_t launch_copy_columns(const float * src, const int * src_col, float * dst, const int * dst_col, int rows, int n, cudaStream_t s);
 
 // Layer-pipeline hand-off over peer memory (pipe.cu). A PipeBox sits at the start of every stage's mailbox allocation, followed by
 // PIPE_SLOTS data areas of slot_floats floats each.

@@ -15,16 +15,22 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 // v4: rwkv_att_wkv_v4 (rwkv_graph.inc:119-161). One thread per channel, sequential over tokens.
 // Every ggml node is its own rounding, so no FMA contraction here.
-// BATCH (seq_stride > 0): one token, column blockIdx.y, on the state of sequence blockIdx.y.
+// MODE SEQ_BATCH: one token, column blockIdx.y, on the state of sequence blockIdx.y.
+// MODE SEQ_RAGGED: the columns [seq_off[y], seq_off[y + 1]) of sequence y = blockIdx.y on its state.
 // ---------------------------------------------------------------------------------------------
-template <bool BATCH>
+template <int MODE>
 __global__ void wkv4_kernel(const Wkv4Params p) {
+    constexpr bool BATCH = MODE == SEQ_BATCH;
     trace_begin(p.trace);
     pdl_prologue();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= p.C) return;
-    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
-    const int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
+    const long long so = MODE != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
+    int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
+    if constexpr (MODE == SEQ_RAGGED) {
+        t_begin = p.seq_off[blockIdx.y]; t_end = p.seq_off[blockIdx.y + 1];
+        if (t_begin == t_end) return;
+    }
     float aa = p.aa_in[so + c], bb = p.bb_in[so + c], pp = p.pp_in[so + c];
     const float tf = p.time_first[c], td = p.time_decay[c];
     for (int t = t_begin; t < t_end; t++) {
@@ -106,13 +112,20 @@ template <int S> struct Wkv6Layout {
 __device__ __forceinline__ void wkv_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void wkv_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-// BATCH (seq_stride > 0): the block walks ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
+// MODE SEQ_BATCH: the block walks ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
+// MODE SEQ_RAGGED: the block walks the columns [seq_off[y], seq_off[y + 1]) of sequence y = blockIdx.y, as a single sequence's
+// block walks its T tokens, on the state of sequence y; a sequence without columns leaves at once.
 // DW2 >= 0 (v6, one token of one sequence): the decay of the head's S channels is the last LoRA GEMV, p.dw2 with weights of type DW2,
 // computed here: its S rows are copied to shared memory before the dependency wait, lora1 is staged after it as the streaming GEMV
 // stages a column, and rows_dot writes exp(-exp(..)) straight into the decay row the recurrence reads.
-template <int S, bool BATCH, int DW2 = -1>
+// DW2 == WKV6_RAGGED (with BATCH_OR_RAGGED = true): the ragged mode. (A value of the third argument rather than a MODE argument of its own, so
+// that the names of the other instantiations stay what they were.)
+constexpr int WKV6_RAGGED = -2;
+template <int S, bool BATCH_OR_RAGGED, int DW2 = -1>
 __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Params p) {
     using LY = Wkv6Layout<S>;
+    constexpr int MODE = DW2 == WKV6_RAGGED ? SEQ_RAGGED : BATCH_OR_RAGGED ? SEQ_BATCH : SEQ_ONE;
+    constexpr bool BATCH = MODE == SEQ_BATCH;
     constexpr int TB = WKV6_TB, NOCT = LY::NOCT, NT = LY::NT, WORK = LY::WORK, BLOCK = LY::BLOCK, NNW = LY::NORM_WARPS, CPL = (S + 31) / 32;
     constexpr int BAR_FULL = 1, BAR_EMPTY = 3, BAR_WORK = 5;        // named barriers: FULL / EMPTY + (chunk & 1), the workers' own
     __shared__ Wkv6Chunk<S> buf[2];
@@ -121,14 +134,20 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int h = blockIdx.x, tid = threadIdx.x, C = p.H * S;
-    const int col0 = BATCH ? blockIdx.y : 0;      // column of the block's first token
-    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
+    constexpr bool RAGGED = MODE == SEQ_RAGGED;
+    int col0 = BATCH ? blockIdx.y : 0;            // column of the block's first token
+    int r_T = 0;                                  // ragged: the sequence's tokens (the other modes: p.T / 1 as written below)
+    if constexpr (RAGGED) {
+        col0 = p.seq_off[blockIdx.y]; r_T = p.seq_off[blockIdx.y + 1] - col0;
+        if (r_T == 0) return;
+    }
+    const long long so = MODE != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
     const bool is_norm = tid >= WORK;
     const bool worker = tid < NT;
     const int oct = worker ? tid % NOCT : 0, jg = worker ? tid / NOCT : 0;
     const int i0 = oct * 8, j0 = jg * 4;
     const int lane = tid & 31;
-    const int nchunks = BATCH ? 1 : (p.T + TB - 1) / TB;
+    const int nchunks = BATCH ? 1 : ((RAGGED ? r_T : p.T) + TB - 1) / TB;
     // the recurrent state (written by the previous token's pass) and the parameters do not depend on the previous
     // kernel: pull them in before the programmatic-dependency wait
     float st[8][4];
@@ -183,7 +202,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         // the recurrence walks a chunk's tokens serially with the state in registers and no barrier inside the chunk.
         auto stage = [&](int c) {
             Wkv6Chunk<S> & B = buf[c & 1];
-            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, (RAGGED ? r_T : p.T) - t0);
             constexpr int PER_ROW = S / 4;
             for (int idx = tid; idx < nt * PER_ROW; idx += WORK) {
                 const int tt = idx / PER_ROW, f = (idx % PER_ROW) * 4;
@@ -196,7 +215,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         };
         // trace marks of CTA 0 (cycles, stored as start + cycles): [0] waiting for the staged chunk, [1] the recurrence,
         // [2] waiting for the normalising warps to hand an output buffer back
-        const bool acct = p.trace != nullptr && blockIdx.x == 0 && (!BATCH || blockIdx.y == 0) && tid == 0;
+        const bool acct = p.trace != nullptr && blockIdx.x == 0 && (MODE == SEQ_ONE || blockIdx.y == 0) && tid == 0;
         long long a0 = 0, a1 = 0, a2 = 0, tq = acct ? clock64() : 0;
         auto tick = [&](long long & a) { if (acct) { const long long now = clock64(); a += now - tq; tq = now; } };
         float tfr[8];     // time_first of my key rows
@@ -214,7 +233,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
             tick(a2);
             const Wkv6Chunk<S> & B = buf[c & 1];
             float (* yb)[S] = ybuf[c & 1];
-            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, (RAGGED ? r_T : p.T) - t0);
             // recurrence (kv = v_j*k_i;  y_j += (kv*tf_i + S_ij) * r_i;  S_ij = S_ij*td_i + kv), 8 + 8 + 8 + 4 operands per token from
             // shared memory
             float kk[8], rr[8], dv[8], vv[4];
@@ -274,7 +293,7 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
         const int nwarp = (tid - WORK) >> 5;
         constexpr int PER = (TB + NNW - 1) / NNW;        // tokens of a chunk per normalising warp
         for (int c = 0; c < nchunks; c++) {
-            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, p.T - t0);
+            const int t0 = c * TB, nt = BATCH ? 1 : min(TB, (RAGGED ? r_T : p.T) - t0);
             // the gate values of my tokens: requested before the wait for the chunk, so their latency hides behind the recurrence
             float gg[PER][CPL];
 #pragma unroll
@@ -331,15 +350,21 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
 // v7: rwkv_att_v7 (rwkv_graph.inc:432-479) around rwkv_wkv_v7_impl (rwkv_operators_wkv_v7.inc:63-101).
 // Thread i owns state row S[i][.] (value index i, key index j).
 // ---------------------------------------------------------------------------------------------
-// BATCH (seq_stride > 0): the block handles ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
-template <int S, bool BATCH>
+// MODE SEQ_BATCH: the block handles ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
+// MODE SEQ_RAGGED: the columns [seq_off[y], seq_off[y + 1]) of sequence y = blockIdx.y on its state; none: the block leaves at once.
+template <int S, int MODE>
 __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
+    constexpr bool BATCH = MODE == SEQ_BATCH;
     __shared__ float sr[S], sw[S], sk[S], sa[S], sb[S], red[S];
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int h = blockIdx.x, i = threadIdx.x, C = p.H * S, c = h * S + i;
-    const long long so = BATCH ? blockIdx.y * p.seq_stride : 0;
-    const int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
+    const long long so = MODE != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
+    int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
+    if constexpr (MODE == SEQ_RAGGED) {
+        t_begin = p.seq_off[blockIdx.y]; t_end = p.seq_off[blockIdx.y + 1];
+        if (t_begin == t_end) return;
+    }
     float st[S];
 #pragma unroll
     for (int j = 0; j < S; j++) st[j] = p.state_in[so + ((size_t) h * S + i) * S + j];
@@ -399,19 +424,22 @@ __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
 
 }  // namespace
 
-// Grid row y is sequence y in batch mode (seq_stride > 0); one sequence has a single row.
+// Grid row y is sequence y in batch mode (seq_stride > 0) and in ragged mode (seq_off set: n_seq rows); one sequence has a single
+// row. The ragged instantiations come after the two others.
 cudaError_t launch_wkv4(const Wkv4Params & p_in, cudaStream_t s) {
     Wkv4Params p = p_in;
     p.trace = trace_slot("wkv4");
     const int threads = 128;
-    return !p.seq_stride ? launch_pdl(wkv4_kernel<false>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
-                         : launch_pdl(wkv4_kernel<true>, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p);
+    return !p.seq_stride ? launch_pdl(wkv4_kernel<SEQ_ONE>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
+         : !p.seq_off    ? launch_pdl(wkv4_kernel<SEQ_BATCH>, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p)
+                         : launch_pdl(wkv4_kernel<SEQ_RAGGED>, dim3((p.C + threads - 1) / threads, p.n_seq), dim3(threads), 0, s, p);
 }
 
 template <int S>
 cudaError_t launch_wkv6_kernel(const Wkv6Params & p, cudaStream_t s) {
     return !p.seq_stride ? launch_pdl(wkv6_kernel<S, false>, dim3(p.H), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
-                         : launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
+         : !p.seq_off    ? launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
+                         : launch_pdl(wkv6_kernel<S, true, WKV6_RAGGED>, dim3(p.H, p.n_seq), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
 }
 
 template <int DW2>
@@ -455,8 +483,9 @@ cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
 
 template <int S>
 cudaError_t launch_wkv7_kernel(const Wkv7Params & p, cudaStream_t s) {
-    return !p.seq_stride ? launch_pdl(wkv7_kernel<S, false>, dim3(p.H), dim3(S), 0, s, p)
-                         : launch_pdl(wkv7_kernel<S, true>, dim3(p.H, p.T), dim3(S), 0, s, p);
+    return !p.seq_stride ? launch_pdl(wkv7_kernel<S, SEQ_ONE>, dim3(p.H), dim3(S), 0, s, p)
+         : !p.seq_off    ? launch_pdl(wkv7_kernel<S, SEQ_BATCH>, dim3(p.H, p.T), dim3(S), 0, s, p)
+                         : launch_pdl(wkv7_kernel<S, SEQ_RAGGED>, dim3(p.H, p.n_seq), dim3(S), 0, s, p);
 }
 
 cudaError_t launch_wkv7(const Wkv7Params & p_in, cudaStream_t s) {

@@ -150,6 +150,8 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_get_state.restype = ctypes.c_bool
         lib.rwkv_b200_batch_eval.argtypes = [vp, P_U32, ctypes.c_bool]
         lib.rwkv_b200_batch_eval.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_eval_ragged.argtypes = [vp, P_U32, P_U32, ctypes.c_bool]
+        lib.rwkv_b200_batch_eval_ragged.restype = ctypes.c_bool
         lib.rwkv_b200_batch_get_logits.argtypes = [vp, ctypes.c_size_t, P_FLOAT]
         lib.rwkv_b200_batch_get_logits.restype = ctypes.c_bool
         lib.rwkv_b200_batch_size.argtypes = [vp]
