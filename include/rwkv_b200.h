@@ -102,6 +102,60 @@ RWKV_API bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows,
                                             const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out,
                                             float * probs_out);
 
+/* Device-side generation: up to max_tokens sample-and-evaluate steps in one call, without the host in any step. For a sequence with
+ * valid logits, step i = 0, 1, ...: (1) if i == max_tokens, stop; (2) draw tok from the current logits with temperature, top_p and
+ * u[i] and the logit bias -(presence_penalty + count[n] * frequency_penalty) on every token n with count[n] > 0 (computed in float32,
+ * the multiply and the add rounded separately) -- bit for bit what rwkv_b200_sample returns with that bias list; (3) tokens_out[i] =
+ * tok; (4) if tok is one of the stop ids, stop: it is reported but neither evaluated nor counted; (5) otherwise count[tok] += 1,
+ * evaluate tok (a single-token resident pass with logits) and continue. This is the loop of the reference's
+ * python/chat_with_bot.py:244-260 and python/generate_completions.py:60-67. Afterwards the state has consumed every evaluated token,
+ * the logits are those of the last evaluated token (the row the last token was drawn from), and n_generated counts the tokens written,
+ * a stop token included.
+ * The penalty counts are a per-sequence table in HBM, allocated on first use. keep_counts false starts the sequence from zero counts;
+ * true continues from its previous generate call, so that a server can generate in short windows (between ragged admissions in a
+ * batch) without losing its penalties. At most RWKV_B200_GENERATE_MAX_STOP stop ids, shared by all sequences, each below n_vocab.
+ * The whole loop is one CUDA-graph launch (a conditional WHILE node; a CUDA driver of 12.4 or newer); only the tokens come back.
+ * Every argument is checked before anything is enqueued, and a rejected call changes no state, logits or count: a context of the
+ * wrong kind (a batch context here, an ordinary one for the batch call, a pipeline or a stage of one) or an older driver gives
+ * RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED; NULL arrays, max_tokens out of range, temperature, top_p or u out of the ranges of
+ * rwkv_b200_sample, non-finite penalties, ids >= n_vocab, more than 16 stop ids, and a context whose last pass skipped the head give
+ * RWKV_ERROR_ARGS. n_vocab <= 65536.
+ * rwkv_b200_generate: a single-sequence context; 1 <= max_tokens <= RWKV_B200_GENERATE_MAX; u holds max_tokens numbers in [0, 1). */
+#define RWKV_B200_GENERATE_MAX 4096
+#define RWKV_B200_GENERATE_MAX_STOP 16
+RWKV_API bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty,
+                                 float frequency_penalty, bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                 uint32_t * tokens_out, size_t * n_generated);
+/* rwkv_b200_batch_generate: a batch context; per-sequence arrays of n_sequences entries: max_tokens (0 .. RWKV_B200_GENERATE_MAX; 0
+ * leaves the sequence exactly as it is), temperature, top_p, penalties, keep_counts (NULL = none kept). With n the largest max_tokens,
+ * u and tokens_out are [n_sequences][n]: sequence b's entries at b * n + i (tokens_out entries past n_generated[b] are 0). Every
+ * sequence gives the tokens, state and logits rwkv_b200_generate gives it alone on the same logits and state (below 16 sequences;
+ * from 16 on the layer matrices take the tensor-core path of rwkv_b200_batch_eval). The pass computes every sequence until the last
+ * one stops; a stopped sequence's state and logits are put back after each pass and after the loop. */
+RWKV_API bool rwkv_b200_batch_generate(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                                       const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts,
+                                       const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated);
+/* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
+ * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
+ * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each
+ * row's next input token (0 when frozen), any_active 1 when a row is still active. Arguments are checked before a device is touched. */
+struct rwkv_b200_generate_step_args {
+    const float * logits;
+    size_t n_rows, n_vocab;                    /* 1 .. 256, 1 .. 65536 */
+    const uint32_t * max_tokens;
+    const float * temperature, * top_p, * presence_penalty, * frequency_penalty;
+    const double * u;
+    const uint32_t * stop_ids;
+    size_t n_stop;
+    uint32_t * step;                           /* in / out, <= max_tokens */
+    uint8_t * frozen;                          /* in / out */
+    uint32_t * counts;                         /* [n_rows, n_vocab] in / out */
+    uint32_t * tokens;                         /* [n_rows][n] in / out */
+    int32_t * next_tokens;                     /* out */
+    uint32_t * any_active;                     /* out */
+};
+RWKV_API bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a);
+
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice
  * of the recurrent state stays resident on that device. Per pass of n_tokens (<= 256):

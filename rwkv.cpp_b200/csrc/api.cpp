@@ -1,6 +1,7 @@
 // The rwkv.h C ABI over the H100 engine, plus the additive rwkv_b200_* entry points.
 // Argument checks, error categories and NULL conventions follow the reference entry points
 // (rwkv.cpp:71-258, rwkv_eval.inc:38-241) so its C tests run unchanged against this library.
+#include <algorithm>
 #include <cinttypes>
 #include <cstdio>
 #include <cstdlib>
@@ -469,6 +470,81 @@ bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows, size_t n
     return true;
 }
 
+static_assert(RWKV_B200_GENERATE_MAX == GENERATE_MAX && RWKV_B200_GENERATE_MAX_STOP == GENERATE_MAX_STOP, "generation limits of the header and the engine");
+
+bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
+                        bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated) {
+    if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(ctx);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
+               "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
+    const uint32_t budget = (uint32_t) max_tokens;
+    const uint8_t keep = keep_counts ? 1 : 0;
+    uint32_t n = 0;
+    if (!generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n)) return false;
+    *n_generated = n;
+    return true;
+}
+
+bool rwkv_b200_batch_generate(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                              const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
+                              const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate");
+    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated);
+}
+
+bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
+               a->step && a->frozen && a->counts && a->next_tokens && a->any_active, "Invalid generate-step arguments");
+    const size_t R = a->n_rows, V = a->n_vocab;
+    if (!check_generate_rows(sink, R, V, a->max_tokens, a->temperature, a->top_p, a->presence_penalty, a->frequency_penalty, a->u, a->stop_ids, a->n_stop,
+                             a->tokens, a->step)) return false;
+    uint32_t n = 0;
+    for (size_t b = 0; b < R; b++) {
+        n = std::max(n, a->max_tokens[b]);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->step[b] <= a->max_tokens[b], "step of row %zu is above its max_tokens", b);
+    }
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n >= 1, "Every row has max_tokens 0");
+    if (!hook_device(sink)) return false;
+    GenShared sh{};
+    for (size_t k = 0; k < a->n_stop; k++) sh.stop[k] = a->stop_ids[k];
+    sh.n_stop = (uint32_t) a->n_stop; sh.stride = n;
+    std::vector<GenRow> rows(R);
+    for (size_t b = 0; b < R; b++)
+        rows[b] = GenRow{a->temperature[b], a->top_p[b], a->presence_penalty[b], a->frequency_penalty[b], a->max_tokens[b], a->step[b], a->frozen[b] ? 1u : 0u, 0};
+    const uint32_t zero = 0;
+    HookBuffers hb;
+    GenStepParams gp{};
+    gp.logits = hb.in(a->logits, R * V); gp.n_vocab = (int) V; gp.n_rows = (int) R;
+    gp.rows = const_cast<GenRow *>(hb.in(rows.data(), R));
+    gp.shared = const_cast<GenShared *>(hb.in(&sh, 1));
+    gp.u = hb.in(a->u, R * n);
+    gp.counts = const_cast<uint32_t *>(hb.in(a->counts, R * V));
+    gp.bias_ids = static_cast<uint32_t *>(hb.alloc(R * V * sizeof(uint32_t)));
+    gp.bias_values = static_cast<float *>(hb.alloc(R * V * sizeof(float)));
+    gp.scratch = static_cast<float *>(hb.alloc(R * V * sizeof(float)));
+    gp.tokens = const_cast<uint32_t *>(hb.in(a->tokens, R * n));
+    gp.n_generated = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
+    gp.passes = const_cast<uint32_t *>(hb.in(&zero, 1));
+    gp.next_tokens = static_cast<int *>(hb.alloc(R * sizeof(int)));
+    const cudaError_t e = hb.ok ? launch_generate_step(gp, 0) : cudaSuccess;
+    bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(a->next_tokens, gp.next_tokens, R * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "generate step failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    for (size_t b = 0; b < R; b++) { a->step[b] = rows[b].step; a->frozen[b] = rows[b].frozen ? 1 : 0; }
+    return true;
+}
+
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }
 
 bool rwkv_b200_stage_eval(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, const float * hidden_in, float * hidden_out, bool want_logits,
@@ -646,7 +722,10 @@ bool rwkv_b200_profile_pass(struct rwkv_context * ctx, const uint32_t * tokens, 
 }
 
 void rwkv_b200_set_graphs(struct rwkv_context * ctx, bool enabled) { C(ctx)->use_graphs = enabled; }
-void rwkv_b200_set_tensor_cores(struct rwkv_context * ctx, bool enabled) { C(ctx)->use_tensor_cores = enabled; }
+void rwkv_b200_set_tensor_cores(struct rwkv_context * ctx, bool enabled) {
+    if (C(ctx)->use_tensor_cores != enabled) drop_generate_graphs(C(ctx));     // a batch's generation graph holds its GEMM routing
+    C(ctx)->use_tensor_cores = enabled;
+}
 void rwkv_b200_set_overlap(struct rwkv_context * ctx, bool enabled) { C(ctx)->overlap_copies = enabled; }
 void rwkv_b200_set_bounce_min_bytes(size_t bytes) { g_bounce_min_bytes.store(bytes); }
 int rwkv_b200_overlap_groups(const struct rwkv_context * ctx) { return C(ctx)->overlap_copies && C(ctx)->n_segments > 1 ? C(ctx)->n_segments : 0; }
@@ -662,6 +741,7 @@ bool rwkv_b200_trace_enable(struct rwkv_context * ctx) {
     if (!c->trace_buf && cudaMalloc((void **) &c->trace_buf, 1024 * sizeof(TraceRec)) != cudaSuccess) return false;
     // graphs captured so far carry no trace slots: drop them so they are re-captured
     for (auto & g : c->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
+    drop_generate_graphs(c);
     return trace_rearm(c);
 }
 
@@ -670,6 +750,7 @@ void rwkv_b200_trace_disable(struct rwkv_context * ctx) {
     if (!c->trace_buf || cudaSetDevice(c->model->dev.device) != cudaSuccess) return;
     cudaStreamSynchronize(c->stream);
     for (auto & g : c->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
+    drop_generate_graphs(c);
     cudaFree(c->trace_buf);
     c->trace_buf = nullptr; c->trace_count = 0;
 }

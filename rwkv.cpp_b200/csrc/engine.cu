@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <cinttypes>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -445,6 +446,7 @@ bool ensure_capacity(Context * ctx, int T) {
         ctx->slot_used[i] = false;
     }
     for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
+    drop_generate_graphs(ctx);
     ctx->capacity_T = 0;
     const size_t n = scratch_floats_for(m, cap);
     cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->scratch), n * sizeof(float));
@@ -477,7 +479,7 @@ bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
     const int C = m.n_embed;
     const Scratch s = carve(m, ctx->scratch, T);
     if (l0 == 0) {
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+        if (!ctx->tokens_on_device) CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
         CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, m.ln0_w.data, m.ln0_b.data, s.x, ctx->stream));
     }   // a later pipeline stage / layer group finds x (and v_first) already in place
     const size_t per_layer = m.state_floats_per_layer();
@@ -693,6 +695,11 @@ void destroy_context(Context * ctx) {
     cudaFree(ctx->sample_rows); cudaFree(ctx->sample_tokens);
     if (ctx->sample_rows_host) cudaFreeHost(ctx->sample_rows_host);
     if (ctx->sample_tokens_host) cudaFreeHost(ctx->sample_tokens_host);
+    drop_generate_graphs(ctx);
+    cudaFree(ctx->gen_in); cudaFree(ctx->gen_out); cudaFree(ctx->gen_counts); cudaFree(ctx->gen_bias_ids); cudaFree(ctx->gen_bias_values);
+    cudaFree(ctx->gen_scratch); cudaFree(ctx->gen_park);
+    if (ctx->gen_in_host) cudaFreeHost(ctx->gen_in_host);
+    if (ctx->gen_out_host) cudaFreeHost(ctx->gen_out_host);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
     if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
@@ -1171,6 +1178,197 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
     if (!check_sample_rows(ctx->sink(), ctx->batch_n, m.n_vocab, temperature, top_p, u, nullptr, nullptr, nullptr, tokens_out)) return false;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.n_vocab <= 65536, "On-device sampling supports n_vocab <= 65536");
     return batch_eval(ctx, tokens, true) && batch_sample(ctx, temperature, top_p, u, nullptr, nullptr, nullptr, tokens_out);
+}
+
+// ---- device-side generation -----------------------------------------------------------------------------------------------------
+// The loop of a generate call is one graph launch: WHILE { step -> IF { pass X -> Y } -> step -> IF { pass Y -> X } }. Each step
+// (generate_sample_kernel) draws every active row's next token and writes it into ctx->tokens, then sets both conditions to "a row is
+// still active". A body holds two passes because the passes double-buffer the state. In a batch context every pass computes all
+// columns, so its shape and graph stay fixed; a frozen row's state is copied back over its output after each pass and its logits,
+// parked by the step that froze it, come back after the loop.
+namespace {
+
+size_t gen_u_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
+size_t gen_out_words(int rows, size_t n) { return (size_t) rows + 1 + (size_t) rows * n; }
+
+GenStepParams generate_step_params(Context * ctx) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    GenStepParams gp{};
+    gp.logits = ctx->logits; gp.n_vocab = ctx->model->n_vocab; gp.n_rows = rows;
+    gp.shared = reinterpret_cast<GenShared *>(ctx->gen_in);
+    gp.rows = reinterpret_cast<GenRow *>(ctx->gen_in + sizeof(GenShared));
+    gp.u = reinterpret_cast<const double *>(ctx->gen_in + gen_u_offset(rows));
+    gp.counts = ctx->gen_counts; gp.bias_ids = ctx->gen_bias_ids; gp.bias_values = ctx->gen_bias_values; gp.scratch = ctx->gen_scratch;
+    gp.n_generated = ctx->gen_out; gp.passes = ctx->gen_out + rows; gp.tokens = ctx->gen_out + rows + 1;
+    gp.next_tokens = ctx->tokens; gp.park = ctx->batch_n ? ctx->gen_park : nullptr;
+    return gp;
+}
+
+// One pass of the loop (state_a -> state_b as they are set now, input tokens already in ctx->tokens) captured into `body`.
+bool capture_generate_pass(Context * ctx, cudaGraph_t body) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(ctx->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    ctx->tokens_on_device = true;
+    bool ok = enqueue_pass(ctx, rows, true, ctx->phase, 0);
+    cudaError_t e = cudaSuccess;
+    if (ok && ctx->batch_n)
+        e = launch_restore_frozen(generate_step_params(ctx).rows, rows, ctx->state_a, ctx->state_b, ctx->batch_stride, ctx->model->state_len(), ctx->stream);
+    ctx->tokens_on_device = false;
+    cudaGraph_t out = nullptr;
+    const cudaError_t ec = cudaStreamEndCapture(ctx->stream, &out);
+    if (e == cudaSuccess) e = ec;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess, "Capturing the generation pass failed: %s", cudaGetErrorString(e));
+    return true;
+}
+
+struct GraphHolder {
+    cudaGraph_t g = nullptr;
+    ~GraphHolder() { if (g) cudaGraphDestroy(g); }
+};
+
+bool build_generate_graph(Context * ctx) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    {   // one uncaptured pass of the loop's shape first, as run_layers does before it captures; its logits go to the step's scratch
+        // and its state to state_b, which holds nothing between passes
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) rows * sizeof(int), ctx->stream));
+        float * logits = ctx->logits;
+        ctx->logits = ctx->gen_scratch;
+        ctx->tokens_on_device = true;
+        const bool ok = enqueue_pass(ctx, rows, true, ctx->phase, 0);
+        ctx->tokens_on_device = false;
+        ctx->logits = logits;
+        if (!ok) return false;
+    }
+    GraphHolder top;
+    CUDA_OK(ctx, cudaGraphCreate(&top.g, 0));
+    cudaGraphConditionalHandle keep_going;
+    CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&keep_going, top.g, 1, cudaGraphCondAssignDefault));
+    cudaGraphNodeParams wp = {};
+    wp.type = cudaGraphNodeTypeConditional;
+    wp.conditional.handle = keep_going; wp.conditional.type = cudaGraphCondTypeWhile; wp.conditional.size = 1;
+    cudaGraphNode_t loop = nullptr;
+    CUDA_OK(ctx, cudaGraphAddNode(&loop, top.g, nullptr, 0, &wp));
+    cudaGraph_t body = wp.conditional.phGraph_out[0];
+    cudaGraphNode_t prev = nullptr;
+    for (int half = 0; half < 2; half++) {
+        cudaGraphConditionalHandle run_pass;
+        CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&run_pass, body, 0, cudaGraphCondAssignDefault));
+        GenStepParams gp = generate_step_params(ctx);
+        gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
+        cudaGraphNode_t step = nullptr, cond = nullptr;
+        CUDA_OK(ctx, add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
+        cudaGraphNodeParams ip = {};
+        ip.type = cudaGraphNodeTypeConditional;
+        ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
+        CUDA_OK(ctx, cudaGraphAddNode(&cond, body, &step, 1, &ip));
+        if (half) std::swap(ctx->state_a, ctx->state_b);      // the second pass reads what the first one wrote
+        const bool ok = capture_generate_pass(ctx, ip.conditional.phGraph_out[0]);
+        if (half) std::swap(ctx->state_a, ctx->state_b);
+        if (!ok) return false;
+        prev = cond;
+    }
+    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase], top.g, 0));
+    return true;
+}
+
+bool ensure_generate_buffers(Context * ctx) {
+    if (ctx->gen_in) return true;
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    const size_t V = (size_t) ctx->model->n_vocab, in_bytes = gen_u_offset(rows) + (size_t) rows * GENERATE_MAX * sizeof(double);
+    const size_t out_bytes = gen_out_words(rows, GENERATE_MAX) * sizeof(uint32_t), table = (size_t) rows * V;
+    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->gen_in_host), in_bytes));
+    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->gen_out_host), out_bytes));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_out), out_bytes));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_counts), table * sizeof(uint32_t)));
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_counts, 0, table * sizeof(uint32_t), ctx->stream));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_bias_ids), table * sizeof(uint32_t)));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_bias_values), table * sizeof(float)));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_scratch), table * sizeof(float)));
+    if (ctx->batch_n) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_park), table * sizeof(float)));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_in), in_bytes));      // last: it marks the set as complete
+    return true;
+}
+
+}  // namespace
+
+void drop_generate_graphs(Context * ctx) {
+    for (auto & e : ctx->gen_graphs) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+}
+
+bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                         const float * presence, const float * frequency, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                         const void * tokens_out, const void * n_generated) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, max_tokens && temperature && top_p && presence && frequency && u && tokens_out && n_generated,
+               "NULL max_tokens, temperature, top_p, penalty, u, tokens_out or n_generated");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_stop <= (size_t) GENERATE_MAX_STOP && (n_stop == 0 || stop_ids), "At most %d stop ids, not NULL", GENERATE_MAX_STOP);
+    for (size_t k = 0; k < n_stop; k++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, stop_ids[k] < n_vocab, "Stop id %u is out of range", stop_ids[k]);
+    size_t n = 0;
+    for (size_t b = 0; b < n_rows; b++) {
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, max_tokens[b] <= (uint32_t) GENERATE_MAX, "max_tokens of row %zu is above %d", b, GENERATE_MAX);
+        n = std::max(n, (size_t) max_tokens[b]);
+    }
+    for (size_t b = 0; b < n_rows; b++) {     // sampling.py:20-23, as check_sample_rows checks a row
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, temperature[b] >= 0.0f, "temperature of row %zu must be >= 0", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, top_p[b] >= 0.0f && top_p[b] <= 1.0f, "top_p of row %zu must be in [0, 1]", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, std::isfinite(presence[b]) && std::isfinite(frequency[b]), "penalties of row %zu must be finite", b);
+        for (size_t i = 0; i < max_tokens[b]; i++)
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, u[b * n + i] >= 0.0 && u[b * n + i] < 1.0, "u[%zu][%zu] must be in [0, 1)", b, i);
+    }
+    return true;
+}
+
+bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
+              const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+              uint32_t * tokens_out, uint32_t * n_generated) {
+    const Model & m = *ctx->model;
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    const size_t V = (size_t) m.n_vocab;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, !ctx->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Generation runs on a whole-model context or batch context, not on a pipeline or one of its stages");
+    if (!check_generate_rows(ctx->sink(), rows, V, max_tokens, temperature, top_p, presence, frequency, u, stop_ids, n_stop, tokens_out, n_generated)) return false;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, V <= 65536, "On-device sampling supports n_vocab <= 65536");
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last evaluation skipped the head");
+    int driver = 0;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaDriverGetVersion(&driver) == cudaSuccess && driver >= 12040,
+               "Device-side generation needs conditional graph nodes: a CUDA driver of 12.4 or newer (found %d)", driver);
+    size_t n = 0;
+    for (int b = 0; b < rows; b++) n = std::max(n, (size_t) max_tokens[b]);
+    CUDA_OK(ctx, cudaSetDevice(m.dev.device));
+    if (!ensure_generate_buffers(ctx) || !ensure_capacity(ctx, rows)) return false;
+    // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
+    GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
+    memset(sh, 0, sizeof(GenShared));
+    for (size_t k = 0; k < n_stop; k++) sh->stop[k] = stop_ids[k];
+    sh->n_stop = (uint32_t) n_stop; sh->stride = (uint32_t) n;
+    GenRow * gr = reinterpret_cast<GenRow *>(ctx->gen_in_host + sizeof(GenShared));
+    for (int b = 0; b < rows; b++) gr[b] = GenRow{temperature[b], top_p[b], presence[b], frequency[b], max_tokens[b], 0, 0, 0};
+    const size_t u_off = gen_u_offset(rows);
+    memcpy(ctx->gen_in_host + u_off, u, (size_t) rows * n * sizeof(double));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_in, ctx->gen_in_host, u_off + (size_t) rows * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    for (int b = 0; b < rows;) {      // counts of the rows that start from zero (runs of them are contiguous)
+        if (keep_counts && keep_counts[b]) { b++; continue; }
+        int e = b;
+        while (e < rows && !(keep_counts && keep_counts[e])) e++;
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_counts + (size_t) b * V, 0, (size_t) (e - b) * V * sizeof(uint32_t), ctx->stream));
+        b = e;
+    }
+    const size_t out_words = gen_out_words(rows, n);
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_out, 0, out_words * sizeof(uint32_t), ctx->stream));
+    const int key = ctx->phase;
+    if (!ctx->gen_graphs[key] && !build_generate_graph(ctx)) return false;
+    CUDA_OK(ctx, cudaGraphLaunch(ctx->gen_graphs[key], ctx->stream));
+    if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    const uint32_t * res = ctx->gen_out_host;
+    memcpy(n_generated, res, (size_t) rows * sizeof(uint32_t));
+    memcpy(tokens_out, res + rows + 1, (size_t) rows * n * sizeof(uint32_t));
+    if (res[rows] & 1u) {      // an odd number of passes leaves the state in state_b
+        std::swap(ctx->state_a, ctx->state_b);
+        ctx->phase ^= 1;
+    }
+    return true;
 }
 
 bool pipe_ensure_box(Context * ctx) {

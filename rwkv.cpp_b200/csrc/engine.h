@@ -116,6 +116,19 @@ struct Context {
     SampleRow * sample_rows = nullptr, * sample_rows_host = nullptr;          // device / pinned
     uint32_t * sample_tokens = nullptr, * sample_tokens_host = nullptr;       // device / pinned
 
+    // Device-side generation (generate), allocated on the first call at GENERATE_MAX tokens per row so that the pointers captured in
+    // the loop's graph never change. gen_in: GenShared, GenRow [rows], u [rows][GENERATE_MAX]; gen_out: n_generated [rows], the
+    // number of passes that ran, tokens [rows][GENERATE_MAX]. Both are packed with the call's row stride, so each crosses PCIe once.
+    unsigned char * gen_in = nullptr, * gen_in_host = nullptr;        // device / pinned
+    uint32_t * gen_out = nullptr, * gen_out_host = nullptr;           // device / pinned
+    uint32_t * gen_counts = nullptr;                                  // [rows, n_vocab] penalty counts
+    uint32_t * gen_bias_ids = nullptr;                                // [rows, n_vocab]
+    float * gen_bias_values = nullptr, * gen_scratch = nullptr;       // [rows, n_vocab] each
+    float * gen_park = nullptr;                                       // batch contexts: [rows, n_vocab] logits of frozen rows
+    // the loop's graph, keyed by phase (which state buffer holds the current state), as the single-token slots are
+    cudaGraphExec_t gen_graphs[2] = {nullptr, nullptr};
+    bool tokens_on_device = false;   // while the loop's passes are captured: ctx->tokens is written by the sampler, no upload
+
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
     bool print_errors = true;
@@ -191,6 +204,20 @@ bool batch_sample(Context * ctx, const float * temperature, const float * top_p,
 // batch_eval(tokens, want_logits = true) + batch_sample without bias. The sampling arguments are checked before the pass, so a
 // rejected call leaves every sequence's state as it was.
 bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * temperature, const float * top_p, const double * u, uint32_t * tokens_out);
+
+// Device-side generation over n_rows rows (1 for a single-sequence context, batch_n for a batch context), the loop of
+// rwkv_b200_generate / rwkv_b200_batch_generate (include/rwkv_b200.h). Host arrays of n_rows entries; u and tokens_out are
+// [n_rows][n] with n the largest max_tokens; keep_counts may be NULL. check_generate_rows checks every argument (also for the test
+// hook); generate checks the context too and runs the whole loop as one graph launch, then copies tokens and counts back. Synchronises.
+constexpr int GENERATE_MAX = 4096;
+bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                         const float * presence, const float * frequency, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                         const void * tokens_out, const void * n_generated);
+bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
+              const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+              uint32_t * tokens_out, uint32_t * n_generated);
+// Drops the loop's graphs (they hold the activation buffers and the GEMM routing of the time they were captured).
+void drop_generate_graphs(Context * ctx);
 
 size_t stage_hidden_len(const Model & m, size_t T);
 

@@ -186,4 +186,44 @@ struct SampleBatchParams {
 };
 cudaError_t launch_sample_batch(const SampleBatchParams & p, cudaStream_t s);
 
+// Device-side generation (rwkv_b200_generate / rwkv_b200_batch_generate): one step of the sample-and-evaluate loop per launch, CTA b
+// for row b. A row that is not frozen freezes when it has drawn max_tokens tokens; otherwise it draws with u[b * stride + step] from
+// its logits with the bias -(presence + count[n] * frequency) on every token n it has counted (sample_row's bias path), writes the
+// token to tokens[b * stride + step], and freezes on a stop token or else counts it and makes it the row's next input token. The
+// last CTA of the step sets both conditional handles to "some row is still active" and, if so, counts one more pass.
+struct GenRow {                       // written by the host per call; step and frozen are then the loop's state
+    float temperature, top_p, presence, frequency;
+    uint32_t max_tokens, step, frozen, pad;
+};
+constexpr int GENERATE_MAX_STOP = 16;
+struct GenShared {                    // written by the host per call (ticket = active = 0)
+    uint32_t stop[GENERATE_MAX_STOP];
+    uint32_t n_stop, stride;
+    uint32_t ticket, active;          // CTAs done with this step / rows active after it; reset by the step's last CTA
+};
+struct GenStepParams {
+    const float * logits;             // [n_rows, n_vocab]
+    int n_vocab, n_rows;
+    GenRow * rows;                    // [n_rows]
+    GenShared * shared;
+    const double * u;                 // [n_rows][stride]
+    uint32_t * counts;                // [n_rows, n_vocab]
+    uint32_t * bias_ids;              // [n_rows, n_vocab] scratch: the bias list of a row, one entry per token (id n_vocab = none)
+    float * bias_values;
+    float * scratch;                  // [n_rows, n_vocab]: the biased logits
+    uint32_t * tokens;                // [n_rows][stride]
+    uint32_t * n_generated;           // [n_rows]: the row's step after this launch
+    uint32_t * passes;                // +1 for every step after which a row is active
+    int * next_tokens;                // [n_rows]: input tokens of the next pass (0 for a frozen row)
+    float * park;                     // [n_rows, n_vocab] or NULL: a row's logits are copied here when it freezes (batch contexts)
+    bool set_handles;                 // inside a conditional graph: set run_pass and keep_going
+    cudaGraphConditionalHandle run_pass, keep_going;
+};
+cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s);
+// The same step as a kernel node of graph g after deps (the body of the generation loop).
+cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node);
+// After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
+// every frozen row, so that its state stays what it was.
+cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);
+
 }  // namespace rwkv

@@ -181,7 +181,113 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) batch_sample_kernel(const Samp
     sample_row<PER>(p);
 }
 
+// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams).
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const GenStepParams gp) {
+    pdl_prologue();
+    __shared__ int draw, park;
+    const int b = blockIdx.x, tid = threadIdx.x, V = gp.n_vocab;
+    const size_t off = (size_t) b * V;
+    GenRow * r = gp.rows + b;
+    GenShared * sh = gp.shared;
+    if (tid == 0) {
+        const bool budget = !r->frozen && r->step == r->max_tokens;
+        if (budget) r->frozen = 1;
+        draw = !r->frozen;
+        park = budget;
+    }
+    __syncthreads();
+    uint32_t tok = 0;
+    if (draw) {
+        const uint32_t step = r->step;
+        const float presence = r->presence, frequency = r->frequency;
+        for (int i = tid; i < V; i += SAMPLE_THREADS) {      // chat_with_bot.py:244-247, as a bias list over every token
+            const uint32_t c = gp.counts[off + i];
+            gp.bias_ids[off + i] = c ? (uint32_t) i : (uint32_t) V;
+            gp.bias_values[off + i] = -__fadd_rn(presence, __fmul_rn((float) c, frequency));
+        }
+        __syncthreads();
+        SampleParams p;
+        p.logits = gp.logits + off; p.n_vocab = V;
+        p.temperature = r->temperature; p.top_p = r->top_p; p.u = gp.u[(size_t) b * sh->stride + step];
+        p.bias_ids = gp.bias_ids + off; p.bias_values = gp.bias_values + off; p.n_bias = V;
+        p.scratch = gp.scratch + off; p.token_out = gp.tokens + (size_t) b * sh->stride + step; p.prob_out = nullptr;
+        sample_row<PER>(p);
+        __syncthreads();
+        if (tid == 0) {
+            tok = *(volatile uint32_t *) p.token_out;
+            r->step = step + 1;
+            bool stop = false;
+            for (uint32_t k = 0; k < sh->n_stop; k++) stop = stop || sh->stop[k] == tok;
+            if (stop) { r->frozen = 1; park = 1; }      // reported, not evaluated, not counted (chat_with_bot.py:249-252)
+            else gp.counts[off + tok] += 1;
+        }
+        __syncthreads();
+    }
+    if (park && gp.park)
+        for (int i = tid; i < V; i += SAMPLE_THREADS) gp.park[off + i] = gp.logits[off + i];
+    if (tid == 0) {
+        const bool active = !r->frozen;
+        gp.n_generated[b] = r->step;
+        gp.next_tokens[b] = active ? (int) tok : 0;
+        if (active) atomicAdd(&sh->active, 1u);
+        __threadfence();
+        if (atomicAdd(&sh->ticket, 1u) == (uint32_t) gridDim.x - 1) {       // the last CTA of the step
+            const uint32_t any = atomicAdd(&sh->active, 0u);
+            sh->active = 0; sh->ticket = 0;
+            if (any) *gp.passes += 1;
+            if (gp.set_handles) {
+                cudaGraphSetConditional(gp.run_pass, any ? 1u : 0u);
+                cudaGraphSetConditional(gp.keep_going, any ? 1u : 0u);
+            }
+        }
+    }
+}
+
+constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
+
+__global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const GenRow * rows, const float * src, float * dst, long long seq_stride, size_t n) {
+    pdl_prologue();
+    const int b = blockIdx.y;
+    if (!rows[b].frozen) return;
+    const size_t base = (size_t) b * (size_t) seq_stride;
+    for (size_t i = (size_t) blockIdx.x * RESTORE_THREADS + threadIdx.x; i < n; i += (size_t) gridDim.x * RESTORE_THREADS) dst[base + i] = src[base + i];
+}
+
+template <int PER> void * generate_step_fn() { return reinterpret_cast<void *>(generate_sample_kernel<PER>); }
+void * generate_step_for(int n_vocab) {
+    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    return per <= 1 ? generate_step_fn<1>() : per <= 4 ? generate_step_fn<4>() : per <= 16 ? generate_step_fn<16>() : per <= 50 ? generate_step_fn<50>()
+                                                                                                                            : generate_step_fn<64>();
+}
+
 }  // namespace
+
+cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s) {
+    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    const dim3 grid(p.n_rows);
+    if (per <= 1) return launch_pdl(generate_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 4) return launch_pdl(generate_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 16) return launch_pdl(generate_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 50) return launch_pdl(generate_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return launch_pdl(generate_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+}
+
+cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node) {
+    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    GenStepParams arg = p;
+    void * args[] = {&arg};
+    cudaKernelNodeParams kp = {};
+    kp.func = generate_step_for(p.n_vocab);
+    kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
+    kp.kernelParams = args; kp.extra = nullptr;
+    return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
+}
+
+cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {
+    return launch_pdl(restore_frozen_kernel, dim3(RESTORE_BLOCKS_PER_ROW, n_rows), dim3(RESTORE_THREADS), 0, s, rows, src, dst, seq_stride, state_len);
+}
 
 cudaError_t launch_sample(const SampleParams & p, cudaStream_t s) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64) return cudaErrorInvalidValue;

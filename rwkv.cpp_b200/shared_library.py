@@ -170,6 +170,14 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_sample_logits_batch.argtypes = [P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, P_FLOAT, P_FLOAT, P_DOUBLE, P_U32, P_U32, P_FLOAT,
                                                       P_U32, P_FLOAT]
         lib.rwkv_b200_sample_logits_batch.restype = ctypes.c_bool
+        lib.rwkv_b200_generate.argtypes = [vp, ctypes.c_size_t, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_bool, P_DOUBLE,
+                                           P_U32, ctypes.c_size_t, P_U32, ctypes.POINTER(ctypes.c_size_t)]
+        lib.rwkv_b200_generate.restype = ctypes.c_bool
+        P_U8 = ctypes.POINTER(ctypes.c_uint8)
+        lib.rwkv_b200_batch_generate.argtypes = [vp, P_U32, P_FLOAT, P_FLOAT, P_FLOAT, P_FLOAT, P_U8, P_DOUBLE, P_U32, ctypes.c_size_t, P_U32, P_U32]
+        lib.rwkv_b200_batch_generate.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step.argtypes = [ctypes.c_void_p]
+        lib.rwkv_b200_test_generate_step.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
