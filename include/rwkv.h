@@ -13,10 +13,12 @@
  *   - a missing / unusable CUDA device makes rwkv_init_from_file return NULL with
  *     RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED -- there is no host execution path;
  *   - rwkv_get_system_info_string describes the CUDA device instead of CPU features;
- *   - tensor data types: FP32, FP16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 -- the formats rwkv.h:212-217 documents. The reference's
- *     type table (rwkv_file_format.inc:28-47) also lets ggml's Q8_1 / K-quant ids (10..16) through; a file that contains
- *     such a tensor is refused by rwkv_init_from_file with RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_UNSUPPORTED, and
- *     rwkv_quantize_model_file refuses those format names with RWKV_ERROR_ARGS | RWKV_ERROR_DATA_TYPE.
+ *   - tensor data types: FP32, FP16, Q4_0, Q4_1, Q4_K, Q5_0, Q5_1, Q5_K, Q8_0 -- the formats the reference's Python binding
+ *     offers. The reference's type table (rwkv_file_format.inc:28-47) also lets ggml's Q8_1, Q2_K, Q3_K, Q6_K and Q8_K ids
+ *     (10, 11, 12, 15, 16) through; a file that contains such a tensor is refused by rwkv_init_from_file with
+ *     RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_UNSUPPORTED, and rwkv_quantize_model_file refuses those format names with
+ *     RWKV_ERROR_ARGS | RWKV_ERROR_DATA_TYPE. The same load error covers a Q4_K / Q5_K emb.weight or head.weight and a Q4_K /
+ *     Q5_K tensor whose rows are not multiples of 256 weights.
  */
 #ifndef RWKV_H
 #define RWKV_H
@@ -92,7 +94,7 @@ RWKV_API bool rwkv_get_print_errors(const struct rwkv_context * ctx);
 RWKV_API enum rwkv_error_flags rwkv_get_last_error(struct rwkv_context * ctx);
 
 /* replaces rwkv.h:91 (rwkv.cpp:71). Reads a ggml-format RWKV file (v4/v5.1/v5.2/v6/v7; FP32, FP16,
- * Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 per tensor), uploads every tensor to HBM. NULL on error. */
+ * Q4_0, Q4_1, Q4_K, Q5_0, Q5_1, Q5_K, Q8_0 per tensor), uploads every tensor to HBM. NULL on error. */
 RWKV_API struct rwkv_context * rwkv_init_from_file(const char * model_file_path, const uint32_t n_threads, const uint32_t n_gpu_layers);
 
 /* replaces rwkv.h:99 (rwkv.cpp:123). New stream/arena/state over the same weights (atomic refcount). */
@@ -132,7 +134,8 @@ RWKV_API void rwkv_init_state(const struct rwkv_context * ctx, float * state);
 RWKV_API void rwkv_free(struct rwkv_context * ctx);
 
 /* replaces rwkv.h:218 (rwkv_quantize.inc:16). Host-side, bit-identical to ggml's quantize_row_*_ref
- * (ggml-quants.c:31-217). format_name in {Q4_0, Q4_1, Q5_0, Q5_1, Q8_0}. */
+ * (ggml-quants.c:31-217, 1208-1480). format_name in {Q4_0, Q4_1, Q4_K, Q5_0, Q5_1, Q5_K, Q8_0}. A Q4_K / Q5_K tensor whose rows
+ * are not multiples of 256 weights is written as Q5_0 / Q5_1 (the reference writes super-blocks that straddle rows there). */
 RWKV_API bool rwkv_quantize_model_file(const char * model_file_path_in, const char * model_file_path_out, const char * format_name);
 
 /* replaces rwkv.h:221 (rwkv.cpp:239). Static storage. */

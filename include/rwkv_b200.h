@@ -378,8 +378,9 @@ struct rwkv_b200_gemv_problem {
     float * y;
 };
 /* One kernel launch: family 0 streaming GEMV, 1 generic GEMV, 2 tensor-core GEMM, 3 fp16 operand conversion, 4 tensor-core weight
- * expansion (of the upload). nc: columns per group (streaming, generic) or distinct inputs (conversion); only: the streaming
- * kernel's single weight type (-1: mixed) or the expanded type; has_ln: the streaming kernel's LayerNorm code; npad: tokens padded
+ * expansion (of the upload), 5 Q4_K / Q5_K streaming GEMV, 6 Q4_K / Q5_K tensor-core weight expansion; a conversion of
+ * Q8_K operands (K-quant weights) reports only = 16. nc: columns per group (streaming, generic, K-quant) or distinct inputs
+ * (conversion); only: the streaming kernel's single weight type (-1: mixed), the expanded type or the K-quant type; has_ln: the streaming kernel's LayerNorm code; npad: tokens padded
  * to 16; cluster: CTAs per cluster of the GEMM. */
 struct rwkv_b200_gemv_launch { int family, nc, only, has_ln, npad, cluster; };
 struct rwkv_b200_gemv_batch_args {

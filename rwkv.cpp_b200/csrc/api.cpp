@@ -781,7 +781,7 @@ int rwkv_b200_trace_read(struct rwkv_context * ctx, double * start_us, double * 
 bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, const float * x, float * y, int epilogue) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, weights && x && y && K > 0 && M > 0 && T > 0 && dtype_supported(data_type) && K % dtype_block_elems(data_type) == 0 && epilogue >= 0 && epilogue <= EPI_RELU_SQR,
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, weights && x && y && K > 0 && M > 0 && T > 0 && dtype_loadable(data_type) && K % dtype_block_elems(data_type) == 0 && epilogue >= 0 && epilogue <= EPI_RELU_SQR,
                "Invalid matvec arguments");
     int dev = default_device(), n_dev = 0;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceCount(&n_dev) == cudaSuccess && dev < n_dev && cudaSetDevice(dev) == cudaSuccess,
@@ -1054,7 +1054,7 @@ bool rwkv_b200_test_wkv7_ragged(const struct rwkv_b200_wkv7_args * a, const uint
 static GemvProblem fold_problem(int type, int K, int M, int epi) {
     GemvProblem p{};
     p.type = type; p.K = K; p.M = M; p.epi = epi; p.ldx = K; p.ldy = M;
-    p.pitch = dtype_supported(type) && K > 0 && K % dtype_block_elems(type) == 0 ? matrix_pitch(type, (uint64_t) K) : 0;
+    p.pitch = dtype_loadable(type) && K > 0 && K % dtype_block_elems(type) == 0 ? matrix_pitch(type, (uint64_t) K) : 0;
     return p;
 }
 
@@ -1124,7 +1124,7 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
     for (int i = 0; args && i < a->n; i++) {
         const rwkv_b200_gemv_problem & q = a->p[i];
         const bool ln = q.pro == PRO_LAYERNORM, res_epi = q.epi == EPI_ADD || q.epi == EPI_MUL_ADD, bias_epi = q.epi >= EPI_BIAS_EXPNEGEXP;
-        args = q.weights && q.y && dtype_supported(q.type) && q.K > 0 && q.M > 0 && q.K % dtype_block_elems(q.type) == 0 &&
+        args = q.weights && q.y && dtype_loadable(q.type) && q.K > 0 && q.M > 0 && q.K % dtype_block_elems(q.type) == 0 &&
                q.input >= 0 && q.input < GEMV_MAX_PROBLEMS && a->x[q.input] && (input_K[q.input] == 0 || input_K[q.input] == q.K) &&
                q.epi >= EPI_NONE && q.epi <= EPI_BIAS_W7 && (q.pro == PRO_NONE || ln) &&
                !q.res == !res_epi && !q.gate == (q.epi != EPI_MUL_ADD) && !q.bias == !bias_epi && (!q.y_aliases_res || q.res) &&
@@ -1132,6 +1132,8 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
                (!q.xq || (a->T == 1 && act::stage_class(q.type) != act::SC_NONE)) &&   // the streaming kernel reads xq of single-token launches only
                (!q.tiled || gemm_tc_eligible(q.type, q.K));
         if (args) input_K[q.input] = q.K;
+        // the streaming path runs one kernel: all problems K-quant of one type (gemv_kq_launch) or none (gemv_tma_launch)
+        if (args && a->path == RWKV_B200_GEMV_STREAMING) args = dtype_kquant(q.type) ? q.type == a->p[0].type : !dtype_kquant(a->p[0].type);
     }
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid gemv_batch arguments");
     if (!hook_device(sink)) return false;
@@ -1186,7 +1188,7 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
     cudaError_t e = cudaSuccess;
     if (b.ok) {
         switch (a->path) {
-            case RWKV_B200_GEMV_STREAMING: e = gemv_tma_launch(batch, di, 0); break;
+            case RWKV_B200_GEMV_STREAMING: e = dtype_kquant(batch.p[0].type) ? gemv_kq_launch(batch, di, 0) : gemv_tma_launch(batch, di, 0); break;
             case RWKV_B200_GEMV_GENERIC: e = gemv_generic_launch(batch, di, 0); break;
             case RWKV_B200_GEMV_TENSOR_CORES: e = gemm_tc_launch(batch, di, 0, ws, ws_bytes); break;
             default: e = gemv_route(batch, di, 0, ws, ws_bytes, a->path == RWKV_B200_GEMV_ENGINE ? 32 : 16); break;

@@ -1,6 +1,7 @@
 // Tensor data types and quant-block geometry of the rwkv.cpp ggml file format.
 // Type ids are the on-disk ids (reference rwkv_file_format.inc:5-24); block layouts are
-// ggml's (ggml/src/ggml-common.h:161-221): 32 weights per block along the input dimension.
+// ggml's (ggml/src/ggml-common.h:161-221): 32 weights per block along the input dimension,
+// 256 per super-block for the K-quants Q4_K / Q5_K (ggml-common.h:296-322).
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -19,14 +20,32 @@ enum DType : int32_t {
 inline bool dtype_supported(int t) {
     return t == DT_F32 || t == DT_F16 || t == DT_Q4_0 || t == DT_Q4_1 || t == DT_Q5_0 || t == DT_Q5_1 || t == DT_Q8_0;
 }
+// Q4_K / Q5_K: matrices only, streamed by their own GEMV (kernels/gemv_kquant.cu). dtype_supported() stays the set of types every
+// legacy-block kernel handles.
+inline bool dtype_kquant(int t) { return t == DT_Q4_K || t == DT_Q5_K; }
+inline bool dtype_loadable(int t) { return dtype_supported(t) || dtype_kquant(t); }
 inline bool dtype_quantized(int t) { return t >= DT_Q4_0 && t != DT_COUNT; }
-inline int dtype_block_elems(int t) { return (t == DT_F32 || t == DT_F16) ? 1 : 32; }
+constexpr int QK_K = 256;
+inline int dtype_block_elems(int t) { return (t == DT_F32 || t == DT_F16) ? 1 : (dtype_kquant(t) ? QK_K : 32); }
 inline int dtype_block_bytes(int t) {
     switch (t) {
         case DT_F32: return 4;  case DT_F16: return 2;
         case DT_Q4_0: return 18; case DT_Q4_1: return 20; case DT_Q5_0: return 22; case DT_Q5_1: return 24; case DT_Q8_0: return 34;
+        case DT_Q4_K: return 144;   // d, dmin (fp16), scales[12] (6-bit scale and min of 8 sub-blocks), qs[128]
+        case DT_Q5_K: return 176;   // d, dmin, scales[12], qh[32] (fifth bits), qs[128]
         default: return 0;
     }
+}
+#if defined(__CUDACC__)
+#define RWKV_FORMATS_HD __host__ __device__
+#else
+#define RWKV_FORMATS_HD
+#endif
+// 6-bit scale and min of sub-block j (32 weights) of a Q4_K / Q5_K super-block, from its packed scales[12] (ggml's get_scale_min_k4).
+// Shared by the host widening, the quantizer and the kernels.
+RWKV_FORMATS_HD inline void kquant_scale_min(const uint8_t * q, int j, int & sc, int & m) {
+    if (j < 4) { sc = q[j] & 63; m = q[j + 4] & 63; }
+    else { sc = (q[j + 4] & 0xF) | ((q[j - 4] >> 6) << 4); m = (q[j + 4] >> 4) | ((q[j] >> 6) << 4); }
 }
 inline const char * dtype_name(int t) {
     static const char * names[DT_COUNT + 1] = {"FP32", "FP16", "Q4_0", "Q4_1", "Q4_1_O", "Q4_2", "Q4_3", "Q5_0", "Q5_1", "Q8_0",

@@ -41,10 +41,18 @@ bool read_tensor_info(FILE * f, TensorInfo & t, ErrorSink sink) {
     RWKV_CHECK(sink, RWKV_ERROR_FILE_READ, false, key_length < (1u << 20), "Implausible tensor name length %" PRIu32, key_length);
     t.name.resize(key_length);
     RWKV_CHECK(sink, RWKV_ERROR_FILE_READ, false, key_length == 0 || fread(&t.name[0], key_length, 1, f) == 1, "Failed to read tensor name");
-    // The reference accepts the K-quant / Q8_1 ids in its table (rwkv_file_format.inc:28-47) but rwkv.h:212-217
-    // documents only the five formats below plus FP16/FP32; this engine has kernels for exactly those.
-    RWKV_CHECK(sink, RWKV_ERROR_UNSUPPORTED, false, dtype_supported((int) t.data_type), "Unsupported data type %s in parameter %s",
+    // The reference accepts every K-quant / Q8_1 id in its table (rwkv_file_format.inc:28-47); its Python binding offers Q4_K and
+    // Q5_K next to the five legacy formats, and this engine has kernels for exactly those plus FP16 / FP32.
+    RWKV_CHECK(sink, RWKV_ERROR_UNSUPPORTED, false, dtype_loadable((int) t.data_type), "Unsupported data type %s in parameter %s",
                dtype_name((int) t.data_type), t.name.c_str());
+    if (dtype_kquant((int) t.data_type)) {
+        // ggml's K-quant rows are whole 256-weight super-blocks; a shorter row has no defined meaning
+        RWKV_CHECK(sink, RWKV_ERROR_UNSUPPORTED, false, t.ne[0] % QK_K == 0,
+                   "Row length %" PRIu64 " of %s is not a multiple of %d, which %s needs; requantize the model with this library's quantizer",
+                   t.ne[0], t.name.c_str(), QK_K, dtype_name((int) t.data_type));
+        RWKV_CHECK(sink, RWKV_ERROR_UNSUPPORTED, false, t.name != "emb.weight" && t.name != "head.weight",
+                   "%s in %s is not supported (the quantizer keeps it in FP16); requantize the model", t.name.c_str(), dtype_name((int) t.data_type));
+    }
     RWKV_CHECK(sink, RWKV_ERROR_SHAPE, false, t.ne[0] % dtype_block_elems((int) t.data_type) == 0,
                "Row length %" PRIu64 " of %s is not a multiple of the %s block size", t.ne[0], t.name.c_str(), dtype_name((int) t.data_type));
     t.nbytes = tensor_nbytes((int) t.data_type, t.ne[0], t.ne[1], t.ne[2]);

@@ -623,9 +623,116 @@ __global__ void __launch_bounds__(TILE_M) tc_expand_kernel(const uint8_t * src, 
     for (int kc = 0; kc < 8; kc++) blk[(kc * (TILE_M / 8) + (r >> 3)) * 8 + (r & 7)] = h[kc];
 }
 
+// Q4_K / Q5_K rows -> the same fp16 operand blocks. A K-step (64 weights) is sub-blocks 2j and 2j + 1 of super-block ks / 4,
+// j = ks % 4: the low and the high nibbles of qs[32j .. 32j + 32). Thread r expands row r: w = d*sc*q - dmin*m, where d*sc, dmin*m
+// and d*sc*q are exact in fp32, so the fp16 conversion of the difference is the one rounding.
+template <int TYPE>
+__global__ void __launch_bounds__(TILE_M) tc_expand_kq_kernel(const uint8_t * src, long long pitch, int M, int nsteps, uint4 * dst) {
+    constexpr int BB = TYPE == DT_Q4_K ? 144 : 176, QS = TYPE == DT_Q4_K ? 16 : 48;
+    const int ks = blockIdx.x, tile = blockIdx.y, r = threadIdx.x, row = tile * TILE_M + r, j = ks & 3;
+    uint4 h[8];
+    if (row < M) {
+        const uint8_t * blk = src + (long long) row * pitch + (long long) (ks >> 2) * BB;
+        const float d = __half2float(__ushort_as_half(*reinterpret_cast<const unsigned short *>(blk)));
+        const float dmin = __half2float(__ushort_as_half(*reinterpret_cast<const unsigned short *>(blk + 2)));
+        float a[2], b[2];
+        for (int hi = 0; hi < 2; hi++) {
+            int sc, mn;
+            kquant_scale_min(blk + 4, 2 * j + hi, sc, mn);
+            a[hi] = d * (float) sc;
+            b[hi] = dmin * (float) mn;
+        }
+        const uint8_t * qs = blk + QS + 32 * j;
+#pragma unroll
+        for (int kc = 0; kc < 8; kc++) {
+            const int hi = kc >> 2;
+            __half v[8];
+#pragma unroll
+            for (int e = 0; e < 8; e++) {
+                const int l = (kc & 3) * 8 + e;
+                int q = (qs[l] >> (4 * hi)) & 0xF;
+                if (TYPE == DT_Q5_K) q |= ((blk[16 + l] >> (2 * j + hi)) & 1) << 4;
+                v[e] = __float2half_rn(__fsub_rn(__fmul_rn(a[hi], (float) q), b[hi]));
+            }
+            h[kc] = *reinterpret_cast<const uint4 *>(v);
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 8; i++) h[i] = make_uint4(0, 0, 0, 0);
+    }
+    uint4 * out = dst + ((size_t) tile * nsteps + ks) * (A_BYTES / 16);
+#pragma unroll
+    for (int kc = 0; kc < 8; kc++) out[(kc * (TILE_M / 8) + (r >> 3)) * 8 + (r & 7)] = h[kc];
+}
+
+// The B operand of K-quant weights: the Q8_K block values q * d the reference multiplies them with (quantize_row_q8_K_ref: d =
+// 1 / (-127 / max) in float32, max the first element of largest magnitude, q = min(127, rint(-127 / max * x))), with the same
+// power-of-two column scale as convert_f16_kernel. A separate kernel, so that convert_f16_kernel's code stays as it is. One CTA =
+// one token column of one input; one warp per super-block, 8 elements per lane (one 16-byte chunk of the canonical layout).
+__global__ void __launch_bounds__(CVT_THREADS) convert_q8k_kernel(const ConvertBatch cb) {
+    __shared__ float red[CVT_THREADS / 32];
+    trace_begin(cb.trace);
+    pdl_prologue();
+    const int q = blockIdx.y, t = blockIdx.x, T = cb.T, npad = cb.npad, K = cb.K[q];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint4 * out = reinterpret_cast<uint4 *>(cb.out[q]);
+    const int NG = npad / 8, g = t >> 3, t8 = t & 7;
+    if (t >= T) {
+        for (int c = tid; c < K / 8; c += CVT_THREADS) out[((size_t) c * NG + g) * 8 + t8] = make_uint4(0, 0, 0, 0);
+        if (tid == 0) cb.colscale[q][t] = 1.0f;
+        return;
+    }
+    const float * x = cb.x[q] + (long long) t * cb.ldx[q];
+    const float4 * x4 = reinterpret_cast<const float4 *>(x);
+    float cmax = 0.f;
+    for (int i = tid; i < K / 4; i += CVT_THREADS) {
+        const float4 v = x4[i];
+        cmax = fmaxf(cmax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(0xffffffffu, cmax, o));
+    if (lane == 0) red[warp] = cmax;
+    __syncthreads();
+    cmax = red[0];
+#pragma unroll
+    for (int i = 1; i < CVT_THREADS / 32; i++) cmax = fmaxf(cmax, red[i]);
+    int ex = 0;
+    if (cmax > 32768.0f && cmax <= 3.0e38f) { (void) frexpf(cmax, &ex); ex -= 15; }
+    const float down = ex > 0 ? exp2f((float) -ex) : 1.0f;
+    if (tid == 0) cb.colscale[q][t] = ex > 0 ? exp2f((float) ex) : 1.0f;
+    for (int s = warp; s < K / QK_K; s += CVT_THREADS / 32) {
+        const float4 a = x4[s * 64 + lane * 2], b = x4[s * 64 + lane * 2 + 1];
+        const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        float amax = 0.f, mx = 0.f;
+        int idx = QK_K;
+#pragma unroll
+        for (int e = 0; e < 8; e++) if (fabsf(v[e]) > amax) { amax = fabsf(v[e]); mx = v[e]; idx = lane * 8 + e; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float oa = __shfl_xor_sync(0xffffffffu, amax, o), om = __shfl_xor_sync(0xffffffffu, mx, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+            if (oa > amax || (oa == amax && oi < idx)) { amax = oa; mx = om; idx = oi; }
+        }
+        __half hv[8];
+        if (amax != 0.f) {
+            const float iscale = __fdiv_rn(-127.f, mx), d = __fmul_rn(__fdiv_rn(1.f, iscale), down);
+#pragma unroll
+            for (int e = 0; e < 8; e++) hv[e] = __float2half_rn(__fmul_rn((float) min(127, __float2int_rn(__fmul_rn(iscale, v[e]))), d));
+        } else {
+#pragma unroll
+            for (int e = 0; e < 8; e++) hv[e] = __float2half_rn(0.f);
+        }
+        out[((size_t) (s * 32 + lane) * NG + g) * 8 + t8] = *reinterpret_cast<const uint4 *>(hv);
+    }
+    trace_end(cb.trace);
+}
+
 }  // namespace tc
 
-bool gemm_tc_eligible(int type, int K) { return type != DT_F32 && K % tc::KSTEP == 0 && K >= tc::KSTEP; }
+// K-quant matrices need whole super-blocks (the loader guarantees them); a K-step never straddles one.
+bool gemm_tc_eligible(int type, int K) {
+    return type != DT_F32 && K % tc::KSTEP == 0 && K >= tc::KSTEP && (!dtype_kquant(type) || K % QK_K == 0);
+}
 
 size_t gemm_tc_tiled_bytes(int type, int M, int K) {
     if (!gemm_tc_eligible(type, K)) return 0;
@@ -639,6 +746,12 @@ cudaError_t gemm_tc_repack(const void * W, long long pitch, int type, int M, int
     const dim3 grid((unsigned) nsteps, (unsigned) ntiles);
     const uint8_t * src = reinterpret_cast<const uint8_t *>(W);
     uint4 * out = reinterpret_cast<uint4 *>(dst);
+    if (dtype_kquant(type)) {
+        log_launch(LF_KQ_EXPAND, 0, type, 0, 0, 0);
+        if (type == DT_Q4_K) tc::tc_expand_kq_kernel<DT_Q4_K><<<grid, tc::TILE_M, 0, stream>>>(src, pitch, M, nsteps, out);
+        else tc::tc_expand_kq_kernel<DT_Q5_K><<<grid, tc::TILE_M, 0, stream>>>(src, pitch, M, nsteps, out);
+        return cudaGetLastError();
+    }
     log_launch(LF_EXPAND, 0, type, 0, 0, 0);
     switch (type) {
         case DT_Q4_0: tc::tc_expand_kernel<DT_Q4_0><<<grid, tc::TILE_M, 0, stream>>>(src, pitch, M, nsteps, out); break;
@@ -673,30 +786,35 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
 
     uint8_t * scratch = reinterpret_cast<uint8_t *>(workspace);
     size_t used = 0;
-    tc::ConvertBatch cvt;
+    // operand kinds: fp16(x) for F16 weights, Q8_0 / Q8_1 block values for the legacy formats (both convert_f16_kernel), Q8_K block
+    // values for K-quant weights (convert_q8k_kernel)
+    tc::ConvertBatch cvt, cvk;
     memset(&cvt, 0, sizeof(cvt));
-    cvt.T = batch.T; cvt.npad = tb.npad;
+    memset(&cvk, 0, sizeof(cvk));
+    cvt.T = cvk.T = batch.T; cvt.npad = cvk.npad = tb.npad;
+    auto kind = [](int type) { return type == DT_F16 ? 0 : (dtype_kquant(type) ? 2 : 1); };
     int share_of[GEMV_MAX_PROBLEMS];
     for (int i = 0; i < batch.n; i++) {
         GemvProblem & p = batch.p[i];
-        const int quant = p.type != DT_F16;
+        const int k = kind(p.type);
+        tc::ConvertBatch & cb = k == 2 ? cvk : cvt;
         const size_t need = (((size_t) tb.npad * p.K * sizeof(__half) + 255) & ~(size_t) 255) + (((size_t) tb.npad * sizeof(float) + 255) & ~(size_t) 255);
         // problems that share an input (and its operand kind) share the converted copy
         int shared = -1;
         for (int j = 0; j < i; j++)
-            if (batch.p[j].x == p.x && batch.p[j].K == p.K && batch.p[j].ldx == p.ldx && (batch.p[j].type != DT_F16) == (quant != 0)) shared = share_of[j];
+            if (batch.p[j].x == p.x && batch.p[j].K == p.K && batch.p[j].ldx == p.ldx && kind(batch.p[j].type) == k) shared = share_of[j];
         if (shared < 0) {
             if (used + need > workspace_bytes) return cudaErrorMemoryAllocation;
-            shared = cvt.n;
-            cvt.x[cvt.n] = p.x; cvt.ldx[cvt.n] = p.ldx; cvt.K[cvt.n] = p.K; cvt.quant[cvt.n] = quant;
-            cvt.out[cvt.n] = reinterpret_cast<__half *>(scratch + used);
-            cvt.colscale[cvt.n] = reinterpret_cast<float *>(scratch + used + (((size_t) tb.npad * p.K * sizeof(__half) + 255) & ~(size_t) 255));
-            cvt.n++;
+            shared = cb.n;
+            cb.x[cb.n] = p.x; cb.ldx[cb.n] = p.ldx; cb.K[cb.n] = p.K; cb.quant[cb.n] = k != 0;
+            cb.out[cb.n] = reinterpret_cast<__half *>(scratch + used);
+            cb.colscale[cb.n] = reinterpret_cast<float *>(scratch + used + (((size_t) tb.npad * p.K * sizeof(__half) + 255) & ~(size_t) 255));
+            cb.n++;
             used += need;
         }
         share_of[i] = shared;
-        tb.act16[i] = cvt.out[shared];
-        tb.colscale[i] = cvt.colscale[shared];
+        tb.act16[i] = cb.out[shared];
+        tb.colscale[i] = cb.colscale[shared];
     }
     // ---- work decomposition: one CTA per (row tile, K-split). Every CTA streams its share of the weights from HBM, so what matters
     // is that close to all SMs have a CTA: launches with few tiles (4096-row matrices: 32; LoRA: 1-2) are cut along K over clusters
@@ -727,10 +845,16 @@ cudaError_t gemm_tc_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream
         next += p.n_cta;
         tb.p[i] = p;
     }
-    {   // every distinct input of the batch -> fp16 canonical layout, one launch: one CTA per (token column, input)
+    if (cvt.n) {   // every distinct input of the batch -> fp16 canonical layout, one launch: one CTA per (token column, input)
         cvt.trace = trace_slot("convert_f16");
         log_launch(LF_CONVERT, cvt.n, 0, 0, tb.npad, 0);
         cudaError_t e = launch_pdl(tc::convert_f16_kernel, dim3(tb.npad, cvt.n), dim3(tc::CVT_THREADS), 0, stream, cvt);
+        if (e != cudaSuccess) return e;
+    }
+    if (cvk.n) {
+        cvk.trace = trace_slot("convert_q8k");
+        log_launch(LF_CONVERT, cvk.n, DT_Q8_K, 0, tb.npad, 0);
+        cudaError_t e = launch_pdl(tc::convert_q8k_kernel, dim3(tb.npad, cvk.n), dim3(tc::CVT_THREADS), 0, stream, cvk);
         if (e != cudaSuccess) return e;
     }
     // shared memory: as many [A | B] ring stages as fit, at most 8

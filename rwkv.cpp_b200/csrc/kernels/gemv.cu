@@ -338,6 +338,24 @@ cudaError_t weights_to_device_layout(void * W, long long pitch, int type, int M,
 
 cudaError_t gemv_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream) {
     if (batch.n <= 0 || batch.T <= 0) return cudaSuccess;
+    bool any_kq = false;
+    for (int i = 0; i < batch.n; i++) any_kq = any_kq || dtype_kquant(batch.p[i].type);
+    if (any_kq) {
+        // one launch per K-quant type present and one for the rest: a v7 layer keeps its LoRA matrices in FP16, a v6 layer's decay
+        // LoRA falls back to a legacy format, so mixed batches are the common case
+        GemvBatch part[3];
+        for (GemvBatch & b : part) { memset(&b, 0, sizeof(b)); b.T = batch.T; }
+        for (int i = 0; i < batch.n; i++) {
+            const int t = batch.p[i].type;
+            GemvBatch & b = part[t == DT_Q4_K ? 0 : (t == DT_Q5_K ? 1 : 2)];
+            b.p[b.n++] = batch.p[i];
+        }
+        for (int k = 0; k < 2; k++) if (part[k].n) {
+            const cudaError_t e = gemv_kq_launch(part[k], dev, stream);
+            if (e != cudaSuccess) return e;
+        }
+        return gemv_launch(part[2], dev, stream);
+    }
     const cudaError_t e = gemv_tma_launch(batch, dev, stream);
     if (e != cudaErrorNotSupported) return e;
     return gemv_generic_launch(batch, dev, stream);
@@ -360,6 +378,7 @@ cudaError_t gemv_route(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t s
 }
 
 cudaError_t gemv_generic_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream) {
+    for (int i = 0; i < batch.n; i++) if (dtype_kquant(batch.p[i].type)) return cudaErrorNotSupported;   // gemv_kq_launch only
     batch.trace = trace_slot("gemv_generic");
     // CTA budget split over the problems in proportion to their weight bytes.
     const int total_ctas = dev.num_sms * CTAS_PER_SM;

@@ -80,6 +80,12 @@ cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStrea
 // The streaming kernel's row plan of p (p.wk, p.g), a function of (type, K, pitch) alone; false if the shape needs the generic kernel.
 bool gemv_tma_plan(GemvProblem & p);
 cudaError_t gemv_generic_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);
+// Q4_K / Q5_K matrices (gemv_kquant.cu): the only kernel that takes them; every problem of `batch` has the same K-quant type and no
+// prologue. gemv_kq_fits: whether rows of K weights fit its streaming plan (the loader refuses a matrix that does not).
+bool gemv_kq_fits(int type, int K);
+cudaError_t gemv_kq_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStream_t stream);
+// Tile height and CTA share of every problem of a streaming launch (gemv_tma.cu), shared by both streaming kernels.
+int assign_tiles_and_ctas(GemvBatch & batch, int total_ctas, long long stage_bytes);
 
 // Brings a freshly uploaded matrix (file bytes, rows `pitch` bytes apart) into the device layout of quant_decode.cuh, in place: the
 // fifth-bit word of every Q5_0 / Q5_1 block is bit-transposed (qh5_to_device); every other type is left as it is. Must run before any
@@ -114,11 +120,11 @@ extern std::atomic<unsigned long long> g_kernel_launches;
 // Which instantiation of the matrix kernels a launch ran, recorded while a log is attached to the calling thread (the GEMV test hook
 // attaches one, so its tests can assert the kernel they reached instead of assuming it). Fields that do not apply to a family are 0,
 // except `only`, -1 where a kernel serves every format.
-enum LaunchFamily : int { LF_STREAMING = 0, LF_GENERIC = 1, LF_TENSOR_CORES = 2, LF_CONVERT = 3, LF_EXPAND = 4 };
+enum LaunchFamily : int { LF_STREAMING = 0, LF_GENERIC = 1, LF_TENSOR_CORES = 2, LF_CONVERT = 3, LF_EXPAND = 4, LF_KQ_STREAMING = 5, LF_KQ_EXPAND = 6 };
 struct LaunchRec {
     int family;
-    int nc;        // streaming / generic: columns per group (NC); convert: distinct inputs
-    int only;      // streaming: ONLY (-1 = mixed formats); expand: the weight type
+    int nc;        // streaming / generic / K-quant streaming: columns per group (NC); convert: distinct inputs
+    int only;      // streaming: ONLY (-1 = mixed formats); expand, K-quant streaming / expand: the weight type; convert: 16 (Q8_K) or 0
     int has_ln;    // streaming: HAS_LN
     int npad;      // tensor cores / convert: tokens padded to 16
     int cluster;   // tensor cores: CTAs per cluster

@@ -195,7 +195,7 @@ cudaError_t launch_tma_single(const GemvBatch & batch, int grid, size_t smem, cu
 
 // Tile height and CTA share of every problem for ring stages of `stage_bytes`: CTAs are split over the problems by weight
 // bytes (largest remainders get the leftovers). Returns the number of CTAs used (<= total_ctas).
-static int assign_tiles_and_ctas(GemvBatch & batch, int total_ctas, long long stage_bytes) {
+int assign_tiles_and_ctas(GemvBatch & batch, int total_ctas, long long stage_bytes) {
     using namespace tma;
     double total_bytes = 0;
     for (int i = 0; i < batch.n; i++) total_bytes += (double) batch.p[i].M * (double) batch.p[i].pitch;
@@ -241,7 +241,7 @@ cudaError_t gemv_tma_launch(GemvBatch & batch, const DeviceInfo & dev, cudaStrea
     size_t max_col = 0;
     for (int i = 0; i < batch.n; i++) {
         GemvProblem & p = batch.p[i];
-        if (!plan_wk(p)) return cudaErrorNotSupported;
+        if (dtype_kquant(p.type) || !plan_wk(p)) return cudaErrorNotSupported;
         const size_t cb = act_bytes_per_column(p.type, p.K);
         if (cb > max_col) max_col = cb;
     }

@@ -354,6 +354,62 @@ __device__ __forceinline__ float group_sum(float v, int G) {
     return v;
 }
 
+// ---- Q4_K / Q5_K rows against Q8_K activation columns (gemv_kquant.cu) ------------------------------------------------------
+// Staged column: qs[nsb][256] (int8), then d[nsb] (float), then bsums[nsb][16] (int16, sums of 16 consecutive qs).
+__host__ __device__ inline size_t kq_act_bytes_per_column(int K) {
+    const size_t nsb = (size_t) K / QK_K;
+    return (nsb * (QK_K + 4 + 32) + 15) & ~(size_t) 15;
+}
+// Lane l of the warp (G = 32) takes sub-block l % 8 of super-blocks wk*per + l/8, + 4, ... The scale x sub-block dot and the
+// min x bsums of a super-block are exact integers summed over its 8 lanes; the lane of sub-block 0 then adds
+// y.d*fp16(d) * sum - y.d*fp16(dmin) * msum to its partial, as ggml_vec_dot_q{4,5}_K_q8_K combines a super-block.
+template <int TYPE, int NC>
+__device__ __forceinline__ void row_partial_kq(const uint8_t * wrow, const uint8_t * act, size_t colb, int nc, int K, const LaneMap & m, float (&acc)[NC]) {
+    constexpr int BB = TYPE == DT_Q4_K ? 144 : 176, QS = TYPE == DT_Q4_K ? 16 : 48;
+    const int nsb = K / QK_K, per = (nsb + m.WK - 1) / m.WK;
+    const int sb0 = m.wk * per, sb1 = min(nsb, sb0 + per);
+    const int j = m.sub & 7;
+#pragma unroll
+    for (int c = 0; c < NC; c++) acc[c] = 0.f;
+    for (int s0 = sb0; s0 < sb1; s0 += 4) {                      // warp-uniform: every lane takes part in the shuffles
+        const bool live = s0 + (m.sub >> 3) < sb1;
+        const int s = live ? s0 + (m.sub >> 3) : s0;
+        const uint8_t * blk = wrow + (size_t) s * BB;
+        const uint32_t dm = *reinterpret_cast<const uint32_t *>(blk);
+        int sc, mn;
+        kquant_scale_min(blk + 4, j, sc, mn);
+        const uint4 qa = *reinterpret_cast<const uint4 *>(blk + QS + 32 * (j >> 1)), qb = *reinterpret_cast<const uint4 *>(blk + QS + 32 * (j >> 1) + 16);
+        uint32_t w[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+        const int shift = 4 * (j & 1);
+#pragma unroll
+        for (int i = 0; i < 8; i++) w[i] = (w[i] >> shift) & 0x0F0F0F0Fu;
+        if constexpr (TYPE == DT_Q5_K) {
+            const uint4 ha = *reinterpret_cast<const uint4 *>(blk + 16), hb = *reinterpret_cast<const uint4 *>(blk + 32);
+            const uint32_t h[8] = {ha.x, ha.y, ha.z, ha.w, hb.x, hb.y, hb.z, hb.w};
+#pragma unroll
+            for (int i = 0; i < 8; i++) w[i] |= ((h[i] >> j) & 0x01010101u) << 4;
+        }
+#pragma unroll
+        for (int c = 0; c < NC; c++) if (c < nc) {
+            const uint8_t * col = act + c * colb;
+            const int4 xa = *reinterpret_cast<const int4 *>(col + (size_t) s * QK_K + 32 * j), xb = *reinterpret_cast<const int4 *>(col + (size_t) s * QK_K + 32 * j + 16);
+            int dot = __dp4a((int) w[0], xa.x, 0);
+            dot = __dp4a((int) w[1], xa.y, dot); dot = __dp4a((int) w[2], xa.z, dot); dot = __dp4a((int) w[3], xa.w, dot);
+            dot = __dp4a((int) w[4], xb.x, dot); dot = __dp4a((int) w[5], xb.y, dot); dot = __dp4a((int) w[6], xb.z, dot); dot = __dp4a((int) w[7], xb.w, dot);
+            const short2 bp = *reinterpret_cast<const short2 *>(col + (size_t) nsb * (QK_K + 4) + (size_t) s * 32 + 4 * j);
+            int isum = dot * sc, msum = ((int) bp.x + (int) bp.y) * mn;
+#pragma unroll
+            for (int o = 1; o < 8; o <<= 1) { isum += __shfl_xor_sync(0xffffffffu, isum, o); msum += __shfl_xor_sync(0xffffffffu, msum, o); }
+            if (live && j == 0) {
+                const float yd = reinterpret_cast<const float *>(col + (size_t) nsb * QK_K)[s];
+                const float d = __fmul_rn(yd, __half2float(__ushort_as_half((unsigned short) (dm & 0xFFFFu))));
+                const float dmin = __fmul_rn(yd, __half2float(__ushort_as_half((unsigned short) (dm >> 16))));
+                acc[c] = __fadd_rn(acc[c], __fsub_rn(__fmul_rn(d, (float) isum), __fmul_rn(dmin, (float) msum)));
+            }
+        }
+    }
+}
+
 // One row's lane partials for NC activation columns in shared memory (colb bytes apart), the lane map's order: lane `sub` of
 // warp slice `wk` takes items wk * per + sub, + G, ... (quantised types: units, each block in order). acc[] starts at 0 and is
 // summed by group_sum, then across the WK warps of the row in warp order. The streaming GEMV and the fused v6 LoRA kernels
@@ -400,6 +456,8 @@ __device__ __forceinline__ void row_partial(const uint8_t * wrow, const uint8_t 
 #pragma unroll
             for (int c = 0; c < NC; c++) if (c < nc) acc[c] = __fmaf_rn(wf, __half2float(reinterpret_cast<const __half *>(act + c * colb)[k]), acc[c]);
         }
+    } else if constexpr (TYPE == DT_Q4_K || TYPE == DT_Q5_K) {
+        row_partial_kq<TYPE, NC>(wrow, act, colb, nc, K, m, acc);
     } else {
         using TR = QTraits<TYPE>;
         constexpr int UB = TR::UNIT_BLOCKS, UW = TR::UNIT_WORDS;

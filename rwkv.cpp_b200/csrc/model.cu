@@ -48,6 +48,25 @@ void widen_to_f32(int type, const uint8_t * src, size_t n, float * dst) {
         return;
     }
     const int bb = dtype_block_bytes(type);
+    if (dtype_kquant(type)) {   // dequantize_row_q4_K / dequantize_row_q5_K (ggml-quants.c:1280, 1482)
+        for (size_t b = 0; b < n / QK_K; b++) {
+            const uint8_t * p = src + b * bb;
+            uint16_t dh, mh; memcpy(&dh, p, 2); memcpy(&mh, p + 2, 2);
+            const float d = fp16_to_fp32(dh), dmin = fp16_to_fp32(mh);
+            const uint8_t * sc = p + 4, * qh = p + 16, * qs = p + (type == DT_Q5_K ? 48 : 16);
+            for (int j = 0; j < 8; j++) {
+                int s, m;
+                kquant_scale_min(sc, j, s, m);
+                const float dj = d * (float) s, mj = dmin * (float) m;
+                for (int l = 0; l < 32; l++) {
+                    int q = (qs[32 * (j / 2) + l] >> (4 * (j & 1))) & 0xF;
+                    if (type == DT_Q5_K) q |= ((qh[l] >> j) & 1) << 4;
+                    dst[b * QK_K + 32 * j + l] = dj * (float) q - mj;
+                }
+            }
+        }
+        return;
+    }
     for (size_t b = 0; b < n / 32; b++) {
         const uint8_t * p = src + b * bb;
         uint16_t dh; memcpy(&dh, p, 2);
@@ -274,6 +293,9 @@ Model * load_model(const char * path, int device, int layer_begin, int layer_end
             }
             RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_SHAPE, nullptr, (r.expect_k == 0 || K == r.expect_k) && (r.expect_m == 0 || M == r.expect_m) && K > 0 && M > 0,
                        "Unexpected shape [%" PRIu64 ", %" PRIu64 "] of parameter %s", K, M, r.name.c_str());
+            // no other kernel takes a K-quant matrix, so one whose rows do not fit the K-quant GEMV's streaming plan cannot run
+            RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_UNSUPPORTED, nullptr, !dtype_kquant((int) t.data_type) || gemv_kq_fits((int) t.data_type, (int) K),
+                       "Rows of %" PRIu64 " weights of %s are too long for the %s kernel; requantize the model in another format", K, r.name.c_str(), dtype_name((int) t.data_type));
             const long long pitch = matrix_pitch((int) t.data_type, K);
             r.arena_offset = arena_bytes;
             arena_bytes += align_up((size_t) M * (size_t) pitch + 256, 256);

@@ -91,6 +91,136 @@ void encode_q8_0(const float * x, uint8_t * out) {
     for (int j = 0; j < 32; j++) out[2 + j] = (uint8_t) (int8_t) roundf(x[j] * id);
 }
 
+// ---- K-quants: quantize_row_q4_K_ref / quantize_row_q5_K_ref (ggml-quants.c:1208-1278, 1395-1480) ----
+
+// round to nearest, ties to even, through the float adder (ggml's nearest_int): valid for |v| < 2^22
+inline int nearest_int(float v) {
+    const float t = v + 12582912.f;
+    int i; memcpy(&i, &t, 4);
+    return (i & 0x007fffff) - 0x00400000;
+}
+
+// make_qkx2_quants (ggml-quants.c:550-629) with use_mad = false: levels L[0..n) in [0, nmax] and the scale of an affine fit
+// x ~ scale*L - the_min, refined over nstep+1 trial scales by weighted least squares.
+float fit_affine_levels(int n, int nmax, const float * x, const float * w, uint8_t * L, float * the_min, uint8_t * Laux,
+                        float rmin, float rdelta, int nstep) {
+    float min = x[0], max = x[0], sum_w = w[0], sum_x = sum_w * x[0];
+    for (int i = 1; i < n; i++) {
+        if (x[i] < min) min = x[i];
+        if (x[i] > max) max = x[i];
+        sum_w += w[i];
+        sum_x += w[i] * x[i];
+    }
+    if (min > 0) min = 0;
+    if (max == min) {
+        for (int i = 0; i < n; i++) L[i] = 0;
+        *the_min = -min;
+        return 0.f;
+    }
+    float iscale = nmax / (max - min), scale = 1 / iscale, best = 0;
+    for (int i = 0; i < n; i++) {
+        const int l = nearest_int(iscale * (x[i] - min));
+        L[i] = (uint8_t) (l < 0 ? 0 : (l > nmax ? nmax : l));
+        const float diff = scale * L[i] + min - x[i];
+        best += w[i] * (diff * diff);
+    }
+    for (int is = 0; is <= nstep; is++) {
+        iscale = (rmin + rdelta * is + nmax) / (max - min);
+        float sum_l = 0, sum_l2 = 0, sum_xl = 0;
+        for (int i = 0; i < n; i++) {
+            int l = nearest_int(iscale * (x[i] - min));
+            l = l < 0 ? 0 : (l > nmax ? nmax : l);
+            Laux[i] = (uint8_t) l;
+            sum_l += w[i] * l;
+            sum_l2 += w[i] * l * l;
+            sum_xl += w[i] * l * x[i];
+        }
+        const float D = sum_w * sum_l2 - sum_l * sum_l;
+        if (D > 0) {
+            float this_scale = (sum_w * sum_xl - sum_x * sum_l) / D;
+            float this_min = (sum_l2 * sum_x - sum_l * sum_xl) / D;
+            if (this_min > 0) {
+                this_min = 0;
+                this_scale = sum_xl / sum_l2;
+            }
+            float mad = 0;
+            for (int i = 0; i < n; i++) {
+                const float diff = this_scale * Laux[i] + this_min - x[i];
+                mad += w[i] * (diff * diff);
+            }
+            if (mad < best) {
+                memcpy(L, Laux, (size_t) n);
+                best = mad;
+                scale = this_scale;
+                min = this_min;
+            }
+        }
+    }
+    *the_min = -min;
+    return scale;
+}
+
+// One 256-weight super-block. Q4_K: nmax 15, 21 trial scales from -1.0; Q5_K: nmax 31, 16 trial scales from -0.5.
+void encode_kquant(const float * x, uint8_t * out, bool five) {
+    const int nmax = five ? 31 : 15;
+    uint8_t L[QK_K], Laux[32];
+    float w[32], mins[8], scales[8], max_scale = 0, max_min = 0;
+    for (int j = 0; j < 8; j++) {
+        const float * xj = x + 32 * j;
+        float sum_x2 = 0;
+        for (int l = 0; l < 32; l++) sum_x2 += xj[l] * xj[l];
+        const float av_x = sqrtf(sum_x2 / 32);
+        for (int l = 0; l < 32; l++) w[l] = av_x + fabsf(xj[l]);
+        scales[j] = fit_affine_levels(32, nmax, xj, w, L + 32 * j, &mins[j], Laux, five ? -0.5f : -1.f, 0.1f, five ? 15 : 20);
+        if (scales[j] > max_scale) max_scale = scales[j];
+        if (mins[j] > max_min) max_min = mins[j];
+    }
+    // 6-bit scales and mins, packed as get_scale_min_k4 unpacks them
+    uint8_t * sc = out + 4;
+    const float inv_scale = max_scale > 0 ? 63.f / max_scale : 0.f, inv_min = max_min > 0 ? 63.f / max_min : 0.f;
+    for (int j = 0; j < 8; j++) {
+        uint8_t ls = (uint8_t) nearest_int(inv_scale * scales[j]), lm = (uint8_t) nearest_int(inv_min * mins[j]);
+        ls = ls < 63 ? ls : 63;
+        lm = lm < 63 ? lm : 63;
+        if (j < 4) {
+            sc[j] = ls;
+            sc[j + 4] = lm;
+        } else {
+            sc[j + 4] = (uint8_t) ((ls & 0xF) | ((lm & 0xF) << 4));
+            sc[j - 4] |= (uint8_t) ((ls >> 4) << 6);
+            sc[j] |= (uint8_t) ((lm >> 4) << 6);
+        }
+    }
+    put_half(out, max_scale / 63.f);
+    put_half(out + 2, max_min / 63.f);
+    // levels again against the rounded scales
+    uint16_t dh, mh; memcpy(&dh, out, 2); memcpy(&mh, out + 2, 2);
+    for (int j = 0; j < 8; j++) {
+        int s, m;
+        kquant_scale_min(sc, j, s, m);
+        const float d = fp16_to_fp32(dh) * s;
+        if (!d) continue;
+        const float dm = fp16_to_fp32(mh) * m;
+        for (int i = 0; i < 32; i++) {
+            const int l = nearest_int((x[32 * j + i] + dm) / d);
+            L[32 * j + i] = (uint8_t) (l < 0 ? 0 : (l > nmax ? nmax : l));
+        }
+    }
+    // sub-blocks 2k and 2k+1 share qs[32k .. 32k+32) as low and high nibbles; Q5_K keeps bit 4 of sub-block j in bit j of qh[l]
+    uint8_t * qh = out + 16, * qs = out + (five ? 48 : 16);
+    if (five) memset(qh, 0, 32);
+    for (int k = 0; k < 4; k++) {
+        for (int l = 0; l < 32; l++) {
+            int lo = L[64 * k + l], hi = L[64 * k + 32 + l];
+            if (five) {
+                if (lo > 15) { lo -= 16; qh[l] |= (uint8_t) (1u << (2 * k)); }
+                if (hi > 15) { hi -= 16; qh[l] |= (uint8_t) (2u << (2 * k)); }
+            }
+            qs[32 * k + l] = (uint8_t) (lo | (hi << 4));
+        }
+    }
+}
+
 // Tensors the reference never quantizes (rwkv_quantize.inc:1-13).
 bool tensor_needs_quant(const std::string & name) {
     static const char * skip[] = {"att.v1", "att.v2", "att.g1", "att.g2", "att.a1", "att.a2", "att.w1", "att.w2", "att.r_k"};
@@ -104,6 +234,10 @@ bool tensor_needs_quant(const std::string & name) {
 size_t quantize_row(int type, const float * x, void * dst, size_t n) {
     uint8_t * out = static_cast<uint8_t *>(dst);
     const int bb = dtype_block_bytes(type);
+    if (dtype_kquant(type)) {
+        for (size_t b = 0; b < n / QK_K; b++) encode_kquant(x + b * QK_K, out + b * bb, type == DT_Q5_K);
+        return n / QK_K * (size_t) bb;
+    }
     for (size_t b = 0; b < n / 32; b++) {
         const float * xb = x + b * 32;
         uint8_t * ob = out + b * bb;
@@ -124,7 +258,8 @@ bool quantize_model_file(const char * in_path, const char * out_path, const char
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, in_path && out_path && format_name, "NULL argument");
     const int out_type = dtype_from_name(format_name);
     RWKV_CHECK(sink, RWKV_ERROR_ARGS | RWKV_ERROR_DATA_TYPE, false,
-               out_type == DT_Q4_0 || out_type == DT_Q4_1 || out_type == DT_Q5_0 || out_type == DT_Q5_1 || out_type == DT_Q8_0,
+               out_type == DT_Q4_0 || out_type == DT_Q4_1 || out_type == DT_Q5_0 || out_type == DT_Q5_1 || out_type == DT_Q8_0 ||
+               dtype_kquant(out_type),
                "Unsupported output data type (%s)", format_name);
     MSG("Loading model from '%s'\n", in_path);
 
@@ -176,11 +311,16 @@ bool quantize_model_file(const char * in_path, const char * out_path, const char
             } else {
                 src = reinterpret_cast<const float *>(raw.data());
             }
-            packed.resize(tensor_nbytes(out_type, t.ne[0], t.ne[1], t.ne[2]));
-            payload_bytes = quantize_row(out_type, src, packed.data(), n);
+            // The reference quantises a K-quant tensor as one flat array, so when rows are not whole super-blocks its blocks straddle
+            // rows and no engine can evaluate the result. Such tensors (v6 decay LoRA, n_embed or ffn widths that are not multiples of
+            // 256) go to the legacy format of the same or more bytes per weight instead, as llama.cpp's quantizer does.
+            int type = out_type;
+            if (dtype_kquant(type) && t.ne[0] % QK_K != 0) type = (type == DT_Q4_K) ? DT_Q5_0 : DT_Q5_1;
+            packed.resize(tensor_nbytes(type, t.ne[0], t.ne[1], t.ne[2]));
+            payload_bytes = quantize_row(type, src, packed.data(), n);
             payload = packed.data();
-            out_dtype = (uint32_t) out_type;
-            MSG("-> %6s size = %8.2f MB -> %8.2f MB\n", dtype_name(out_type), t.nbytes / 1024.0 / 1024.0, payload_bytes / 1024.0 / 1024.0);
+            out_dtype = (uint32_t) type;
+            MSG("-> %6s size = %8.2f MB -> %8.2f MB\n", dtype_name(type), t.nbytes / 1024.0 / 1024.0, payload_bytes / 1024.0 / 1024.0);
         } else {
             MSG("size = %8.3f MB\n", t.nbytes / 1024.0 / 1024.0);
         }

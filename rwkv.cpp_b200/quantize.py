@@ -1,5 +1,7 @@
 """Quantizes an rwkv.cpp model file from FP32 or FP16 (CLI of the reference's python/quantize.py:8-32 over this library's
-rwkv_quantize_model_file, which is byte-identical to the reference's for all five formats and needs no GPU).
+rwkv_quantize_model_file, which is byte-identical to the reference's for all seven formats and needs no GPU; the one exception: a
+Q4_K / Q5_K tensor whose rows are not whole 256-weight super-blocks is written as Q5_0 / Q5_1, where the reference writes blocks that
+straddle rows).
 
     python rwkv.cpp_b200/quantize.py model-FP16.bin model-Q5_1.bin Q5_1
 """
@@ -8,7 +10,7 @@ import importlib.util
 import os
 import sys
 
-FORMAT_NAMES = ("Q4_0", "Q4_1", "Q5_0", "Q5_1", "Q8_0")      # rwkv.h:212-217
+FORMAT_NAMES = ("Q4_0", "Q4_1", "Q4_K", "Q5_0", "Q5_1", "Q5_K", "Q8_0")      # the reference binding's list, in its order
 
 
 def _load_package():

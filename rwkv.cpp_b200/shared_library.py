@@ -11,7 +11,7 @@ from typing import Optional
 P_FLOAT = ctypes.POINTER(ctypes.c_float)
 P_U32 = ctypes.POINTER(ctypes.c_uint32)
 
-QUANTIZED_FORMAT_NAMES = ("Q4_0", "Q4_1", "Q5_0", "Q5_1", "Q8_0")   # rwkv.h:212-217
+QUANTIZED_FORMAT_NAMES = ("Q4_0", "Q4_1", "Q4_K", "Q5_0", "Q5_1", "Q5_K", "Q8_0")   # the reference binding's list, in its order
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 

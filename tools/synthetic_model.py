@@ -218,7 +218,46 @@ _QINFO = {  # fmt -> (type id, block bytes, offset of qs, qs bytes, has_qh, has_
 }
 
 
+# Q4_K / Q5_K super-blocks: random levels and 6-bit scales / mins; d, dmin fp16 chosen so weights have std ~ target_std.
+_KQINFO = {"Q4_K": (13, 144, 15), "Q5_K": (14, 176, 31)}
+
+
+def _write_kquant_file(path, n_vocab, n_embed, n_layer, data_type, tensors):
+    """The file layout of ggml_file.write_model_file, for files that hold Q4_K / Q5_K records (ggml_file reads the legacy formats only)."""
+    import struct
+    per_elem = {t: bb / 256 for t, bb, _ in _KQINFO.values()}
+    with open(path, "wb") as f:
+        f.write(struct.pack("<6I", gf.RWKV_FILE_MAGIC, 101, n_vocab, n_embed, n_layer, data_type))
+        for name, dtype, ne, raw in tensors:
+            key = name.encode("utf-8")
+            f.write(struct.pack("<3I", len(ne), len(key), dtype))
+            f.write(struct.pack("<%dI" % len(ne), *ne))
+            f.write(key)
+            raw = np.ascontiguousarray(raw).view(np.uint8).reshape(-1)
+            want = int(np.prod(ne) * per_elem[dtype]) if dtype in per_elem else gf.tensor_nbytes(dtype, ne)
+            assert raw.size == want, (name, raw.size, want)
+            f.write(raw.tobytes())
+
+
+def _random_kquant(fmt, ne, rng, target_std):
+    """The quantizer's per-tensor rule: rows that are not whole 256-weight super-blocks fall back to Q5_0 (Q4_K) / Q5_1 (Q5_K)."""
+    K, M = ne[0], int(np.prod(ne[1:]))
+    if K % 256:
+        return _random_blocks("Q5_0" if fmt == "Q4_K" else "Q5_1", ne, rng, target_std)
+    tid, bb, lev = _KQINFO[fmt]
+    nb = M * (K // 256)
+    b = rng.integers(0, 256, size=(nb, bb), dtype=np.uint8)
+    # level std ~ lev/sqrt(12), mean scale ~ 32: d*32*lev/sqrt(12) ~ 2 target_std; the min removes the mean
+    d = (2.0 * target_std * np.sqrt(12) / (32 * lev) * rng.uniform(0.8, 1.2, nb)).astype(np.float16)
+    dmin = (target_std * rng.uniform(0.8, 1.2, nb) / 32).astype(np.float16)
+    b[:, 0:2] = d.view(np.uint8).reshape(nb, 2)
+    b[:, 2:4] = dmin.view(np.uint8).reshape(nb, 2)
+    return tid, b.reshape(-1)
+
+
 def _random_blocks(fmt, ne, rng, target_std):
+    if fmt in _KQINFO:
+        return _random_kquant(fmt, ne, rng, target_std)
     tid, bb, qoff, qbytes, has_qh, has_min, istd = _QINFO[fmt]
     K, M = ne[0], int(np.prod(ne[1:]))
     nb = M * (K // 32)
@@ -240,7 +279,7 @@ def write_direct(path, preset, fmt, seed=0):
     follows rwkv_quantize.inc:1-13,133-140: 2-D, not emb/head, not the v7 LoRA / r_k tensors."""
     p = PRESETS[preset] if isinstance(preset, str) else preset
     rng = np.random.default_rng(seed)
-    quant = fmt in _QINFO
+    quant = fmt in _QINFO or fmt in _KQINFO
 
     def gen():
         for name, kind, ne, _ in _Spec(p).tensors():
@@ -269,7 +308,10 @@ def write_direct(path, preset, fmt, seed=0):
                 t, a = _vec(_small_values(kind, ne, rng))
                 yield name, t, ne, a
 
-    gf.write_model_file(path, p["V"], p["C"], p["L"], gf.TYPE_IDS[fmt], gen(), version=101)
+    if fmt in _KQINFO:
+        _write_kquant_file(path, p["V"], p["C"], p["L"], _KQINFO[fmt][0], gen())
+    else:
+        gf.write_model_file(path, p["V"], p["C"], p["L"], gf.TYPE_IDS[fmt], gen(), version=101)
     return p
 
 
