@@ -135,6 +135,43 @@ RWKV_API bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, f
 RWKV_API bool rwkv_b200_batch_generate(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                                        const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts,
                                        const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated);
+
+/* Streaming generation: the loops of rwkv_b200_generate / rwkv_b200_batch_generate, with every token handed to on_token while the loop
+ * runs, so that an interactive caller can print it and end a sequence on a condition of its own (a decoded text, say) exactly after
+ * any token. The arguments and their checks are those of the blocking calls, the same context kinds are refused, and on_token must
+ * not be NULL (RWKV_ERROR_ARGS); a rejected call changes nothing.
+ * 1. Delivery: on_token(user, sequence, index, token) runs on the calling thread exactly once for every token written to tokens_out
+ *    (index: the token's position in this call), in index order per sequence; calls for different sequences interleave in the order
+ *    their tokens arrive. Every call happens before the API call returns. A stop id is delivered too and ends its sequence whatever
+ *    on_token returns.
+ * 2. Gate: token j + 1 of a sequence is not drawn until on_token has returned for token j. The pass that evaluates token j runs while
+ *    on_token runs, so the device waits only when a callback takes longer than a pass (in a batch, the step waits for every sequence).
+ * 3. Ending a sequence: a nonzero return for token j ends that sequence after token j, which has been evaluated and counted, as
+ *    python/chat_with_bot.py does. Its tokens, n_generated, state, logits and penalty counts are then bit-identical to the blocking
+ *    call with max_tokens = j + 1 for that sequence and the same u; in a batch the other sequences are unaffected.
+ * 4. Otherwise nothing changes: when on_token always returns 0, the results are bit-identical to the blocking call, and so are the
+ *    results of later calls.
+ * 5. Re-entrancy: from inside on_token, every call that would enqueue work on the generating context's stream or wait on it
+ *    (rwkv_eval*, rwkv_b200_eval_resident, rwkv_b200_eval_sample, rwkv_b200_state_load / _store, rwkv_b200_synchronize,
+ *    rwkv_b200_sample, rwkv_b200_generate*, rwkv_b200_batch_*, rwkv_b200_stage_eval / _logits on that context) returns false with
+ *    RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED and enqueues nothing. Other contexts, clones of the same model included, stay usable; a
+ *    call that has to allocate or free device memory (a first pass of a new size, creating or freeing a context) may wait for the
+ *    whole device and belongs outside the callback. rwkv_free of the generating context from on_token is not allowed.
+ * 6. Bounded wait: the device waits at most RWKV_B200_STREAM_TIMEOUT_MS for a callback. When the bound runs out it ends that sequence as
+ *    if on_token had asked it to; once the callback has returned, the call returns false with RWKV_ERROR_CTX, and tokens_out,
+ *    n_generated, state and logits keep what was delivered up to then. This is a safety net against a kernel spinning on a stuck host.
+ * The calling thread busy-polls (yielding between polls) for the length of the call. While the device waits on the gate, each
+ * waiting sequence holds one CTA of 1024 threads on an SM. */
+#define RWKV_B200_STREAM_TIMEOUT_MS 10000
+/* Return 0 to go on, nonzero to end `sequence` after `token` (its index-th token of this call). */
+typedef int (*rwkv_b200_token_fn)(void * user, size_t sequence, size_t index, uint32_t token);
+RWKV_API bool rwkv_b200_generate_stream(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty,
+                                        float frequency_penalty, bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                        rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated);
+RWKV_API bool rwkv_b200_batch_generate_stream(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature,
+                                              const float * top_p, const float * presence_penalty, const float * frequency_penalty,
+                                              const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                              rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated);
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each

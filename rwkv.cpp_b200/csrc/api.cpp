@@ -123,6 +123,11 @@ struct RaggedMap {
 
 }  // namespace
 
+// Entry points that enqueue work on a context's stream, or wait on it, refuse while a streaming generation of that context calls
+// its callback: the device waits for that callback to return, so the work would deadlock against it. Nothing is enqueued.
+#define RWKV_NOT_STREAMING(c) RWKV_CHECK((c)->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, !(c)->in_stream, \
+                                         "This context is inside a streaming generation; use another context from its callback")
+
 extern "C" {
 
 struct rwkv_context * rwkv_b200_init_from_file_ex(const char * file_path, int device, int layer_begin, int layer_end) {
@@ -190,6 +195,7 @@ struct rwkv_context * rwkv_clone_context(struct rwkv_context * ctx, const uint32
 bool rwkv_eval(struct rwkv_context * ctx, const uint32_t token, const float * state_in, float * state_out, float * logits_out) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     const size_t n_vocab = (size_t) c->model->n_vocab;
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, token < n_vocab, "Token (%" PRIu32 ") is out of range (0 .. %zu)", token, n_vocab - 1);
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, whole_model(c),
@@ -201,6 +207,7 @@ bool rwkv_eval(struct rwkv_context * ctx, const uint32_t token, const float * st
 bool rwkv_eval_sequence(struct rwkv_context * ctx, const uint32_t * sequence, const size_t sequence_len, const float * state_in, float * state_out, float * logits_out) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, sequence_len > 0, "Sequence length is 0");
     if (!sequence) return true;   // "build the graph only" in the reference (rwkv_eval.inc:122); nothing to build here
     const size_t n_vocab = (size_t) c->model->n_vocab;
@@ -218,6 +225,7 @@ bool rwkv_eval_sequence_in_chunks(struct rwkv_context * ctx, const uint32_t * to
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, sequence_len > 0, "Sequence length is 0");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, chunk_size > 0, "Chunk size is 0");
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     if (!tokens) return true;
     const size_t n_vocab = (size_t) c->model->n_vocab;
     for (size_t i = 0; i < sequence_len; i++)
@@ -310,13 +318,24 @@ bool rwkv_b200_inspect_file(const char * path, struct rwkv_b200_file_info * out)
     return true;
 }
 
-bool rwkv_b200_state_load(struct rwkv_context * ctx, const float * state_in) { C(ctx)->last_error = 0; return C(ctx)->batch_n == 0 && upload_state(C(ctx), state_in); }
-bool rwkv_b200_state_store(struct rwkv_context * ctx, float * state_out) { return C(ctx)->batch_n == 0 && download_outputs(C(ctx), state_out, nullptr); }
-bool rwkv_b200_synchronize(struct rwkv_context * ctx) { return download_outputs(C(ctx), nullptr, nullptr); }
+bool rwkv_b200_state_load(struct rwkv_context * ctx, const float * state_in) {
+    C(ctx)->last_error = 0;
+    RWKV_NOT_STREAMING(C(ctx));
+    return C(ctx)->batch_n == 0 && upload_state(C(ctx), state_in);
+}
+bool rwkv_b200_state_store(struct rwkv_context * ctx, float * state_out) {
+    RWKV_NOT_STREAMING(C(ctx));
+    return C(ctx)->batch_n == 0 && download_outputs(C(ctx), state_out, nullptr);
+}
+bool rwkv_b200_synchronize(struct rwkv_context * ctx) {
+    RWKV_NOT_STREAMING(C(ctx));
+    return download_outputs(C(ctx), nullptr, nullptr);
+}
 
 bool rwkv_b200_eval_resident(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, bool want_logits, float * logits_out) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens && n_tokens > 0, "No tokens");
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_eval");
     const size_t n_vocab = (size_t) c->model->n_vocab;
@@ -362,15 +381,18 @@ struct rwkv_context * rwkv_b200_batch_create(struct rwkv_context * ctx, size_t n
 }
 bool rwkv_b200_batch_set_state(struct rwkv_context * batch, size_t sequence, const float * state_in) {
     C(batch)->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(C(batch));
     return batch_set_state(C(batch), (int) sequence, state_in);
 }
 bool rwkv_b200_batch_get_state(struct rwkv_context * batch, size_t sequence, float * state_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(C(batch));
     return batch_get_state(C(batch), (int) sequence, state_out);
 }
 bool rwkv_b200_batch_eval(struct rwkv_context * batch, const uint32_t * tokens, bool want_logits) {
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->batch_n > 0 && tokens, "Not a batch context or NULL tokens");
     for (int i = 0; i < c->batch_n; i++)
         RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) c->model->n_vocab, "Token of sequence %d (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], c->model->n_vocab - 1);
@@ -379,10 +401,12 @@ bool rwkv_b200_batch_eval(struct rwkv_context * batch, const uint32_t * tokens, 
 bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     return batch_eval_ragged(c, tokens, counts, want_logits);
 }
 bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(C(batch));
     return batch_get_logits(C(batch), (int) sequence, logits_out);
 }
 size_t rwkv_b200_batch_size(const struct rwkv_context * ctx) { return (size_t) C(ctx)->batch_n; }
@@ -391,6 +415,7 @@ bool rwkv_b200_sample(struct rwkv_context * ctx, float temperature, float top_p,
                       uint32_t * token_out) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     return sample_token(c, temperature, top_p, u, bias_ids, bias_values, n_bias, token_out);
 }
 
@@ -431,6 +456,7 @@ bool rwkv_b200_eval_sample(struct rwkv_context * ctx, uint32_t token, float temp
 bool rwkv_b200_batch_sample(struct rwkv_context * batch, const float * temperature, const float * top_p, const double * u, const uint32_t * bias_offsets,
                             const uint32_t * bias_ids, const float * bias_values, uint32_t * tokens_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(C(batch));
     return batch_sample(C(batch), temperature, top_p, u, bias_offsets, bias_ids, bias_values, tokens_out);
 }
 
@@ -438,6 +464,7 @@ bool rwkv_b200_batch_eval_sample(struct rwkv_context * batch, const uint32_t * t
                                  uint32_t * tokens_out) {
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->batch_n > 0 && tokens, "Not a batch context or NULL tokens");
     for (int i = 0; i < c->batch_n; i++)
         RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) c->model->n_vocab, "Token of sequence %d (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], c->model->n_vocab - 1);
@@ -472,30 +499,68 @@ bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows, size_t n
 
 static_assert(RWKV_B200_GENERATE_MAX == GENERATE_MAX && RWKV_B200_GENERATE_MAX_STOP == GENERATE_MAX_STOP, "generation limits of the header and the engine");
 
-bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
-                        bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated) {
+static_assert(RWKV_B200_STREAM_TIMEOUT_MS == STREAM_TIMEOUT_MS, "streaming wait bound of the header and the kernel");
+
+// The single-sequence generate calls; on_token NULL is the blocking loop.
+static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
+                            bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated,
+                            bool streaming, TokenFn on_token, void * user) {
     if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
-    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate");
+    RWKV_NOT_STREAMING(c);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s",
+               streaming ? "_stream" : "");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
                "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
     const uint32_t budget = (uint32_t) max_tokens;
     const uint8_t keep = keep_counts ? 1 : 0;
     uint32_t n = 0;
-    if (!generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n)) return false;
-    *n_generated = n;
-    return true;
+    const bool ok = generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n, on_token, user);
+    if (ok || n) *n_generated = n;      // a callback that kept the device waiting too long still gets what was delivered
+    return ok;
+}
+
+// The batch generate calls; on_token NULL is the blocking loop.
+static bool generate_batch(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                           const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
+                           const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s", streaming ? "_stream" : "");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
+    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user);
+}
+
+bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
+                        bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated) {
+    return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                           false, nullptr, nullptr);
 }
 
 bool rwkv_b200_batch_generate(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                               const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
                               const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated) {
-    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
-    Context * c = C(batch);
-    c->last_error = RWKV_ERROR_NONE;
-    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate");
-    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated);
+    return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                          false, nullptr, nullptr);
+}
+
+bool rwkv_b200_generate_stream(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty,
+                               float frequency_penalty, bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                               rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated) {
+    return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                           true, on_token, user);
+}
+
+bool rwkv_b200_batch_generate_stream(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
+                                     const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
+                                     const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
+                                     uint32_t * n_generated) {
+    return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                          true, on_token, user);
 }
 
 bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) {
@@ -551,6 +616,7 @@ bool rwkv_b200_stage_eval(struct rwkv_context * ctx, const uint32_t * tokens, si
                           void * cuda_stream) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     const Model & m = *c->model;
     const bool first = m.layer_begin == 0, last = m.layer_end == m.n_layer;
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_tokens > 0 && n_tokens <= (size_t) MAX_TOKENS_PER_PASS, "A stage pass takes 1 .. %d tokens", MAX_TOKENS_PER_PASS);
@@ -648,6 +714,7 @@ bool rwkv_b200_pipe_eval(struct rwkv_context * ctx, const uint32_t * tokens, siz
 bool rwkv_b200_stage_logits(struct rwkv_context * ctx, float * logits_out, void * cuda_stream) {
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, logits_out && c->model->layer_end == c->model->n_layer, "Only the last stage holds logits");
     cudaStream_t s = cuda_stream ? reinterpret_cast<cudaStream_t>(cuda_stream) : c->stream;
     cudaError_t e = cudaMemcpyAsync(logits_out, c->logits, (size_t) c->model->n_vocab * sizeof(float), cudaMemcpyDeviceToHost, s);

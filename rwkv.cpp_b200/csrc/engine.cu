@@ -700,6 +700,8 @@ void destroy_context(Context * ctx) {
     cudaFree(ctx->gen_scratch); cudaFree(ctx->gen_park);
     if (ctx->gen_in_host) cudaFreeHost(ctx->gen_in_host);
     if (ctx->gen_out_host) cudaFreeHost(ctx->gen_out_host);
+    if (ctx->stream_host) cudaFreeHost(ctx->stream_host);
+    if (ctx->stream_done) cudaEventDestroy(ctx->stream_done);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
     if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
@@ -1186,6 +1188,9 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // still active". A body holds two passes because the passes double-buffer the state. In a batch context every pass computes all
 // columns, so its shape and graph stay fixed; a frozen row's state is copied back over its output after each pass and its logits,
 // parked by the step that froze it, come back after the loop.
+// A streaming loop runs generate_stream_sample_kernel instead: after each draw it publishes the token to mapped host memory, and
+// before the next draw of that row it waits for the calling thread to acknowledge it (stream_tokens), so that the pass evaluating
+// token j overlaps the callback of token j, and a callback can end its row before token j + 1 is drawn.
 namespace {
 
 size_t gen_u_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
@@ -1226,7 +1231,18 @@ struct GraphHolder {
     ~GraphHolder() { if (g) cudaGraphDestroy(g); }
 };
 
-bool build_generate_graph(Context * ctx) {
+size_t stream_token_offset(int rows) { return 2 * (size_t) rows + 1; }
+
+GenStreamParams generate_stream_params(Context * ctx) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    GenStreamParams sp{};
+    sp.step = generate_step_params(ctx);
+    sp.published = ctx->stream_dev; sp.acked = ctx->stream_dev + rows; sp.timed_out = ctx->stream_dev + 2 * rows;
+    sp.tokens = ctx->stream_dev + stream_token_offset(rows);
+    return sp;
+}
+
+bool build_generate_graph(Context * ctx, bool streaming) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     {   // one uncaptured pass of the loop's shape first, as run_layers does before it captures; its logits go to the step's scratch
         // and its state to state_b, which holds nothing between passes
@@ -1253,10 +1269,12 @@ bool build_generate_graph(Context * ctx) {
     for (int half = 0; half < 2; half++) {
         cudaGraphConditionalHandle run_pass;
         CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&run_pass, body, 0, cudaGraphCondAssignDefault));
-        GenStepParams gp = generate_step_params(ctx);
+        GenStreamParams sp = generate_stream_params(ctx);
+        GenStepParams & gp = sp.step;
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
-        CUDA_OK(ctx, add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
+        CUDA_OK(ctx, streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
+                               : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
         cudaGraphNodeParams ip = {};
         ip.type = cudaGraphNodeTypeConditional;
         ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
@@ -1267,7 +1285,7 @@ bool build_generate_graph(Context * ctx) {
         if (!ok) return false;
         prev = cond;
     }
-    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase], top.g, 0));
+    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase][streaming], top.g, 0));
     return true;
 }
 
@@ -1289,10 +1307,49 @@ bool ensure_generate_buffers(Context * ctx) {
     return true;
 }
 
+bool ensure_stream_buffers(Context * ctx) {
+    if (ctx->stream_dev) return true;
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    const size_t bytes = (stream_token_offset(rows) + (size_t) rows * GENERATE_MAX) * sizeof(uint32_t);
+    if (!ctx->stream_done) CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->stream_done, cudaEventDisableTiming));
+    if (!ctx->stream_host) CUDA_OK(ctx, cudaHostAlloc(reinterpret_cast<void **>(&ctx->stream_host), bytes, cudaHostAllocMapped));
+    CUDA_OK(ctx, cudaHostGetDevicePointer(reinterpret_cast<void **>(&ctx->stream_dev), ctx->stream_host, 0));
+    return true;
+}
+
+// The calling thread's side of a streaming loop that has been enqueued up to ctx->stream_done: calls on_token for every token the
+// step kernel publishes, in order per row, and acknowledges each one (the stop bit set when on_token returned nonzero), until the
+// stream has passed the event and every published token is delivered. Busy-polls, yielding between empty sweeps. Returns false when
+// a wait of the device for an acknowledgement ran out.
+bool stream_tokens(Context * ctx, TokenFn on_token, void * user) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    uint32_t * published = ctx->stream_host, * acked = published + rows, * tokens = published + stream_token_offset(rows);
+    std::vector<uint32_t> delivered((size_t) rows, 0);
+    ctx->in_stream = true;
+    for (bool done = false; !done;) {
+        done = cudaEventQuery(ctx->stream_done) != cudaErrorNotReady;      // before the sweep, so that the last sweep sees every token
+        bool any = false;
+        for (int b = 0; b < rows; b++) {
+            const uint32_t n = __atomic_load_n(published + b, __ATOMIC_ACQUIRE);
+            for (uint32_t j = delivered[b]; j < n; j++) {
+                const uint32_t tok = __atomic_load_n(tokens + (size_t) b * GENERATE_MAX + j, __ATOMIC_RELAXED);
+                const uint32_t stop = on_token(user, (size_t) b, j, tok) != 0 ? 1u : 0u;
+                __atomic_store_n(acked + b, 2 * (j + 1) + stop, __ATOMIC_RELEASE);
+                any = true;
+            }
+            delivered[b] = std::max(delivered[b], n);
+        }
+        if (!any && !done) std::this_thread::yield();
+    }
+    ctx->in_stream = false;
+    return __atomic_load_n(published + 2 * rows, __ATOMIC_ACQUIRE) == 0;
+}
+
 }  // namespace
 
 void drop_generate_graphs(Context * ctx) {
-    for (auto & e : ctx->gen_graphs) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+    for (auto & by_phase : ctx->gen_graphs)
+        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
 }
 
 bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
@@ -1320,7 +1377,7 @@ bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const ui
 
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
-              uint32_t * tokens_out, uint32_t * n_generated) {
+              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token, void * user) {
     const Model & m = *ctx->model;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     const size_t V = (size_t) m.n_vocab;
@@ -1335,7 +1392,8 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     size_t n = 0;
     for (int b = 0; b < rows; b++) n = std::max(n, (size_t) max_tokens[b]);
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    if (!ensure_generate_buffers(ctx) || !ensure_capacity(ctx, rows)) return false;
+    const bool streaming = on_token != nullptr;
+    if (!ensure_generate_buffers(ctx) || (streaming && !ensure_stream_buffers(ctx)) || !ensure_capacity(ctx, rows)) return false;
     // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
     GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
     memset(sh, 0, sizeof(GenShared));
@@ -1355,11 +1413,17 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     }
     const size_t out_words = gen_out_words(rows, n);
     CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_out, 0, out_words * sizeof(uint32_t), ctx->stream));
-    const int key = ctx->phase;
-    if (!ctx->gen_graphs[key] && !build_generate_graph(ctx)) return false;
-    CUDA_OK(ctx, cudaGraphLaunch(ctx->gen_graphs[key], ctx->stream));
+    if (streaming) memset(ctx->stream_host, 0, stream_token_offset(rows) * sizeof(uint32_t));     // published, acked, timed_out
+    cudaGraphExec_t & graph = ctx->gen_graphs[ctx->phase][streaming];
+    if (!graph && !build_generate_graph(ctx, streaming)) return false;
+    CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    bool in_time = true;
+    if (streaming) {
+        CUDA_OK(ctx, cudaEventRecord(ctx->stream_done, ctx->stream));
+        in_time = stream_tokens(ctx, on_token, user);
+    }
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     const uint32_t * res = ctx->gen_out_host;
     memcpy(n_generated, res, (size_t) rows * sizeof(uint32_t));
@@ -1368,6 +1432,8 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
         std::swap(ctx->state_a, ctx->state_b);
         ctx->phase ^= 1;
     }
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX, false, in_time, "A token callback kept the device waiting for more than %d ms; its sequence was ended there",
+               STREAM_TIMEOUT_MS);
     return true;
 }
 

@@ -125,9 +125,16 @@ struct Context {
     uint32_t * gen_bias_ids = nullptr;                                // [rows, n_vocab]
     float * gen_bias_values = nullptr, * gen_scratch = nullptr;       // [rows, n_vocab] each
     float * gen_park = nullptr;                                       // batch contexts: [rows, n_vocab] logits of frozen rows
-    // the loop's graph, keyed by phase (which state buffer holds the current state), as the single-token slots are
-    cudaGraphExec_t gen_graphs[2] = {nullptr, nullptr};
+    // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, and by whether
+    // the loop streams its tokens to a callback
+    cudaGraphExec_t gen_graphs[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
     bool tokens_on_device = false;   // while the loop's passes are captured: ctx->tokens is written by the sampler, no upload
+    // Streaming generation, allocated on the first streaming call: mapped pinned words shared by the step kernel and the calling
+    // thread (GenStreamParams), at device addresses the streaming graph captures. Layout: published [rows], acked [rows], timed_out,
+    // then tokens [rows][GENERATE_MAX].
+    uint32_t * stream_host = nullptr, * stream_dev = nullptr;
+    cudaEvent_t stream_done = nullptr;   // recorded after the streaming loop's copies
+    bool in_stream = false;          // the calling thread is inside a streaming call's callbacks: this context's stream is busy
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -209,13 +216,15 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // rwkv_b200_generate / rwkv_b200_batch_generate (include/rwkv_b200.h). Host arrays of n_rows entries; u and tokens_out are
 // [n_rows][n] with n the largest max_tokens; keep_counts may be NULL. check_generate_rows checks every argument (also for the test
 // hook); generate checks the context too and runs the whole loop as one graph launch, then copies tokens and counts back. Synchronises.
-constexpr int GENERATE_MAX = 4096;
+// With on_token, the loop streams: the calling thread busy-polls the published tokens, calls on_token(user, row, index, token) for
+// each, in order per row, and acknowledges it; a nonzero return ends the row after that token (rwkv_b200_generate_stream).
+using TokenFn = int (*)(void * user, size_t sequence, size_t index, uint32_t token);
 bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                          const float * presence, const float * frequency, const double * u, const uint32_t * stop_ids, size_t n_stop,
                          const void * tokens_out, const void * n_generated);
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
-              uint32_t * tokens_out, uint32_t * n_generated);
+              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr);
 // Drops the loop's graphs (they hold the activation buffers and the GEMM routing of the time they were captured).
 void drop_generate_graphs(Context * ctx);
 

@@ -222,6 +222,22 @@ struct GenStepParams {
 cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s);
 // The same step as a kernel node of graph g after deps (the body of the generation loop).
 cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node);
+
+// Streaming generation (rwkv_b200_generate_stream / rwkv_b200_batch_generate_stream): the same step with a gate and a publisher over
+// words in mapped pinned host memory. Gate: before a row that is not frozen draws token step (0 < step < max_tokens), thread 0 waits
+// until acked[b] >> 1 == step, i.e. the host has acknowledged token step - 1; acked bit 0 asks the row to stop, which freezes it as an
+// exhausted budget does. A wait longer than STREAM_TIMEOUT_MS freezes the row the same way and sets *timed_out. Publisher: after a
+// draw, tokens[b * GENERATE_MAX + step] = token, then (release, system scope) published[b] = step + 1.
+constexpr int GENERATE_MAX = 4096;
+constexpr int STREAM_TIMEOUT_MS = 10000;
+struct GenStreamParams {
+    GenStepParams step;
+    uint32_t * tokens;                // mapped [n_rows][GENERATE_MAX]
+    uint32_t * published;             // mapped [n_rows]: tokens published this call
+    const uint32_t * acked;           // mapped [n_rows]: 2 * tokens acknowledged + stop request
+    uint32_t * timed_out;             // mapped: set when a wait ran out
+};
+cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node);
 // After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);

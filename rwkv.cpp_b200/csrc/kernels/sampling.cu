@@ -181,20 +181,60 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) batch_sample_kernel(const Samp
     sample_row<PER>(p);
 }
 
-// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams).
-template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const GenStepParams gp) {
-    pdl_prologue();
+// The blocking loop's gate: a row never waits, nothing is published.
+struct NoGate {
+    __device__ __forceinline__ bool stop_before(int, uint32_t) const { return false; }
+    __device__ __forceinline__ void publish(int, uint32_t, uint32_t) const {}
+};
+
+__device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// The streaming loop's gate over the mapped words of GenStreamParams (ops.h).
+struct StreamGate {
+    uint32_t * tokens, * published;
+    const uint32_t * acked;
+    uint32_t * timed_out;
+    // Thread 0, before row b draws token step (> 0): waits for the host's acknowledgement of token step - 1. True: the host asked
+    // the row to stop, or the wait ran out.
+    __device__ __forceinline__ bool stop_before(int b, uint32_t step) const {
+        const unsigned long long deadline = global_ns() + (unsigned long long) STREAM_TIMEOUT_MS * 1000000ull;
+        for (unsigned int ns = 32;; ns = min(2 * ns, 1024u)) {
+            uint32_t a;
+            asm volatile("ld.acquire.sys.u32 %0, [%1];" : "=r"(a) : "l"(acked + b) : "memory");
+            if ((a >> 1) >= step) return a & 1u;
+            if (global_ns() > deadline) {
+                *(volatile uint32_t *) timed_out = 1;
+                return true;
+            }
+            __nanosleep(ns);
+        }
+    }
+    // Thread 0, after row b drew token step: the token first, then the count that makes it visible to the host.
+    __device__ __forceinline__ void publish(int b, uint32_t step, uint32_t tok) const {
+        *(volatile uint32_t *) (tokens + (size_t) b * GENERATE_MAX + step) = tok;
+        asm volatile("st.release.sys.u32 [%0], %1;" :: "l"(published + b), "r"(step + 1) : "memory");
+    }
+};
+
+// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`.
+template <int PER, class Gate>
+__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate) {
     __shared__ int draw, park;
     const int b = blockIdx.x, tid = threadIdx.x, V = gp.n_vocab;
     const size_t off = (size_t) b * V;
     GenRow * r = gp.rows + b;
     GenShared * sh = gp.shared;
     if (tid == 0) {
-        const bool budget = !r->frozen && r->step == r->max_tokens;
-        if (budget) r->frozen = 1;
+        bool freeze = !r->frozen && r->step == r->max_tokens;
+        // a stop request (or a wait that ran out) freezes the row exactly as an exhausted budget does
+        if (!r->frozen && !freeze && r->step > 0 && gate.stop_before(b, r->step)) freeze = true;
+        if (freeze) r->frozen = 1;
         draw = !r->frozen;
-        park = budget;
+        park = freeze;
     }
     __syncthreads();
     uint32_t tok = 0;
@@ -227,6 +267,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const G
     if (park && gp.park)
         for (int i = tid; i < V; i += SAMPLE_THREADS) gp.park[off + i] = gp.logits[off + i];
     if (tid == 0) {
+        if (draw) gate.publish(b, r->step - 1, tok);
         const bool active = !r->frozen;
         gp.n_generated[b] = r->step;
         gp.next_tokens[b] = active ? (int) tok : 0;
@@ -244,6 +285,20 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const G
     }
 }
 
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const GenStepParams gp) {
+    pdl_prologue();
+    generate_step<PER>(gp, NoGate{});
+}
+
+// At one CTA per SM ptxas may give every thread 64 registers: with the default bound it holds PER <= 4 to 32, and the gate's wait
+// loop then spills more than generate_sample_kernel does. Only a step of more than one row per SM pays for it, with a second wave.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sample_kernel(const GenStreamParams sp) {
+    pdl_prologue();
+    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out});
+}
+
 constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
 
 __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const GenRow * rows, const float * src, float * dst, long long seq_stride, size_t n) {
@@ -254,11 +309,26 @@ __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const G
     for (size_t i = (size_t) blockIdx.x * RESTORE_THREADS + threadIdx.x; i < n; i += (size_t) gridDim.x * RESTORE_THREADS) dst[base + i] = src[base + i];
 }
 
-template <int PER> void * generate_step_fn() { return reinterpret_cast<void *>(generate_sample_kernel<PER>); }
-void * generate_step_for(int n_vocab) {
+template <int PER> void * generate_step_fn(bool stream) {
+    return stream ? reinterpret_cast<void *>(generate_stream_sample_kernel<PER>) : reinterpret_cast<void *>(generate_sample_kernel<PER>);
+}
+void * generate_step_for(int n_vocab, bool stream) {
     const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? generate_step_fn<1>() : per <= 4 ? generate_step_fn<4>() : per <= 16 ? generate_step_fn<16>() : per <= 50 ? generate_step_fn<50>()
-                                                                                                                            : generate_step_fn<64>();
+    return per <= 1 ? generate_step_fn<1>(stream) : per <= 4 ? generate_step_fn<4>(stream) : per <= 16 ? generate_step_fn<16>(stream)
+         : per <= 50 ? generate_step_fn<50>(stream) : generate_step_fn<64>(stream);
+}
+
+// A step kernel node of graph g after deps with the single kernel parameter `arg`.
+template <class P>
+cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, bool stream, cudaGraphNode_t * node) {
+    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    P copy = arg;
+    void * args[] = {&copy};
+    cudaKernelNodeParams kp = {};
+    kp.func = generate_step_for(p.n_vocab, stream);
+    kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
+    kp.kernelParams = args; kp.extra = nullptr;
+    return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
 }
 
 }  // namespace
@@ -275,14 +345,11 @@ cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s) {
 }
 
 cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node) {
-    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    GenStepParams arg = p;
-    void * args[] = {&arg};
-    cudaKernelNodeParams kp = {};
-    kp.func = generate_step_for(p.n_vocab);
-    kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
-    kp.kernelParams = args; kp.extra = nullptr;
-    return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
+    return add_step_node(g, deps, n_deps, p, p, false, node);
+}
+
+cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node) {
+    return add_step_node(g, deps, n_deps, p.step, p, true, node);
 }
 
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {

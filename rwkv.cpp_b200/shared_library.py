@@ -10,6 +10,8 @@ from typing import Optional
 
 P_FLOAT = ctypes.POINTER(ctypes.c_float)
 P_U32 = ctypes.POINTER(ctypes.c_uint32)
+# rwkv_b200_token_fn (include/rwkv_b200.h): int (*)(void * user, size_t sequence, size_t index, uint32_t token)
+RWKV_TOKEN_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint32)
 
 QUANTIZED_FORMAT_NAMES = ("Q4_0", "Q4_1", "Q4_K", "Q5_0", "Q5_1", "Q5_K", "Q8_0")   # the reference binding's list, in its order
 
@@ -176,6 +178,12 @@ class RWKVSharedLibrary:
         P_U8 = ctypes.POINTER(ctypes.c_uint8)
         lib.rwkv_b200_batch_generate.argtypes = [vp, P_U32, P_FLOAT, P_FLOAT, P_FLOAT, P_FLOAT, P_U8, P_DOUBLE, P_U32, ctypes.c_size_t, P_U32, P_U32]
         lib.rwkv_b200_batch_generate.restype = ctypes.c_bool
+        lib.rwkv_b200_generate_stream.argtypes = [vp, ctypes.c_size_t, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_bool,
+                                                  P_DOUBLE, P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, ctypes.POINTER(ctypes.c_size_t)]
+        lib.rwkv_b200_generate_stream.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_generate_stream.argtypes = [vp, P_U32, P_FLOAT, P_FLOAT, P_FLOAT, P_FLOAT, P_U8, P_DOUBLE, P_U32, ctypes.c_size_t,
+                                                        RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, P_U32]
+        lib.rwkv_b200_batch_generate_stream.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step.argtypes = [ctypes.c_void_p]
         lib.rwkv_b200_test_generate_step.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
