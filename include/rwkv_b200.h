@@ -172,6 +172,46 @@ RWKV_API bool rwkv_b200_batch_generate_stream(struct rwkv_context * batch, const
                                               const float * top_p, const float * presence_penalty, const float * frequency_penalty,
                                               const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
                                               rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated);
+/* Constrained generation: the loops above with every sequence's tokens restricted by a token automaton, so that structured output
+ * (a number, a choice from a list, a fixed schema, tool-call syntax) stays on the device instead of a host loop of rwkv_b200_sample
+ * calls with an n_vocab-entry -inf bias list.
+ * An automaton is a dense transition table next[s * n_vocab + t] over the vocabulary of ctx's model, 1 <= n_states <= 65535: the state
+ * after token t in state s, or RWKV_B200_AUTOMATON_DEAD when t is not allowed in s. next may be a host or a device pointer.
+ * rwkv_b200_automaton_create checks every entry (< n_states or dead) and the context (a whole-model or a batch context) before it
+ * allocates anything, then uploads the table once to the HBM of the model's device (n_states * n_vocab * 2 bytes, 128 KB per state at
+ * n_vocab 65536) with a flag per state that says whether it allows any token. It returns NULL with RWKV_ERROR_ARGS for a NULL context
+ * or a bad table, and RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED for a pipeline or one of its stages (flags read with
+ * rwkv_get_last_error(NULL)). The automaton serves every context of that model (clones, batch contexts created from it); a context
+ * of another model refuses it with RWKV_ERROR_ARGS. Free it with rwkv_b200_automaton_free once no call uses it, never from a token
+ * callback.
+ * The generate calls take the arguments of rwkv_b200_generate / rwkv_b200_batch_generate with the same checks, plus the automaton
+ * and the caller's automaton state (in / out); on_token NULL is the blocking loop, otherwise the loop streams with every rule of
+ * rwkv_b200_generate_stream. A rejected call changes no state, logits, counts or automaton state: a NULL automaton or state
+ * pointer, a state >= n_states and an automaton of another model give RWKV_ERROR_ARGS. A constrained sequence in state s, at each step:
+ * 1. if s allows no token, the sequence stops before it draws, exactly as at an exhausted budget (one that starts there generates 0
+ *    tokens and is left as it is);
+ * 2. it draws with the bias -inf on every token s does not allow, in place of any penalty, and the penalty on every other counted
+ *    token: bit for bit what rwkv_b200_sample returns from the same logits, u and that bias list;
+ * 3. a stop id can be drawn only where s allows it; it is reported, neither evaluated nor counted, and s stays;
+ * 4. any other token is counted and evaluated, and s becomes next[s][token].
+ * automaton_state receives the state after the last evaluated token. A callback that ends a sequence after token j gives the results
+ * of max_tokens = j + 1, automaton state included. A one-state automaton that allows every token gives the bytes of the unconstrained
+ * call. In a batch, automata[b] == NULL leaves sequence b unconstrained and automaton_states[b] untouched; such a row gives what
+ * rwkv_b200_batch_generate gives it. */
+#define RWKV_B200_AUTOMATON_DEAD 0xFFFF
+struct rwkv_b200_automaton;
+RWKV_API struct rwkv_b200_automaton * rwkv_b200_automaton_create(struct rwkv_context * ctx, const uint16_t * next, size_t n_states);
+RWKV_API void rwkv_b200_automaton_free(struct rwkv_b200_automaton * automaton);
+RWKV_API bool rwkv_b200_generate_constrained(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state,
+                                             size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
+                                             bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                             rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated);
+RWKV_API bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata,
+                                                   uint32_t * automaton_states, const uint32_t * max_tokens, const float * temperature,
+                                                   const float * top_p, const float * presence_penalty, const float * frequency_penalty,
+                                                   const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                                   rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each
@@ -192,6 +232,10 @@ struct rwkv_b200_generate_step_args {
     uint32_t * any_active;                     /* out */
 };
 RWKV_API bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a);
+/* The same step of the constrained kernel: row b follows the table next (n_states x n_vocab, as for rwkv_b200_automaton_create) from
+ * states[b], which receives its new state; states[b] == UINT32_MAX marks an unconstrained row. */
+RWKV_API bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states,
+                                                       uint32_t * states);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

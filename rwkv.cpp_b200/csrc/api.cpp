@@ -501,23 +501,27 @@ static_assert(RWKV_B200_GENERATE_MAX == GENERATE_MAX && RWKV_B200_GENERATE_MAX_S
 
 static_assert(RWKV_B200_STREAM_TIMEOUT_MS == STREAM_TIMEOUT_MS, "streaming wait bound of the header and the kernel");
 
-// The single-sequence generate calls; on_token NULL is the blocking loop.
+// The single-sequence generate calls; on_token NULL is the blocking loop. `constrained`: the row follows *automaton from
+// *automaton_state (both checked here, the rest by generate).
 static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
                             bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated,
-                            bool streaming, TokenFn on_token, void * user) {
+                            bool streaming, TokenFn on_token, void * user, bool constrained = false, const Automaton * automaton = nullptr,
+                            uint32_t * automaton_state = nullptr) {
     if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
-    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s",
-               streaming ? "_stream" : "");
+    const char * suffix = constrained ? "_constrained" : streaming ? "_stream" : "";
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s", suffix);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
                "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automaton && automaton_state), "NULL automaton or automaton_state");
     const uint32_t budget = (uint32_t) max_tokens;
     const uint8_t keep = keep_counts ? 1 : 0;
     uint32_t n = 0;
-    const bool ok = generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n, on_token, user);
+    const bool ok = generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n, on_token, user,
+                             constrained ? &automaton : nullptr, automaton_state);
     if (ok || n) *n_generated = n;      // a callback that kept the device waiting too long still gets what was delivered
     return ok;
 }
@@ -525,14 +529,18 @@ static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float 
 // The batch generate calls; on_token NULL is the blocking loop.
 static bool generate_batch(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                            const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
-                           const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user) {
+                           const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user,
+                           bool constrained = false, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr) {
     if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
-    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s", streaming ? "_stream" : "");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s",
+               constrained ? "_constrained" : streaming ? "_stream" : "");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
-    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automata && automaton_states), "NULL automata or automaton_states");
+    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user,
+                    automata, automaton_states);
 }
 
 bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
@@ -563,7 +571,47 @@ bool rwkv_b200_batch_generate_stream(struct rwkv_context * batch, const uint32_t
                           true, on_token, user);
 }
 
-bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) {
+}  // extern "C"
+
+// The opaque handle of the automaton API is the engine's Automaton.
+struct rwkv_b200_automaton : public rwkv::Automaton {};
+
+extern "C" {
+
+struct rwkv_b200_automaton * rwkv_b200_automaton_create(struct rwkv_context * ctx, const uint16_t * next, size_t n_states) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, ctx, "NULL context");
+    const Model & m = *C(ctx)->model;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, !C(ctx)->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Automata serve whole-model and batch contexts, not a pipeline or one of its stages");
+    return static_cast<struct rwkv_b200_automaton *>(create_automaton(&m, next, n_states, sink));
+}
+
+void rwkv_b200_automaton_free(struct rwkv_b200_automaton * a) { destroy_automaton(a); }
+
+bool rwkv_b200_generate_constrained(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state, size_t max_tokens,
+                                    float temperature, float top_p, float presence_penalty, float frequency_penalty, bool keep_counts, const double * u,
+                                    const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
+                                    size_t * n_generated) {
+    return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                           false, on_token, user, true, automaton, automaton_state);
+}
+
+bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata, uint32_t * automaton_states,
+                                          const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence_penalty,
+                                          const float * frequency_penalty, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids,
+                                          size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated) {
+    static_assert(sizeof(struct rwkv_b200_automaton) == sizeof(Automaton), "the handle is the engine's automaton");
+    return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                          false, on_token, user, true, reinterpret_cast<const Automaton * const *>(automata), automaton_states);
+}
+
+static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");
+
+// One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
+// the table from states[b] (UINT32_MAX: unconstrained).
+static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
@@ -577,6 +625,16 @@ bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a)
         RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->step[b] <= a->max_tokens[b], "step of row %zu is above its max_tokens", b);
     }
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n >= 1, "Every row has max_tokens 0");
+    const bool constrained = next != nullptr;
+    std::vector<uint8_t> live;
+    if (constrained) {
+        if (!check_automaton_table(sink, next, n_states, V)) return false;
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, states, "NULL states");
+        for (size_t b = 0; b < R; b++)
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, states[b] < n_states || states[b] == UINT32_MAX, "state of row %zu is out of range", b);
+        live.resize(n_states);
+        automaton_live(next, n_states, V, live.data());
+    }
     if (!hook_device(sink)) return false;
     GenShared sh{};
     for (size_t k = 0; k < a->n_stop; k++) sh.stop[k] = a->stop_ids[k];
@@ -599,15 +657,37 @@ bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a)
     gp.n_generated = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
     gp.passes = const_cast<uint32_t *>(hb.in(&zero, 1));
     gp.next_tokens = static_cast<int *>(hb.alloc(R * sizeof(int)));
-    const cudaError_t e = hb.ok ? launch_generate_step(gp, 0) : cudaSuccess;
+    GenConstrainedParams cp{};
+    cp.stream.step = gp;
+    std::vector<uint32_t> states_out(R);
+    if (constrained) {
+        const uint16_t * d_next = hb.in(next, n_states * V);
+        const uint8_t * d_live = hb.in(live.data(), n_states);
+        std::vector<GenMaskRow> mask(R);
+        for (size_t b = 0; b < R; b++)
+            mask[b] = states[b] == UINT32_MAX ? GenMaskRow{nullptr, nullptr, 0, 0} : GenMaskRow{d_next, d_live, states[b], 0};
+        cp.mask = const_cast<GenMaskRow *>(hb.in(mask.data(), R));
+        cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
+    }
+    const cudaError_t e = !hb.ok ? cudaSuccess : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->next_tokens, gp.next_tokens, R * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess &&
-              cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess;
+              cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              (!constrained || cudaMemcpy(states_out.data(), cp.states_out, R * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "generate step failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     for (size_t b = 0; b < R; b++) { a->step[b] = rows[b].step; a->frozen[b] = rows[b].frozen ? 1 : 0; }
+    for (size_t b = 0; constrained && b < R; b++)
+        if (states[b] != UINT32_MAX) states[b] = states_out[b];
     return true;
+}
+
+bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) { return generate_step_hook(a, nullptr, 0, nullptr); }
+
+bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states) {
+    if (!next) { g_last_error = RWKV_ERROR_NONE; ErrorSink sink = global_sink(); RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL table"); }
+    return generate_step_hook(a, next, n_states, states);
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

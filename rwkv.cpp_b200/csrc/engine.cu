@@ -1193,8 +1193,10 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // token j overlaps the callback of token j, and a callback can end its row before token j + 1 is drawn.
 namespace {
 
-size_t gen_u_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
-size_t gen_out_words(int rows, size_t n) { return (size_t) rows + 1 + (size_t) rows * n; }
+size_t gen_mask_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
+size_t gen_u_offset(int rows) { return gen_mask_offset(rows) + (size_t) rows * sizeof(GenMaskRow); }
+size_t gen_tokens_word(int rows) { return 2 * (size_t) rows + 1; }
+size_t gen_out_words(int rows, size_t n) { return gen_tokens_word(rows) + (size_t) rows * n; }
 
 GenStepParams generate_step_params(Context * ctx) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
@@ -1204,7 +1206,7 @@ GenStepParams generate_step_params(Context * ctx) {
     gp.rows = reinterpret_cast<GenRow *>(ctx->gen_in + sizeof(GenShared));
     gp.u = reinterpret_cast<const double *>(ctx->gen_in + gen_u_offset(rows));
     gp.counts = ctx->gen_counts; gp.bias_ids = ctx->gen_bias_ids; gp.bias_values = ctx->gen_bias_values; gp.scratch = ctx->gen_scratch;
-    gp.n_generated = ctx->gen_out; gp.passes = ctx->gen_out + rows; gp.tokens = ctx->gen_out + rows + 1;
+    gp.n_generated = ctx->gen_out; gp.passes = ctx->gen_out + rows; gp.tokens = ctx->gen_out + gen_tokens_word(rows);
     gp.next_tokens = ctx->tokens; gp.park = ctx->batch_n ? ctx->gen_park : nullptr;
     return gp;
 }
@@ -1242,7 +1244,7 @@ GenStreamParams generate_stream_params(Context * ctx) {
     return sp;
 }
 
-bool build_generate_graph(Context * ctx, bool streaming) {
+bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     {   // one uncaptured pass of the loop's shape first, as run_layers does before it captures; its logits go to the step's scratch
         // and its state to state_b, which holds nothing between passes
@@ -1273,8 +1275,10 @@ bool build_generate_graph(Context * ctx, bool streaming) {
         GenStepParams & gp = sp.step;
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
-        CUDA_OK(ctx, streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
-                               : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
+        const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen_in + gen_mask_offset(rows)), ctx->gen_out + rows + 1};
+        CUDA_OK(ctx, constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
+                     : streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
+                                 : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
         cudaGraphNodeParams ip = {};
         ip.type = cudaGraphNodeTypeConditional;
         ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
@@ -1285,7 +1289,7 @@ bool build_generate_graph(Context * ctx, bool streaming) {
         if (!ok) return false;
         prev = cond;
     }
-    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase][streaming], top.g, 0));
+    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
     return true;
 }
 
@@ -1349,7 +1353,63 @@ bool stream_tokens(Context * ctx, TokenFn on_token, void * user) {
 
 void drop_generate_graphs(Context * ctx) {
     for (auto & by_phase : ctx->gen_graphs)
-        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+        for (auto & by_streaming : by_phase)
+            for (auto & e : by_streaming) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+}
+
+bool check_automaton_table(ErrorSink sink, const uint16_t * next, size_t n_states, size_t n_vocab) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, next && n_states >= 1 && n_states <= 65535, "An automaton needs a table and 1 .. 65535 states");
+    for (size_t i = 0, n = n_states * n_vocab; i < n; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, next[i] < n_states || next[i] == GEN_MASK_DEAD, "Transition %zu of state %zu (%u) is neither a state nor dead",
+                   i % n_vocab, i / n_vocab, (unsigned) next[i]);
+    return true;
+}
+
+void automaton_live(const uint16_t * next, size_t n_states, size_t n_vocab, uint8_t * live) {
+    for (size_t s = 0; s < n_states; s++) {
+        const uint16_t * row = next + s * n_vocab;
+        live[s] = std::any_of(row, row + n_vocab, [](uint16_t t) { return t != GEN_MASK_DEAD; }) ? 1 : 0;
+    }
+}
+
+Automaton * create_automaton(const Model * model, const uint16_t * next, size_t n_states, ErrorSink sink) {
+    const size_t V = (size_t) model->n_vocab;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, next && n_states >= 1 && n_states <= 65535, "An automaton needs a table and 1 .. 65535 states");
+    // a device table is checked from a host copy; nothing is allocated before the checks pass
+    std::vector<uint16_t> staged;
+    const uint16_t * host = next;
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, next) == cudaSuccess && (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged)) {
+        staged.resize(n_states * V);
+        RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, cudaMemcpy(staged.data(), next, staged.size() * sizeof(uint16_t), cudaMemcpyDefault) == cudaSuccess,
+                   "Reading the automaton's device table failed");
+        host = staged.data();
+    }
+    cudaGetLastError();     // a host pointer unknown to CUDA is not an error
+    if (!check_automaton_table(sink, host, n_states, V)) return nullptr;
+    std::vector<uint8_t> live(n_states);
+    automaton_live(host, n_states, V, live.data());
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, cudaSetDevice(model->dev.device) == cudaSuccess, "Cannot select the model's device");
+    Automaton * a = new Automaton;
+    a->model = model; a->device = model->dev.device; a->n_vocab = V; a->n_states = (uint32_t) n_states;
+    const bool ok = cudaMalloc(reinterpret_cast<void **>(&a->next), n_states * V * sizeof(uint16_t)) == cudaSuccess &&
+                    cudaMalloc(reinterpret_cast<void **>(&a->live), n_states) == cudaSuccess &&
+                    cudaMemcpy(a->next, next, n_states * V * sizeof(uint16_t), cudaMemcpyDefault) == cudaSuccess &&
+                    cudaMemcpy(a->live, live.data(), n_states, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (!ok) {
+        const cudaError_t e = cudaGetLastError();
+        destroy_automaton(a);
+        RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, false, "Uploading the automaton failed: %s", cudaGetErrorString(e));
+    }
+    return a;
+}
+
+void destroy_automaton(Automaton * a) {
+    if (!a) return;
+    cudaSetDevice(a->device);
+    if (a->next) cudaFree(a->next);
+    if (a->live) cudaFree(a->live);
+    delete a;
 }
 
 bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
@@ -1377,13 +1437,25 @@ bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const ui
 
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
-              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token, void * user) {
+              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token, void * user, const Automaton * const * automata,
+              uint32_t * automaton_states) {
     const Model & m = *ctx->model;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     const size_t V = (size_t) m.n_vocab;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, !ctx->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
                "Generation runs on a whole-model context or batch context, not on a pipeline or one of its stages");
     if (!check_generate_rows(ctx->sink(), rows, V, max_tokens, temperature, top_p, presence, frequency, u, stop_ids, n_stop, tokens_out, n_generated)) return false;
+    const bool constrained = automata != nullptr;
+    if (constrained) {
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, automaton_states, "NULL automaton states");
+        for (int b = 0; b < rows; b++) {
+            if (!automata[b]) continue;
+            RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, automata[b]->model == ctx->model && automata[b]->n_vocab == V,
+                       "The automaton of sequence %d was created for another model", b);
+            RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, automaton_states[b] < automata[b]->n_states, "Automaton state %u of sequence %d is not below %u",
+                       automaton_states[b], b, automata[b]->n_states);
+        }
+    }
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, V <= 65536, "On-device sampling supports n_vocab <= 65536");
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last evaluation skipped the head");
     int driver = 0;
@@ -1401,6 +1473,9 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     sh->n_stop = (uint32_t) n_stop; sh->stride = (uint32_t) n;
     GenRow * gr = reinterpret_cast<GenRow *>(ctx->gen_in_host + sizeof(GenShared));
     for (int b = 0; b < rows; b++) gr[b] = GenRow{temperature[b], top_p[b], presence[b], frequency[b], max_tokens[b], 0, 0, 0};
+    GenMaskRow * mr = reinterpret_cast<GenMaskRow *>(ctx->gen_in_host + gen_mask_offset(rows));
+    for (int b = 0; b < rows; b++)
+        mr[b] = constrained && automata[b] ? GenMaskRow{automata[b]->next, automata[b]->live, automaton_states[b], 0} : GenMaskRow{nullptr, nullptr, 0, 0};
     const size_t u_off = gen_u_offset(rows);
     memcpy(ctx->gen_in_host + u_off, u, (size_t) rows * n * sizeof(double));
     CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_in, ctx->gen_in_host, u_off + (size_t) rows * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -1414,8 +1489,8 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     const size_t out_words = gen_out_words(rows, n);
     CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_out, 0, out_words * sizeof(uint32_t), ctx->stream));
     if (streaming) memset(ctx->stream_host, 0, stream_token_offset(rows) * sizeof(uint32_t));     // published, acked, timed_out
-    cudaGraphExec_t & graph = ctx->gen_graphs[ctx->phase][streaming];
-    if (!graph && !build_generate_graph(ctx, streaming)) return false;
+    cudaGraphExec_t & graph = ctx->gen_graphs[ctx->phase][streaming][constrained];
+    if (!graph && !build_generate_graph(ctx, streaming, constrained)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1427,7 +1502,9 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     const uint32_t * res = ctx->gen_out_host;
     memcpy(n_generated, res, (size_t) rows * sizeof(uint32_t));
-    memcpy(tokens_out, res + rows + 1, (size_t) rows * n * sizeof(uint32_t));
+    memcpy(tokens_out, res + gen_tokens_word(rows), (size_t) rows * n * sizeof(uint32_t));
+    for (int b = 0; constrained && b < rows; b++)
+        if (automata[b]) automaton_states[b] = res[rows + 1 + b];
     if (res[rows] & 1u) {      // an odd number of passes leaves the state in state_b
         std::swap(ctx->state_a, ctx->state_b);
         ctx->phase ^= 1;

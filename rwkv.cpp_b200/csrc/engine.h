@@ -117,17 +117,18 @@ struct Context {
     uint32_t * sample_tokens = nullptr, * sample_tokens_host = nullptr;       // device / pinned
 
     // Device-side generation (generate), allocated on the first call at GENERATE_MAX tokens per row so that the pointers captured in
-    // the loop's graph never change. gen_in: GenShared, GenRow [rows], u [rows][GENERATE_MAX]; gen_out: n_generated [rows], the
-    // number of passes that ran, tokens [rows][GENERATE_MAX]. Both are packed with the call's row stride, so each crosses PCIe once.
+    // the loop's graph never change. gen_in: GenShared, GenRow [rows], GenMaskRow [rows], u [rows][GENERATE_MAX]; gen_out:
+    // n_generated [rows], the number of passes that ran, automaton states [rows], tokens [rows][GENERATE_MAX]. Both are packed with
+    // the call's row stride, so each crosses PCIe once.
     unsigned char * gen_in = nullptr, * gen_in_host = nullptr;        // device / pinned
     uint32_t * gen_out = nullptr, * gen_out_host = nullptr;           // device / pinned
     uint32_t * gen_counts = nullptr;                                  // [rows, n_vocab] penalty counts
     uint32_t * gen_bias_ids = nullptr;                                // [rows, n_vocab]
     float * gen_bias_values = nullptr, * gen_scratch = nullptr;       // [rows, n_vocab] each
     float * gen_park = nullptr;                                       // batch contexts: [rows, n_vocab] logits of frozen rows
-    // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, and by whether
-    // the loop streams its tokens to a callback
-    cudaGraphExec_t gen_graphs[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
+    // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by whether
+    // the loop streams its tokens to a callback, and by whether its draws are constrained by automata
+    cudaGraphExec_t gen_graphs[2][2][2] = {};
     bool tokens_on_device = false;   // while the loop's passes are captured: ctx->tokens is written by the sampler, no upload
     // Streaming generation, allocated on the first streaming call: mapped pinned words shared by the step kernel and the calling
     // thread (GenStreamParams), at device addresses the streaming graph captures. Layout: published [rows], acked [rows], timed_out,
@@ -222,9 +223,30 @@ using TokenFn = int (*)(void * user, size_t sequence, size_t index, uint32_t tok
 bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                          const float * presence, const float * frequency, const double * u, const uint32_t * stop_ids, size_t n_stop,
                          const void * tokens_out, const void * n_generated);
+// With automata (rwkv_b200_generate_constrained), row b is restricted by automata[b] from state automaton_states[b] (a NULL entry:
+// unconstrained), and automaton_states[b] receives the row's final state.
+struct Automaton;
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
-              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr);
+              uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr,
+              const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr);
+
+// A token automaton of rwkv_b200_automaton_create: the transition table next[s * n_vocab + t] (GEN_MASK_DEAD: t not allowed in s)
+// and live[s] (s allows some token) in the HBM of the model's device. It serves every context of that model.
+struct Automaton {
+    const Model * model = nullptr;
+    int device = 0;
+    size_t n_vocab = 0;
+    uint32_t n_states = 0;
+    uint16_t * next = nullptr;
+    uint8_t * live = nullptr;
+};
+// Host checks of a table (1 <= n_states <= 65535, every entry below n_states or dead) and its live flags, [n_states].
+bool check_automaton_table(ErrorSink sink, const uint16_t * next, size_t n_states, size_t n_vocab);
+void automaton_live(const uint16_t * next, size_t n_states, size_t n_vocab, uint8_t * live);
+// The automaton's table on the model's device; `next` may be a host or a device pointer. NULL on failure, with the flags set.
+Automaton * create_automaton(const Model * model, const uint16_t * next, size_t n_states, ErrorSink sink);
+void destroy_automaton(Automaton * a);
 // Drops the loop's graphs (they hold the activation buffers and the GEMM routing of the time they were captured).
 void drop_generate_graphs(Context * ctx);
 

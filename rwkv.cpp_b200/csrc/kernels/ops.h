@@ -238,6 +238,26 @@ struct GenStreamParams {
     uint32_t * timed_out;             // mapped: set when a wait ran out
 };
 cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node);
+// Constrained generation (rwkv_b200_generate_constrained / rwkv_b200_batch_generate_constrained): the same steps, blocking or streaming,
+// with row b restricted by a token automaton, next[s * n_vocab + t] the state after token t in state s or GEN_MASK_DEAD. A row in a
+// state s with !live[s] freezes before it draws, as an exhausted budget freezes it; otherwise every token t with next[s][t] dead
+// gets the bias -inf in place of its penalty, and a drawn token that is evaluated (not a stop id) moves the row to next[s][tok].
+// After every step states_out[b] = the row's state. A row with next == NULL is unconstrained. The rows live in the per-call upload,
+// so that the graph holds only their address and serves every automaton.
+constexpr uint16_t GEN_MASK_DEAD = 0xFFFF;
+struct GenMaskRow {                   // written by the host per call; state is then the loop's
+    const uint16_t * next;            // [n_states, n_vocab] device, or NULL
+    const uint8_t * live;             // [n_states]: the state allows some token
+    uint32_t state, pad;
+};
+struct GenConstrainedParams {
+    GenStreamParams stream;           // the step's parameters; the mapped words are used by the streaming kernel only
+    GenMaskRow * mask;                // [n_rows]
+    uint32_t * states_out;            // [n_rows]
+};
+cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s);     // the blocking kernel
+cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
+                                               cudaGraphNode_t * node);
 // After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);

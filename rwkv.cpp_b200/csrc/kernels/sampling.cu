@@ -220,16 +220,47 @@ struct StreamGate {
     }
 };
 
-// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`.
-template <int PER, class Gate>
-__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate) {
+// The unconstrained loop's mask: every token is allowed, no state is kept.
+struct NoMask {
+    __device__ __forceinline__ bool dead_end(int) const { return false; }
+    __device__ __forceinline__ const uint16_t * table_row(int, int) const { return nullptr; }
+    __device__ __forceinline__ void advance(int, int, uint32_t) const {}
+    __device__ __forceinline__ void report(int) const {}
+};
+
+// The constrained loop's mask over the per-row automata of GenConstrainedParams (ops.h); a row with a NULL table is unconstrained.
+struct TableMask {
+    GenMaskRow * rows;
+    uint32_t * states_out;
+    // Thread 0, before the row draws: its state allows no token.
+    __device__ __forceinline__ bool dead_end(int b) const { const GenMaskRow m = rows[b]; return m.next && !m.live[m.state]; }
+    // Every thread: the row's transitions out of its current state, or NULL.
+    __device__ __forceinline__ const uint16_t * table_row(int b, int V) const {
+        const GenMaskRow m = rows[b];
+        return m.next ? m.next + (size_t) m.state * V : nullptr;
+    }
+    // Thread 0, after the row evaluated tok. Only a row whose allowed tokens all have logit -inf or NaN can draw a token its state
+    // does not allow; that keeps the state.
+    __device__ __forceinline__ void advance(int b, int V, uint32_t tok) const {
+        GenMaskRow & m = rows[b];
+        if (!m.next) return;
+        const uint16_t s = m.next[(size_t) m.state * V + tok];
+        if (s != GEN_MASK_DEAD) m.state = s;
+    }
+    __device__ __forceinline__ void report(int b) const { states_out[b] = rows[b].state; }
+};
+
+// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`, its draws restricted by `mask`.
+template <int PER, class Gate, class Mask>
+__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate, const Mask mask) {
     __shared__ int draw, park;
     const int b = blockIdx.x, tid = threadIdx.x, V = gp.n_vocab;
     const size_t off = (size_t) b * V;
     GenRow * r = gp.rows + b;
     GenShared * sh = gp.shared;
     if (tid == 0) {
-        bool freeze = !r->frozen && r->step == r->max_tokens;
+        // a state that allows no token freezes the row exactly as an exhausted budget does
+        bool freeze = !r->frozen && (r->step == r->max_tokens || mask.dead_end(b));
         // a stop request (or a wait that ran out) freezes the row exactly as an exhausted budget does
         if (!r->frozen && !freeze && r->step > 0 && gate.stop_before(b, r->step)) freeze = true;
         if (freeze) r->frozen = 1;
@@ -241,10 +272,12 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
     if (draw) {
         const uint32_t step = r->step;
         const float presence = r->presence, frequency = r->frequency;
+        const uint16_t * allowed = mask.table_row(b, V);
         for (int i = tid; i < V; i += SAMPLE_THREADS) {      // chat_with_bot.py:244-247, as a bias list over every token
             const uint32_t c = gp.counts[off + i];
-            gp.bias_ids[off + i] = c ? (uint32_t) i : (uint32_t) V;
-            gp.bias_values[off + i] = -__fadd_rn(presence, __fmul_rn((float) c, frequency));
+            const bool dead = allowed && allowed[i] == GEN_MASK_DEAD;     // a token the state does not allow: -inf, whatever its count
+            gp.bias_ids[off + i] = (c || dead) ? (uint32_t) i : (uint32_t) V;
+            gp.bias_values[off + i] = dead ? -INFINITY : -__fadd_rn(presence, __fmul_rn((float) c, frequency));
         }
         __syncthreads();
         SampleParams p;
@@ -260,7 +293,7 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
             bool stop = false;
             for (uint32_t k = 0; k < sh->n_stop; k++) stop = stop || sh->stop[k] == tok;
             if (stop) { r->frozen = 1; park = 1; }      // reported, not evaluated, not counted (chat_with_bot.py:249-252)
-            else gp.counts[off + tok] += 1;
+            else { gp.counts[off + tok] += 1; mask.advance(b, V, tok); }
         }
         __syncthreads();
     }
@@ -270,6 +303,7 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
         if (draw) gate.publish(b, r->step - 1, tok);
         const bool active = !r->frozen;
         gp.n_generated[b] = r->step;
+        mask.report(b);
         gp.next_tokens[b] = active ? (int) tok : 0;
         if (active) atomicAdd(&sh->active, 1u);
         __threadfence();
@@ -288,7 +322,7 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
 template <int PER>
 __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    generate_step<PER>(gp, NoGate{});
+    generate_step<PER>(gp, NoGate{}, NoMask{});
 }
 
 // At one CTA per SM ptxas may give every thread 64 registers: with the default bound it holds PER <= 4 to 32, and the gate's wait
@@ -296,7 +330,23 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const G
 template <int PER>
 __global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sample_kernel(const GenStreamParams sp) {
     pdl_prologue();
-    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out});
+    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, NoMask{});
+}
+
+// The constrained twins of the two step kernels (rwkv_b200_generate_constrained); the blocking one ignores cp.stream's mapped words.
+// Both are bounded at one CTA per SM: with the default bound the mask's table read makes PER = 4 spill more than
+// generate_sample_kernel<4>.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_constrained_sample_kernel(const GenConstrainedParams cp) {
+    pdl_prologue();
+    generate_step<PER>(cp.stream.step, NoGate{}, TableMask{cp.mask, cp.states_out});
+}
+
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_constrained_sample_kernel(const GenConstrainedParams cp) {
+    pdl_prologue();
+    const GenStreamParams & sp = cp.stream;
+    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, TableMask{cp.mask, cp.states_out});
 }
 
 constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
@@ -309,23 +359,26 @@ __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const G
     for (size_t i = (size_t) blockIdx.x * RESTORE_THREADS + threadIdx.x; i < n; i += (size_t) gridDim.x * RESTORE_THREADS) dst[base + i] = src[base + i];
 }
 
-template <int PER> void * generate_step_fn(bool stream) {
+template <int PER> void * generate_step_fn(bool stream, bool constrained) {
+    if (constrained)
+        return stream ? reinterpret_cast<void *>(generate_stream_constrained_sample_kernel<PER>) : reinterpret_cast<void *>(generate_constrained_sample_kernel<PER>);
     return stream ? reinterpret_cast<void *>(generate_stream_sample_kernel<PER>) : reinterpret_cast<void *>(generate_sample_kernel<PER>);
 }
-void * generate_step_for(int n_vocab, bool stream) {
+void * generate_step_for(int n_vocab, bool stream, bool constrained) {
     const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? generate_step_fn<1>(stream) : per <= 4 ? generate_step_fn<4>(stream) : per <= 16 ? generate_step_fn<16>(stream)
-         : per <= 50 ? generate_step_fn<50>(stream) : generate_step_fn<64>(stream);
+    return per <= 1 ? generate_step_fn<1>(stream, constrained) : per <= 4 ? generate_step_fn<4>(stream, constrained)
+         : per <= 16 ? generate_step_fn<16>(stream, constrained) : per <= 50 ? generate_step_fn<50>(stream, constrained) : generate_step_fn<64>(stream, constrained);
 }
 
 // A step kernel node of graph g after deps with the single kernel parameter `arg`.
 template <class P>
-cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, bool stream, cudaGraphNode_t * node) {
+cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, bool stream, bool constrained,
+                          cudaGraphNode_t * node) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
     P copy = arg;
     void * args[] = {&copy};
     cudaKernelNodeParams kp = {};
-    kp.func = generate_step_for(p.n_vocab, stream);
+    kp.func = generate_step_for(p.n_vocab, stream, constrained);
     kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
     kp.kernelParams = args; kp.extra = nullptr;
     return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
@@ -345,11 +398,28 @@ cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s) {
 }
 
 cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p, p, false, node);
+    return add_step_node(g, deps, n_deps, p, p, false, false, node);
 }
 
 cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.step, p, true, node);
+    return add_step_node(g, deps, n_deps, p.step, p, true, false, node);
+}
+
+cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s) {
+    const GenStepParams & gp = p.stream.step;
+    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    const dim3 grid(gp.n_rows);
+    if (per <= 1) return launch_pdl(generate_constrained_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 4) return launch_pdl(generate_constrained_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 16) return launch_pdl(generate_constrained_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 50) return launch_pdl(generate_constrained_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return launch_pdl(generate_constrained_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+}
+
+cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
+                                               cudaGraphNode_t * node) {
+    return add_step_node(g, deps, n_deps, p.stream.step, p, stream, true, node);
 }
 
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {

@@ -186,6 +186,20 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_generate_stream.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step.argtypes = [ctypes.c_void_p]
         lib.rwkv_b200_test_generate_step.restype = ctypes.c_bool
+        P_U16 = ctypes.POINTER(ctypes.c_uint16)
+        lib.rwkv_b200_automaton_create.argtypes = [vp, P_U16, ctypes.c_size_t]
+        lib.rwkv_b200_automaton_create.restype = vp
+        lib.rwkv_b200_automaton_free.argtypes = [vp]
+        lib.rwkv_b200_automaton_free.restype = None
+        lib.rwkv_b200_generate_constrained.argtypes = [vp, vp, P_U32, ctypes.c_size_t, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                                       ctypes.c_bool, P_DOUBLE, P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32,
+                                                       ctypes.POINTER(ctypes.c_size_t)]
+        lib.rwkv_b200_generate_constrained.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_generate_constrained.argtypes = [vp, ctypes.POINTER(vp), P_U32, P_U32, P_FLOAT, P_FLOAT, P_FLOAT, P_FLOAT, P_U8, P_DOUBLE,
+                                                             P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, P_U32]
+        lib.rwkv_b200_batch_generate_constrained.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step_constrained.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32]
+        lib.rwkv_b200_test_generate_step_constrained.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
