@@ -74,6 +74,11 @@ RWKV_API size_t rwkv_b200_batch_size(const struct rwkv_context * ctx);   /* 0 fo
  * cutoff, power by 1/temperature, renormalise, inverse-CDF draw); only the 4-byte token id crosses PCIe instead of n_vocab floats.
  * `u` is a uniform number in [0, 1) from the caller's generator -- with u = numpy's RandomState.random_sample() the result is the
  * token numpy.random.choice would return in the reference. temperature >= 0, 0 <= top_p <= 1 (0 means 1), n_vocab <= 65536.
+ * Every draw (these calls, the batch calls and every generate step) follows three rules:
+ * - the drawn token has positive probability after bias, top-p and temperature, unless every biased logit is -inf or NaN;
+ * - tempering is relative to the largest kept probability, (p / p_max)^(1 / temperature), so no temperature > 0 underflows: a kept
+ *   token is lost only if its share is below 2^-149;
+ * - a bias list that names a token twice, or a token >= n_vocab, is refused with RWKV_ERROR_ARGS.
  * rwkv_b200_eval_sample = rwkv_b200_eval_resident(token, with logits) + rwkv_b200_sample without bias. */
 RWKV_API bool rwkv_b200_sample(struct rwkv_context * ctx, float temperature, float top_p, double u, const uint32_t * bias_ids, const float * bias_values,
                                size_t n_bias, uint32_t * token_out);

@@ -44,6 +44,54 @@ def sample_logits_u(logits: np.ndarray, temperature: float, top_p: float, u: flo
     return sample_probs_u(softmax(np.asarray(logits, dtype=np.float32).copy()), temperature, top_p, u, logit_bias)
 
 
+def probs64(logits: np.ndarray, temperature: float, top_p: float, logit_bias=None, float32_range: bool = True) -> np.ndarray:
+    """Each token's probability in float64 after bias, top-p and temperature: what the draw samples from, computed without the
+    float32 rounding of the reference and the kernel. The biased logit is the float32 sum logits + bias, as the C API defines it;
+    -inf becomes probability 0. With float32_range, so does a softmax probability below 2^-150, which the reference's float32
+    softmax rounds to 0 (at T = 8 such tokens would otherwise hold whole percents of the mass). Top-p is the rule of
+    sampling.py:42-45, keeping whole tie groups; tempering is exp((log p - log p_max) / T) over the kept tokens. temperature 0
+    gives the one-hot of the first maximum."""
+    x = np.asarray(logits, dtype=np.float32).copy()
+    if logit_bias:
+        for k, v in logit_bias.items():
+            x[k] = np.float32(x[k] + np.float32(v))
+    if temperature == 0.0:
+        out = np.zeros(x.size)
+        out[int(np.argmax(x))] = 1.0
+        return out
+    x = x.astype(np.float64)
+    e = np.exp(x - x.max())
+    p = e / e.sum()
+    if float32_range:
+        p[p < 2.0 ** -150] = 0.0
+    tp = 1.0 if top_p == 0.0 else float(top_p)
+    if tp < 1.0:
+        sp = np.sort(p)[::-1]
+        cutoff = sp[np.argmax(np.cumsum(sp) > tp)]
+        p = np.where(p >= cutoff, p, 0.0)
+    if temperature != 1.0:
+        kept = p > 0
+        lp = np.full(p.size, -np.inf)
+        lp[kept] = np.log(p[kept])
+        p = np.exp((lp - lp[kept].max()) / float(temperature))
+    return p / p.sum()
+
+
+def cdf64(probs: np.ndarray) -> np.ndarray:
+    """The float64 CDF of probs64: token t owns [cdf[t - 1], cdf[t])."""
+    c = np.cumsum(probs)
+    return c / c[-1]
+
+
+def top_p_boundaries(logits: np.ndarray, logit_bias=None) -> tuple:
+    """(values, cumulative) of the float64 probabilities' tie groups, largest first: top_p in [cumulative[k - 1], cumulative[k])
+    keeps groups 0 .. k."""
+    p = probs64(logits, 1.0, 1.0, logit_bias)
+    vals, counts = np.unique(p[p > 0], return_counts=True)
+    vals, counts = vals[::-1], counts[::-1]
+    return vals, np.cumsum(vals * counts)
+
+
 def boundary_distance(logits: np.ndarray, temperature: float, top_p: float, u: float, logit_bias=None) -> float:
     """How far u is from the nearest edge of the chosen token's CDF interval (tests skip knife-edge draws)."""
     probs = softmax(np.asarray(logits, dtype=np.float32).copy())

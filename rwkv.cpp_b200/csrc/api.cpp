@@ -425,6 +425,8 @@ bool rwkv_b200_sample_logits(const float * logits, size_t n_vocab, float tempera
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, logits && token_out && n_vocab > 0 && n_vocab <= 65536 && temperature >= 0.0f && top_p >= 0.0f && top_p <= 1.0f &&
                u >= 0.0 && u < 1.0 && (n_bias == 0 || (bias_ids && bias_values)), "Invalid sampling arguments");
+    std::vector<uint64_t> seen;
+    if (!check_bias_ids(sink, bias_ids, n_bias, n_vocab, seen)) return false;
     int dev = default_device(), n_dev = 0;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceCount(&n_dev) == cudaSuccess && dev < n_dev && cudaSetDevice(dev) == cudaSuccess,
                "No usable CUDA device; this engine has no CPU execution path");

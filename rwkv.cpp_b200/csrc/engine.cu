@@ -1104,8 +1104,8 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
         CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_token), 2 * sizeof(uint32_t)));
         CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_token_host), 2 * sizeof(uint32_t)));
     }
-    for (size_t i = 0; i < n_bias; i++)
-        RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, bias_ids[i] < (uint32_t) m.n_vocab, "logit bias id %u is out of range", bias_ids[i]);
+    std::vector<uint64_t> seen;
+    if (!check_bias_ids(ctx->sink(), bias_ids, n_bias, (size_t) m.n_vocab, seen)) return false;
     if (n_bias > 0 && !upload_bias(ctx, bias_ids, bias_values, n_bias, (size_t) m.n_vocab)) return false;
     SampleParams sp{};
     sp.logits = ctx->logits; sp.n_vocab = m.n_vocab; sp.temperature = temperature; sp.top_p = top_p; sp.u = u;
@@ -1119,6 +1119,20 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
 }
 
 static_assert(SAMPLE_MAX_ROWS == MAX_TOKENS_PER_PASS, "the batched sampling launch takes a row per sequence of the largest batch");
+
+bool check_bias_ids(ErrorSink sink, const uint32_t * bias_ids, size_t n_bias, size_t n_vocab, std::vector<uint64_t> & seen) {
+    if (seen.size() < (n_vocab + 63) / 64) seen.assign((n_vocab + 63) / 64, 0);
+    bool ok = true;
+    size_t i = 0;
+    for (; i < n_bias && ok; i++) {
+        const uint32_t id = bias_ids[i];
+        ok = id < n_vocab && !(seen[id >> 6] >> (id & 63) & 1);
+        if (ok) seen[id >> 6] |= 1ull << (id & 63);
+    }
+    for (size_t k = 0; k < i; k++) if (bias_ids[k] < n_vocab) seen[bias_ids[k] >> 6] = 0;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, ok, "logit bias id %u is %s", bias_ids[i - 1], bias_ids[i - 1] < n_vocab ? "given twice" : "out of range");
+    return true;
+}
 
 bool check_sample_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const float * temperature, const float * top_p, const double * u,
                        const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values, const uint32_t * tokens_out) {
@@ -1135,8 +1149,9 @@ bool check_sample_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const floa
     const size_t n_bias = bias_offsets[n_rows];
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_bias <= (size_t) INT32_MAX, "More than 2^31 - 1 logit bias entries");
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_bias == 0 || (bias_ids && bias_values), "logit bias arrays are NULL");
-    for (size_t i = 0; i < n_bias; i++)
-        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, bias_ids[i] < n_vocab, "logit bias id %u is out of range", bias_ids[i]);
+    std::vector<uint64_t> seen;
+    for (size_t b = 0; b < n_rows; b++)
+        if (!check_bias_ids(sink, bias_ids + bias_offsets[b], bias_offsets[b + 1] - bias_offsets[b], n_vocab, seen)) return false;
     return true;
 }
 

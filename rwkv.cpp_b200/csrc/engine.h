@@ -196,8 +196,13 @@ bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * 
 // [0, 1) in place of numpy's RandomState draw); only the token id is copied back. Requires a preceding pass that computed logits.
 bool sample_token(Context * ctx, float temperature, float top_p, double u, const uint32_t * bias_ids, const float * bias_values, size_t n_bias, uint32_t * token_out);
 
+// One row's logit bias ids: each below n_vocab and none twice (the kernel adds the entries without atomics, and the reference takes
+// a dict). `seen` is a bitmap of n_vocab bits, all clear on entry and on return.
+bool check_bias_ids(ErrorSink sink, const uint32_t * bias_ids, size_t n_bias, size_t n_vocab, std::vector<uint64_t> & seen);
+
 // The arguments of a draw for each of n_rows rows (batch_sample, the batched kernel's test hook): non-NULL arrays, every row's
-// temperature, top_p and u in range, and, with bias_offsets, offsets from 0 that never decrease and bias ids below n_vocab.
+// temperature, top_p and u in range, and, with bias_offsets, offsets from 0 that never decrease and bias ids below n_vocab, none
+// twice within a row.
 bool check_sample_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const float * temperature, const float * top_p, const double * u,
                        const uint32_t * bias_offsets, const uint32_t * bias_ids, const float * bias_values, const uint32_t * tokens_out);
 // rows[b] <- row b's parameters and its bias range (empty without bias_offsets); the arguments passed check_sample_rows.

@@ -50,10 +50,10 @@ template <int PER>
 __device__ __forceinline__ void sample_row(const SampleParams & p) {
     __shared__ double dslots[SAMPLE_WARPS];
     __shared__ float fslots[SAMPLE_WARPS];
-    __shared__ int first_flagged;
+    __shared__ int first_flagged, last_massive;
     const int tid = threadIdx.x, V = p.n_vocab, base = tid * PER;
     const float * src = p.logits;
-    if (p.n_bias > 0) {     // logits + bias through the scratch copy (a dict has no duplicate ids, :30-33)
+    if (p.n_bias > 0) {     // logits + bias through the scratch copy (a dict has no duplicate ids, :30-33; the callers reject them)
         for (int i = tid; i < V; i += SAMPLE_THREADS) p.scratch[i] = p.logits[i];
         __syncthreads();
         for (int i = tid; i < p.n_bias; i += SAMPLE_THREADS) if (p.bias_ids[i] < (uint32_t) V) p.scratch[p.bias_ids[i]] += p.bias_values[i];
@@ -112,10 +112,12 @@ __device__ __forceinline__ void sample_row(const SampleParams & p) {
 #pragma unroll
         for (int j = 0; j < PER; j++) if (v[j] < cutoff) v[j] = 0.f;
     }
-    if (p.temperature != 1.0f) {    // :47-48
-        const float inv_t = 1.0f / p.temperature;
+    if (p.temperature != 1.0f) {    // :47-48, relative to the largest probability so that no T > 0 underflows every kept token
+        // expf(0) = 1 is the largest softmax numerator and top-p always keeps it, so 1 / total is the largest kept probability.
+        // The largest tempered mass is then exactly 1, and a kept token is lost only if its share is below 2^-149.
+        const float inv_t = 1.0f / p.temperature, p_max = __fdiv_rn(1.0f, total);
 #pragma unroll
-        for (int j = 0; j < PER; j++) v[j] = (v[j] > 0.f) ? powf(v[j], inv_t) : 0.f;
+        for (int j = 0; j < PER; j++) v[j] = (v[j] > 0.f) ? powf(__fdiv_rn(v[j], p_max), inv_t) : 0.f;
     }
     double s2 = 0;
 #pragma unroll
@@ -134,28 +136,42 @@ __device__ __forceinline__ void sample_row(const SampleParams & p) {
     }
     __syncthreads();
     if ((tid & 31) == 31) dslots[tid >> 5] = incl;
-    if (tid == 0) first_flagged = SAMPLE_THREADS;
+    if (tid == 0) { first_flagged = SAMPLE_THREADS; last_massive = -1; }
     __syncthreads();
     double warp_base = 0, grand = 0;
     for (int w = 0; w < SAMPLE_WARPS; w++) { const double t = dslots[w]; if (w < (tid >> 5)) warp_base += t; grand += t; }
     const double before = warp_base + incl - mine;
-    if ((before + mine) / grand > p.u) atomicMin(&first_flagged, tid);
+    // The warp scan, the sum of the warp totals and the owner's element sum round differently, so near u = 1 a thread without mass
+    // can see its end above u while the last thread with mass does not: only a thread with mass may own the draw.
+    if (mine > 0.0 && (before + mine) / grand > p.u) atomicMin(&first_flagged, tid);
     __syncthreads();
     const int owner = first_flagged;
-    if (owner == SAMPLE_THREADS) {                 // u >= cdf[-1] (only for u == 1.0): the last token with any mass
-        if (tid == 0) { *p.token_out = (uint32_t) (V - 1); if (p.prob_out) *p.prob_out = 0.f; }
+    if (owner == SAMPLE_THREADS) {      // no end above u (u within rounding of 1): the last token with mass, or V - 1 if none has any
+        int last = -1;
+        float last_p = 0.f;
+#pragma unroll
+        for (int j = 0; j < PER; j++) if (v[j] > 0.f) { last = base + j; last_p = v[j]; }
+        if (last >= 0) atomicMax(&last_massive, last);
+        __syncthreads();
+        const int pick = last_massive;
+        if (pick < 0 ? tid == 0 : pick == last) {
+            *p.token_out = (uint32_t) (pick < 0 ? V - 1 : pick);
+            if (p.prob_out) *p.prob_out = last_p;
+        }
         return;
     }
     if (tid == owner) {
         double c = before;
-        int pick = min(base + PER - 1, V - 1);
+        int pick = base;
         float pp = 0.f;
 #pragma unroll
         for (int j = 0; j < PER; j++) {
+            if (!(v[j] > 0.f)) continue;
             c += (double) v[j];
-            if (c / grand > p.u) { pick = base + j; pp = v[j]; break; }
+            pick = base + j; pp = v[j];         // the owner has mass: if its own sum falls short of u, its last token with mass
+            if (c / grand > p.u) break;
         }
-        *p.token_out = (uint32_t) min(pick, V - 1);
+        *p.token_out = (uint32_t) pick;
         if (p.prob_out) *p.prob_out = pp;
     }
 }
@@ -239,8 +255,8 @@ struct TableMask {
         const GenMaskRow m = rows[b];
         return m.next ? m.next + (size_t) m.state * V : nullptr;
     }
-    // Thread 0, after the row evaluated tok. Only a row whose allowed tokens all have logit -inf or NaN can draw a token its state
-    // does not allow; that keeps the state.
+    // Thread 0, after the row evaluated tok. A draw never picks a token of zero mass while any token has mass, so only a row whose
+    // allowed tokens all have logit -inf or NaN can draw a token its state does not allow; that keeps the state.
     __device__ __forceinline__ void advance(int b, int V, uint32_t tok) const {
         GenMaskRow & m = rows[b];
         if (!m.next) return;

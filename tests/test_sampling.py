@@ -31,6 +31,26 @@ def test_oracle_matches_reference_sampling():
         assert got == c["token"], c
 
 
+def test_float64_restatement_holds_the_golden_draws():
+    """Every golden draw of the reference module lies in its token's interval of the float64 CDF (so.probs64 / so.cdf64), or within
+    eps = 2e-6 * max(1, 1 / T) of its edge where the reference's float32 rounding decides; temperature 0 is the float64 argmax."""
+    worst = 0.0
+    for c in CASES:
+        logits = make_logits(c["logits_seed"], c["n_vocab"], c["scale"])
+        p = so.probs64(logits, c["temperature"], c["top_p"], bias_of(c))
+        tok = c["token"]
+        assert p[tok] > 0, c
+        if c["temperature"] == 0.0:
+            continue
+        cdf = so.cdf64(p)
+        eps = 2e-6 * max(1.0, 1.0 / c["temperature"])
+        left = cdf[tok - 1] if tok > 0 else 0.0
+        err = max(left - c["u"], c["u"] - cdf[tok], 0.0)
+        worst = max(worst, err / eps)
+        assert err <= eps, (c, left, cdf[tok])
+    print("worst distance outside the float64 interval / eps: %.3g" % worst)
+
+
 def test_oracle_argument_errors():
     with pytest.raises(ValueError):
         so.sample_logits_u(np.zeros(8, np.float32), -1.0, 0.5, 0.1)
