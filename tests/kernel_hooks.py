@@ -209,7 +209,7 @@ class GemvBatchArgs(ctypes.Structure):
 
 
 GEMV_PATHS = {"engine": 0, "engine_batch_ctx": 1, "streaming": 2, "generic": 3, "tensor_cores": 4}
-LAUNCH_FAMILIES = ("streaming", "generic", "tensor_cores", "convert", "expand")
+LAUNCH_FAMILIES = ("streaming", "generic", "tensor_cores", "convert", "expand", "kquant", "kquant_expand")
 
 
 def gemv_batch(lib, T, problems, xs, path="engine"):

@@ -220,10 +220,10 @@ def random_raw(fmt, M, K, seed=0):
     return tid, blk.reshape(-1)
 
 
-def problem(fmt, M, K, T, rng, input=0, epi=kr.EPI_NONE, tiled=None, alias=True):
-    """One problem of a batch: weights, and the residual / gate / bias its epilogue reads. The bias puts a quarter of the rows deep
-    into the saturation of the sigmoid / exp(-exp) epilogues, on both sides."""
-    tid, raw = random_raw(fmt, M, K)
+def problem(fmt, M, K, T, rng, input=0, epi=kr.EPI_NONE, tiled=None, alias=True, weights=None):
+    """One problem of a batch: weights (random_raw's, or `weights` = (type, bytes) given), and the residual / gate / bias its epilogue
+    reads. The bias puts a quarter of the rows deep into the saturation of the sigmoid / exp(-exp) epilogues, on both sides."""
+    tid, raw = weights or random_raw(fmt, M, K)
     p = dict(type=tid, K=K, M=M, raw=raw, input=input, epi=epi, fmt=fmt,
              tiled=fmt != "FP32" and K % 64 == 0 if tiled is None else tiled)
     if epi in kr.RES_EPIS:
