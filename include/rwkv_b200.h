@@ -32,6 +32,14 @@ RWKV_API struct rwkv_context * rwkv_b200_init_from_file_ex(const char * model_fi
  *   rwkv_b200_state_load : state_in (host, may be NULL = fresh) -> device
  *   rwkv_b200_eval_resident: run n tokens from the resident state; logits stay on the device unless logits_out != NULL
  *   rwkv_b200_state_store: device -> state_out (host) */
+/* The resident state is the state after the context's most recent evaluation of any kind: rwkv_eval, rwkv_eval_sequence and
+ * rwkv_eval_sequence_in_chunks leave the state they computed resident too (whether or not state_out was given; state_in NULL starts
+ * them from a fresh state), so rwkv_b200_state_store after one of them returns the bytes of its state_out. rwkv_b200_profile_pass and
+ * rwkv_b200_time_resident are resident passes and advance it. rwkv_clone_context gives a new context that shares the weights and
+ * nothing else: its resident state is unspecified until rwkv_b200_state_load or a rwkv_eval* call sets it, it has no logits (a draw
+ * is refused until a pass computes them) and its penalty counts start from zero.
+ * The logits are those of the most recent pass that ran the head; a pass that skips it (want_logits false and logits_out NULL,
+ * rwkv_eval* with logits_out NULL) makes rwkv_b200_sample and rwkv_b200_generate* refuse with RWKV_ERROR_ARGS until the next one. */
 RWKV_API bool rwkv_b200_state_load(struct rwkv_context * ctx, const float * state_in);
 RWKV_API bool rwkv_b200_eval_resident(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, bool want_logits, float * logits_out);
 RWKV_API bool rwkv_b200_state_store(struct rwkv_context * ctx, float * state_out);
@@ -64,7 +72,10 @@ RWKV_API bool rwkv_b200_batch_eval(struct rwkv_context * batch, const uint32_t *
  * not a batch context gives RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED; NULL arrays, a sum of 0 or above 256 and a token >= n_vocab give
  * RWKV_ERROR_ARGS. Per sequence the result is bit-identical to feeding its tokens to a single-sequence context one at a time while the
  * sum stays below 16, and with rwkv_b200_set_tensor_cores(batch, false) at any sum. rwkv_b200_batch_sample / get_logits / get_state
- * work after it unchanged; an idle sequence's row draws from the column it still holds. */
+ * work after it unchanged; an idle sequence's row draws from the column it still holds. Validity is per context, the bytes per column:
+ * after a pass that skipped the head (rwkv_b200_batch_eval with want_logits false, or a ragged pass without logits on a context whose
+ * logits were not valid), a ragged pass with want_logits makes the logits valid again, and an idle sequence's column then holds the logits
+ * of the last pass that ran the head for it (zeros if none ever did), not those of its latest token. */
 RWKV_API bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits);
 RWKV_API bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out);
 RWKV_API size_t rwkv_b200_batch_size(const struct rwkv_context * ctx);   /* 0 for an ordinary context */
@@ -118,7 +129,9 @@ RWKV_API bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows,
  * a stop token included.
  * The penalty counts are a per-sequence table in HBM, allocated on first use. keep_counts false starts the sequence from zero counts;
  * true continues from its previous generate call, so that a server can generate in short windows (between ragged admissions in a
- * batch) without losing its penalties. At most RWKV_B200_GENERATE_MAX_STOP stop ids, shared by all sequences, each below n_vocab.
+ * batch) without losing its penalties. keep_counts applies to every sequence of an accepted call, also one that generates nothing
+ * (max_tokens[b] = 0, or a constrained sequence that starts in a state that allows no token): its state and logits are left as they
+ * are, its counts are cleared unless keep_counts[b] is set. At most RWKV_B200_GENERATE_MAX_STOP stop ids, shared by all sequences, each below n_vocab.
  * The whole loop is one CUDA-graph launch (a conditional WHILE node; a CUDA driver of 12.4 or newer); only the tokens come back.
  * Every argument is checked before anything is enqueued, and a rejected call changes no state, logits or count: a context of the
  * wrong kind (a batch context here, an ordinary one for the batch call, a pipeline or a stage of one) or an older driver gives
@@ -286,6 +299,7 @@ RWKV_API bool rwkv_b200_pipe_eval(struct rwkv_context * ctx, const uint32_t * to
 /* Measurement hooks. */
 RWKV_API float rwkv_b200_last_device_ms(const struct rwkv_context * ctx);     /* CUDA-event time of the last pass */
 RWKV_API uint64_t rwkv_b200_kernel_launch_count(void);                         /* kernels enqueued by this process */
+RWKV_API uint64_t rwkv_b200_graph_launch_count(void);   /* CUDA graphs launched by this process: single-token replays, generation loops */
 RWKV_API uint64_t rwkv_b200_bytes_per_token(const struct rwkv_context * ctx, bool with_logits);
 /* The part of that byte model the GEMV launches of the context's decode pass stream: every layer matrix (+ the head), at file
  * precision -- except, in a single-sequence context, the v6 LoRA matrices maa_w1 / decay_w2 of the layers whose single-token pass folds

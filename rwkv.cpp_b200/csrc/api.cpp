@@ -814,6 +814,7 @@ float rwkv_b200_last_device_ms(const struct rwkv_context * ctx) {
 }
 
 uint64_t rwkv_b200_kernel_launch_count(void) { return g_kernel_launches; }
+uint64_t rwkv_b200_graph_launch_count(void) { return g_graph_launches; }
 
 uint64_t rwkv_b200_gemv_bytes_per_token(const struct rwkv_context * ctx, bool with_logits) {
     const Model & m = *C(ctx)->model;

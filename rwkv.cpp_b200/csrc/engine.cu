@@ -550,6 +550,7 @@ bool run_layers(Context * ctx, int T, bool want_logits, int seg) {
     if (g && g->exec) {
         CUDA_OK(ctx, cudaGraphLaunch(g->exec, ctx->stream));
         g_kernel_launches += g->launches;
+        g_graph_launches++;
     } else if (g && g->uses >= 1) {
         // second use of this slot: capture the launch sequence once, replay from now on
         const unsigned long long before = g_kernel_launches;
@@ -563,6 +564,7 @@ bool run_layers(Context * ctx, int T, bool want_logits, int seg) {
         cudaGraphDestroy(graph);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, e == cudaSuccess, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
         CUDA_OK(ctx, cudaGraphLaunch(g->exec, ctx->stream));
+        g_graph_launches++;
     } else {
         if (g) g->uses++;
         if (!enqueue_pass(ctx, T, want_logits, phase, seg)) return false;
@@ -744,6 +746,7 @@ static bool bounce_enabled() {
 }
 // states below this size go the plain way (two helper threads cost ~0.1 ms); rwkv_b200_set_bounce_min_bytes moves the bar (tests)
 std::atomic<size_t> g_bounce_min_bytes{(size_t) 4 << 20};
+std::atomic<unsigned long long> g_graph_launches{0};
 CopyPool * new_copy_pool();
 static bool ensure_bounce(Context * ctx) {
     if (ctx->bounce_in) return true;
@@ -1507,6 +1510,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     cudaGraphExec_t & graph = ctx->gen_graphs[ctx->phase][streaming][constrained];
     if (!graph && !build_generate_graph(ctx, streaming, constrained)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
+    g_graph_launches++;
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     bool in_time = true;

@@ -148,6 +148,7 @@ struct Context {
 // Largest number of tokens pushed through the kernels in one go; longer sequences are cut into
 // pieces of this size with the state staying on the device.
 constexpr int MAX_TOKENS_PER_PASS = 256;
+extern std::atomic<unsigned long long> g_graph_launches;   // CUDA graphs launched by this process: single-token replays and generation loops
 extern std::atomic<size_t> g_bounce_min_bytes;   // pageable caller states of at least this many bytes travel through pinned bounce buffers
 
 Context * create_context(Model * model, ErrorSink sink, int batch_n = 0);   // batch_n > 0: a batch context for that many sequences

@@ -104,6 +104,8 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_last_device_ms.restype = ctypes.c_float
         lib.rwkv_b200_kernel_launch_count.argtypes = []
         lib.rwkv_b200_kernel_launch_count.restype = ctypes.c_uint64
+        lib.rwkv_b200_graph_launch_count.argtypes = []
+        lib.rwkv_b200_graph_launch_count.restype = ctypes.c_uint64
         lib.rwkv_b200_bytes_per_token.argtypes = [vp, ctypes.c_bool]
         lib.rwkv_b200_bytes_per_token.restype = ctypes.c_uint64
         lib.rwkv_b200_time_resident.argtypes = [vp, P_U32, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_bool]
