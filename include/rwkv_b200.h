@@ -80,6 +80,38 @@ RWKV_API bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uin
 RWKV_API bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out);
 RWKV_API size_t rwkv_b200_batch_size(const struct rwkv_context * ctx);   /* 0 for an ordinary context */
 
+/* Scoring a known text (perplexity, likelihood-based evaluation, "echo + logprobs"): the log-probability the model gives each of
+ * caller-given targets, computed on the device; no per-position logits cross PCIe.
+ *   rwkv_b200_score: advances the resident state of a single-sequence context over tokens[0 .. n_tokens) exactly as
+ *     rwkv_b200_eval_resident(ctx, tokens, n_tokens, true, NULL) does (same passes, same layer kernels). With z_i the logits after
+ *     tokens[0 .. i], for every i whose targets[i] is not RWKV_B200_SCORE_NO_TARGET: logprobs_out[i] = log_softmax(z_i)[targets[i]] and
+ *     greedy_out[i] = 1 if targets[i] is the first index of max(z_i), else 0 (greedy_out may be NULL). Other positions are not written.
+ *     For perplexity, targets[i] = tokens[i + 1] and the last target is the first token of the next window, or NO_TARGET.
+ *     Afterwards the resident state is what rwkv_b200_eval_resident leaves, the logits are z_{n-1} as the scoring head computed them
+ *     (rwkv_b200_sample / rwkv_b200_generate* can follow), and the penalty counts are untouched.
+ *   rwkv_b200_batch_score_ragged: the same over a ragged pass of a batch context, with the rules of rwkv_b200_batch_eval_ragged (with
+ *     want_logits); targets, logprobs_out and greedy_out are indexed like tokens. Multiple-choice scoring: set k sequences to one prefix
+ *     state and score k continuations in one pass over the weights.
+ * The output pointers may be host or device memory; both calls synchronise before they return. A log-probability is computed from the
+ * head's float logits in double (sum of expf(z - max), then log); -inf logits contribute nothing, a -inf target gives -inf, and a
+ * position whose logits hold a NaN or +inf, or nothing finite, gives NaN with greedy 0. Passes of >= 32 tokens (batch contexts: >= 16)
+ * with tensor cores on run the head on the tensor cores, from a tile-major copy of the head (2 bytes per weight) that the first such
+ * pass builds and the model keeps until its last context is freed; their logits carry the rounding of that path. Every other pass
+ * runs the head's GEMV on every column, which gives each position the bits rwkv_eval gives it token by token.
+ * Refusals change no state, logits or validity: RWKV_ERROR_ARGS for NULL tokens, targets or logprobs_out, no tokens, a token >= n_vocab,
+ * a target >= n_vocab other than NO_TARGET, n_vocab > 65536 and the ragged count rules; RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED for the
+ * wrong kind of context, a pipeline handle or stage, and a call from inside a streaming callback of the context. A failed allocation of
+ * the head's copy gives RWKV_ERROR_CTX | RWKV_ERROR_ALLOC before anything is enqueued. */
+#define RWKV_B200_SCORE_NO_TARGET 0xFFFFFFFFu
+RWKV_API bool rwkv_b200_score(struct rwkv_context * ctx, const uint32_t * tokens, const uint32_t * targets, size_t n_tokens,
+                              float * logprobs_out, uint8_t * greedy_out);
+RWKV_API bool rwkv_b200_batch_score_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts,
+                                           const uint32_t * targets, float * logprobs_out, uint8_t * greedy_out);
+/* Test hook: the scoring kernel on n_rows x n_vocab host logits (row-major), no model needed. Rows whose target is NO_TARGET keep what
+ * logprobs_out / greedy_out held. */
+RWKV_API bool rwkv_b200_score_logits(const float * logits, size_t n_rows, size_t n_vocab, const uint32_t * targets,
+                                     float * logprobs_out, uint8_t * greedy_out);
+
 /* On-device sampling (SURVEY.md 8f-4): the next token is drawn on the GPU from the logits of the most recent evaluation that
  * computed them, following the reference's python/sampling.py:10-52 (softmax, optional logit bias, temperature 0 = argmax, top-p
  * cutoff, power by 1/temperature, renormalise, inverse-CDF draw); only the 4-byte token id crosses PCIe instead of n_vocab floats.

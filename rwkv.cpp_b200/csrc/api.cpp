@@ -411,6 +411,63 @@ bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, fl
 }
 size_t rwkv_b200_batch_size(const struct rwkv_context * ctx) { return (size_t) C(ctx)->batch_n; }
 
+static_assert(RWKV_B200_SCORE_NO_TARGET == SCORE_NO_TARGET, "no-target marker of the header and the kernel");
+
+// The arguments every scoring entry point checks: non-NULL arrays, n > 0, n_vocab <= 65536 and every target below n_vocab or
+// SCORE_NO_TARGET (tokens: tokens_checked, or here).
+static bool score_args_ok(ErrorSink sink, size_t n_vocab, const uint32_t * tokens, bool tokens_checked, const uint32_t * targets, size_t n,
+                          const float * logprobs_out) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, tokens && targets && logprobs_out, "NULL tokens, targets or logprobs_out");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n > 0, "No tokens");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n_vocab > 0 && n_vocab <= 65536, "Scoring supports n_vocab <= 65536, not %zu", n_vocab);
+    for (size_t i = 0; !tokens_checked && i < n; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, tokens[i] < n_vocab, "Token at index %zu (%" PRIu32 ") is out of range (0 .. %zu)", i, tokens[i], n_vocab - 1);
+    for (size_t i = 0; i < n; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, targets[i] < n_vocab || targets[i] == SCORE_NO_TARGET,
+                   "Target at index %zu (%" PRIu32 ") is out of range (0 .. %zu, or RWKV_B200_SCORE_NO_TARGET)", i, targets[i], n_vocab - 1);
+    return true;
+}
+
+bool rwkv_b200_score(struct rwkv_context * ctx, const uint32_t * tokens, const uint32_t * targets, size_t n_tokens, float * logprobs_out, uint8_t * greedy_out) {
+    Context * c = C(ctx);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0 && !c->group && whole_model(c),
+               "Scoring takes a single-sequence context of the whole model: use rwkv_b200_batch_score_ragged on a batch context; pipelines are not supported");
+    if (!score_args_ok(c->sink(), (size_t) c->model->n_vocab, tokens, false, targets, n_tokens, logprobs_out)) return false;
+    return score(c, tokens, targets, n_tokens, logprobs_out, greedy_out);
+}
+
+bool rwkv_b200_batch_score_ragged(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, const uint32_t * targets,
+                                  float * logprobs_out, uint8_t * greedy_out) {
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    size_t total = 0;
+    if (!check_ragged(c, tokens, counts, total)) return false;
+    if (!score_args_ok(c->sink(), (size_t) c->model->n_vocab, tokens, true, targets, total, logprobs_out)) return false;
+    return batch_score_ragged(c, tokens, counts, targets, logprobs_out, greedy_out);
+}
+
+bool rwkv_b200_score_logits(const float * logits, size_t n_rows, size_t n_vocab, const uint32_t * targets, float * logprobs_out, uint8_t * greedy_out) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, logits && n_rows <= (size_t) 1 << 24, "NULL logits or more than 2^24 rows");
+    if (!score_args_ok(sink, n_vocab, targets, true, targets, n_rows, logprobs_out)) return false;
+    if (!hook_device(sink)) return false;
+    HookBuffers hb;     // the results start as the caller's buffers (rows without a target are not written) and return at their exact size
+    ScoreParams sp{};
+    sp.logits = hb.in(logits, n_rows * n_vocab); sp.n_vocab = (int) n_vocab; sp.T = (int) n_rows;
+    sp.targets = hb.in(targets, n_rows);
+    sp.logprobs = const_cast<float *>(hb.in(logprobs_out, n_rows));
+    sp.greedy = greedy_out ? const_cast<uint8_t *>(hb.in(greedy_out, n_rows)) : nullptr;
+    const cudaError_t e = hb.ok ? launch_score(sp, 0) : cudaSuccess;
+    bool ok = hb.finish(e) && cudaMemcpy(logprobs_out, sp.logprobs, n_rows * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess;
+    if (ok && greedy_out) ok = cudaMemcpy(greedy_out, sp.greedy, n_rows, cudaMemcpyDeviceToHost) == cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "scoring failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
 bool rwkv_b200_sample(struct rwkv_context * ctx, float temperature, float top_p, double u, const uint32_t * bias_ids, const float * bias_values, size_t n_bias,
                       uint32_t * token_out) {
     Context * c = C(ctx);

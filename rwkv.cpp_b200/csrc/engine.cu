@@ -469,6 +469,41 @@ bool ensure_capacity(Context * ctx, int T) {
     return true;
 }
 
+// The head of a scoring pass of T columns runs on the tensor cores when the layers of such a pass would (T >= 32 in a single-sequence
+// context, >= BATCH_TC_MIN in a batch context, tensor cores on) and the head's type and width have a tile-major form.
+bool score_on_tensor_cores(const Context * ctx, int T) {
+    const Model & m = *ctx->model;
+    return T >= (ctx->batch_n > 0 ? BATCH_TC_MIN : 32) && ctx->use_tensor_cores && getenv("RWKV_B200_NO_TC") == nullptr &&
+           gemm_tc_eligible(m.head.type, m.head.K);
+}
+
+// Head of a scoring pass: logits of every column into score_logits [T, n_vocab], the scoring kernel over them, and the last column of
+// every advancing sequence (of the pass, for a single sequence) into its logits column.
+bool score_head(Context * ctx, const Scratch & s, int T) {
+    const Model & m = *ctx->model;
+    const int C = m.n_embed, V = m.n_vocab;
+    Batch b(T);
+    if (score_on_tensor_cores(ctx, T)) {
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.head_tiled && ctx->act16, "The head has no tile-major copy");
+        // the columns' LayerNorm goes to mix[0], which the layers no longer need
+        CUDA_OK(ctx, launch_layer_norm_columns(s.x, m.ln_out_w.data, m.ln_out_b.data, C, T, s.mix[0], ctx->stream));
+        GemvProblem & p = b.add(m.head, s.mix[0], ctx->score_logits);
+        p.Wt = m.head_tiled;
+        CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, ctx->stream, ctx->act16, ctx->act16_bytes));
+    } else {
+        GemvProblem & p = b.add(m.head, s.x, ctx->score_logits);
+        p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
+        if (!run_batch(ctx, b)) return false;
+    }
+    ScoreParams sp{};
+    sp.logits = ctx->score_logits; sp.n_vocab = V; sp.T = T;
+    sp.targets = ctx->pass_targets; sp.logprobs = ctx->pass_lp; sp.greedy = ctx->pass_greedy;
+    CUDA_OK(ctx, launch_score(sp, ctx->stream));
+    if (ctx->pass_seq_off) CUDA_OK(ctx, launch_copy_columns(ctx->score_logits, ctx->pass_head_col, ctx->logits, ctx->pass_head_seq, V, ctx->pass_n_active, ctx->stream));
+    else CUDA_OK(ctx, launch_copy_columns(ctx->score_logits + (size_t) (T - 1) * V, nullptr, ctx->logits, nullptr, V, 1, ctx->stream));
+    return true;
+}
+
 // Enqueues one pass (token upload + every kernel) on ctx->stream; pure stream work, so it can be captured.
 bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
     const Model & m = *ctx->model;
@@ -497,7 +532,9 @@ bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
         }
         if (!ok || !ffn(ctx, L, s, T, flp)) return false;
     }
-    if (want_logits && l1 == m.n_layer && ctx->pass_seq_off) {
+    if (ctx->pass_targets && l1 == m.n_layer) {
+        if (!score_head(ctx, s, T)) return false;
+    } else if (want_logits && l1 == m.n_layer && ctx->pass_seq_off) {
         // ragged: the head on the last column of every advancing sequence, gathered; its columns go to those sequences' logits
         const int n = ctx->pass_n_active;
         CUDA_OK(ctx, launch_copy_columns(s.x, ctx->pass_head_col, ctx->head_x, nullptr, C, n, ctx->stream));
@@ -683,6 +720,7 @@ void destroy_context(Context * ctx) {
         if (ctx->slot_free[i]) cudaEventDestroy(ctx->slot_free[i]);
     }
     cudaFree(ctx->ragged_map); cudaFree(ctx->head_x); cudaFree(ctx->head_y);
+    cudaFree(ctx->score_logits); cudaFree(ctx->score_targets); cudaFree(ctx->score_lp); cudaFree(ctx->score_greedy);
     for (auto & g : ctx->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (ctx->copy_pool) destroy_copy_pool(ctx->copy_pool);
     if (ctx->bounce_in) { cudaFreeHost(ctx->bounce_in); cudaFreeHost(ctx->bounce_out); cudaFreeHost(ctx->bounce_logits); }
@@ -1008,16 +1046,23 @@ bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits) {
 // Ints of one ragged map (Context::ragged_host): offsets [B + 1], column sequences [MAX_TOKENS_PER_PASS], head columns and sequences [B each].
 static size_t ragged_map_ints(int B) { return (size_t) 3 * B + 1 + MAX_TOKENS_PER_PASS; }
 
-bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
+bool check_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, size_t & total) {
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ctx->batch_n > 0, "Not a batch context");
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, tokens && counts, "NULL tokens or counts");
     const Model & m = *ctx->model;
-    const int B = ctx->batch_n;
-    size_t total = 0;
-    for (int b = 0; b < B; b++) total += counts[b];
+    total = 0;
+    for (int b = 0; b < ctx->batch_n; b++) total += counts[b];
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, total >= 1 && total <= (size_t) MAX_TOKENS_PER_PASS, "A ragged pass takes 1 .. %d tokens in all, not %zu", MAX_TOKENS_PER_PASS, total);
     for (size_t i = 0; i < total; i++)
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, tokens[i] < (uint32_t) m.n_vocab, "Token at index %zu (%" PRIu32 ") is out of range (0 .. %d)", i, tokens[i], m.n_vocab - 1);
+    return true;
+}
+
+bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
+    size_t total = 0;
+    if (!check_ragged(ctx, tokens, counts, total)) return false;
+    const Model & m = *ctx->model;
+    const int B = ctx->batch_n;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     const size_t map_bytes = ragged_map_ints(B) * sizeof(int);
     if (!ctx->ragged_map) {
@@ -1070,6 +1115,103 @@ bool batch_get_logits(Context * ctx, int seq, float * logits_out) {
     CUDA_OK(ctx, cudaMemcpyAsync(logits_out, ctx->logits + (size_t) seq * V, V * sizeof(float), cudaMemcpyDefault, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return true;
+}
+
+namespace {
+
+// The head's tile-major copy (Model::head_tiled), built once per model by the first scoring pass that routes its head to the tensor
+// cores: 2 bytes per weight, so a model that is never scored that way does not pay for it.
+bool ensure_head_tiled(Context * ctx) {
+    Model & m = *ctx->model;
+    std::lock_guard<std::mutex> lk(m.head_tiled_lock);
+    if (m.head_tiled) return true;
+    const size_t bytes = gemm_tc_tiled_bytes(m.head.type, m.head.M, m.head.K);
+    void * p = nullptr;
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) cudaGetLastError();
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes for the head's tile-major copy: %s", bytes, cudaGetErrorString(e));
+    e = gemm_tc_repack(m.head.data, m.head.pitch, m.head.type, m.head.M, m.head.K, p, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // other contexts' streams use it from now on
+    if (e != cudaSuccess) cudaFree(p);
+    CUDA_OK(ctx, e);
+    m.head_tiled = static_cast<uint8_t *>(p);
+    return true;
+}
+
+// The scoring buffers for a call of n tokens (the targets and results grow to the largest call so far), and the head's tile-major copy
+// if any pass of the call routes its head to the tensor cores. Allocates, enqueues nothing.
+bool prepare_score(Context * ctx, size_t n, bool any_tc) {
+    const Model & m = *ctx->model;
+    CUDA_OK(ctx, cudaSetDevice(m.dev.device));
+    auto alloc = [&](void ** p, size_t bytes) {
+        const cudaError_t e = cudaMalloc(p, bytes);
+        if (e != cudaSuccess) { cudaGetLastError(); *p = nullptr; }
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes of scoring buffers: %s", bytes, cudaGetErrorString(e));
+        return true;
+    };
+    if (!ctx->score_logits && !alloc(reinterpret_cast<void **>(&ctx->score_logits), (size_t) MAX_TOKENS_PER_PASS * m.n_vocab * sizeof(float))) return false;
+    if (n > ctx->score_capacity) {
+        CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+        cudaFree(ctx->score_targets); cudaFree(ctx->score_lp); cudaFree(ctx->score_greedy);
+        ctx->score_targets = nullptr; ctx->score_lp = nullptr; ctx->score_greedy = nullptr; ctx->score_capacity = 0;
+        size_t cap = 256;
+        while (cap < n) cap *= 2;
+        if (!alloc(reinterpret_cast<void **>(&ctx->score_targets), cap * sizeof(uint32_t)) || !alloc(reinterpret_cast<void **>(&ctx->score_lp), cap * sizeof(float)) ||
+            !alloc(reinterpret_cast<void **>(&ctx->score_greedy), cap)) return false;
+        ctx->score_capacity = cap;
+    }
+    return !any_tc || ensure_head_tiled(ctx);
+}
+
+// Targets in, and the caller's outputs too, so that positions without a target come back as they were.
+bool score_copy_in(Context * ctx, const uint32_t * targets, size_t n, const float * logprobs_out, const uint8_t * greedy_out) {
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_targets, targets, n * sizeof(uint32_t), cudaMemcpyDefault, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_lp, logprobs_out, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_greedy, greedy_out, n, cudaMemcpyDefault, ctx->stream));
+    return true;
+}
+
+bool score_copy_out(Context * ctx, size_t n, float * logprobs_out, uint8_t * greedy_out) {
+    CUDA_OK(ctx, cudaMemcpyAsync(logprobs_out, ctx->score_lp, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(greedy_out, ctx->score_greedy, n, cudaMemcpyDefault, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return true;
+}
+
+void end_score_pass(Context * ctx) { ctx->pass_targets = nullptr; ctx->pass_lp = nullptr; ctx->pass_greedy = nullptr; }
+
+}  // namespace
+
+bool score(Context * ctx, const uint32_t * tokens, const uint32_t * targets, size_t n, float * logprobs_out, uint8_t * greedy_out) {
+    // the passes of forward(): MAX_TOKENS_PER_PASS tokens each, then the rest; only the first can be the longest
+    const int first = (int) std::min(n, (size_t) MAX_TOKENS_PER_PASS);
+    if (!prepare_score(ctx, n, score_on_tensor_cores(ctx, first))) return false;
+    if (!score_copy_in(ctx, targets, n, logprobs_out, greedy_out)) return false;
+    for (size_t done = 0; done < n;) {
+        const int T = (int) std::min(n - done, (size_t) MAX_TOKENS_PER_PASS);
+        ctx->pass_targets = ctx->score_targets + done;
+        ctx->pass_lp = ctx->score_lp + done;
+        ctx->pass_greedy = greedy_out ? ctx->score_greedy + done : nullptr;
+        // enqueue_pass directly: a scoring pass is never captured into a graph or replayed from one
+        const bool ok = begin_pass(ctx, tokens + done, T) && enqueue_pass(ctx, T, true, ctx->phase, 0) && end_pass(ctx, T, true);
+        end_score_pass(ctx);
+        if (!ok) return false;
+        done += (size_t) T;
+    }
+    return score_copy_out(ctx, n, logprobs_out, greedy_out);
+}
+
+bool batch_score_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, const uint32_t * targets, float * logprobs_out, uint8_t * greedy_out) {
+    size_t total = 0;
+    if (!check_ragged(ctx, tokens, counts, total)) return false;
+    if (!prepare_score(ctx, total, score_on_tensor_cores(ctx, (int) total))) return false;
+    if (!score_copy_in(ctx, targets, total, logprobs_out, greedy_out)) return false;
+    ctx->pass_targets = ctx->score_targets;
+    ctx->pass_lp = ctx->score_lp;
+    ctx->pass_greedy = greedy_out ? ctx->score_greedy : nullptr;
+    const bool ok = batch_eval_ragged(ctx, tokens, counts, true);
+    end_score_pass(ctx);
+    return ok && score_copy_out(ctx, total, logprobs_out, greedy_out);
 }
 
 namespace {

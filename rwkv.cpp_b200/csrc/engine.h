@@ -105,6 +105,17 @@ struct Context {
     // while a ragged pass is being enqueued: its device map, and how many sequences advance (the head's columns)
     const int * pass_seq_off = nullptr, * pass_col_seq = nullptr, * pass_head_col = nullptr, * pass_head_seq = nullptr;
     int pass_n_active = 0;
+    // Scoring passes (score, batch_score_ragged), allocated on the first: the head's output for every column of a pass
+    // ([MAX_TOKENS_PER_PASS, n_vocab]), and the targets and results of a call's tokens (score_capacity entries each).
+    float * score_logits = nullptr;
+    uint32_t * score_targets = nullptr;
+    float * score_lp = nullptr;
+    uint8_t * score_greedy = nullptr;
+    size_t score_capacity = 0;
+    // while a scoring pass is being enqueued: the targets of its columns and where their results go (greedy may be NULL)
+    const uint32_t * pass_targets = nullptr;
+    float * pass_lp = nullptr;
+    uint8_t * pass_greedy = nullptr;
 
     // On-device sampling (kernels/sampling.cu): result word, scratch for biased logits, device copy of the caller's logit bias.
     bool logits_valid = false;       // ctx->logits holds the head output of the most recent pass
@@ -188,6 +199,18 @@ bool batch_set_state(Context * ctx, int seq, const float * state_in);
 bool batch_get_state(Context * ctx, int seq, float * state_out);
 bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits);
 bool batch_get_logits(Context * ctx, int seq, float * logits_out);
+// Ragged pass arguments (batch_eval_ragged, batch_score_ragged): a batch context, non-NULL arrays, 1 <= sum of counts <= MAX_TOKENS_PER_PASS
+// (returned in total), every token below n_vocab.
+bool check_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, size_t & total);
+
+// Scoring (rwkv_b200_score / rwkv_b200_batch_score_ragged, include/rwkv_b200.h): the passes of forward(tokens, n, want_logits) or of
+// batch_eval_ragged(tokens, counts, want_logits), with the head over every column of a pass and the scoring kernel over its output:
+// logprobs_out[i] / greedy_out[i] (host or device pointers; greedy_out may be NULL) for every i whose target is not SCORE_NO_TARGET, the
+// others left as they were. The logits of the last column (of every advancing sequence) go to ctx->logits. The head runs on the tensor
+// cores (score_on_tensor_cores) or as the GEMV with the LayerNorm prologue. The arguments are checked by the caller, except the ragged
+// counts, which batch_score_ragged checks before it enqueues anything. Never a CUDA graph. Synchronises.
+bool score(Context * ctx, const uint32_t * tokens, const uint32_t * targets, size_t n, float * logprobs_out, uint8_t * greedy_out);
+bool batch_score_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, const uint32_t * targets, float * logprobs_out, uint8_t * greedy_out);
 // Ragged pass: sequence b advances counts[b] tokens (tokens back to back in sequence order; 0 leaves it exactly as it was), all in one
 // pass over the weights. Checks every argument before it enqueues anything. want_logits: the logits column of every sequence with
 // counts[b] > 0 receives the logits of its last token, the other columns keep what they held. Never replays a CUDA graph.

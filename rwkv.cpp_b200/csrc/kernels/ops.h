@@ -137,6 +137,23 @@ cudaError_t launch_wkv7(const Wkv7Params & p, cudaStream_t s);
 // ragged pass of a batch context gathers the last column of every advancing sequence for the head and scatters the head's output.
 cudaError_t launch_copy_columns(const float * src, const int * src_col, float * dst, const int * dst_col, int rows, int n, cudaStream_t s);
 
+// Scoring passes (score.cu). y[:, t] = LN(x[:, t]; w, b) for t < T, columns of C floats, with the arithmetic of the head GEMV's
+// PRO_LAYERNORM prologue: the tensor-core head of a scoring pass contracts these columns.
+cudaError_t launch_layer_norm_columns(const float * x, const float * w, const float * b, int C, int T, float * y, cudaStream_t s);
+// One CTA per column t < T of logits ([T, n_vocab], column t at logits + t * n_vocab): unless targets[t] is SCORE_NO_TARGET,
+// logprobs[t] = log_softmax(column)[targets[t]] and, if greedy, greedy[t] = 1 when targets[t] is the first index of the column's
+// maximum, else 0. A column with a NaN or +inf, or with no finite value, gives NaN and 0. Columns without a target are not written.
+constexpr uint32_t SCORE_NO_TARGET = 0xFFFFFFFFu;
+struct ScoreParams {
+    TraceRec * trace = nullptr;
+    const float * logits;
+    int n_vocab, T;
+    const uint32_t * targets;         // [T]
+    float * logprobs;                 // [T]
+    uint8_t * greedy;                 // [T] or NULL
+};
+cudaError_t launch_score(const ScoreParams & p, cudaStream_t s);
+
 // Layer-pipeline hand-off over peer memory (pipe.cu). A PipeBox sits at the start of every stage's mailbox allocation, followed by
 // PIPE_SLOTS data areas of slot_floats floats each.
 constexpr int PIPE_SLOTS = 2;

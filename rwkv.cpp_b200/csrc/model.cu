@@ -15,7 +15,8 @@
 namespace rwkv {
 
 Model::~Model() {
-    if (arena || link.box) cudaSetDevice(dev.device);
+    if (arena || link.box || head_tiled) cudaSetDevice(dev.device);
+    cudaFree(head_tiled);
     if (link.prev && link.prev_ipc) cudaIpcCloseMemHandle(link.prev);
     if (link.next && link.next_ipc) cudaIpcCloseMemHandle(link.next);
     cudaFree(link.box);
@@ -300,7 +301,8 @@ Model * load_model(const char * path, int device, int layer_begin, int layer_end
             r.arena_offset = arena_bytes;
             arena_bytes += align_up((size_t) M * (size_t) pitch + 256, 256);
             // every per-layer matrix also gets the tile-major copy the tensor-core prefill kernel streams (gemm_tc.cu); the
-            // embedding is a gather and the head only ever sees the last token of a pass
+            // embedding is a gather, and every pass but a scoring pass runs the head on one column per sequence (a scoring pass builds
+            // the head's copy when it first needs it, Model::head_tiled)
             if (tc_copies && r.name != "emb.weight" && r.name != "head.weight") {
                 r.tiled_bytes = gemm_tc_tiled_bytes((int) t.data_type, (int) M, (int) K);
                 r.tiled_offset = arena_bytes;

@@ -5,6 +5,7 @@
 #pragma once
 #include <atomic>
 #include <cstdint>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -80,6 +81,10 @@ struct Model {
     size_t head_bytes = 0;
     size_t gemv_bytes_per_token = 0;     // of which: matrices streamed by the fused dequantize-GEMV (layer matrices + head)
     size_t head_matrix_bytes = 0;
+    // The head's tile-major copy for the tensor-core head of scoring passes (engine.cu: ensure_head_tiled), built by the first one
+    // that needs it, under head_tiled_lock, and freed with the model. Every other pass streams the head with the GEMV.
+    uint8_t * head_tiled = nullptr;
+    std::mutex head_tiled_lock;
     std::atomic<int> refcount{0};
     PipeLink link;
     std::string device_name;

@@ -13,6 +13,7 @@ P_U32 = ctypes.POINTER(ctypes.c_uint32)
 # rwkv_b200_token_fn (include/rwkv_b200.h): int (*)(void * user, size_t sequence, size_t index, uint32_t token)
 RWKV_TOKEN_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_uint32)
 
+SCORE_NO_TARGET = 0xFFFFFFFF   # RWKV_B200_SCORE_NO_TARGET (include/rwkv_b200.h)
 QUANTIZED_FORMAT_NAMES = ("Q4_0", "Q4_1", "Q4_K", "Q5_0", "Q5_1", "Q5_K", "Q8_0")   # the reference binding's list, in its order
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -202,6 +203,12 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_generate_constrained.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_constrained.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32]
         lib.rwkv_b200_test_generate_step_constrained.restype = ctypes.c_bool
+        lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
+        lib.rwkv_b200_score.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
+        lib.rwkv_b200_batch_score_ragged.restype = ctypes.c_bool
+        lib.rwkv_b200_score_logits.argtypes = [P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, P_U32, P_FLOAT, P_U8]
+        lib.rwkv_b200_score_logits.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
