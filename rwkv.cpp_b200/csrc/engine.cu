@@ -1,6 +1,6 @@
 // Forward pass over a resident model: the per-architecture launch sequences.
 // Math follows rwkv_graph.inc (serial graph :611-720, sequence graph :744-866); every stage below
-// names the graph lines it covers. All launches go to ctx->stream; nothing here blocks the host
+// names the graph lines it covers. All launches of a pass go to its stream (Pass::stream); nothing here blocks the host
 // except the token upload.
 #include "engine.h"
 
@@ -95,6 +95,30 @@ Scratch carve(const Model & m, float * base, int T) {
     return s;
 }
 
+// Everything one pass reads that is not the context's standing state: make_pass fills in the defaults, an entry point changes what
+// its pass needs. Nothing of a pass is left on the context for the next one to find.
+struct Pass {
+    int T = 0;
+    bool want_logits = false;
+    int phase = 0;                        // ctx->phase: the pinned token slot, and the graph slot of a single-token pass
+    cudaStream_t stream = nullptr;        // ctx->stream, or the stream of a pipeline stage's caller
+    float * state_in = nullptr, * state_out = nullptr;   // ctx->state_a -> ctx->state_b
+    float * logits = nullptr;             // where the head writes: ctx->logits
+    Scratch s{};                          // ctx->scratch carved for T tokens
+    bool tokens_in_place = false;         // ctx->tokens already holds the tokens (the generation loop's step writes them): no upload
+    // Pipeline-stage hand-off (SURVEY.md 8e): device pointers of the caller, or NULL.
+    // Layout: x f32[C x T], then (v7 only) v_first f32[C x T].
+    const float * hidden_in = nullptr;
+    float * hidden_out = nullptr;
+    // a ragged pass: its device map (Context::ragged_map), and how many sequences advance (the head's columns)
+    const int * seq_off = nullptr, * col_seq = nullptr, * head_col = nullptr, * head_seq = nullptr;
+    int n_active = 0;
+    // a scoring pass: the targets of its columns and where their results go (greedy may be NULL)
+    const uint32_t * targets = nullptr;
+    float * lp = nullptr;
+    uint8_t * greedy = nullptr;
+};
+
 // ---- GEMV batch builder -------------------------------------------------------------------------
 struct Batch {
     GemvBatch b;
@@ -136,24 +160,24 @@ void xq_bind(GemvProblem & p, const unsigned char * q, int q_type) {
 // wherever the reference's tests compare states. Every eligible problem goes, however small: a tensor-core launch has a fixed cost
 // of tens of microseconds even for the 160 x 4096 LoRA matrix of a v6 layer, but the multi-column GEMV is worse for such a matrix
 // at T = 128 (32 column groups), and a 7B chunk measured slower with a 2^20-weight threshold than with none.
-bool launch_batch(Context * ctx, GemvBatch & b) {
+bool launch_batch(Context * ctx, GemvBatch & b, cudaStream_t stream) {
     // tensor cores: chunks of >= 32 tokens; batch contexts (one token of each of B sequences: nothing to stay bit-identical with
     // across pass sizes) from 16 sequences on, where the multi-column SIMT consumer is instruction-bound
     void * ws = ctx->use_tensor_cores ? ctx->act16 : nullptr;
-    CUDA_OK(ctx, gemv_route(b, ctx->model->dev, ctx->stream, ws, ctx->act16_bytes, ctx->batch_n > 0 ? BATCH_TC_MIN : 32));
+    CUDA_OK(ctx, gemv_route(b, ctx->model->dev, stream, ws, ctx->act16_bytes, ctx->batch_n > 0 ? BATCH_TC_MIN : 32));
     return true;
 }
 
-bool run_batch(Context * ctx, Batch & batch) {
-    if (!ctx->profiling) return launch_batch(ctx, batch.b);
+bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
+    if (!ctx->profiling) return launch_batch(ctx, batch.b, p.stream);
     Context::ProfRecord rec{};
     CUDA_OK(ctx, cudaEventCreate(&rec.start));
     CUDA_OK(ctx, cudaEventCreate(&rec.stop));
     for (int i = 0; i < batch.b.n; i++)
         rec.bytes += (double) tensor_nbytes(batch.b.p[i].type, (uint64_t) batch.b.p[i].K, (uint64_t) batch.b.p[i].M, 1);
-    CUDA_OK(ctx, cudaEventRecord(rec.start, ctx->stream));
-    if (!launch_batch(ctx, batch.b)) return false;
-    CUDA_OK(ctx, cudaEventRecord(rec.stop, ctx->stream));
+    CUDA_OK(ctx, cudaEventRecord(rec.start, p.stream));
+    if (!launch_batch(ctx, batch.b, p.stream)) return false;
+    CUDA_OK(ctx, cudaEventRecord(rec.stop, p.stream));
     ctx->prof.push_back(rec);
     return true;
 }
@@ -174,123 +198,123 @@ bool run_batch(Context * ctx, Batch & batch) {
 //     robustness test of the 64-channel fixture (not understood). 1 % was not worth an unexplained failure.
 
 // LayerNorm + mix parameters of the channel-mixing block (rwkv_ffn_v4_v5 :484-511, rwkv_ffn_v6 :513-531, rwkv_ffn_v7 :533-543).
-LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out) {
+LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out) {
     const Model & m = *ctx->model;
     LnMixParams lp{};
-    lp.x = s.x; lp.ln_w = L.ln2_w.data; lp.ln_b = L.ln2_b.data;
-    lp.state_in = st_in; lp.state_out = st_out; lp.C = m.n_embed; lp.T = T; lp.seq_stride = ctx->batch_stride;
-    lp.seq_off = ctx->pass_seq_off; lp.col_seq = ctx->pass_col_seq;
+    lp.x = p.s.x; lp.ln_w = L.ln2_w.data; lp.ln_b = L.ln2_b.data;
+    lp.state_in = st_in; lp.state_out = st_out; lp.C = m.n_embed; lp.T = p.T; lp.seq_stride = ctx->batch_stride;
+    lp.seq_off = p.seq_off; lp.col_seq = p.col_seq;
     if (m.arch_major == 7) {
-        lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.ffn_x_k.data; lp.out[0] = s.mix[0];
+        lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.ffn_x_k.data; lp.out[0] = p.s.mix[0];
     } else if (m.arch_major == 6) {
         lp.formula = 1; lp.n_out = 2;
-        lp.coef[0] = L.ffn_maa_k.data; lp.out[0] = s.mix[0];
-        lp.coef[1] = L.ffn_maa_r.data; lp.out[1] = s.mix[1];
+        lp.coef[0] = L.ffn_maa_k.data; lp.out[0] = p.s.mix[0];
+        lp.coef[1] = L.ffn_maa_r.data; lp.out[1] = p.s.mix[1];
     } else {
         lp.formula = 0; lp.n_out = 2;
-        lp.coef[0] = L.ffn_time_mix_k.data; lp.out[0] = s.mix[0];
-        lp.coef[1] = L.ffn_time_mix_r.data; lp.out[1] = s.mix[1];
+        lp.coef[0] = L.ffn_time_mix_k.data; lp.out[0] = p.s.mix[0];
+        lp.coef[1] = L.ffn_time_mix_r.data; lp.out[1] = p.s.mix[1];
     }
     return lp;
 }
 
 // Channel mixing, all versions.
-bool ffn(Context * ctx, const Layer & L, const Scratch & s, int T, const LnMixParams & lp) {
+bool ffn(Context * ctx, const Layer & L, const Pass & p, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
-    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
     {
-        Batch b(T);
-        b.add(L.ffn_key, s.mix[0], s.ffn_k, EPI_RELU_SQR);
-        if (m.arch_major != 7) b.add(L.ffn_receptance, s.mix[1], s.ffn_r, EPI_SIGMOID);
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        b.add(L.ffn_key, p.s.mix[0], p.s.ffn_k, EPI_RELU_SQR);
+        if (m.arch_major != 7) b.add(L.ffn_receptance, p.s.mix[1], p.s.ffn_r, EPI_SIGMOID);
+        if (!run_batch(ctx, p, b)) return false;
     }
     {
-        Batch b(T);
-        GemvProblem & p = b.add(L.ffn_value, s.ffn_k, s.x, m.arch_major == 7 ? EPI_ADD : EPI_MUL_ADD);
-        p.res = s.x; p.ldres = C;
-        p.gate = s.ffn_r; p.ldgate = C;
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        GemvProblem & q = b.add(L.ffn_value, p.s.ffn_k, p.s.x, m.arch_major == 7 ? EPI_ADD : EPI_MUL_ADD);
+        q.res = p.s.x; q.ldres = C;
+        q.gate = p.s.ffn_r; q.ldgate = C;
+        if (!run_batch(ctx, p, b)) return false;
     }
     return true;
 }
 
 // yq: y as a staged column (written by the WKV kernel) or NULL
-bool att_output(Context * ctx, const Layer & L, const Scratch & s, int T, const unsigned char * yq) {
-    Batch b(T);
-    GemvProblem & p = b.add(L.att_output, s.y, s.x, EPI_ADD);   // x + Wo.y  (:182/:291/:384/:481 + residual :667-679)
-    p.res = s.x; p.ldres = ctx->model->n_embed;
-    xq_bind(p, yq, L.att_output.type);
-    return run_batch(ctx, b);
+bool att_output(Context * ctx, const Layer & L, const Pass & p, const unsigned char * yq) {
+    Batch b(p.T);
+    GemvProblem & q = b.add(L.att_output, p.s.y, p.s.x, EPI_ADD);   // x + Wo.y  (:182/:291/:384/:481 + residual :667-679)
+    q.res = p.s.x; q.ldres = ctx->model->n_embed;
+    xq_bind(q, yq, L.att_output.type);
+    return run_batch(ctx, p, b);
 }
 
 // LayerNorm + mix parameters of the time-mixing block, per architecture (:94-97, :306-311, :400-413).
-LnMixParams att_ln(const Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out) {
+LnMixParams att_ln(const Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     LnMixParams lp{};
-    lp.x = s.x; lp.ln_w = L.ln1_w.data; lp.ln_b = L.ln1_b.data;
-    lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = T; lp.seq_stride = ctx->batch_stride;
-    lp.seq_off = ctx->pass_seq_off; lp.col_seq = ctx->pass_col_seq;
+    lp.x = p.s.x; lp.ln_w = L.ln1_w.data; lp.ln_b = L.ln1_b.data;
+    lp.state_in = st_in + C; lp.state_out = st_out + C; lp.C = C; lp.T = p.T; lp.seq_stride = ctx->batch_stride;
+    lp.seq_off = p.seq_off; lp.col_seq = p.col_seq;
     if (m.arch_major == 7) {
         lp.formula = 1; lp.n_out = 6;
-        for (int j = 0; j < 6; j++) { lp.coef[j] = L.att_x_rwkvag.data + (size_t) j * C; lp.out[j] = s.mix[j]; }   // r w k v a g
+        for (int j = 0; j < 6; j++) { lp.coef[j] = L.att_x_rwkvag.data + (size_t) j * C; lp.out[j] = p.s.mix[j]; }   // r w k v a g
     } else if (m.arch_major == 6) {
-        lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.att_maa_x.data; lp.out[0] = s.mix[0];
-        lp.out_xx = s.xx; lp.out_sx = s.sx;
+        lp.formula = 1; lp.n_out = 1; lp.coef[0] = L.att_maa_x.data; lp.out[0] = p.s.mix[0];
+        lp.out_xx = p.s.xx; lp.out_sx = p.s.sx;
     } else {
         const bool v52 = m.arch_major == 5 && m.arch_minor >= 2;
         lp.formula = 0; lp.n_out = v52 ? 4 : 3;
-        lp.coef[0] = L.att_time_mix_k.data; lp.out[0] = s.mix[0];
-        lp.coef[1] = L.att_time_mix_v.data; lp.out[1] = s.mix[1];
-        lp.coef[2] = L.att_time_mix_r.data; lp.out[2] = s.mix[2];
-        if (v52) { lp.coef[3] = L.att_time_mix_g.data; lp.out[3] = s.mix[3]; }
+        lp.coef[0] = L.att_time_mix_k.data; lp.out[0] = p.s.mix[0];
+        lp.coef[1] = L.att_time_mix_v.data; lp.out[1] = p.s.mix[1];
+        lp.coef[2] = L.att_time_mix_r.data; lp.out[2] = p.s.mix[2];
+        if (v52) { lp.coef[3] = L.att_time_mix_g.data; lp.out[3] = p.s.mix[3]; }
     }
     return lp;
 }
 
-bool att_v4(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
+bool att_v4(Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out, const LnMixParams & lp) {
     const int C = ctx->model->n_embed;
-    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
-    Batch b(T);
-    b.add(L.att_receptance, s.mix[2], s.r, EPI_SIGMOID);
-    b.add(L.att_key, s.mix[0], s.k);
-    b.add(L.att_value, s.mix[1], s.v);
-    if (!run_batch(ctx, b)) return false;
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    Batch b(p.T);
+    b.add(L.att_receptance, p.s.mix[2], p.s.r, EPI_SIGMOID);
+    b.add(L.att_key, p.s.mix[0], p.s.k);
+    b.add(L.att_value, p.s.mix[1], p.s.v);
+    if (!run_batch(ctx, p, b)) return false;
     Wkv4Params wp{};
-    wp.k = s.k; wp.v = s.v; wp.r = s.r;
+    wp.k = p.s.k; wp.v = p.s.v; wp.r = p.s.r;
     wp.time_first = L.att_time_first.data; wp.time_decay = L.att_time_decay.data;
     wp.aa_in = st_in + 2 * C; wp.bb_in = st_in + 3 * C; wp.pp_in = st_in + 4 * C;
     wp.aa_out = st_out + 2 * C; wp.bb_out = st_out + 3 * C; wp.pp_out = st_out + 4 * C;
-    wp.y = s.y; wp.C = C; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
-    wp.q_out = (C % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, launch_wkv4(wp, ctx->stream));
-    return att_output(ctx, L, s, T, wp.q_out);
+    wp.y = p.s.y; wp.C = C; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
+    wp.q_out = (C % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    CUDA_OK(ctx, launch_wkv4(wp, p.stream));
+    return att_output(ctx, L, p, wp.q_out);
 }
 
-bool att_v5(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
+bool att_v5(Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     const bool v52 = m.arch_minor >= 2;
-    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
-    Batch b(T);
-    b.add(L.att_receptance, s.mix[2], s.r);
-    b.add(L.att_key, s.mix[0], s.k);
-    b.add(L.att_value, s.mix[1], s.v);
-    if (v52) b.add(L.att_gate, s.mix[3], s.g, EPI_SILU);
-    if (!run_batch(ctx, b)) return false;
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    Batch b(p.T);
+    b.add(L.att_receptance, p.s.mix[2], p.s.r);
+    b.add(L.att_key, p.s.mix[0], p.s.k);
+    b.add(L.att_value, p.s.mix[1], p.s.v);
+    if (v52) b.add(L.att_gate, p.s.mix[3], p.s.g, EPI_SILU);
+    if (!run_batch(ctx, p, b)) return false;
     Wkv6Params wp{};
-    wp.r = s.r; wp.k = s.k; wp.v = s.v;
+    wp.r = p.s.r; wp.k = p.s.k; wp.v = p.s.v;
     wp.td = L.att_time_decay.data; wp.td_per_token = 0;
     wp.tf = v52 ? L.att_time_faaaa.data : L.att_time_first.data;
     wp.per_head_scalars = v52 ? 0 : 1;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
-    wp.g = v52 ? s.g : nullptr;
-    wp.y = s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
-    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
-    return att_output(ctx, L, s, T, wp.q_out);
+    wp.g = v52 ? p.s.g : nullptr;
+    wp.y = p.s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
+    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    CUDA_OK(ctx, launch_wkv6(wp, p.stream));
+    return att_output(ctx, L, p, wp.q_out);
 }
 
 }  // namespace
@@ -338,100 +362,100 @@ size_t v6_folded_gemv_bytes(const Model & m) {
 
 namespace {
 
-bool att_v6(Context * ctx, const Layer & L, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
+bool att_v6(Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     // single-token passes of one sequence: maa_w1 folded into the LayerNorm-mix launch and decay_w2 into the WKV launch
     GemvProblem w1{}, dw2{};
-    const bool fold = T == 1 && !ctx->batch_stride && v6_lora_fold(L, m.n_embed, m.head_size, w1, dw2);
+    const bool fold = p.T == 1 && !ctx->batch_stride && v6_lora_fold(L, m.n_embed, m.head_size, w1, dw2);
     if (fold) {
-        w1.x = s.mix[0]; w1.y = s.lora[0];
-        dw2.x = s.lora[1]; dw2.bias = L.att_time_decay.data;     // dw2's output is the WKV kernel's decay row in shared memory
-        CUDA_OK(ctx, launch_v6_prologue(lp, w1, ctx->stream));
+        w1.x = p.s.mix[0]; w1.y = p.s.lora[0];
+        dw2.x = p.s.lora[1]; dw2.bias = L.att_time_decay.data;     // dw2's output is the WKV kernel's decay row in shared memory
+        CUDA_OK(ctx, launch_v6_prologue(lp, w1, p.stream));
     } else {
-        CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
-        Batch b(T);   // :313-321  tanh(W1 . xxx)
-        b.add(L.att_maa_w1, s.mix[0], s.lora[0], EPI_TANH);
-        if (!run_batch(ctx, b)) return false;
+        CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+        Batch b(p.T);   // :313-321  tanh(W1 . xxx)
+        b.add(L.att_maa_w1, p.s.mix[0], p.s.lora[0], EPI_TANH);
+        if (!run_batch(ctx, p, b)) return false;
     }
     V6LerpParams vp{};   // :323-346
-    vp.w2 = L.att_maa_w2.data; vp.z = s.lora[0]; vp.xx = s.xx; vp.sx = s.sx;
+    vp.w2 = L.att_maa_w2.data; vp.z = p.s.lora[0]; vp.xx = p.s.xx; vp.sx = p.s.sx;
     vp.maa[0] = L.att_maa_w.data; vp.maa[1] = L.att_maa_k.data; vp.maa[2] = L.att_maa_v.data;
     vp.maa[3] = L.att_maa_r.data; vp.maa[4] = L.att_maa_g.data;
-    for (int j = 0; j < 5; j++) vp.out[j] = s.mix[1 + j];   // w, k, v, r, g
-    vp.C = C; vp.T = T; vp.mix = L.maa_mix;
+    for (int j = 0; j < 5; j++) vp.out[j] = p.s.mix[1 + j];   // w, k, v, r, g
+    vp.C = C; vp.T = p.T; vp.mix = L.maa_mix;
     {   // staged columns for the five consumers (w, k, v, r, g order of the lerp outputs): all or none
         const DevMatrix * cons[5] = {&L.att_decay_w1, &L.att_key, &L.att_value, &L.att_receptance, &L.att_gate};
         bool all = C % 32 == 0;
-        for (int j = 0; j < 5; j++) { vp.q_out[j] = xq_slot(ctx, T, XQ_LERP + j, *cons[j]); vp.q_type[j] = cons[j]->type; all = all && vp.q_out[j]; }
+        for (int j = 0; j < 5; j++) { vp.q_out[j] = xq_slot(ctx, p.T, XQ_LERP + j, *cons[j]); vp.q_type[j] = cons[j]->type; all = all && vp.q_out[j]; }
         if (!all) for (int j = 0; j < 5; j++) vp.q_out[j] = nullptr;
     }
-    CUDA_OK(ctx, launch_v6_lerp(vp, ctx->stream));
+    CUDA_OK(ctx, launch_v6_lerp(vp, p.stream));
     {   // :349-363
-        Batch b(T);
-        xq_bind(b.add(L.att_receptance, s.mix[4], s.r), vp.q_out[3], vp.q_type[3]);
-        xq_bind(b.add(L.att_key, s.mix[2], s.k), vp.q_out[1], vp.q_type[1]);
-        xq_bind(b.add(L.att_value, s.mix[3], s.v), vp.q_out[2], vp.q_type[2]);
-        xq_bind(b.add(L.att_gate, s.mix[5], s.g, EPI_SILU), vp.q_out[4], vp.q_type[4]);
-        xq_bind(b.add(L.att_decay_w1, s.mix[1], s.lora[1], EPI_TANH), vp.q_out[0], vp.q_type[0]);
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        xq_bind(b.add(L.att_receptance, p.s.mix[4], p.s.r), vp.q_out[3], vp.q_type[3]);
+        xq_bind(b.add(L.att_key, p.s.mix[2], p.s.k), vp.q_out[1], vp.q_type[1]);
+        xq_bind(b.add(L.att_value, p.s.mix[3], p.s.v), vp.q_out[2], vp.q_type[2]);
+        xq_bind(b.add(L.att_gate, p.s.mix[5], p.s.g, EPI_SILU), vp.q_out[4], vp.q_type[4]);
+        xq_bind(b.add(L.att_decay_w1, p.s.mix[1], p.s.lora[1], EPI_TANH), vp.q_out[0], vp.q_type[0]);
+        if (!run_batch(ctx, p, b)) return false;
     }
     if (!fold) {   // :357-367  w = exp(-exp(Wd2 . tanh(..) + time_decay))
-        Batch b(T);
-        GemvProblem & p = b.add(L.att_decay_w2, s.lora[1], s.w, EPI_BIAS_EXPNEGEXP);
-        p.bias = L.att_time_decay.data;
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        GemvProblem & q = b.add(L.att_decay_w2, p.s.lora[1], p.s.w, EPI_BIAS_EXPNEGEXP);
+        q.bias = L.att_time_decay.data;
+        if (!run_batch(ctx, p, b)) return false;
     }
     Wkv6Params wp{};   // :370-382
-    wp.r = s.r; wp.k = s.k; wp.v = s.v;
-    wp.td = fold ? nullptr : s.w; wp.td_per_token = fold ? 0 : 1; wp.tf = L.att_time_faaaa.data; wp.per_head_scalars = 0;
+    wp.r = p.s.r; wp.k = p.s.k; wp.v = p.s.v;
+    wp.td = fold ? nullptr : p.s.w; wp.td_per_token = fold ? 0 : 1; wp.tf = L.att_time_faaaa.data; wp.per_head_scalars = 0;
     if (fold) wp.dw2 = dw2;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
-    wp.g = s.g; wp.y = s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
-    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, launch_wkv6(wp, ctx->stream));
-    return att_output(ctx, L, s, T, wp.q_out);
+    wp.g = p.s.g; wp.y = p.s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
+    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    CUDA_OK(ctx, launch_wkv6(wp, p.stream));
+    return att_output(ctx, L, p, wp.q_out);
 }
 
-bool att_v7(Context * ctx, const Layer & L, int layer, const Scratch & s, int T, const float * st_in, float * st_out, const LnMixParams & lp) {
+bool att_v7(Context * ctx, const Layer & L, int layer, const Pass & p, const float * st_in, float * st_out, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     const bool first = layer == 0;
-    float * v_dst = first ? s.v_first : s.v;
-    CUDA_OK(ctx, launch_ln_mix(lp, ctx->stream));
+    float * v_dst = first ? p.s.v_first : p.s.v;
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
     {   // :415-432, 439, 447 -- first halves of the LoRA pairs
-        Batch b(T);
-        b.add(L.att_receptance, s.mix[0], s.r);
-        b.add(L.att_key, s.mix[2], s.k);
-        b.add(L.att_value, s.mix[3], v_dst);
-        b.add(L.att_w1, s.mix[1], s.lora[0], EPI_TANH);
-        b.add(L.att_a1, s.mix[4], s.lora[1]);
-        b.add(L.att_g1, s.mix[5], s.lora[2], EPI_SIGMOID);
-        if (!first) b.add(L.att_v1, s.mix[3], s.lora[3]);
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        b.add(L.att_receptance, p.s.mix[0], p.s.r);
+        b.add(L.att_key, p.s.mix[2], p.s.k);
+        b.add(L.att_value, p.s.mix[3], v_dst);
+        b.add(L.att_w1, p.s.mix[1], p.s.lora[0], EPI_TANH);
+        b.add(L.att_a1, p.s.mix[4], p.s.lora[1]);
+        b.add(L.att_g1, p.s.mix[5], p.s.lora[2], EPI_SIGMOID);
+        if (!first) b.add(L.att_v1, p.s.mix[3], p.s.lora[3]);
+        if (!run_batch(ctx, p, b)) return false;
     }
     {   // second halves
-        Batch b(T);
-        GemvProblem & pw = b.add(L.att_w2, s.lora[0], s.w, EPI_BIAS_W7);      pw.bias = L.att_w0.data;
-        GemvProblem & pa = b.add(L.att_a2, s.lora[1], s.a, EPI_BIAS_SIGMOID); pa.bias = L.att_a0.data;
-        b.add(L.att_g2, s.lora[2], s.g);
-        if (!first) { GemvProblem & pv = b.add(L.att_v2, s.lora[3], s.vgate, EPI_BIAS_SIGMOID); pv.bias = L.att_v0.data; }
-        if (!run_batch(ctx, b)) return false;
+        Batch b(p.T);
+        GemvProblem & pw = b.add(L.att_w2, p.s.lora[0], p.s.w, EPI_BIAS_W7);      pw.bias = L.att_w0.data;
+        GemvProblem & pa = b.add(L.att_a2, p.s.lora[1], p.s.a, EPI_BIAS_SIGMOID); pa.bias = L.att_a0.data;
+        b.add(L.att_g2, p.s.lora[2], p.s.g);
+        if (!first) { GemvProblem & pv = b.add(L.att_v2, p.s.lora[3], p.s.vgate, EPI_BIAS_SIGMOID); pv.bias = L.att_v0.data; }
+        if (!run_batch(ctx, p, b)) return false;
     }
     Wkv7Params wp{};   // :433-479
-    wp.r = s.r; wp.w = s.w; wp.k = s.k; wp.v = v_dst; wp.a = s.a; wp.g = s.g;
-    wp.vgate = first ? nullptr : s.vgate; wp.v_first = s.v_first; wp.v_out = nullptr;
+    wp.r = p.s.r; wp.w = p.s.w; wp.k = p.s.k; wp.v = v_dst; wp.a = p.s.a; wp.g = p.s.g;
+    wp.vgate = first ? nullptr : p.s.vgate; wp.v_first = p.s.v_first; wp.v_out = nullptr;
     wp.k_k = L.att_k_k.data; wp.k_a = L.att_k_a.data; wp.r_k = L.att_r_k.data;
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
-    wp.y = s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = T; wp.seq_stride = ctx->batch_stride; wp.seq_off = ctx->pass_seq_off; wp.n_seq = ctx->batch_n;
-    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
-    CUDA_OK(ctx, launch_wkv7(wp, ctx->stream));
-    return att_output(ctx, L, s, T, wp.q_out);
+    wp.y = p.s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
+    wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    CUDA_OK(ctx, launch_wkv7(wp, p.stream));
+    return att_output(ctx, L, p, wp.q_out);
 }
 
-bool ensure_capacity(Context * ctx, int T) {
+bool ensure_capacity(Context * ctx, int T, cudaStream_t stream) {
     if (T <= ctx->capacity_T) return true;
     const Model & m = *ctx->model;
     int cap = ctx->capacity_T ? ctx->capacity_T : 1;
@@ -440,7 +464,7 @@ bool ensure_capacity(Context * ctx, int T) {
     if (ctx->scratch) { cudaFree(ctx->scratch); ctx->scratch = nullptr; }
     if (ctx->act16) { cudaFree(ctx->act16); ctx->act16 = nullptr; ctx->act16_bytes = 0; }
     if (ctx->tokens) { cudaFree(ctx->tokens); ctx->tokens = nullptr; }
-    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(stream));
     for (int i = 0; i < 2; i++) {
         if (ctx->tokens_host[i]) { cudaFreeHost(ctx->tokens_host[i]); ctx->tokens_host[i] = nullptr; }
         ctx->slot_used[i] = false;
@@ -469,6 +493,17 @@ bool ensure_capacity(Context * ctx, int T) {
     return true;
 }
 
+// A pass of T tokens with the defaults of Pass on `stream` (NULL: the context's), once the context has room for T tokens.
+bool make_pass(Context * ctx, int T, bool want_logits, cudaStream_t stream, Pass & p) {
+    p = Pass{};
+    p.stream = stream ? stream : ctx->stream;
+    if (!ensure_capacity(ctx, T, p.stream)) return false;
+    p.T = T; p.want_logits = want_logits; p.phase = ctx->phase;
+    p.state_in = ctx->state_a; p.state_out = ctx->state_b; p.logits = ctx->logits;
+    p.s = carve(*ctx->model, ctx->scratch, T);
+    return true;
+}
+
 // The head of a scoring pass of T columns runs on the tensor cores when the layers of such a pass would (T >= 32 in a single-sequence
 // context, >= BATCH_TC_MIN in a batch context, tensor cores on) and the head's type and width have a tile-major form.
 bool score_on_tensor_cores(const Context * ctx, int T) {
@@ -479,75 +514,74 @@ bool score_on_tensor_cores(const Context * ctx, int T) {
 
 // Head of a scoring pass: logits of every column into score_logits [T, n_vocab], the scoring kernel over them, and the last column of
 // every advancing sequence (of the pass, for a single sequence) into its logits column.
-bool score_head(Context * ctx, const Scratch & s, int T) {
+bool score_head(Context * ctx, const Pass & p) {
     const Model & m = *ctx->model;
-    const int C = m.n_embed, V = m.n_vocab;
+    const int C = m.n_embed, V = m.n_vocab, T = p.T;
     Batch b(T);
     if (score_on_tensor_cores(ctx, T)) {
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.head_tiled && ctx->act16, "The head has no tile-major copy");
         // the columns' LayerNorm goes to mix[0], which the layers no longer need
-        CUDA_OK(ctx, launch_layer_norm_columns(s.x, m.ln_out_w.data, m.ln_out_b.data, C, T, s.mix[0], ctx->stream));
-        GemvProblem & p = b.add(m.head, s.mix[0], ctx->score_logits);
-        p.Wt = m.head_tiled;
-        CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, ctx->stream, ctx->act16, ctx->act16_bytes));
+        CUDA_OK(ctx, launch_layer_norm_columns(p.s.x, m.ln_out_w.data, m.ln_out_b.data, C, T, p.s.mix[0], p.stream));
+        GemvProblem & q = b.add(m.head, p.s.mix[0], ctx->score_logits);
+        q.Wt = m.head_tiled;
+        CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, p.stream, ctx->act16, ctx->act16_bytes));
     } else {
-        GemvProblem & p = b.add(m.head, s.x, ctx->score_logits);
-        p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
-        if (!run_batch(ctx, b)) return false;
+        GemvProblem & q = b.add(m.head, p.s.x, ctx->score_logits);
+        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        if (!run_batch(ctx, p, b)) return false;
     }
     ScoreParams sp{};
     sp.logits = ctx->score_logits; sp.n_vocab = V; sp.T = T;
-    sp.targets = ctx->pass_targets; sp.logprobs = ctx->pass_lp; sp.greedy = ctx->pass_greedy;
-    CUDA_OK(ctx, launch_score(sp, ctx->stream));
-    if (ctx->pass_seq_off) CUDA_OK(ctx, launch_copy_columns(ctx->score_logits, ctx->pass_head_col, ctx->logits, ctx->pass_head_seq, V, ctx->pass_n_active, ctx->stream));
-    else CUDA_OK(ctx, launch_copy_columns(ctx->score_logits + (size_t) (T - 1) * V, nullptr, ctx->logits, nullptr, V, 1, ctx->stream));
+    sp.targets = p.targets; sp.logprobs = p.lp; sp.greedy = p.greedy;
+    CUDA_OK(ctx, launch_score(sp, p.stream));
+    if (p.seq_off) CUDA_OK(ctx, launch_copy_columns(ctx->score_logits, p.head_col, p.logits, p.head_seq, V, p.n_active, p.stream));
+    else CUDA_OK(ctx, launch_copy_columns(ctx->score_logits + (size_t) (T - 1) * V, nullptr, p.logits, nullptr, V, 1, p.stream));
     return true;
 }
 
-// Enqueues one pass (token upload + every kernel) on ctx->stream; pure stream work, so it can be captured.
-bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
+// Enqueues segment `seg` of pass p (token upload + every kernel) on its stream; pure stream work, so it can be captured.
+bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
     const Model & m = *ctx->model;
     int l0, l1;
     segment_range(ctx, seg, l0, l1);
     g_trace_base = ctx->trace_buf;
     g_trace_next = 0;
-    const int C = m.n_embed;
-    const Scratch s = carve(m, ctx->scratch, T);
+    const int C = m.n_embed, T = p.T;
     if (l0 == 0) {
-        if (!ctx->tokens_on_device) CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, m.ln0_w.data, m.ln0_b.data, s.x, ctx->stream));
+        if (!p.tokens_in_place) CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[p.phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, p.stream));
+        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, m.ln0_w.data, m.ln0_b.data, p.s.x, p.stream));
     }   // a later pipeline stage / layer group finds x (and v_first) already in place
     const size_t per_layer = m.state_floats_per_layer();
     for (int i = l0; i < l1; i++) {
         const Layer & L = m.layers[i];
-        const float * st_in = ctx->state_a + (size_t) i * per_layer;
-        float * st_out = ctx->state_b + (size_t) i * per_layer;
-        const LnMixParams alp = att_ln(ctx, L, s, T, st_in, st_out), flp = ffn_ln(ctx, L, s, T, st_in, st_out);
+        const float * st_in = p.state_in + (size_t) i * per_layer;
+        float * st_out = p.state_out + (size_t) i * per_layer;
+        const LnMixParams alp = att_ln(ctx, L, p, st_in, st_out), flp = ffn_ln(ctx, L, p, st_in, st_out);
         bool ok;
         switch (m.arch_major) {
-            case 7: ok = att_v7(ctx, L, i, s, T, st_in, st_out, alp); break;
-            case 6: ok = att_v6(ctx, L, s, T, st_in, st_out, alp); break;
-            case 5: ok = att_v5(ctx, L, s, T, st_in, st_out, alp); break;
-            default: ok = att_v4(ctx, L, s, T, st_in, st_out, alp); break;
+            case 7: ok = att_v7(ctx, L, i, p, st_in, st_out, alp); break;
+            case 6: ok = att_v6(ctx, L, p, st_in, st_out, alp); break;
+            case 5: ok = att_v5(ctx, L, p, st_in, st_out, alp); break;
+            default: ok = att_v4(ctx, L, p, st_in, st_out, alp); break;
         }
-        if (!ok || !ffn(ctx, L, s, T, flp)) return false;
+        if (!ok || !ffn(ctx, L, p, flp)) return false;
     }
-    if (ctx->pass_targets && l1 == m.n_layer) {
-        if (!score_head(ctx, s, T)) return false;
-    } else if (want_logits && l1 == m.n_layer && ctx->pass_seq_off) {
+    if (p.targets && l1 == m.n_layer) {
+        if (!score_head(ctx, p)) return false;
+    } else if (p.want_logits && l1 == m.n_layer && p.seq_off) {
         // ragged: the head on the last column of every advancing sequence, gathered; its columns go to those sequences' logits
-        const int n = ctx->pass_n_active;
-        CUDA_OK(ctx, launch_copy_columns(s.x, ctx->pass_head_col, ctx->head_x, nullptr, C, n, ctx->stream));
+        const int n = p.n_active;
+        CUDA_OK(ctx, launch_copy_columns(p.s.x, p.head_col, ctx->head_x, nullptr, C, n, p.stream));
         Batch b(n);
-        GemvProblem & p = b.add(m.head, ctx->head_x, ctx->head_y);
-        p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
-        if (!run_batch(ctx, b)) return false;
-        CUDA_OK(ctx, launch_copy_columns(ctx->head_y, nullptr, ctx->logits, ctx->pass_head_seq, m.n_vocab, n, ctx->stream));
-    } else if (want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
+        GemvProblem & q = b.add(m.head, ctx->head_x, ctx->head_y);
+        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        if (!run_batch(ctx, p, b)) return false;
+        CUDA_OK(ctx, launch_copy_columns(ctx->head_y, nullptr, p.logits, p.head_seq, m.n_vocab, n, p.stream));
+    } else if (p.want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
         Batch b(ctx->batch_n ? T : 1);
-        GemvProblem & p = b.add(m.head, ctx->batch_n ? s.x : s.x + (size_t) (T - 1) * C, ctx->logits);
-        p.pro = PRO_LAYERNORM; p.ln_w = m.ln_out_w.data; p.ln_b = m.ln_out_b.data;
-        if (!run_batch(ctx, b)) return false;
+        GemvProblem & q = b.add(m.head, ctx->batch_n ? p.s.x : p.s.x + (size_t) (T - 1) * C, p.logits);
+        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        if (!run_batch(ctx, p, b)) return false;
     }
     if (ctx->trace_buf) {
         ctx->trace_count = g_trace_next;
@@ -558,77 +592,72 @@ bool enqueue_pass(Context * ctx, int T, bool want_logits, int phase, int seg) {
 }
 
 // One pass of at most MAX_TOKENS_PER_PASS tokens (state_a -> state_b, then swap) in three steps, so that the overlapped path can
-// put copies between the layer groups: begin_pass (capacity, token staging, hand-off in), run_layers per segment, end_pass.
-bool begin_pass(Context * ctx, const uint32_t * tokens, int T) {
-    if (!ensure_capacity(ctx, T)) return false;
-    const int phase = ctx->phase;
+// put copies between the layer groups: begin_pass (token staging, hand-off in), run_layers per segment, end_pass.
+bool begin_pass(Context * ctx, const uint32_t * tokens, const Pass & p) {
+    const int phase = p.phase, T = p.T;
     if (ctx->slot_used[phase]) CUDA_OK(ctx, cudaEventSynchronize(ctx->slot_free[phase]));   // pass n-2 has consumed this slot
     const Model & m = *ctx->model;
     if (m.layer_begin == 0) for (int t = 0; t < T; t++) ctx->tokens_host[phase][t] = (int) tokens[t];
-    const Scratch hs = carve(m, ctx->scratch, T);
     const size_t ct = (size_t) m.n_embed * (size_t) T * sizeof(float);
-    CUDA_OK(ctx, cudaEventRecord(ctx->ev_start, ctx->stream));
-    if (ctx->hidden_in) {    // outside the captured graph: the caller's pointers may change from call to call
-        CUDA_OK(ctx, cudaMemcpyAsync(hs.x, ctx->hidden_in, ct, cudaMemcpyDeviceToDevice, ctx->stream));
-        if (m.arch_major == 7) CUDA_OK(ctx, cudaMemcpyAsync(hs.v_first, ctx->hidden_in + (size_t) m.n_embed * T, ct, cudaMemcpyDeviceToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_start, p.stream));
+    if (p.hidden_in) {    // outside the captured graph: the caller's pointers may change from call to call
+        CUDA_OK(ctx, cudaMemcpyAsync(p.s.x, p.hidden_in, ct, cudaMemcpyDeviceToDevice, p.stream));
+        if (m.arch_major == 7) CUDA_OK(ctx, cudaMemcpyAsync(p.s.v_first, p.hidden_in + (size_t) m.n_embed * T, ct, cudaMemcpyDeviceToDevice, p.stream));
     }
     return true;
 }
 
 // The kernels of segment `seg` (0 = all resident layers) for the pass begun by begin_pass.
-bool run_layers(Context * ctx, int T, bool want_logits, int seg) {
+bool run_layers(Context * ctx, const Pass & p, int seg) {
     const Model & m = *ctx->model;
-    const int phase = ctx->phase;
     int l0, l1;
     segment_range(ctx, seg, l0, l1);
-    want_logits = want_logits && l1 == m.n_layer;        // only the group that ends the model can run the head
-    const int slot = Context::slot_index(want_logits, phase, seg);
-    Context::GraphSlot * g = (T == 1 && ctx->use_graphs && !ctx->profiling) ? &ctx->graphs[slot] : nullptr;
+    // only the group that ends the model can run the head
+    const int slot = Context::slot_index(p.want_logits && l1 == m.n_layer, p.phase, seg);
+    Context::GraphSlot * g = (p.T == 1 && ctx->use_graphs && !ctx->profiling) ? &ctx->graphs[slot] : nullptr;
     if (g && g->exec) {
-        CUDA_OK(ctx, cudaGraphLaunch(g->exec, ctx->stream));
+        CUDA_OK(ctx, cudaGraphLaunch(g->exec, p.stream));
         g_kernel_launches += g->launches;
         g_graph_launches++;
     } else if (g && g->uses >= 1) {
         // second use of this slot: capture the launch sequence once, replay from now on
         const unsigned long long before = g_kernel_launches;
-        CUDA_OK(ctx, cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
-        const bool ok = enqueue_pass(ctx, T, want_logits, phase, seg);
+        CUDA_OK(ctx, cudaStreamBeginCapture(p.stream, cudaStreamCaptureModeThreadLocal));
+        const bool ok = enqueue_pass(ctx, p, seg);
         cudaGraph_t graph = nullptr;
-        cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
+        cudaError_t e = cudaStreamEndCapture(p.stream, &graph);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess && graph, "CUDA graph capture failed: %s", cudaGetErrorString(e));
         g->launches = g_kernel_launches - before;
         e = cudaGraphInstantiate(&g->exec, graph, 0);
         cudaGraphDestroy(graph);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, e == cudaSuccess, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
-        CUDA_OK(ctx, cudaGraphLaunch(g->exec, ctx->stream));
+        CUDA_OK(ctx, cudaGraphLaunch(g->exec, p.stream));
         g_graph_launches++;
     } else {
         if (g) g->uses++;
-        if (!enqueue_pass(ctx, T, want_logits, phase, seg)) return false;
+        if (!enqueue_pass(ctx, p, seg)) return false;
     }
     return true;
 }
 
-bool end_pass(Context * ctx, int T, bool want_logits) {
+bool end_pass(Context * ctx, const Pass & p) {
     const Model & m = *ctx->model;
-    const int phase = ctx->phase;
-    if (ctx->hidden_out) {
-        const Scratch hs = carve(m, ctx->scratch, T);
-        const size_t ct = (size_t) m.n_embed * (size_t) T * sizeof(float);
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->hidden_out, hs.x, ct, cudaMemcpyDeviceToDevice, ctx->stream));
-        if (m.arch_major == 7) CUDA_OK(ctx, cudaMemcpyAsync(ctx->hidden_out + (size_t) m.n_embed * T, hs.v_first, ct, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (p.hidden_out) {
+        const size_t ct = (size_t) m.n_embed * (size_t) p.T * sizeof(float);
+        CUDA_OK(ctx, cudaMemcpyAsync(p.hidden_out, p.s.x, ct, cudaMemcpyDeviceToDevice, p.stream));
+        if (m.arch_major == 7) CUDA_OK(ctx, cudaMemcpyAsync(p.hidden_out + (size_t) m.n_embed * p.T, p.s.v_first, ct, cudaMemcpyDeviceToDevice, p.stream));
     }
-    CUDA_OK(ctx, cudaEventRecord(ctx->ev_stop, ctx->stream));
-    CUDA_OK(ctx, cudaEventRecord(ctx->slot_free[phase], ctx->stream));
-    ctx->slot_used[phase] = true;
+    CUDA_OK(ctx, cudaEventRecord(ctx->ev_stop, p.stream));
+    CUDA_OK(ctx, cudaEventRecord(ctx->slot_free[p.phase], p.stream));
+    ctx->slot_used[p.phase] = true;
     float * tmp = ctx->state_a; ctx->state_a = ctx->state_b; ctx->state_b = tmp;
     ctx->phase ^= 1;
-    ctx->logits_valid = want_logits && m.layer_end == m.n_layer;
+    ctx->logits_valid = p.want_logits && m.layer_end == m.n_layer;
     return true;
 }
 
-bool forward_pass(Context * ctx, const uint32_t * tokens, int T, bool want_logits) {
-    return begin_pass(ctx, tokens, T) && run_layers(ctx, T, want_logits, 0) && end_pass(ctx, T, want_logits);
+bool forward_pass(Context * ctx, const uint32_t * tokens, const Pass & p) {
+    return begin_pass(ctx, tokens, p) && run_layers(ctx, p, 0) && end_pass(ctx, p);
 }
 
 bool ensure_copy_streams(Context * ctx) {
@@ -930,8 +959,8 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
     } else if (!state_in && !resident_in) {
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a, ctx->state_init, m.state_len() * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     }
-    if (!begin_pass(ctx, tokens, T)) return false;
-    const bool want_logits = logits_out != nullptr;
+    Pass p;
+    if (!make_pass(ctx, T, logits_out != nullptr, nullptr, p) || !begin_pass(ctx, tokens, p)) return false;
     for (int g = 1; g <= G; g++) {
         if (b_in) {      // the slice is in pinned memory once every lane has delivered its part
             while (bp.in_parts[g - 1].load(std::memory_order_acquire) < LANES) std::this_thread::yield();
@@ -940,7 +969,7 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
             CUDA_OK(ctx, cudaEventRecord(ctx->seg_in[g - 1], ctx->copy_in));
         }
         if (state_in) CUDA_OK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->seg_in[g - 1], 0));
-        if (!run_layers(ctx, T, want_logits, g)) return false;
+        if (!run_layers(ctx, p, g)) return false;
         CUDA_OK(ctx, cudaEventRecord(ctx->seg_out[g - 1], ctx->stream));
         if (b_out && g > 1) {      // one group behind: the copy-out stream never waits for something that has not been enqueued
             size_t off, cnt; slice(g - 1, off, cnt);
@@ -951,7 +980,7 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
             bp.out_posted.store(g - 1, std::memory_order_release);
         }
     }
-    if (!end_pass(ctx, T, want_logits)) return false;      // the new state is ctx->state_a from here on
+    if (!end_pass(ctx, p)) return false;      // the new state is ctx->state_a from here on
     if (logits_out) CUDA_OK(ctx, cudaMemcpyAsync(b_log ? ctx->bounce_logits : logits_out, ctx->logits, (size_t) m.n_vocab * sizeof(float), cudaMemcpyDefault, ctx->stream));
     if (state_out && b_out) {
         size_t off, cnt; slice(G, off, cnt);
@@ -1012,7 +1041,8 @@ bool forward(Context * ctx, const uint32_t * tokens, size_t T, bool want_logits)
     while (done < T) {
         const size_t n = (T - done < (size_t) MAX_TOKENS_PER_PASS) ? T - done : (size_t) MAX_TOKENS_PER_PASS;
         const bool last = done + n == T;
-        if (!forward_pass(ctx, tokens + done, (int) n, want_logits && last)) return false;
+        Pass p;
+        if (!make_pass(ctx, (int) n, want_logits && last, nullptr, p) || !forward_pass(ctx, tokens + done, p)) return false;
         done += n;
     }
     return true;
@@ -1040,7 +1070,8 @@ bool batch_get_state(Context * ctx, int seq, float * state_out) {
 bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits) {
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->batch_n > 0 && tokens, "Not a batch context or NULL tokens");
     CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
-    return forward_pass(ctx, tokens, ctx->batch_n, want_logits);
+    Pass p;
+    return make_pass(ctx, ctx->batch_n, want_logits, nullptr, p) && forward_pass(ctx, tokens, p);
 }
 
 // Ints of one ragged map (Context::ragged_host): offsets [B + 1], column sequences [MAX_TOKENS_PER_PASS], head columns and sequences [B each].
@@ -1058,9 +1089,10 @@ bool check_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * count
     return true;
 }
 
-bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
-    size_t total = 0;
-    if (!check_ragged(ctx, tokens, counts, total)) return false;
+// batch_eval_ragged on arguments that passed check_ragged (T tokens in all); with targets, a scoring pass whose results go to lp and
+// greedy (greedy may be NULL).
+static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t * counts, int T, bool want_logits, const uint32_t * targets,
+                        float * lp, uint8_t * greedy) {
     const Model & m = *ctx->model;
     const int B = ctx->batch_n;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
@@ -1071,40 +1103,40 @@ bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * 
         CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->head_y), (size_t) B * m.n_vocab * sizeof(float)));
         CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->ragged_map), map_bytes));
     }
-    const int T = (int) total;
-    if (!begin_pass(ctx, tokens, T)) return false;      // waits until the pass that last used this phase's slots has read them
-    const int phase = ctx->phase;
-    int * off = ctx->ragged_host[phase], * col_seq = off + B + 1, * head_col = col_seq + MAX_TOKENS_PER_PASS, * head_seq = head_col + B;
-    int n_active = 0;
+    Pass p;
+    if (!make_pass(ctx, T, want_logits, nullptr, p) || !begin_pass(ctx, tokens, p)) return false;   // waits until the pass that last used this phase's slots has read them
+    int * off = ctx->ragged_host[p.phase], * col_seq = off + B + 1, * head_col = col_seq + MAX_TOKENS_PER_PASS, * head_seq = head_col + B;
     off[0] = 0;
     for (int b = 0; b < B; b++) {
         off[b + 1] = off[b] + (int) counts[b];
         for (int t = off[b]; t < off[b + 1]; t++) col_seq[t] = b;
-        if (counts[b]) { head_col[n_active] = off[b + 1] - 1; head_seq[n_active] = b; n_active++; }
+        if (counts[b]) { head_col[p.n_active] = off[b + 1] - 1; head_seq[p.n_active] = b; p.n_active++; }
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->ragged_map, off, map_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->ragged_map, off, map_bytes, cudaMemcpyHostToDevice, p.stream));
     // the state of every idle sequence (runs of them are contiguous) goes to state_b as it is: end_pass swaps the whole buffers
     const size_t n = m.state_len();
     for (int b = 0; b < B;) {
         if (counts[b]) { b++; continue; }
         int e = b;
         while (e < B && !counts[e]) e++;
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_b + (size_t) b * n, ctx->state_a + (size_t) b * n, (size_t) (e - b) * n * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(p.state_out + (size_t) b * n, p.state_in + (size_t) b * n, (size_t) (e - b) * n * sizeof(float), cudaMemcpyDeviceToDevice, p.stream));
         b = e;
     }
-    ctx->pass_seq_off = ctx->ragged_map;
-    ctx->pass_col_seq = ctx->ragged_map + B + 1;
-    ctx->pass_head_col = ctx->pass_col_seq + MAX_TOKENS_PER_PASS;
-    ctx->pass_head_seq = ctx->pass_head_col + B;
-    ctx->pass_n_active = n_active;
-    const bool ok = enqueue_pass(ctx, T, want_logits, phase, 0);     // never a graph: the map changes from call to call
-    ctx->pass_seq_off = ctx->pass_col_seq = ctx->pass_head_col = ctx->pass_head_seq = nullptr;
-    ctx->pass_n_active = 0;
-    if (!ok) return false;
+    p.seq_off = ctx->ragged_map;
+    p.col_seq = p.seq_off + B + 1;
+    p.head_col = p.col_seq + MAX_TOKENS_PER_PASS;
+    p.head_seq = p.head_col + B;
+    p.targets = targets; p.lp = lp; p.greedy = greedy;
+    if (!enqueue_pass(ctx, p, 0)) return false;     // never a graph: the map changes from call to call
     const bool had_logits = ctx->logits_valid;
-    if (!end_pass(ctx, T, want_logits)) return false;
+    if (!end_pass(ctx, p)) return false;
     ctx->logits_valid = had_logits || want_logits;     // idle columns keep what they held
     return true;
+}
+
+bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
+    size_t total = 0;
+    return check_ragged(ctx, tokens, counts, total) && ragged_pass(ctx, tokens, counts, (int) total, want_logits, nullptr, nullptr, nullptr);
 }
 
 bool batch_get_logits(Context * ctx, int seq, float * logits_out) {
@@ -1178,8 +1210,6 @@ bool score_copy_out(Context * ctx, size_t n, float * logprobs_out, uint8_t * gre
     return true;
 }
 
-void end_score_pass(Context * ctx) { ctx->pass_targets = nullptr; ctx->pass_lp = nullptr; ctx->pass_greedy = nullptr; }
-
 }  // namespace
 
 bool score(Context * ctx, const uint32_t * tokens, const uint32_t * targets, size_t n, float * logprobs_out, uint8_t * greedy_out) {
@@ -1189,13 +1219,13 @@ bool score(Context * ctx, const uint32_t * tokens, const uint32_t * targets, siz
     if (!score_copy_in(ctx, targets, n, logprobs_out, greedy_out)) return false;
     for (size_t done = 0; done < n;) {
         const int T = (int) std::min(n - done, (size_t) MAX_TOKENS_PER_PASS);
-        ctx->pass_targets = ctx->score_targets + done;
-        ctx->pass_lp = ctx->score_lp + done;
-        ctx->pass_greedy = greedy_out ? ctx->score_greedy + done : nullptr;
+        Pass p;
+        if (!make_pass(ctx, T, true, nullptr, p)) return false;
+        p.targets = ctx->score_targets + done;
+        p.lp = ctx->score_lp + done;
+        p.greedy = greedy_out ? ctx->score_greedy + done : nullptr;
         // enqueue_pass directly: a scoring pass is never captured into a graph or replayed from one
-        const bool ok = begin_pass(ctx, tokens + done, T) && enqueue_pass(ctx, T, true, ctx->phase, 0) && end_pass(ctx, T, true);
-        end_score_pass(ctx);
-        if (!ok) return false;
+        if (!begin_pass(ctx, tokens + done, p) || !enqueue_pass(ctx, p, 0) || !end_pass(ctx, p)) return false;
         done += (size_t) T;
     }
     return score_copy_out(ctx, n, logprobs_out, greedy_out);
@@ -1206,12 +1236,8 @@ bool batch_score_ragged(Context * ctx, const uint32_t * tokens, const uint32_t *
     if (!check_ragged(ctx, tokens, counts, total)) return false;
     if (!prepare_score(ctx, total, score_on_tensor_cores(ctx, (int) total))) return false;
     if (!score_copy_in(ctx, targets, total, logprobs_out, greedy_out)) return false;
-    ctx->pass_targets = ctx->score_targets;
-    ctx->pass_lp = ctx->score_lp;
-    ctx->pass_greedy = greedy_out ? ctx->score_greedy : nullptr;
-    const bool ok = batch_eval_ragged(ctx, tokens, counts, true);
-    end_score_pass(ctx);
-    return ok && score_copy_out(ctx, total, logprobs_out, greedy_out);
+    return ragged_pass(ctx, tokens, counts, (int) total, true, ctx->score_targets, ctx->score_lp, greedy_out ? ctx->score_greedy : nullptr) &&
+           score_copy_out(ctx, total, logprobs_out, greedy_out);
 }
 
 namespace {
@@ -1371,18 +1397,15 @@ GenStepParams generate_step_params(Context * ctx) {
     return gp;
 }
 
-// One pass of the loop (state_a -> state_b as they are set now, input tokens already in ctx->tokens) captured into `body`.
-bool capture_generate_pass(Context * ctx, cudaGraph_t body) {
-    const int rows = ctx->batch_n ? ctx->batch_n : 1;
-    CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(ctx->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    ctx->tokens_on_device = true;
-    bool ok = enqueue_pass(ctx, rows, true, ctx->phase, 0);
+// Pass p of the loop (input tokens already in ctx->tokens) captured into `body`.
+bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p) {
+    CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(p.stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    bool ok = enqueue_pass(ctx, p, 0);
     cudaError_t e = cudaSuccess;
     if (ok && ctx->batch_n)
-        e = launch_restore_frozen(generate_step_params(ctx).rows, rows, ctx->state_a, ctx->state_b, ctx->batch_stride, ctx->model->state_len(), ctx->stream);
-    ctx->tokens_on_device = false;
+        e = launch_restore_frozen(generate_step_params(ctx).rows, p.T, p.state_in, p.state_out, ctx->batch_stride, ctx->model->state_len(), p.stream);
     cudaGraph_t out = nullptr;
-    const cudaError_t ec = cudaStreamEndCapture(ctx->stream, &out);
+    const cudaError_t ec = cudaStreamEndCapture(p.stream, &out);
     if (e == cudaSuccess) e = ec;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess, "Capturing the generation pass failed: %s", cudaGetErrorString(e));
     return true;
@@ -1406,16 +1429,15 @@ GenStreamParams generate_stream_params(Context * ctx) {
 
 bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    Pass p;
+    if (!make_pass(ctx, rows, true, nullptr, p)) return false;
+    p.tokens_in_place = true;
     {   // one uncaptured pass of the loop's shape first, as run_layers does before it captures; its logits go to the step's scratch
         // and its state to state_b, which holds nothing between passes
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) rows * sizeof(int), ctx->stream));
-        float * logits = ctx->logits;
-        ctx->logits = ctx->gen_scratch;
-        ctx->tokens_on_device = true;
-        const bool ok = enqueue_pass(ctx, rows, true, ctx->phase, 0);
-        ctx->tokens_on_device = false;
-        ctx->logits = logits;
-        if (!ok) return false;
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) rows * sizeof(int), p.stream));
+        Pass warm = p;
+        warm.logits = ctx->gen_scratch;
+        if (!enqueue_pass(ctx, warm, 0)) return false;
     }
     GraphHolder top;
     CUDA_OK(ctx, cudaGraphCreate(&top.g, 0));
@@ -1443,10 +1465,8 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
         ip.type = cudaGraphNodeTypeConditional;
         ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
         CUDA_OK(ctx, cudaGraphAddNode(&cond, body, &step, 1, &ip));
-        if (half) std::swap(ctx->state_a, ctx->state_b);      // the second pass reads what the first one wrote
-        const bool ok = capture_generate_pass(ctx, ip.conditional.phGraph_out[0]);
-        if (half) std::swap(ctx->state_a, ctx->state_b);
-        if (!ok) return false;
+        if (!capture_generate_pass(ctx, ip.conditional.phGraph_out[0], p)) return false;
+        std::swap(p.state_in, p.state_out);      // the second pass reads what the first one wrote
         prev = cond;
     }
     CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
@@ -1625,7 +1645,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     for (int b = 0; b < rows; b++) n = std::max(n, (size_t) max_tokens[b]);
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     const bool streaming = on_token != nullptr;
-    if (!ensure_generate_buffers(ctx) || (streaming && !ensure_stream_buffers(ctx)) || !ensure_capacity(ctx, rows)) return false;
+    if (!ensure_generate_buffers(ctx) || (streaming && !ensure_stream_buffers(ctx)) || !ensure_capacity(ctx, rows, ctx->stream)) return false;
     // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
     GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
     memset(sh, 0, sizeof(GenShared));
@@ -1694,20 +1714,15 @@ bool pipe_forward(Context * ctx, const uint32_t * tokens, size_t T, bool want_lo
     const bool first = m.layer_begin == 0, last = m.layer_end == m.n_layer;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, m.link.box && (first || m.link.prev) && (last || m.link.next), "The stage is not connected to its neighbours");
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    cudaStream_t own = ctx->stream;
-    if (stream) ctx->stream = stream;
-    bool ok = begin_pass(ctx, tokens, (int) T);
-    if (ok) {
-        const Scratch hs = carve(m, ctx->scratch, (int) T);
-        const size_t n = (size_t) m.n_embed * T, nv = m.arch_major == 7 ? n : 0;
-        cudaError_t e = cudaSuccess;
-        if (!first) e = launch_pipe_recv(m.link.box, m.link.prev, m.link.counters, m.link.slot_floats, hs.x, n, hs.v_first, nv, ctx->stream);
-        ok = e == cudaSuccess && run_layers(ctx, (int) T, want_logits && last, 0);
-        if (ok && !last) e = launch_pipe_send(m.link.box, m.link.next, m.link.counters, m.link.slot_floats, hs.x, n, hs.v_first, nv, ctx->stream);
-        ok = ok && e == cudaSuccess && end_pass(ctx, (int) T, want_logits && last);
-        if (e != cudaSuccess) { ctx->last_error |= RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED; if (ctx->print_errors) fprintf(stderr, "pipeline hand-off launch failed: %s\n", cudaGetErrorString(e)); }
-    }
-    ctx->stream = own;
+    Pass p;
+    if (!make_pass(ctx, (int) T, want_logits && last, stream, p) || !begin_pass(ctx, tokens, p)) return false;
+    const size_t n = (size_t) m.n_embed * T, nv = m.arch_major == 7 ? n : 0;
+    cudaError_t e = cudaSuccess;
+    if (!first) e = launch_pipe_recv(m.link.box, m.link.prev, m.link.counters, m.link.slot_floats, p.s.x, n, p.s.v_first, nv, p.stream);
+    bool ok = e == cudaSuccess && run_layers(ctx, p, 0);
+    if (ok && !last) e = launch_pipe_send(m.link.box, m.link.next, m.link.counters, m.link.slot_floats, p.s.x, n, p.s.v_first, nv, p.stream);
+    ok = ok && e == cudaSuccess && end_pass(ctx, p);
+    if (e != cudaSuccess) { ctx->last_error |= RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED; if (ctx->print_errors) fprintf(stderr, "pipeline hand-off launch failed: %s\n", cudaGetErrorString(e)); }
     return ok;
 }
 
@@ -1867,14 +1882,11 @@ size_t stage_hidden_len(const Model & m, size_t T) { return (size_t) (m.arch_maj
 bool stage_forward(Context * ctx, const uint32_t * tokens, size_t T, const float * hidden_in, float * hidden_out, bool want_logits, cudaStream_t stream) {
     const Model & m = *ctx->model;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    cudaStream_t own = ctx->stream;
-    if (stream) ctx->stream = stream;
-    ctx->hidden_in = m.layer_begin == 0 ? nullptr : hidden_in;
-    ctx->hidden_out = m.layer_end == m.n_layer ? nullptr : hidden_out;
-    const bool ok = forward_pass(ctx, tokens, (int) T, want_logits);
-    ctx->hidden_in = nullptr; ctx->hidden_out = nullptr;
-    ctx->stream = own;
-    return ok;
+    Pass p;
+    if (!make_pass(ctx, (int) T, want_logits, stream, p)) return false;
+    p.hidden_in = m.layer_begin == 0 ? nullptr : hidden_in;
+    p.hidden_out = m.layer_end == m.n_layer ? nullptr : hidden_out;
+    return forward_pass(ctx, tokens, p);
 }
 
 }  // namespace rwkv

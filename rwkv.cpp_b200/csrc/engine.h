@@ -85,11 +85,6 @@ struct Context {
     int trace_count = 0;             // slots used by the last enqueued / captured pass
     const char * trace_names[1024] = {};   // kernel name per slot (string literals)
 
-    // Pipeline-stage hand-off (SURVEY.md 8e): device pointers of the caller for the pass being enqueued, or NULL.
-    // Layout: x f32[C x T], then (v7 only) v_first f32[C x T].
-    const float * hidden_in = nullptr;
-    float * hidden_out = nullptr;
-
     // Batched multi-sequence decode (rwkv_b200_batch_*): batch_n > 0 makes this a batch context whose state
     // buffers hold batch_n states back to back (batch_stride = state_len floats apart) and whose logits buffer holds batch_n columns;
     // every pass evaluates exactly one token of each sequence.
@@ -102,9 +97,6 @@ struct Context {
     int * ragged_host[2] = {nullptr, nullptr};
     int * ragged_map = nullptr;
     float * head_x = nullptr, * head_y = nullptr;
-    // while a ragged pass is being enqueued: its device map, and how many sequences advance (the head's columns)
-    const int * pass_seq_off = nullptr, * pass_col_seq = nullptr, * pass_head_col = nullptr, * pass_head_seq = nullptr;
-    int pass_n_active = 0;
     // Scoring passes (score, batch_score_ragged), allocated on the first: the head's output for every column of a pass
     // ([MAX_TOKENS_PER_PASS, n_vocab]), and the targets and results of a call's tokens (score_capacity entries each).
     float * score_logits = nullptr;
@@ -112,10 +104,6 @@ struct Context {
     float * score_lp = nullptr;
     uint8_t * score_greedy = nullptr;
     size_t score_capacity = 0;
-    // while a scoring pass is being enqueued: the targets of its columns and where their results go (greedy may be NULL)
-    const uint32_t * pass_targets = nullptr;
-    float * pass_lp = nullptr;
-    uint8_t * pass_greedy = nullptr;
 
     // On-device sampling (kernels/sampling.cu): result word, scratch for biased logits, device copy of the caller's logit bias.
     bool logits_valid = false;       // ctx->logits holds the head output of the most recent pass
@@ -140,7 +128,6 @@ struct Context {
     // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by whether
     // the loop streams its tokens to a callback, and by whether its draws are constrained by automata
     cudaGraphExec_t gen_graphs[2][2][2] = {};
-    bool tokens_on_device = false;   // while the loop's passes are captured: ctx->tokens is written by the sampler, no upload
     // Streaming generation, allocated on the first streaming call: mapped pinned words shared by the step kernel and the calling
     // thread (GenStreamParams), at device addresses the streaming graph captures. Layout: published [rows], acked [rows], timed_out,
     // then tokens [rows][GENERATE_MAX].
