@@ -403,6 +403,10 @@ RWKV_API bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * 
 RWKV_API bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, int n_vocab, const int * tokens, int T, int C,
                                        const float * ln_w, const float * ln_b, float * x);
 
+/* y[:, t] = LN(x[:, t]; w, b) for t < T (launch_layer_norm_columns: the LayerNorm of the tensor-core head of scoring passes).
+ * x, y: [C, T]; T at most 256, the columns of one pass. */
+RWKV_API bool rwkv_b200_test_layer_norm_columns(const float * x, const float * w, const float * b, int C, int T, float * y);
+
 /* LayerNorm + token shift + mix (launch_ln_mix). formula 0: out_j = xx*m_j + (prev - prev*m_j);
  * formula 1: out_j = (prev - xx)*m_j + xx. state_in / state_out: the carried LN(x) of the previous token, [C] per sequence. */
 struct rwkv_b200_ln_mix_args {

@@ -1041,6 +1041,20 @@ bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, 
     return true;
 }
 
+bool rwkv_b200_test_layer_norm_columns(const float * x, const float * w, const float * b, int C, int T, float * y) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, x && w && b && y && C > 0 && T > 0 && T <= 256, "Invalid layer_norm_columns arguments");
+    if (!hook_device(sink)) return false;
+    HookBuffers hb;
+    const float * d_x = hb.in(x, (size_t) C * T), * d_w = hb.in(w, C), * d_b = hb.in(b, C);
+    float * d_y = hb.out(y, (size_t) C * T);
+    const cudaError_t e = hb.ok ? launch_layer_norm_columns(d_x, d_w, d_b, C, T, d_y, 0) : cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, hb.finish(e), "layer_norm_columns failed: %s",
+               cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
 bool rwkv_b200_test_ln_mix(const struct rwkv_b200_ln_mix_args * a) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();

@@ -107,6 +107,17 @@ def embed_ln0(lib, emb, tokens, w, b):
     return x
 
 
+def layer_norm_columns(lib, x, w, b):
+    """x: [C, T]; w, b: [C] (None passes NULL). Returns Out of C*T floats: LN(x[:, t]; w, b) of every column."""
+    C, T = x.shape
+    i = Inputs()
+    y = Out(C * T)
+    ok = lib.library.rwkv_b200_test_layer_norm_columns(VP(i(x, True)), VP(i(w)), VP(i(b)), ctypes.c_int(C), ctypes.c_int(T), VP(y.ptr))
+    if not ok:
+        raise HookError(lib.rwkv_get_last_error(None))
+    return y
+
+
 def ln_mix(lib, x, w, b, state_in, coefs, formula, n_seq=0, seq_stride=0, xx=True, sx=True):
     """x: [C, T] (or [C, n_seq] with n_seq > 0, state_in then holding n_seq states seq_stride floats apart).
     Returns dict of Out: out0.., xx, sx, state."""

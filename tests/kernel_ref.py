@@ -41,6 +41,22 @@ def layer_norm(x, w, b, dt, eps=1e-5):
     return norm(x, eps, dt) * w.astype(dt)[:, None] + b.astype(dt)[:, None]
 
 
+def layer_norm_columns(x, w, b, dt, bug=None):
+    """layer_norm_columns_kernel (csrc/kernels/score.cu): layer_norm of every column of x [C, T], the head's LayerNorm of a scoring
+    pass on the tensor cores. bug: "eps" (1e-6 instead of 1e-5), "wb_neighbour" (w and b of the next channel), "no_bias", "no_mean"
+    (the mean not subtracted), "var_c_minus_1" (the variance divided by C - 1)."""
+    if bug is None:
+        return layer_norm(x, w, b, dt)
+    x, w, b = x.astype(dt), w.astype(dt), b.astype(dt)
+    n = dt(x.shape[0])
+    v = x if bug == "no_mean" else x - x.sum(axis=0, dtype=dt) / n
+    var = (v * v).sum(axis=0, dtype=dt) / (n - 1 if bug == "var_c_minus_1" else n)
+    if bug == "wb_neighbour":
+        w, b = np.roll(w, -1), np.roll(b, -1)
+    y = v / np.sqrt(var + dt(1e-6 if bug == "eps" else 1e-5)) * w[:, None]
+    return y if bug == "no_bias" else y + b[:, None]
+
+
 def head_norm(y, H, eps, dt):
     """Per-head ggml_norm after the reshape to [S, H, T] (rwkv_graph.inc:281-284, 376-379)."""
     C, T = y.shape
@@ -400,19 +416,43 @@ def _f16_tie_distance(v):
     return dist / np.where(up > 0, up, 1.0)
 
 
-def ln_bias_away_from_roundings(x, ln_w, ln_b, w_type, rng, margin=1e-3, tie_margin=1e-2):
+def ln_columns_f32(x, w):
+    """(x - mean) * rstd * w of layer_norm_columns_kernel (and of the GEMV's LayerNorm prologue) in float32, before the bias: the mean
+    and the sum of squares in double, everything else one float32 rounding per operation in the kernel's order."""
+    x = np.asarray(x, np.float32)
+    C = x.shape[0]
+    mean = (x.astype(F64).sum(axis=0) / C).astype(np.float32)
+    v = x - mean
+    s2 = (v * v).astype(F64).sum(axis=0)
+    rstd = np.float32(1) / np.sqrt((s2 / C).astype(np.float32) + np.float32(1e-5))
+    return (v * rstd) * np.asarray(w, np.float32)[:, None]
+
+
+def ln_bias_away_from_roundings(x, ln_w, ln_b, w_type, rng, margin=1e-3, tie_margin=1e-2, kernel_error=False):
     """ln_b nudged element by element until the float64 LayerNorm output of x gives the same operands as any faithful fp32 LayerNorm:
     every Q8 value x 127 / amax at least `margin` (in units of q) away from a rint half-way point, and every block's amax / 127, every
     Q8_1 s and every fp16 operand at least `tie_margin` of an fp16 spacing away from an fp16 tie. ln_b enters after the normalisation,
-    element by element, so moving ln_b[k] moves row k of the output and nothing else."""
+    element by element, so moving ln_b[k] moves row k of the output and nothing else.
+
+    With kernel_error, an fp16 operand is instead held four times its distance from the LayerNorm of the kernels (ln_columns_f32 + ln_b in
+    float32 numpy) away from a tie: a margin that a single ln_b[k] can keep for all of a row's 256 columns at once, where tie_margin is
+    out of reach for more than about 64. Operands below 2^-8 are left where they fall: their fp16 spacing is at most 2^-19, so another
+    rounding of one moves a product with a head weight by less than the bar's floor of 1e-6 of the output."""
     b = np.asarray(ln_b, np.float32).copy()
     if w_type == TYPE_F32:
         return b
     n = norm(x, 1e-5, F64) * np.asarray(ln_w, F64)[:, None]
     K, T = n.shape
+    if kernel_error:
+        nw32 = ln_columns_f32(x, ln_w)
     for _ in range(200):
         y = n + b.astype(F64)[:, None]
-        if w_type == TYPE_F16:
+        if w_type == TYPE_F16 and kernel_error:
+            gap = _f16_tie_distance(y) * np.spacing(np.abs(y).astype(np.float16)).astype(F64)
+            err = np.abs((nw32 + b[:, None]).astype(F64) - y) + 2.0 ** -24 * np.abs(y)
+            bad = ((gap < 4 * err) & (np.abs(y) >= 2.0 ** -8)).any(axis=1)
+            unit = np.abs(y).max(axis=1) * 2.0 ** -10 + 1e-8
+        elif w_type == TYPE_F16:
             bad = (_f16_tie_distance(y) < tie_margin).any(axis=1)
             unit = np.abs(y).max(axis=1) * 2.0 ** -10 + 1e-8
         else:

@@ -238,12 +238,13 @@ def problem(fmt, M, K, T, rng, input=0, epi=kr.EPI_NONE, tiled=None, alias=True,
     return p
 
 
-def with_layernorm(p, x, rng):
-    """Give p the head's LayerNorm prologue, with ln_b chosen so that fp32 and float64 LayerNorms give the same operands."""
+def with_layernorm(p, x, rng, **margins):
+    """Give p the head's LayerNorm prologue, with ln_b chosen so that fp32 and float64 LayerNorms give the same operands (margins: of
+    kernel_ref.ln_bias_away_from_roundings)."""
     K = p["K"]
     w = (1 + 0.2 * rng.standard_normal(K)).astype(F32)
     b = (0.2 * rng.standard_normal(K)).astype(F32)
-    p.update(pro=1, ln_w=w, ln_b=kr.ln_bias_away_from_roundings(x, w, b, p["type"], rng))
+    p.update(pro=1, ln_w=w, ln_b=kr.ln_bias_away_from_roundings(x, w, b, p["type"], rng, **margins))
     return p
 
 

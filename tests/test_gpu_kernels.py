@@ -372,6 +372,36 @@ def test_ln_mix_batch(lib, C, n_seq, formula):
         check("ln_mix_b", "state", batch["state"].value[s * stride:s * stride + C], r64[3], r32[3])
 
 
+# ---- LayerNorm of columns (the tensor-core head of scoring passes) --------------------------------------------------------
+
+def ln_columns_inputs(C, T, rng):
+    """Unit-scale columns and, cycling from the second column on, ones the LayerNorm's conditioning or its eps decides: a large
+    common offset over a spread of 1, a variance of the order of eps (1e-5) on an offset of 0.5, and a constant column."""
+    x = rng.standard_normal((C, T)).astype(F32) * 1.5
+    for t in range(1, T):
+        if t % 4 == 1:
+            x[:, t] = (1e4 + rng.standard_normal(C)).astype(F32)
+        elif t % 4 == 2:
+            x[:, t] = (0.5 + 3e-3 * rng.standard_normal(C)).astype(F32)
+        elif t % 4 == 3:
+            x[:, t] = F32(3.7)
+    w = (1 + 0.2 * rng.standard_normal(C)).astype(F32)
+    b = (0.2 * rng.standard_normal(C)).astype(F32)
+    return x, w, b
+
+
+LN_COLUMN_WIDTHS = [100, 300, 768, 1000, 1024, 2048, 2560, 4096, 5120]      # the published n_embed and widths off the 256-thread stride
+
+
+@pytest.mark.parametrize("C", LN_COLUMN_WIDTHS)
+@pytest.mark.parametrize("T", [1, 17, 256])
+def test_layer_norm_columns_matches_float64(lib, C, T):
+    x, w, b = ln_columns_inputs(C, T, rng_for("ln_columns", C, T))
+    y = kh.layer_norm_columns(lib, x, w, b)
+    assert y.guard_intact(), "write past the end of y"
+    check("ln_columns", "y", y.cols(C), *both(lambda dt: kr.layer_norm_columns(x, w, b, dt)))
+
+
 # ---- v6 lerp -----------------------------------------------------------------------------------------------------------
 
 def lerp_inputs(C, T, mix, rng):

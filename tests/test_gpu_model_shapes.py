@@ -6,16 +6,19 @@ shares, the fallback to the generic kernel, the tensor-core cluster size and npa
 SHAPES lists the published RWKV-4 / 5.2 / 6 / 7 layer shapes; each matrix gets the type the quantiser writes for it (file_types), and
 the batches are built as engine.cu builds them (engine_batches), on every route of the eval path: a single context's SIMT launches
 (T = 1 / 3 / 31) and tensor-core launches (T = 32 / 128 / 256), a batch context's (B = 5 / 15 SIMT, B = 16 / 64 / 256 tensor cores),
-and the head with its LayerNorm prologue at the real vocabulary. Each launch record is checked against a host restatement of the plan
-(routing, NC, generic fallback, cluster size, npad). The float64 reference restates only some rows -- all rows of the first and last
+the head with its LayerNorm prologue at the real vocabulary (single tokens, scoring passes of up to 256 columns, batch contexts of up
+to 256 sequences), and the tensor-core head of scoring passes (LayerNorm of columns, the GEMM, the score kernel). Each launch record is
+checked against a host restatement of the plan (routing, NC, generic fallback, cluster size, npad). The float64 reference restates only some rows -- all rows of the first and last
 128-row tile, both edge rows of every tensor-core tile and of the first tile of every streaming CTA, and a seeded sample -- and every
 column, and no output may keep the NaN of the 0xFF fill in any row. The state kernels run at the same shapes (part A). One-layer model
 files at the smallest and largest shape of each architecture and at RWKV-4 14B check the engine's own invariants there: serial ==
-sequence == chunks, batch == alone, tensor-core passes within the end-to-end bars, and where the v6 LoRA fold runs (part B).
+sequence == chunks, batch == alone, tensor-core passes within the end-to-end bars, where the v6 LoRA fold runs, and scoring at the
+real vocabulary: GEMV-head passes and ragged passes below 16 columns bit for bit, tensor-core ones within the end-to-end bars (part B).
 tests/test_model_shapes_host.py checks the table and the bars without a GPU."""
 import collections
 import ctypes
 import functools
+import types
 
 import numpy as np
 import pytest
@@ -27,6 +30,8 @@ import kquant_ref as kq
 import test_gpu_gemv as tg
 from test_gpu_kernels import (F32, F64, ln_mix_inputs, lerp_inputs, ref_wkv4, ref_wkv6, ref_wkv7, run_wkv4, run_wkv6, run_wkv7, wkv4_inputs,
                               wkv6_inputs, wkv7_inputs)
+from test_gpu_score import (NO, P_F, P_U, P_U8, SENTINEL, bits, check_rows, lp64, ragged_case, score_logits, text_targets, u32,
+                            traced_names as score_trace)
 
 pytestmark = pytest.mark.gpu
 
@@ -158,12 +163,49 @@ def weights(fmt, M, K):
     return tg.random_raw.__wrapped__(fmt, M, K)
 
 
-def problem(fmt, M, K, T, rng, input=0, epi=0, tiled=None):
-    """tg.problem with the weights above; the tile-major copy exists where gemm_tc_eligible (engine.cu keeps one for every layer
-    matrix), which for K-quant rows means whole super-blocks."""
+def head_weights(V, C, tiles=None):
+    """float32 head weights of about 1 / sqrt(C), [rows of `tiles`, C]: every 128-row tile drawn from its own seed, so that a test can
+    restate some tiles of a 65536-row head without drawing the rest (all tiles when None)."""
+    tiles = range(-(-V // 128)) if tiles is None else tiles
+    w = np.empty((sum(min(128, V - 128 * t) for t in tiles), C), F32)
+    r = 0
+    for t in tiles:
+        n = min(128, V - 128 * t)
+        w[r:r + n] = tg.rng_for("shape-head", V, C, t).standard_normal((n, C), dtype=F32)
+        r += n
+    w *= F32(1 / np.sqrt(C))
+    return w
+
+
+def head_raw(fmt, w):
+    return TYPE[fmt], w.astype(np.float16 if fmt == "FP16" else F32).view(np.uint8).reshape(-1)
+
+
+@pytest.fixture(scope="module")
+def head():
+    """head(fmt, V, C) -> (type, bytes) of a shape's head. The FP16 bytes of every head drawn stay for the module (11 heads, 3 GB); of
+    the FP32 bytes only the last head's do (shapes of one vocabulary and width share a head)."""
+    f16, f32 = {}, {}
+
+    def get(fmt, V, C):
+        if (V, C) not in (f32 if fmt == "FP32" else f16):
+            w = head_weights(V, C)
+            f16[(V, C)] = head_raw("FP16", w)
+            if fmt == "FP32":
+                f32.clear()
+                f32[(V, C)] = head_raw("FP32", w)
+        return (f32 if fmt == "FP32" else f16)[(V, C)]
+    yield get
+    f16.clear()
+    f32.clear()
+
+
+def problem(fmt, M, K, T, rng, input=0, epi=0, tiled=None, raw=None):
+    """tg.problem with the weights above (or `raw` = (type, bytes)); the tile-major copy exists where gemm_tc_eligible (engine.cu keeps
+    one for every layer matrix), which for K-quant rows means whole super-blocks."""
     if tiled is None:
         tiled = fmt != "FP32" and K % (256 if fmt in KQ_FALLBACK else 64) == 0
-    return tg.problem(fmt, M, K, T, rng, input=input, epi=epi, tiled=tiled, weights=weights(fmt, M, K))
+    return tg.problem(fmt, M, K, T, rng, input=input, epi=epi, tiled=tiled, weights=raw or weights(fmt, M, K))
 
 
 def build(s, fmt, batch, T, rng):
@@ -403,6 +445,7 @@ def tc_factor(p):
 WORST = collections.defaultdict(float)
 NEEDED = collections.defaultdict(float)
 TC_NEEDED = collections.defaultdict(float)    # (M, K) -> error / float32 distance of its tensor-core launches
+HEADS_ON_TC = set()                           # (V, C) of the heads run on the tensor cores
 RAN = set()                                   # (shape, route) pairs that ran
 KEYS = collections.defaultdict(set)           # shape -> launch keys reached
 
@@ -414,6 +457,9 @@ def report_worst():
         print("\n%-13s worst error / bar = %.3f (error / fp32 distance %.2f)" % (family, WORST[family], NEEDED[family]), end="")
     for (M, K), f in sorted(TC_NEEDED.items(), key=lambda kv: -kv[1])[:12]:
         print("\ntensor cores %5d x %5d: error / fp32 distance %.2f (bar factor %d)" % (M, K, f, tc_factor(dict(M=M, K=K))), end="")
+    for V, C in sorted(HEADS_ON_TC):
+        print("\ntensor-core head %5d x %4d: error / fp32 distance %.2f (bar factor %d)" % (V, C, TC_NEEDED[(V, C)], tc_factor(dict(M=V, K=C))),
+              end="")
     print()
 
 
@@ -436,12 +482,13 @@ def check(family, name, got, r64, r32, factor, shape=None):
     err, d32 = np.abs(got - r64).max(axis=0), np.abs(r32 - r64).max(axis=0)
     needed = float((err / np.maximum(d32, 1e-30))[err > kr.bar(r64, r32, 0)].max(initial=0))
     NEEDED[family] = max(NEEDED[family], needed)
-    if family == "tensor_cores":
+    if family.startswith("tensor_cores"):
         TC_NEEDED[shape] = max(TC_NEEDED[shape], needed)
     assert ratio <= 1, (family, name, ratio, np.abs(got - r64).max())
 
 
-def run_and_check(lib, shape, name, T, probs, xs, path, sms):
+def run_and_check(lib, shape, name, T, probs, xs, path, sms, tc_family="tensor_cores"):
+    """Runs the batch, checks it and returns its outputs and launch record; tensor-core outputs count towards tc_family."""
     outs, launches = kh.gemv_batch(lib, T, probs, xs, path)
     for o in outs:
         assert o.guard_intact(), (name, "write past the end of an output")
@@ -450,7 +497,7 @@ def run_and_check(lib, shape, name, T, probs, xs, path, sms):
     fams = {l[0] for l in launches}
     for j, (p, o) in enumerate(zip(probs, outs)):
         tc = takes_tc(p, T, path)
-        fam = "tensor_cores" if tc else "kquant" if p["fmt"] in KQ_BYTES else "generic" if "generic" in fams else "streaming"
+        fam = tc_family if tc else "kquant" if p["fmt"] in KQ_BYTES else "generic" if "generic" in fams else "streaming"
         # every row was written (no NaN of the 0xFF fill anywhere), before the float64 comparison of the sampled rows
         assert not np.isnan(o.cols(p["M"])).any(), (name, p["fmt"], p["M"], p["K"], "NaN left in the output")
         rows = sample_rows(p, T, path, probs, sms, tg.rng_for("rows", name, j))
@@ -458,6 +505,7 @@ def run_and_check(lib, shape, name, T, probs, xs, path, sms):
         got = o.cols(p["M"])[rows]
         check(fam, (name, p["fmt"], p["M"], p["K"], p["epi"]), got, reference(sub, xs, F64, tc), reference(sub, xs, F32, tc),
               tc_factor(p) if tc else 4, (p["M"], p["K"]))
+    return outs, launches
 
 
 # ---- A. the matrix kernels at every shape ------------------------------------------------------------------------------------
@@ -478,20 +526,64 @@ def test_engine_batches_at_model_shape(lib, sms, shape, fmt, path, T):
     RAN.add((shape, "gemv", fmt, path, T))
 
 
-HEAD_ROUTES = [("engine", 1), ("engine_batch_ctx", 4), ("engine_batch_ctx", 20)]
+# The GEMV with its LayerNorm prologue: a single token; the GEMV-head scoring passes of a single context (up to 31 tokens with tensor
+# cores on, up to 256 with them off); batch contexts of 4 .. 256 sequences, whose head the tensor cores never take (they refuse the
+# prologue).
+HEAD_ROUTES = [("engine", 1), ("engine", 31), ("engine", 256), ("engine_batch_ctx", 4), ("engine_batch_ctx", 20), ("engine_batch_ctx", 64),
+               ("engine_batch_ctx", 256)]
 
 
 @pytest.mark.parametrize("shape", [s.name for s in SHAPES])
 @pytest.mark.parametrize("fmt", ["FP16", "FP32"])
-def test_head_at_model_shape(lib, sms, shape, fmt):
-    """LN(x; ln_out) . W at the shape's real vocabulary (engine.cu's head), single token and batch contexts of 4 and 20."""
+def test_head_at_model_shape(lib, sms, head, shape, fmt):
+    """LN(x; ln_out) . W at the shape's real vocabulary (engine.cu's head and the GEMV head of score_head) on every route of
+    HEAD_ROUTES. Beyond 64 columns ln_b keeps the fp16 operands of every column four times the kernel's own LayerNorm error away from
+    a tie instead of a hundredth of an fp16 spacing, which no ln_b achieves for 256 columns at once."""
     s = BY_NAME[shape]
     for path, T in HEAD_ROUTES:
         rng = tg.rng_for("shape-head", shape, fmt, path, T)
         xs = tg.inputs([s.C], T, rng, scale=1.5)
-        p = tg.with_layernorm(problem(fmt, s.V, s.C, T, rng, tiled=False), xs[0], rng)
+        p = problem(fmt, s.V, s.C, T, rng, tiled=False, raw=head(fmt, s.V, s.C))
+        tg.with_layernorm(p, xs[0], rng, kernel_error=T > 64)
         run_and_check(lib, shape, (shape, "head", fmt, path, T), T, [p], xs, path, sms)
         RAN.add((shape, "head", fmt, path, T))
+
+
+# Columns of the tensor-core head: a batch context's smallest passes (16, 17) and a single context's (32 and up), ragged ones included.
+SCORE_HEAD_T = [16, 17, 32, 33, 100, 256]
+
+
+def score_head_targets(V, T, rng):
+    """Targets of a [T, V] pass: every column's argmax is scored separately (score_head_case); these mix positions without a target,
+    rows of the last row tile (101 rows at V = 50277) and any row."""
+    last = (V - 1) // 128 * 128
+    return [NO if t % 3 == 0 else int(rng.integers(last, V)) if t % 3 == 1 else int(rng.integers(0, V)) for t in range(T)]
+
+
+@pytest.mark.parametrize("shape", [s.name for s in SHAPES])
+def test_score_head_at_model_shape(lib, sms, head, shape):
+    """score_head on the tensor cores at the shape's real vocabulary: layer_norm_columns (through its hook), then the FP16 head from
+    its tile-major copy (gemm_tc_repack, as ensure_head_tiled builds it) on the tensor cores, then the score kernel on the [T, V]
+    logits. The GEMM is checked as every tensor-core launch of this file is (launch record, no NaN anywhere, the sampled rows -- all
+    of the first and last tile and both edges of every tile -- against float64), and the score kernel against float64 log_softmax of
+    the logits the GEMM returned, so a GEMM error cannot hide one of the score kernel."""
+    s = BY_NAME[shape]
+    HEADS_ON_TC.add((s.V, s.C))
+    for T in SCORE_HEAD_T:
+        rng = tg.rng_for("shape-score-head", shape, T)
+        x = tg.inputs([s.C], T, rng, scale=1.5)[0]
+        w, b = (1 + 0.2 * rng.standard_normal(s.C)).astype(F32), (0.2 * rng.standard_normal(s.C)).astype(F32)
+        ln = kh.layer_norm_columns(lib, x, w, b)
+        assert ln.guard_intact() and not np.isnan(ln.value).any(), (shape, T)
+        p = problem("FP16", s.V, s.C, T, rng, tiled=True, raw=head("FP16", s.V, s.C))
+        (out,), launches = run_and_check(lib, shape, (shape, "score_head", T), T, [p], [ln.cols(s.C).copy()], "tensor_cores", sms,
+                                         tc_family="tensor_cores_head")
+        assert launches[0] == ("expand", 0, TYPE["FP16"], 0, 0, 0), launches       # the tile-major upload
+        logits = out.value.reshape(T, s.V)
+        for targets in ([int(a) for a in logits.argmax(axis=1)], score_head_targets(s.V, T, rng)):
+            lp, g = score_logits(lib, logits, targets)
+            check_rows(lp, g, logits, targets)
+        RAN.add((shape, "score_head", T))
 
 
 # ---- A.4 the state kernels at the same shapes --------------------------------------------------------------------------------
@@ -718,6 +810,7 @@ def test_one_layer_file_invariants(lib, tmp_path, shape, fmt):
         if s.arch[0] == 6:
             names = traced_names(lib, ctx, toks[0])
             assert names.count("v6_prologue") == int(fold_expected(s, fmt)), names
+        score_at_real_vocabulary(lib, ctx, toks, serial, tol)
         if s.C > 4096:      # batch contexts take n_embed <= 4096 (rwkv_b200_batch_create): the 14B shape is refused
             assert not lib.library.rwkv_b200_batch_create(ctx.ptr, 16)
             assert lib.rwkv_get_last_error(None) & ((6 << 8) | 9) == (6 << 8) | 9      # RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED
@@ -742,19 +835,72 @@ def test_one_layer_file_invariants(lib, tmp_path, shape, fmt):
     finally:
         lib.rwkv_free(ctx)
     check_batch(lib, path, n_seq=5, n_steps=5)            # a batch of 5 == each sequence alone, bit for bit
+    # ragged scoring passes: below 16 columns the GEMV head, bit for bit each sequence alone; from 16 on the tensor-core head
+    ragged_case(lib, path, [3, 0, 5, 1, 0, 6], tensor_cores=True, exact=True)
+    ragged_case(lib, path, [20, 0, 13, 1], tensor_cores=True, exact=False, bar=2 * tol)
     RAN.add((shape, "one_layer", fmt))
+
+
+def score_at_real_vocabulary(lib, ctx, toks, serial, tol):
+    """rwkv_b200_score over the 128 tokens from a fresh state, tensor cores on. In calls below 32 tokens (the GEMV head): the bits
+    rwkv_b200_score_logits gives on the serial logits, and the last serial logits left resident. In one call (the tensor-core head,
+    trace ending layer_norm_columns, convert_f16, gemm_tc, score): within twice the end-to-end logits bar of float64 log_softmax over
+    the serial logits (the error of log p is at most that of z_t plus that of the logsumexp), and the state eval_resident leaves."""
+    L = lib.library
+    V = len(serial[0][1])
+    ref = np.stack([lg for _, lg in serial])
+    targets = text_targets(toks, V)
+    has = np.array([t != NO for t in targets])
+
+    def score(lo, hi):
+        lp, g = np.full(hi - lo, SENTINEL, F32), np.full(hi - lo, 7, np.uint8)
+        assert L.rwkv_b200_score(ctx.ptr, u32(toks[lo:hi]).ctypes.data_as(P_U), u32(targets[lo:hi]).ctypes.data_as(P_U), hi - lo,
+                                 lp.ctypes.data_as(P_F), g.ctypes.data_as(P_U8)), L.rwkv_get_last_error(ctx.ptr)
+        return lp, g
+
+    def state():
+        st = np.zeros(len(serial[0][0]), F32)
+        assert L.rwkv_b200_state_store(ctx.ptr, st.ctypes.data_as(P_F))
+        return st
+    L.rwkv_b200_set_tensor_cores(ctx.ptr, True)
+    want_lp, want_g = score_logits(lib, ref, targets)
+    assert L.rwkv_b200_state_load(ctx.ptr, None)
+    parts, off = [], 0
+    for n in (31, 1, 20, 18, 31, 27):
+        parts.append(score(off, off + n))
+        off += n
+    assert off == len(toks)
+    assert bits(np.concatenate([a for a, _ in parts])) == bits(want_lp) and bits(np.concatenate([g for _, g in parts])) == bits(want_g)
+    lg = np.zeros(V, F32)
+    assert L.rwkv_b200_stage_logits(ctx.ptr, lg.ctypes.data_as(P_F), None)
+    assert bits(lg) == bits(serial[-1][1]), "resident logits"
+    # the tensor-core head
+    assert L.rwkv_b200_state_load(ctx.ptr, None)
+    assert L.rwkv_b200_eval_resident(ctx.ptr, u32(toks).ctypes.data_as(P_U), len(toks), True, None)
+    want_state = state()
+    assert L.rwkv_b200_state_load(ctx.ptr, None) and L.rwkv_b200_trace_enable(ctx.ptr)
+    lp, g = score(0, len(toks))
+    names = score_trace(types.SimpleNamespace(L=L, ptr=ctx.ptr))
+    L.rwkv_b200_trace_disable(ctx.ptr)
+    assert names[-4:] == ["layer_norm_columns", "convert_f16", "gemm_tc", "score"], names[-6:]
+    err = np.abs(lp[has].astype(F64) - lp64(ref, np.where(has, targets, 0))[has])
+    print(" score on the tensor cores - float64 over serial: %.2e" % err.max(), end="")
+    assert np.isfinite(lp[has]).all() and err.max() <= 2 * tol, err.max()
+    assert (lp[~has] == SENTINEL).all() and (g[~has] == 7).all()
+    assert bits(state()) == bits(want_state), "state after scoring on the tensor cores"
 
 
 # ---- A.6 every (shape, route) of the table ran ---------------------------------------------------------------------------------
 
 def test_every_shape_and_route_ran(request):
-    """Runs last: every (shape, format, route) of GEMV_CASES, every head route, every state kernel of every shape and every one-layer
-    file ran. Prints the launch keys each shape reached. A run of part of the file (-k, a node id) skips it."""
-    n_items = len(GEMV_CASES) + 4 * len(SHAPES) + len(V6) * (1 + len(FOLD_FORMATS)) + len(ONE_LAYER) + 1
+    """Runs last: every (shape, format, route) of GEMV_CASES, every head route (the GEMV ones and the tensor-core one of scoring), every
+    state kernel of every shape and every one-layer file ran. Prints the launch keys each shape reached. A run of part of the file (-k, a node id) skips it."""
+    n_items = len(GEMV_CASES) + 5 * len(SHAPES) + len(V6) * (1 + len(FOLD_FORMATS)) + len(ONE_LAYER) + 1
     if sum(i.fspath == request.node.fspath for i in request.session.items) < n_items:
         pytest.skip("only part of the file was selected")
     want = {(sh, "gemv", f, p, T) for sh, f, p, T in GEMV_CASES}
     want |= {(s.name, "head", f, p, T) for s in SHAPES for f in ("FP16", "FP32") for p, T in HEAD_ROUTES}
+    want |= {(s.name, "score_head", T) for s in SHAPES for T in SCORE_HEAD_T}
     want |= {(s.name, k) for s in SHAPES for k in ("ln_mix", "wkv")} | {(n, "v6_lerp") for n in V6}
     want |= {(n, "v6_fold", f) for n in V6 for f in FOLD_FORMATS} | {(n, "one_layer", f) for n, f in ONE_LAYER}
     for s in SHAPES:

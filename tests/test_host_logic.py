@@ -129,7 +129,7 @@ def test_kernel_hooks_reject_invalid_arguments(lib):
     passes in which whole warps emit whole 32-blocks (head size a multiple of 32 for the v5/6/7 WKV, not just n_embed) and for a
     weight type that has a stage class, batch passes of one token with non-overlapping states (and float4-aligned ones for the v5/6
     WKV), known formulas, tokens inside the table, embedding rows aligned to their element type, the lerp's staged columns
-    all or none."""
+    all or none, LayerNorm columns of at least one channel, one to 256 of them."""
     import kernel_hooks as kh
     f = lambda *shape: np.ones(shape, np.float32)
     Q = gf.TYPE_IDS["Q5_0"]
@@ -148,6 +148,11 @@ def test_kernel_hooks_reject_invalid_arguments(lib):
         lambda: kh.ln_mix(lib, f(64, 2), f(64), f(64), f(64 + 64), [f(64)], 0, n_seq=2, seq_stride=32),
         lambda: kh.ln_mix(lib, f(64, 1), f(64), f(64), f(64), [f(64)], 2),
         lambda: kh.embed_ln0(lib, np.ones((4, 64), np.float32), [0, 4], f(64), f(64)),
+        lambda: kh.layer_norm_columns(lib, f(64, 2), None, f(64)),             # no LayerNorm weight
+        lambda: kh.layer_norm_columns(lib, f(64, 2), f(64), None),             # no LayerNorm bias
+        lambda: kh.layer_norm_columns(lib, f(0, 2), f(0), f(0)),               # no channels
+        lambda: kh.layer_norm_columns(lib, f(64, 0), f(64), f(64)),            # no columns
+        lambda: kh.layer_norm_columns(lib, f(64, 257), f(64), f(64)),          # more columns than a pass holds
     ]
     # the GEMV batch hook: operands present exactly when the epilogue / prologue reads them, whole blocks, known inputs
     Q51 = gf.TYPE_IDS["Q5_1"]
@@ -184,6 +189,11 @@ def test_kernel_hooks_reject_invalid_arguments(lib):
     assert not lib.library.rwkv_b200_test_embed_ln0(ctypes.c_void_p(emb.ctypes.data), 0, ctypes.c_size_t(258), 3, ctypes.c_void_p(tok.ctypes.data), 1, 64,
                                                     ctypes.c_void_p(one.ctypes.data), ctypes.c_void_p(one.ctypes.data), ctypes.c_void_p(emb.ctypes.data))
     assert lib.rwkv_get_last_error(None) == ERR["ARGS"]
+    cols = np.ones(64 * 2, np.float32)
+    col = ctypes.c_void_p(cols.ctypes.data)
+    for x, y in ((None, col), (col, None)):          # no input, no output
+        assert not lib.library.rwkv_b200_test_layer_norm_columns(x, col, col, 64, 2, y)
+        assert lib.rwkv_get_last_error(None) == ERR["ARGS"]
     a = kh.V6LerpArgs(C=64, T=1, mix=32)          # staged columns for two of the five outputs
     buf = np.zeros(4096, np.float32)
     a.w2 = a.z = a.xx = a.sx = buf.ctypes.data

@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 import kernel_ref as kr
-from test_gpu_kernels import F32, F64, ln_mix_inputs, lerp_inputs, ref_wkv6, rng_for, wkv4_inputs, wkv6_inputs
+from test_gpu_kernels import (F32, F64, LN_COLUMN_WIDTHS, ln_columns_inputs, ln_mix_inputs, lerp_inputs, ref_wkv6, rng_for, wkv4_inputs,
+                              wkv6_inputs)
 
 
 def assert_caught(r64, r32, bugged):
@@ -55,6 +56,16 @@ def test_token_shift_off_by_one_is_caught(C, formula, T):
     bugged = kr.ln_mix(x, w, b, state, coefs, formula, F64, bug="shift")
     for j in range(3):
         assert_caught(r64[0][j], r32[0][j], bugged[0][j])
+
+
+@pytest.mark.parametrize("C", LN_COLUMN_WIDTHS)
+@pytest.mark.parametrize("T", [17, 256])
+@pytest.mark.parametrize("bug", ["eps", "wb_neighbour", "no_bias", "no_mean", "var_c_minus_1"])
+def test_layer_norm_columns_bugs_are_caught(C, T, bug):
+    """On the inputs of test_layer_norm_columns_matches_float64 (the ones with a column of variance ~eps, which eps 1e-6 needs)."""
+    x, w, b = ln_columns_inputs(C, T, rng_for("ln_columns", C, T))
+    r64, r32 = kr.layer_norm_columns(x, w, b, F64), kr.layer_norm_columns(x, w, b, F32)
+    assert_caught(r64, r32, kr.layer_norm_columns(x, w, b, F64, bug=bug))
 
 
 @pytest.mark.parametrize("T,mix,C", [(1, 32, 200), (33, 64, 1000), (8, 30, 200)])

@@ -167,3 +167,41 @@ def test_host_plan_matches_the_documented_routes():
     assert ms.tc_plan(32, [dict(M=5120, K=20480)], SMS)[1] == 2
     assert ms.tc_plan(32, [dict(M=768, K=3072)], SMS)[1] == 8
     assert ms.tc_plan(32, [dict(M=768, K=768)], SMS)[1] == 1          # 12 K-steps: too few for four per split of a cluster of 2+
+
+
+# ---- the tensor-core head of scoring passes at every head shape ----------------------------------------------------------------
+
+HEAD_SHAPES = sorted({(s.V, s.C) for s in ms.SHAPES})
+
+
+def head_case(V, C, T, tiles):
+    """Some row tiles of the head test_score_head_at_model_shape uploads, and an input of the same make: LayerNorm of columns of
+    scale 1.5 with random w / b, here in float32 on the host."""
+    rng = tg.rng_for("bars-head", V, C, T)
+    x = tg.inputs([C], T, rng, scale=1.5)[0]
+    w, b = (1 + 0.2 * rng.standard_normal(C)).astype(F32), (0.2 * rng.standard_normal(C)).astype(F32)
+    _, raw = ms.head_raw("FP16", ms.head_weights(V, C, tiles))
+    p = dict(type=ms.TYPE["FP16"], K=C, M=raw.size // (2 * C), raw=raw, input=0, epi=0, fmt="FP16", tiled=True)
+    return p, [kr.layer_norm(x, w, b, F32).astype(F32)]
+
+
+@pytest.mark.parametrize("V,C", HEAD_SHAPES)
+@pytest.mark.parametrize("defect", ["neighbouring_row_tile", "shifted_npad_column", "drop_last_tile", "no_colscale"])
+def test_head_defects_are_caught(V, C, defect):
+    """At the head's own bar (tc_factor of V x C): row tile 1 written with tile 2's output (T = 32); column 1 of a 17-column pass (npad
+    32) written with column 2's; the partial last row tile never written (101 rows at V = 50277); a column beyond the fp16 range
+    without its power-of-two scale."""
+    last = (V - 1) // 128
+    T = {"shifted_npad_column": 17, "drop_last_tile": 33}.get(defect, 32)
+    p, xs = head_case(V, C, T, [last] if defect == "drop_last_tile" else [1] if defect == "neighbouring_row_tile" else [0])
+    if defect == "no_colscale":
+        xs[0][:, 3] *= F32(3.0e5)
+    r64, r32 = ms.reference(p, xs, F64, True), ms.reference(p, xs, F32, True)
+    if defect == "neighbouring_row_tile":
+        bugged = ms.reference(head_case(V, C, T, [2])[0], xs, F64, True)
+    elif defect == "shifted_npad_column":
+        bugged = r64.copy()
+        bugged[:, 1] = bugged[:, 2]
+    else:
+        bugged = ms.reference(p, xs, F64, True, bug=defect)
+    assert kr.error_over_bar(bugged, r64, r32, ms.tc_factor(dict(M=V, K=C))) > 1, (V, C, defect)
