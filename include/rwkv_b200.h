@@ -262,6 +262,51 @@ RWKV_API bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, 
                                                    const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
                                                    rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated);
 
+/* Generation with log-probabilities: the loops above that also report, for every token they draw, how likely it was, as completion
+ * servers (logprobs / top_logprobs), evaluation and RL callers need, without per-token logits crossing PCIe.
+ * The arguments, checks, context kinds and refusals are those of rwkv_b200_generate_constrained / rwkv_b200_batch_generate_constrained,
+ * except that automaton may be NULL (no constraint; automaton_state is then not used) and automata may be NULL (no sequence
+ * constrained); on_token NULL is the blocking loop. The outputs are host arrays indexed like tokens_out ([rows][n], n the largest
+ * max_tokens, rows 1 or n_sequences); the top arrays are [rows][n][top_n]. With z the logits token i of a sequence was drawn from:
+ * 1. Generation itself does not change: tokens, n_generated, state, logits, penalty counts and automaton states are bit-identical to
+ *    the call without log-probabilities (rwkv_b200_generate* or its _constrained twin) with the same arguments.
+ * 2. logprobs[i] = log_softmax(z)[token i] of the raw logits, before penalties, mask, top-p and temperature: bit for bit what
+ *    rwkv_b200_score_logits returns for z and that target (a -inf logit gives -inf; a column with a NaN or +inf, or without a finite
+ *    value, gives NaN). So rwkv_b200_score over the same text from the same state returns the same bits wherever it runs the GEMV head.
+ * 3. top_ids[i][0 .. top_n) are the top_n largest entries of z in descending order, the smaller id first among equal logits, and
+ *    top_logprobs their log-probabilities, each bit for bit rwkv_b200_score_logits with that id as target. -inf entries appear only when
+ *    fewer than top_n are finite. For a column with a NaN or +inf, or without a finite value, every id is RWKV_B200_SCORE_NO_TARGET and
+ *    every log-probability NaN.
+ * 4. sample_probs[i] (optional) is the probability the token had under the distribution it was drawn from, after penalty bias,
+ *    automaton mask, top-p and temperature: bit for bit rwkv_b200_sample_logits' prob_out for z, u and that bias list (1 at
+ *    temperature 0).
+ * 5. A stop id's entries are written too. Entries at or past n_generated[b] are NaN (floats) and RWKV_B200_SCORE_NO_TARGET (ids).
+ * 6. Streaming: entry i of every output array is written before on_token(..., i, ...) is called; ending a sequence after token i gives
+ *    the outputs of max_tokens = i + 1.
+ * 7. RWKV_ERROR_ARGS, changing nothing, for a NULL lp or lp->logprobs, top_n > RWKV_B200_TOP_LOGPROBS_MAX or > n_vocab, and NULL top
+ *    arrays with top_n > 0.
+ * The first call that asks for log-probabilities allocates their buffers (rows * n * (2 + 2 * top_n) words on the device and pinned on
+ * the host, grown to the largest call, and for streaming a small mapped ring); contexts that never ask allocate nothing. */
+#define RWKV_B200_TOP_LOGPROBS_MAX 20
+struct rwkv_b200_logprobs {
+    size_t top_n;                              /* 0 .. RWKV_B200_TOP_LOGPROBS_MAX, and <= n_vocab */
+    float * logprobs;                          /* [rows][n], required */
+    uint32_t * top_ids;                        /* [rows][n][top_n], NULL iff top_n == 0 */
+    float * top_logprobs;                      /* [rows][n][top_n], NULL iff top_n == 0 */
+    float * sample_probs;                      /* [rows][n], optional */
+};
+RWKV_API bool rwkv_b200_generate_logprobs(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state,
+                                          size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
+                                          bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                          rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated,
+                                          const struct rwkv_b200_logprobs * lp);
+RWKV_API bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata,
+                                                uint32_t * automaton_states, const uint32_t * max_tokens, const float * temperature,
+                                                const float * top_p, const float * presence_penalty, const float * frequency_penalty,
+                                                const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                                rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
+                                                const struct rwkv_b200_logprobs * lp);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each
@@ -286,6 +331,10 @@ RWKV_API bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_
  * states[b], which receives its new state; states[b] == UINT32_MAX marks an unconstrained row. */
 RWKV_API bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states,
                                                        uint32_t * states);
+/* The same step of the logprob kernel: next NULL leaves every row unconstrained (states not used), otherwise as above. The outputs of
+ * lp ([n_rows][n], top arrays [n_rows][n][top_n]) are written at [b][step] for every row that draws; other entries keep what they held. */
+RWKV_API bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states,
+                                                    uint32_t * states, const struct rwkv_b200_logprobs * lp);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

@@ -560,27 +560,36 @@ static_assert(RWKV_B200_GENERATE_MAX == GENERATE_MAX && RWKV_B200_GENERATE_MAX_S
 
 static_assert(RWKV_B200_STREAM_TIMEOUT_MS == STREAM_TIMEOUT_MS, "streaming wait bound of the header and the kernel");
 
+// The public logprob request as the engine's; NULL is refused.
+static bool logprobs_arg(ErrorSink sink, const struct rwkv_b200_logprobs * lp, LogprobsOut & out) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp, "NULL logprob request");
+    out = LogprobsOut{lp->top_n, lp->logprobs, lp->top_ids, lp->top_logprobs, lp->sample_probs};
+    return true;
+}
+
 // The single-sequence generate calls; on_token NULL is the blocking loop. `constrained`: the row follows *automaton from
 // *automaton_state (both checked here, the rest by generate).
 static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
                             bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated,
                             bool streaming, TokenFn on_token, void * user, bool constrained = false, const Automaton * automaton = nullptr,
-                            uint32_t * automaton_state = nullptr) {
+                            uint32_t * automaton_state = nullptr, bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr) {
     if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
-    const char * suffix = constrained ? "_constrained" : streaming ? "_stream" : "";
+    const char * suffix = logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "";
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s", suffix);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
                "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automaton && automaton_state), "NULL automaton or automaton_state");
+    LogprobsOut out{};
+    if (logprobs && !logprobs_arg(c->sink(), lp, out)) return false;
     const uint32_t budget = (uint32_t) max_tokens;
     const uint8_t keep = keep_counts ? 1 : 0;
     uint32_t n = 0;
     const bool ok = generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n, on_token, user,
-                             constrained ? &automaton : nullptr, automaton_state);
+                             constrained ? &automaton : nullptr, automaton_state, logprobs ? &out : nullptr);
     if (ok || n) *n_generated = n;      // a callback that kept the device waiting too long still gets what was delivered
     return ok;
 }
@@ -589,17 +598,20 @@ static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float 
 static bool generate_batch(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                            const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
                            const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user,
-                           bool constrained = false, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr) {
+                           bool constrained = false, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr,
+                           bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr) {
     if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s",
-               constrained ? "_constrained" : streaming ? "_stream" : "");
+               logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automata && automaton_states), "NULL automata or automaton_states");
+    LogprobsOut out{};
+    if (logprobs && !logprobs_arg(c->sink(), lp, out)) return false;
     return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user,
-                    automata, automaton_states);
+                    automata, automaton_states, logprobs ? &out : nullptr);
 }
 
 bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
@@ -666,11 +678,31 @@ bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, const str
                           false, on_token, user, true, reinterpret_cast<const Automaton * const *>(automata), automaton_states);
 }
 
+bool rwkv_b200_generate_logprobs(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state, size_t max_tokens,
+                                 float temperature, float top_p, float presence_penalty, float frequency_penalty, bool keep_counts, const double * u,
+                                 const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
+                                 size_t * n_generated, const struct rwkv_b200_logprobs * lp) {
+    return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                           on_token != nullptr, on_token, user, automaton != nullptr, automaton, automaton_state, true, lp);
+}
+
+bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata, uint32_t * automaton_states,
+                                       const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence_penalty,
+                                       const float * frequency_penalty, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids,
+                                       size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
+                                       const struct rwkv_b200_logprobs * lp) {
+    return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                          on_token != nullptr, on_token, user, automata != nullptr, reinterpret_cast<const Automaton * const *>(automata), automaton_states,
+                          true, lp);
+}
+
 static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");
+static_assert(RWKV_B200_TOP_LOGPROBS_MAX == GEN_TOP_MAX, "top log-probabilities of the header and the kernel");
 
 // One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
-// the table from states[b] (UINT32_MAX: unconstrained).
-static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states) {
+// the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained).
+static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
+                               const LogprobsOut * lp = nullptr) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
@@ -684,6 +716,7 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->step[b] <= a->max_tokens[b], "step of row %zu is above its max_tokens", b);
     }
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n >= 1, "Every row has max_tokens 0");
+    if (lp && !check_logprobs(sink, V, lp)) return false;
     const bool constrained = next != nullptr;
     std::vector<uint8_t> live;
     if (constrained) {
@@ -728,13 +761,34 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         cp.mask = const_cast<GenMaskRow *>(hb.in(mask.data(), R));
         cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
     }
-    const cudaError_t e = !hb.ok ? cudaSuccess : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
+    GenLogprobParams lpp{};
+    GenLogprobRequest req{};
+    const size_t cells = R * n, k = lp ? lp->top_n : 0;
+    if (lp) {       // every row unconstrained without a table; the outputs start as the caller's arrays
+        if (!constrained) {
+            const std::vector<GenMaskRow> none(R, GenMaskRow{nullptr, nullptr, 0, 0});
+            cp.mask = const_cast<GenMaskRow *>(hb.in(none.data(), R));
+            cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
+        }
+        req.top_n = (uint32_t) k;
+        req.logprobs = const_cast<float *>(hb.in(lp->logprobs, cells));
+        req.sample_probs = lp->sample_probs ? const_cast<float *>(hb.in(lp->sample_probs, cells)) : static_cast<float *>(hb.alloc(cells * sizeof(float)));
+        req.top_ids = k ? const_cast<uint32_t *>(hb.in(lp->top_ids, cells * k)) : nullptr;
+        req.top_logprobs = k ? const_cast<float *>(hb.in(lp->top_logprobs, cells * k)) : nullptr;
+        lpp.gen = cp;
+        lpp.req = hb.in(&req, 1);
+    }
+    const cudaError_t e = !hb.ok ? cudaSuccess : lp ? launch_generate_logprob_step(lpp, 0) : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->next_tokens, gp.next_tokens, R * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
-              (!constrained || cudaMemcpy(states_out.data(), cp.states_out, R * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess);
+              (!constrained || cudaMemcpy(states_out.data(), cp.states_out, R * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess) &&
+              (!lp || cudaMemcpy(lp->logprobs, req.logprobs, cells * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess) &&
+              (!lp || !lp->sample_probs || cudaMemcpy(lp->sample_probs, req.sample_probs, cells * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess) &&
+              (!k || (cudaMemcpy(lp->top_ids, req.top_ids, cells * k * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                      cudaMemcpy(lp->top_logprobs, req.top_logprobs, cells * k * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess));
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "generate step failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     for (size_t b = 0; b < R; b++) { a->step[b] = rows[b].step; a->frozen[b] = rows[b].frozen ? 1 : 0; }
     for (size_t b = 0; constrained && b < R; b++)
@@ -747,6 +801,15 @@ bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a)
 bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states) {
     if (!next) { g_last_error = RWKV_ERROR_NONE; ErrorSink sink = global_sink(); RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL table"); }
     return generate_step_hook(a, next, n_states, states);
+}
+
+bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
+                                           const struct rwkv_b200_logprobs * lp) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    LogprobsOut out{};
+    if (!logprobs_arg(sink, lp, out)) return false;
+    return generate_step_hook(a, next, n_states, states, &out);
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

@@ -771,6 +771,10 @@ void destroy_context(Context * ctx) {
     if (ctx->gen_out_host) cudaFreeHost(ctx->gen_out_host);
     if (ctx->stream_host) cudaFreeHost(ctx->stream_host);
     if (ctx->stream_done) cudaEventDestroy(ctx->stream_done);
+    cudaFree(ctx->lp_req); cudaFree(ctx->lp_dev);
+    if (ctx->lp_req_host) cudaFreeHost(ctx->lp_req_host);
+    if (ctx->lp_host) cudaFreeHost(ctx->lp_host);
+    if (ctx->lp_ring_host) cudaFreeHost(ctx->lp_ring_host);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
     if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
@@ -1377,6 +1381,9 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // A streaming loop runs generate_stream_sample_kernel instead: after each draw it publishes the token to mapped host memory, and
 // before the next draw of that row it waits for the calling thread to acknowledge it (stream_tokens), so that the pass evaluating
 // token j overlaps the callback of token j, and a callback can end its row before token j + 1 is drawn.
+// A loop that reports log-probabilities runs the logprob step kernels instead, in graphs of their own (gen_lp_graphs); they read the
+// call's GenLogprobRequest from ctx->lp_req, and the streaming one writes each token's record into the mapped ring before it publishes
+// the token, so that stream_tokens can hand the record to the caller before on_token.
 namespace {
 
 size_t gen_mask_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
@@ -1427,7 +1434,7 @@ GenStreamParams generate_stream_params(Context * ctx) {
     return sp;
 }
 
-bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
+bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool logprobs) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     Pass p;
     if (!make_pass(ctx, rows, true, nullptr, p)) return false;
@@ -1458,7 +1465,8 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
         const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen_in + gen_mask_offset(rows)), ctx->gen_out + rows + 1};
-        CUDA_OK(ctx, constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
+        CUDA_OK(ctx, logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req}, streaming, &step)
+                     : constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
                      : streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
                                  : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
         cudaGraphNodeParams ip = {};
@@ -1469,7 +1477,7 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained) {
         std::swap(p.state_in, p.state_out);      // the second pass reads what the first one wrote
         prev = cond;
     }
-    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
+    CUDA_OK(ctx, cudaGraphInstantiate(logprobs ? &ctx->gen_lp_graphs[ctx->phase][streaming] : &ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
     return true;
 }
 
@@ -1501,11 +1509,40 @@ bool ensure_stream_buffers(Context * ctx) {
     return true;
 }
 
+// The request and output buffers of a logprob call whose outputs take `words` 32-bit words, and for a streaming one the ring.
+bool ensure_logprob_buffers(Context * ctx, size_t words, bool streaming) {
+    const int rows = ctx->batch_n ? ctx->batch_n : 1;
+    if (!ctx->lp_req_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->lp_req_host), sizeof(GenLogprobRequest)));
+    if (!ctx->lp_req) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->lp_req), sizeof(GenLogprobRequest)));
+    if (words > ctx->lp_words) {      // no graph holds these addresses: they travel in the request
+        cudaFree(ctx->lp_dev);
+        if (ctx->lp_host) cudaFreeHost(ctx->lp_host);
+        ctx->lp_dev = ctx->lp_host = nullptr;
+        ctx->lp_words = 0;
+        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->lp_dev), words * sizeof(uint32_t)));
+        CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->lp_host), words * sizeof(uint32_t)));
+        ctx->lp_words = words;
+    }
+    if (streaming && !ctx->lp_ring_dev) {
+        if (!ctx->lp_ring_host)
+            CUDA_OK(ctx, cudaHostAlloc(reinterpret_cast<void **>(&ctx->lp_ring_host), (size_t) rows * 2 * GEN_LP_RECORD * sizeof(uint32_t), cudaHostAllocMapped));
+        CUDA_OK(ctx, cudaHostGetDevicePointer(reinterpret_cast<void **>(&ctx->lp_ring_dev), ctx->lp_ring_host, 0));
+    }
+    return true;
+}
+
+// Entry at = b * n + j of the caller's logprob arrays <- words[w] of a record laid out as the ring's (GenLogprobRequest, ops.h).
+void put_logprob_entry(const LogprobsOut & lp, size_t at, float logprob, float sample_prob, const uint32_t * ids, const float * top_lps) {
+    lp.logprobs[at] = logprob;
+    if (lp.sample_probs) lp.sample_probs[at] = sample_prob;
+    for (size_t k = 0; k < lp.top_n; k++) { lp.top_ids[at * lp.top_n + k] = ids[k]; lp.top_logprobs[at * lp.top_n + k] = top_lps[k]; }
+}
+
 // The calling thread's side of a streaming loop that has been enqueued up to ctx->stream_done: calls on_token for every token the
 // step kernel publishes, in order per row, and acknowledges each one (the stop bit set when on_token returned nonzero), until the
 // stream has passed the event and every published token is delivered. Busy-polls, yielding between empty sweeps. Returns false when
-// a wait of the device for an acknowledgement ran out.
-bool stream_tokens(Context * ctx, TokenFn on_token, void * user) {
+// a wait of the device for an acknowledgement ran out. With lp, token j's ring record goes to entry j of lp's arrays (`stride` entries per row) first.
+bool stream_tokens(Context * ctx, TokenFn on_token, void * user, const LogprobsOut * lp, size_t stride) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     uint32_t * published = ctx->stream_host, * acked = published + rows, * tokens = published + stream_token_offset(rows);
     std::vector<uint32_t> delivered((size_t) rows, 0);
@@ -1517,6 +1554,15 @@ bool stream_tokens(Context * ctx, TokenFn on_token, void * user) {
             const uint32_t n = __atomic_load_n(published + b, __ATOMIC_ACQUIRE);
             for (uint32_t j = delivered[b]; j < n; j++) {
                 const uint32_t tok = __atomic_load_n(tokens + (size_t) b * GENERATE_MAX + j, __ATOMIC_RELAXED);
+                if (lp) {
+                    uint32_t rec[GEN_LP_RECORD];
+                    const uint32_t * src = ctx->lp_ring_host + ((size_t) b * 2 + (j & 1u)) * GEN_LP_RECORD;
+                    for (int w = 0; w < GEN_LP_RECORD; w++) rec[w] = __atomic_load_n(src + w, __ATOMIC_RELAXED);
+                    float f[2 + GEN_TOP_MAX];
+                    memcpy(f, rec, 2 * sizeof(float));
+                    memcpy(f + 2, rec + 2 + GEN_TOP_MAX, GEN_TOP_MAX * sizeof(float));
+                    put_logprob_entry(*lp, (size_t) b * stride + j, f[0], f[1], rec + 2, f + 2);
+                }
                 const uint32_t stop = on_token(user, (size_t) b, j, tok) != 0 ? 1u : 0u;
                 __atomic_store_n(acked + b, 2 * (j + 1) + stop, __ATOMIC_RELEASE);
                 any = true;
@@ -1535,6 +1581,16 @@ void drop_generate_graphs(Context * ctx) {
     for (auto & by_phase : ctx->gen_graphs)
         for (auto & by_streaming : by_phase)
             for (auto & e : by_streaming) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+    for (auto & by_phase : ctx->gen_lp_graphs)
+        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+}
+
+bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp && lp->logprobs, "NULL logprob request or logprobs array");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp->top_n <= (size_t) GEN_TOP_MAX && lp->top_n <= n_vocab, "top_n (%zu) must be at most %d and n_vocab",
+               lp->top_n, GEN_TOP_MAX);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp->top_n == 0 || (lp->top_ids && lp->top_logprobs), "NULL top_ids or top_logprobs with top_n > 0");
+    return true;
 }
 
 bool check_automaton_table(ErrorSink sink, const uint16_t * next, size_t n_states, size_t n_vocab) {
@@ -1618,7 +1674,7 @@ bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const ui
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
               uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token, void * user, const Automaton * const * automata,
-              uint32_t * automaton_states) {
+              uint32_t * automaton_states, const LogprobsOut * lp) {
     const Model & m = *ctx->model;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     const size_t V = (size_t) m.n_vocab;
@@ -1636,6 +1692,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
                        automaton_states[b], b, automata[b]->n_states);
         }
     }
+    if (lp && !check_logprobs(ctx->sink(), V, lp)) return false;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, V <= 65536, "On-device sampling supports n_vocab <= 65536");
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last evaluation skipped the head");
     int driver = 0;
@@ -1646,6 +1703,8 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     const bool streaming = on_token != nullptr;
     if (!ensure_generate_buffers(ctx) || (streaming && !ensure_stream_buffers(ctx)) || !ensure_capacity(ctx, rows, ctx->stream)) return false;
+    const size_t lp_cells = (size_t) rows * n, lp_words = lp ? lp_cells * (2 + 2 * lp->top_n) : 0;
+    if (lp && !ensure_logprob_buffers(ctx, lp_words, streaming)) return false;
     // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
     GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
     memset(sh, 0, sizeof(GenShared));
@@ -1669,16 +1728,23 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     const size_t out_words = gen_out_words(rows, n);
     CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_out, 0, out_words * sizeof(uint32_t), ctx->stream));
     if (streaming) memset(ctx->stream_host, 0, stream_token_offset(rows) * sizeof(uint32_t));     // published, acked, timed_out
-    cudaGraphExec_t & graph = ctx->gen_graphs[ctx->phase][streaming][constrained];
-    if (!graph && !build_generate_graph(ctx, streaming, constrained)) return false;
+    if (lp) {
+        float * f = reinterpret_cast<float *>(ctx->lp_dev);
+        *ctx->lp_req_host = GenLogprobRequest{(uint32_t) lp->top_n, 0, f, f + lp_cells, ctx->lp_dev + 2 * lp_cells, f + 2 * lp_cells + lp_cells * lp->top_n,
+                                              streaming ? ctx->lp_ring_dev : nullptr};
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_req, ctx->lp_req_host, sizeof(GenLogprobRequest), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    cudaGraphExec_t & graph = lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
+    if (!graph && !build_generate_graph(ctx, streaming, constrained, lp != nullptr)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (lp_words) CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_host, ctx->lp_dev, lp_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     bool in_time = true;
     if (streaming) {
         CUDA_OK(ctx, cudaEventRecord(ctx->stream_done, ctx->stream));
-        in_time = stream_tokens(ctx, on_token, user);
+        in_time = stream_tokens(ctx, on_token, user, lp, n);
     }
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     const uint32_t * res = ctx->gen_out_host;
@@ -1686,6 +1752,17 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     memcpy(tokens_out, res + gen_tokens_word(rows), (size_t) rows * n * sizeof(uint32_t));
     for (int b = 0; constrained && b < rows; b++)
         if (automata[b]) automaton_states[b] = res[rows + 1 + b];
+    if (lp) {       // drawn entries from the device, the rest NaN / SCORE_NO_TARGET
+        const float * f = reinterpret_cast<const float *>(ctx->lp_host);
+        const std::vector<uint32_t> none(lp->top_n, SCORE_NO_TARGET);
+        const std::vector<float> nans(lp->top_n, NAN);
+        for (int b = 0; b < rows; b++)
+            for (size_t i = 0; i < n; i++) {
+                const size_t at = (size_t) b * n + i, k = lp->top_n;
+                if (i < res[b]) put_logprob_entry(*lp, at, f[at], f[lp_cells + at], ctx->lp_host + 2 * lp_cells + at * k, f + 2 * lp_cells + lp_cells * k + at * k);
+                else put_logprob_entry(*lp, at, NAN, NAN, none.data(), nans.data());
+            }
+    }
     if (res[rows] & 1u) {      // an odd number of passes leaves the state in state_b
         std::swap(ctx->state_a, ctx->state_b);
         ctx->phase ^= 1;

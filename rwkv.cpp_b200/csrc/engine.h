@@ -24,6 +24,7 @@ struct PipeGroup {
 };
 
 struct SampleRow;                       // per-sequence sampling parameters (kernels/ops.h)
+struct GenLogprobRequest;               // the per-call request of the logprob generation kernels (kernels/ops.h)
 struct CopyPool;                        // helper threads of the pageable-buffer bounce path (engine.cu)
 void destroy_copy_pool(CopyPool * p);
 
@@ -134,6 +135,15 @@ struct Context {
     uint32_t * stream_host = nullptr, * stream_dev = nullptr;
     cudaEvent_t stream_done = nullptr;   // recorded after the streaming loop's copies
     bool in_stream = false;          // the calling thread is inside a streaming call's callbacks: this context's stream is busy
+    // Log-probabilities of generated tokens (generate with a LogprobsOut), allocated only by calls that ask for them. lp_req: the
+    // call's GenLogprobRequest, at a device address the logprob graphs capture (pinned copy lp_req_host). lp_dev / lp_host: the call's
+    // outputs [rows][n] logprobs, sample probs, then [rows][n][top_n] ids and log-probabilities, lp_words 32-bit words each, grown to
+    // the largest rows * n * (2 + 2 * top_n) asked for. lp_ring: mapped [rows][2][GEN_LP_RECORD] records of the streaming loop.
+    GenLogprobRequest * lp_req = nullptr, * lp_req_host = nullptr;
+    uint32_t * lp_dev = nullptr, * lp_host = nullptr;
+    size_t lp_words = 0;
+    uint32_t * lp_ring_host = nullptr, * lp_ring_dev = nullptr;
+    cudaGraphExec_t gen_lp_graphs[2][2] = {};    // the logprob loops' graphs, keyed by phase and streaming
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -241,11 +251,22 @@ bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const ui
                          const void * tokens_out, const void * n_generated);
 // With automata (rwkv_b200_generate_constrained), row b is restricted by automata[b] from state automaton_states[b] (a NULL entry:
 // unconstrained), and automaton_states[b] receives the row's final state.
+// With lp (rwkv_b200_generate_logprobs), every drawn token's log-probability, top alternatives and sampling probability go to lp's
+// host arrays, [n_rows][n] (top arrays [n_rows][n][top_n]), entries past n_generated[b] NaN / SCORE_NO_TARGET; the loop runs the logprob
+// kernels, which take automata == NULL as "no row constrained". check_logprobs checks lp (also for the test hook).
 struct Automaton;
+struct LogprobsOut {
+    size_t top_n;
+    float * logprobs;
+    uint32_t * top_ids;
+    float * top_logprobs;
+    float * sample_probs;             // may be NULL
+};
+bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp);
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
               uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr,
-              const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr);
+              const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr, const LogprobsOut * lp = nullptr);
 
 // A token automaton of rwkv_b200_automaton_create: the transition table next[s * n_vocab + t] (GEN_MASK_DEAD: t not allowed in s)
 // and live[s] (s allows some token) in the HBM of the model's device. It serves every context of that model.

@@ -275,6 +275,31 @@ struct GenConstrainedParams {
 cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s);     // the blocking kernel
 cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
                                                cudaGraphNode_t * node);
+// Generation with log-probabilities (rwkv_b200_generate_logprobs / rwkv_b200_batch_generate_logprobs): the constrained steps (a row
+// with a NULL table is unconstrained) that also report, for every token they draw at [b][step] of the request's [n_rows][stride]
+// arrays: logprobs = log_softmax(z)[tok] of the raw logits z the token was drawn from, in the arithmetic and order of score_kernel;
+// the top_n largest logits of z (descending, the smaller id first among equals) with their log-probabilities; and sample_probs = the
+// probability the token had after bias, mask, top-p and temperature (sample_row's prob_out). A column with a NaN or +inf, or without a
+// finite logit, gives NaN log-probabilities and SCORE_NO_TARGET ids. The streaming kernel also writes the token's record into the
+// mapped ring (row b, slot step % 2: logprob, sample prob, top_n ids, top_n log-probabilities) before it publishes the token.
+// The request lives in the per-call upload, so that one graph serves every top_n and output buffer.
+constexpr int GEN_TOP_MAX = 20;
+constexpr int GEN_LP_RECORD = 2 + 2 * GEN_TOP_MAX;     // words of a ring record
+struct GenLogprobRequest {            // written by the host per call
+    uint32_t top_n, pad;
+    float * logprobs;                 // [n_rows][stride] device
+    float * sample_probs;             // [n_rows][stride] device
+    uint32_t * top_ids;               // [n_rows][stride][top_n] device
+    float * top_logprobs;             // [n_rows][stride][top_n] device
+    uint32_t * ring;                  // mapped [n_rows][2][GEN_LP_RECORD], streaming only
+};
+struct GenLogprobParams {
+    GenConstrainedParams gen;
+    const GenLogprobRequest * req;    // device
+};
+cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_t s);     // the blocking kernel
+cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
+                                           cudaGraphNode_t * node);
 // After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);

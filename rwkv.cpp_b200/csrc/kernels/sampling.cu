@@ -13,6 +13,7 @@
 // its own parameters and bias; both kernels call the same sample_row body.
 #include "ops.h"
 #include "gemv.h"
+#include "score_row.cuh"
 
 namespace rwkv {
 namespace {
@@ -266,9 +267,102 @@ struct TableMask {
     __device__ __forceinline__ void report(int b) const { states_out[b] = rows[b].state; }
 };
 
-// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`, its draws restricted by `mask`.
-template <int PER, class Gate, class Mask>
-__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate, const Mask mask) {
+// The loops without log-probabilities: sample_row gets no prob_out, nothing is recorded.
+struct NoLogprobs {
+    __device__ __forceinline__ float * prob_slot(size_t) const { return nullptr; }
+    __device__ __forceinline__ void record(int, size_t, uint32_t, const float *, int, uint32_t) const {}
+};
+
+// Top-N order over (logit, id): a larger logit first, the smaller id first among equal logits. The key holds the logit's bits mapped to
+// an unsigned order in its upper half (-0 counted as +0, so that equal values differ by id alone) and ~id in its lower half, so every
+// entry of a column has its own key and the largest keys are the top entries. No entry maps to key 0 (upper half 0xFFFFFFFF and id
+// 0xFFFFFFFF together), so 0 stands for "none".
+__device__ __forceinline__ unsigned long long top_key(float v, int i) {
+    const uint32_t u = __float_as_uint(__fadd_rn(v, 0.0f));
+    return ((unsigned long long) ((u & 0x80000000u) ? ~u : (u | 0x80000000u)) << 32) | (uint32_t) ~(uint32_t) i;
+}
+// The largest key below `limit` among this thread's entries tid + k * SAMPLE_THREADS of z, or 0.
+template <int PER>
+__device__ __forceinline__ unsigned long long top_below(const float * z, int V, int tid, unsigned long long limit) {
+    unsigned long long best = 0;
+#pragma unroll 4
+    for (int k = 0; k < PER; k++) {
+        const int i = tid + k * SAMPLE_THREADS;
+        if (i < V) {
+            const unsigned long long key = top_key(z[i], i);
+            if (key < limit && key > best) best = key;
+        }
+    }
+    return best;
+}
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+        v = w > v ? w : v;
+    }
+    return v;
+}
+
+// The log-probability policy of the logprob kernels (GenLogprobRequest, ops.h). After the draw of token tok from row b's raw logits z:
+// warps 0-7 run score_kernel's reduction (score_row.cuh) under named barrier 1 while every warp selects its top_n entries by
+// top_n rounds of a warp-wide key maximum (a round's winner rescans its own entries below the key it gave up). Warp 0 then merges the
+// 32 sorted lists in shared memory the same way, and its lane 0 writes the outputs at `at` (and, streaming, the ring record).
+template <int PER>
+struct Logprobs {
+    const GenLogprobRequest * req;
+    bool ring;
+    __device__ __forceinline__ float * prob_slot(size_t at) const { return req->sample_probs + at; }
+    __device__ __forceinline__ void record(int b, size_t at, uint32_t step, const float * z, int V, uint32_t tok) const {
+        __shared__ float s_max[LP_SCORE_WARPS];
+        __shared__ int s_arg[LP_SCORE_WARPS], s_bad[LP_SCORE_WARPS];
+        __shared__ double s_sum[LP_SCORE_WARPS];
+        __shared__ unsigned long long s_top[SAMPLE_WARPS][GEN_TOP_MAX];
+        const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, top_n = (int) req->top_n;
+        float mx = 0.f;
+        bool valid = false;
+        double log_sum = 0.0;
+        if (tid < LP_SCORE_THREADS)
+            score_column(tid, z, V, s_max, s_arg, s_bad, s_sum, [] { asm volatile("bar.sync 1, %0;" :: "n"(LP_SCORE_THREADS) : "memory"); },
+                         [&](float m, int, bool v, double sum) { mx = m; valid = v; if (v) log_sum = log(sum); });
+        if (top_n > 0) {
+            unsigned long long mine = top_below<PER>(z, V, tid, ~0ull);
+            for (int k = 0; k < top_n; k++) {
+                const unsigned long long w = warp_max_u64(mine);
+                if (lane == 0) s_top[warp][k] = w;
+                if (w != 0 && mine == w) mine = top_below<PER>(z, V, tid, w);
+            }
+        }
+        __syncthreads();
+        if (warp != 0) return;
+        uint32_t * rec = ring ? req->ring + ((size_t) b * 2 + (step & 1u)) * GEN_LP_RECORD : nullptr;
+        int head = 0;
+        unsigned long long cur = top_n > 0 ? s_top[lane][0] : 0ull;
+        for (int k = 0; k < top_n; k++) {
+            const unsigned long long w = warp_max_u64(cur);
+            if (lane == 0) {
+                const uint32_t id = ~(uint32_t) w;
+                const uint32_t out_id = valid ? id : SCORE_NO_TARGET;
+                const float out_lp = valid ? score_logprob(z[id], mx, log_sum) : NAN;
+                req->top_ids[at * top_n + k] = out_id;
+                req->top_logprobs[at * top_n + k] = out_lp;
+                if (rec) { ((volatile uint32_t *) rec)[2 + k] = out_id; ((volatile float *) rec)[2 + GEN_TOP_MAX + k] = out_lp; }
+            }
+            if (cur == w) { head++; cur = head < top_n ? s_top[lane][head] : 0ull; }
+        }
+        if (lane == 0) {
+            const float lp = valid ? score_logprob(z[tok], mx, log_sum) : NAN;
+            const float prob = req->sample_probs[at];
+            req->logprobs[at] = lp;
+            if (rec) { ((volatile float *) rec)[0] = lp; ((volatile float *) rec)[1] = prob; }
+        }
+    }
+};
+
+// One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`, its draws restricted by `mask`, every
+// draw reported by `lp`.
+template <int PER, class Gate, class Mask, class Lp = NoLogprobs>
+__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate, const Mask mask, const Lp lp = Lp{}) {
     __shared__ int draw, park;
     const int b = blockIdx.x, tid = threadIdx.x, V = gp.n_vocab;
     const size_t off = (size_t) b * V;
@@ -300,7 +394,8 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
         p.logits = gp.logits + off; p.n_vocab = V;
         p.temperature = r->temperature; p.top_p = r->top_p; p.u = gp.u[(size_t) b * sh->stride + step];
         p.bias_ids = gp.bias_ids + off; p.bias_values = gp.bias_values + off; p.n_bias = V;
-        p.scratch = gp.scratch + off; p.token_out = gp.tokens + (size_t) b * sh->stride + step; p.prob_out = nullptr;
+        p.scratch = gp.scratch + off; p.token_out = gp.tokens + (size_t) b * sh->stride + step;
+        p.prob_out = lp.prob_slot((size_t) b * sh->stride + step);
         sample_row<PER>(p);
         __syncthreads();
         if (tid == 0) {
@@ -312,6 +407,7 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
             else { gp.counts[off + tok] += 1; mask.advance(b, V, tok); }
         }
         __syncthreads();
+        lp.record(b, (size_t) b * sh->stride + step, step, gp.logits + off, V, tok);
     }
     if (park && gp.park)
         for (int i = tid; i < V; i += SAMPLE_THREADS) gp.park[off + i] = gp.logits[off + i];
@@ -365,6 +461,22 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_constrained
     generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, TableMask{cp.mask, cp.states_out});
 }
 
+// The constrained steps that also report log-probabilities (GenLogprobParams); a row with a NULL table is unconstrained, so these two
+// serve the logprob calls with and without automata.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_logprob_sample_kernel(const GenLogprobParams lp) {
+    pdl_prologue();
+    generate_step<PER>(lp.gen.stream.step, NoGate{}, TableMask{lp.gen.mask, lp.gen.states_out}, Logprobs<PER>{lp.req, false});
+}
+
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_logprob_sample_kernel(const GenLogprobParams lp) {
+    pdl_prologue();
+    const GenStreamParams & sp = lp.gen.stream;
+    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, TableMask{lp.gen.mask, lp.gen.states_out},
+                       Logprobs<PER>{lp.req, true});
+}
+
 constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
 
 __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const GenRow * rows, const float * src, float * dst, long long seq_stride, size_t n) {
@@ -386,15 +498,24 @@ void * generate_step_for(int n_vocab, bool stream, bool constrained) {
          : per <= 16 ? generate_step_fn<16>(stream, constrained) : per <= 50 ? generate_step_fn<50>(stream, constrained) : generate_step_fn<64>(stream, constrained);
 }
 
-// A step kernel node of graph g after deps with the single kernel parameter `arg`.
+template <int PER> void * generate_logprob_step_fn(bool stream) {
+    return stream ? reinterpret_cast<void *>(generate_stream_logprob_sample_kernel<PER>) : reinterpret_cast<void *>(generate_logprob_sample_kernel<PER>);
+}
+void * generate_logprob_step_for(int n_vocab, bool stream) {
+    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    return per <= 1 ? generate_logprob_step_fn<1>(stream) : per <= 4 ? generate_logprob_step_fn<4>(stream) : per <= 16 ? generate_logprob_step_fn<16>(stream)
+         : per <= 50 ? generate_logprob_step_fn<50>(stream) : generate_logprob_step_fn<64>(stream);
+}
+
+// A node of graph g after deps running step kernel `func` with the single kernel parameter `arg`.
 template <class P>
-cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, bool stream, bool constrained,
+cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, void * func,
                           cudaGraphNode_t * node) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
     P copy = arg;
     void * args[] = {&copy};
     cudaKernelNodeParams kp = {};
-    kp.func = generate_step_for(p.n_vocab, stream, constrained);
+    kp.func = func;
     kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
     kp.kernelParams = args; kp.extra = nullptr;
     return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
@@ -414,11 +535,11 @@ cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s) {
 }
 
 cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p, p, false, false, node);
+    return add_step_node(g, deps, n_deps, p, p, generate_step_for(p.n_vocab, false, false), node);
 }
 
 cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.step, p, true, false, node);
+    return add_step_node(g, deps, n_deps, p.step, p, generate_step_for(p.step.n_vocab, true, false), node);
 }
 
 cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s) {
@@ -435,7 +556,24 @@ cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cud
 
 cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
                                                cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.stream.step, p, stream, true, node);
+    return add_step_node(g, deps, n_deps, p.stream.step, p, generate_step_for(p.stream.step.n_vocab, stream, true), node);
+}
+
+cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_t s) {
+    const GenStepParams & gp = p.gen.stream.step;
+    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    const dim3 grid(gp.n_rows);
+    if (per <= 1) return launch_pdl(generate_logprob_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 4) return launch_pdl(generate_logprob_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 16) return launch_pdl(generate_logprob_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 50) return launch_pdl(generate_logprob_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return launch_pdl(generate_logprob_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+}
+
+cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
+                                           cudaGraphNode_t * node) {
+    return add_step_node(g, deps, n_deps, p.gen.stream.step, p, generate_logprob_step_for(p.gen.stream.step.n_vocab, stream), node);
 }
 
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {

@@ -34,6 +34,11 @@ class ProfileResult(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200
                [(n, ctypes.c_uint32) for n in ("gemv_launches", "total_launches")]
 
 
+class Logprobs(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_logprobs
+    _fields_ = [("top_n", ctypes.c_size_t), ("logprobs", ctypes.POINTER(ctypes.c_float)), ("top_ids", ctypes.POINTER(ctypes.c_uint32)),
+                ("top_logprobs", ctypes.POINTER(ctypes.c_float)), ("sample_probs", ctypes.POINTER(ctypes.c_float))]
+
+
 class RWKVContext:
     def __init__(self, ptr: ctypes.c_void_p) -> None:
         self.ptr = ptr
@@ -203,6 +208,16 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_generate_constrained.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_constrained.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32]
         lib.rwkv_b200_test_generate_step_constrained.restype = ctypes.c_bool
+        P_LOGPROBS = ctypes.POINTER(Logprobs)
+        lib.rwkv_b200_generate_logprobs.argtypes = [vp, vp, P_U32, ctypes.c_size_t, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                                    ctypes.c_bool, P_DOUBLE, P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32,
+                                                    ctypes.POINTER(ctypes.c_size_t), P_LOGPROBS]
+        lib.rwkv_b200_generate_logprobs.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_generate_logprobs.argtypes = [vp, ctypes.POINTER(vp), P_U32, P_U32, P_FLOAT, P_FLOAT, P_FLOAT, P_FLOAT, P_U8, P_DOUBLE,
+                                                          P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, P_U32, P_LOGPROBS]
+        lib.rwkv_b200_batch_generate_logprobs.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step_logprobs.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS]
+        lib.rwkv_b200_test_generate_step_logprobs.restype = ctypes.c_bool
         lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
         lib.rwkv_b200_score.restype = ctypes.c_bool
         lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
