@@ -307,6 +307,48 @@ RWKV_API bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, con
                                                 rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
                                                 const struct rwkv_b200_logprobs * lp);
 
+/* Generation with a sampler per sequence: the knobs completion servers send on ordinary requests (top_k, min_p, logit_bias) inside the
+ * device-side loop, so that such a request does not take every token's logits to the host. The arguments, checks, context kinds,
+ * streaming, automata (NULL: unconstrained) and outputs are those of rwkv_b200_generate_logprobs / rwkv_b200_batch_generate_logprobs,
+ * except that temperature, top_p and the penalties come from the sampler (samplers[b] for sequence b) and lp may be NULL (no
+ * log-probabilities; nothing is allocated for them). One draw of a sequence in automaton state s with penalty counts c, logits z and
+ * user bias ub (ub[n] for the ids bias_ids lists):
+ * 1. Bias entry of token n: -inf if s does not allow n, whatever c[n] or ub[n]. Otherwise, with pen = presence + c[n] * frequency
+ *    (float32, multiply and add rounded separately): c[n] > 0 with a user entry: ub[n] - pen (one more rounding); c[n] > 0 without one:
+ *    -pen; c[n] = 0 with one: ub[n]; otherwise no entry. The biased logits are y = z + entry, as rwkv_b200_sample's bias list adds them.
+ * 2. Temperature 0: the first index of max(y); top_k and min_p have no effect.
+ * 3. p = softmax(y), the float32 values rwkv_b200_sample computes, and p_max = 1 / total its largest entry.
+ * 4. Token n is kept iff p[n] >= the top-p cutoff of rwkv_b200_sample, p[n] >= the top_k-th largest entry of p counted with
+ *    multiplicity (every tie at the k-th value is kept; top_k = 0 is off), and p[n] >= fl(min_p * p_max) (min_p = 0 is off). All three
+ *    come from the same p, so the kept set is their intersection, in any order; the largest probability is always kept.
+ * 5. Tempering relative to p_max, normalisation and the inverse-CDF draw with u are those of rwkv_b200_sample. lp->sample_probs is the
+ *    chosen token's probability after all of this; lp->logprobs and the top entries are those of the raw z.
+ * A column with a NaN or +inf draws as rwkv_b200_sample draws it. With top_k = 0, min_p = 0 and n_bias = 0 on every sequence, a call
+ * returns the bits of the matching rwkv_b200_generate / _stream / _constrained / _logprobs call (tokens, n_generated, state, logits,
+ * counts, automaton states, lp outputs). RWKV_ERROR_ARGS, changing nothing, for NULL sampler(s), top_k > n_vocab, min_p NaN or outside
+ * [0, 1], n_bias > RWKV_B200_LOGIT_BIAS_MAX or n_bias > 0 with NULL arrays, a duplicate id or an id >= n_vocab in one sampler, and a
+ * bias value that is NaN or +inf. The first call allocates the sampler upload (rows * RWKV_B200_LOGIT_BIAS_MAX * 8 bytes plus the rows,
+ * on the device and pinned); contexts that never call these allocate nothing for it. */
+#define RWKV_B200_LOGIT_BIAS_MAX 1024
+struct rwkv_b200_sampler {
+    float temperature, top_p;                  /* as rwkv_b200_sample */
+    uint32_t top_k;                            /* 0 = off; <= n_vocab */
+    float min_p;                               /* 0 = off; 0 .. 1 */
+    float presence_penalty, frequency_penalty; /* as rwkv_b200_generate */
+    size_t n_bias;                             /* 0 .. RWKV_B200_LOGIT_BIAS_MAX */
+    const uint32_t * bias_ids;                 /* host, n_bias distinct ids < n_vocab */
+    const float * bias_values;                 /* host, finite or -inf (a ban) */
+};
+RWKV_API bool rwkv_b200_generate_sampled(struct rwkv_context * ctx, const struct rwkv_b200_sampler * sampler, const struct rwkv_b200_automaton * automaton,
+                                         uint32_t * automaton_state, size_t max_tokens, bool keep_counts, const double * u, const uint32_t * stop_ids,
+                                         size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated,
+                                         const struct rwkv_b200_logprobs * lp /* NULL = none */);
+RWKV_API bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct rwkv_b200_sampler * samplers /* [n_sequences] */,
+                                               const struct rwkv_b200_automaton * const * automata, uint32_t * automaton_states,
+                                               const uint32_t * max_tokens, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids,
+                                               size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
+                                               const struct rwkv_b200_logprobs * lp /* NULL = none */);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each
@@ -335,6 +377,10 @@ RWKV_API bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_ge
  * lp ([n_rows][n], top arrays [n_rows][n][top_n]) are written at [b][step] for every row that draws; other entries keep what they held. */
 RWKV_API bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states,
                                                     uint32_t * states, const struct rwkv_b200_logprobs * lp);
+/* The same step of the sampled kernel. a->temperature, top_p, presence_penalty and frequency_penalty must be NULL; samplers[n_rows]
+ * supplies them. next may be NULL (unconstrained) and lp may be NULL, otherwise as for rwkv_b200_test_generate_step_logprobs. */
+RWKV_API bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers,
+                                                   const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

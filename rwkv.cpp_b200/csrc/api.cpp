@@ -567,17 +567,22 @@ static bool logprobs_arg(ErrorSink sink, const struct rwkv_b200_logprobs * lp, L
     return true;
 }
 
+// The engine's part of a public sampler (temperature, top_p and the penalties travel in GenRow).
+static SamplerIn sampler_in(const struct rwkv_b200_sampler & s) { return SamplerIn{s.top_k, s.min_p, s.n_bias, s.bias_ids, s.bias_values}; }
+
 // The single-sequence generate calls; on_token NULL is the blocking loop. `constrained`: the row follows *automaton from
-// *automaton_state (both checked here, the rest by generate).
+// *automaton_state (both checked here, the rest by generate). `sampled`: *sampler (checked here) replaces temperature, top_p and the
+// penalties, and lp may be NULL.
 static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
                             bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated,
                             bool streaming, TokenFn on_token, void * user, bool constrained = false, const Automaton * automaton = nullptr,
-                            uint32_t * automaton_state = nullptr, bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr) {
+                            uint32_t * automaton_state = nullptr, bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr,
+                            bool sampled = false, const struct rwkv_b200_sampler * sampler = nullptr) {
     if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
-    const char * suffix = logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "";
+    const char * suffix = sampled ? "_sampled" : logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "";
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s", suffix);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
                "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
@@ -585,33 +590,54 @@ static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float 
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automaton && automaton_state), "NULL automaton or automaton_state");
     LogprobsOut out{};
     if (logprobs && !logprobs_arg(c->sink(), lp, out)) return false;
+    SamplerIn smp{};
+    if (sampled) {
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, sampler, "NULL sampler");
+        temperature = sampler->temperature; top_p = sampler->top_p;
+        presence_penalty = sampler->presence_penalty; frequency_penalty = sampler->frequency_penalty;
+        smp = sampler_in(*sampler);
+    }
     const uint32_t budget = (uint32_t) max_tokens;
     const uint8_t keep = keep_counts ? 1 : 0;
     uint32_t n = 0;
     const bool ok = generate(c, &budget, &temperature, &top_p, &presence_penalty, &frequency_penalty, &keep, u, stop_ids, n_stop, tokens_out, &n, on_token, user,
-                             constrained ? &automaton : nullptr, automaton_state, logprobs ? &out : nullptr);
+                             constrained ? &automaton : nullptr, automaton_state, logprobs ? &out : nullptr, sampled ? &smp : nullptr);
     if (ok || n) *n_generated = n;      // a callback that kept the device waiting too long still gets what was delivered
     return ok;
 }
 
-// The batch generate calls; on_token NULL is the blocking loop.
+// The batch generate calls; on_token NULL is the blocking loop. `sampled`: samplers[n_sequences] (checked here) replace the
+// temperature, top_p and penalty arrays.
 static bool generate_batch(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                            const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
                            const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user,
                            bool constrained = false, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr,
-                           bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr) {
+                           bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr, bool sampled = false,
+                           const struct rwkv_b200_sampler * samplers = nullptr) {
     if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s",
-               logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "");
+               sampled ? "_sampled" : logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automata && automaton_states), "NULL automata or automaton_states");
     LogprobsOut out{};
     if (logprobs && !logprobs_arg(c->sink(), lp, out)) return false;
-    return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user,
-                    automata, automaton_states, logprobs ? &out : nullptr);
+    if (!sampled)
+        return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
+                        on_token, user, automata, automaton_states, logprobs ? &out : nullptr);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
+    const size_t rows = (size_t) c->batch_n;
+    std::vector<float> t(rows), p(rows), pres(rows), freq(rows);
+    std::vector<SamplerIn> smp(rows);
+    for (size_t b = 0; b < rows; b++) {
+        t[b] = samplers[b].temperature; p[b] = samplers[b].top_p;
+        pres[b] = samplers[b].presence_penalty; freq[b] = samplers[b].frequency_penalty;
+        smp[b] = sampler_in(samplers[b]);
+    }
+    return generate(c, max_tokens, t.data(), p.data(), pres.data(), freq.data(), keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token, user,
+                    automata, automaton_states, logprobs ? &out : nullptr, smp.data());
 }
 
 bool rwkv_b200_generate(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
@@ -696,13 +722,31 @@ bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, const struct
                           true, lp);
 }
 
+bool rwkv_b200_generate_sampled(struct rwkv_context * ctx, const struct rwkv_b200_sampler * sampler, const struct rwkv_b200_automaton * automaton,
+                                uint32_t * automaton_state, size_t max_tokens, bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
+                                rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated, const struct rwkv_b200_logprobs * lp) {
+    return generate_single(ctx, max_tokens, 0.0f, 0.0f, 0.0f, 0.0f, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token != nullptr, on_token, user,
+                           automaton != nullptr, automaton, automaton_state, lp != nullptr, lp, true, sampler);
+}
+
+bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct rwkv_b200_sampler * samplers, const struct rwkv_b200_automaton * const * automata,
+                                      uint32_t * automaton_states, const uint32_t * max_tokens, const uint8_t * keep_counts, const double * u,
+                                      const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
+                                      uint32_t * n_generated, const struct rwkv_b200_logprobs * lp) {
+    return generate_batch(batch, max_tokens, nullptr, nullptr, nullptr, nullptr, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token != nullptr,
+                          on_token, user, automata != nullptr, reinterpret_cast<const Automaton * const *>(automata), automaton_states, lp != nullptr, lp,
+                          true, samplers);
+}
+
 static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");
 static_assert(RWKV_B200_TOP_LOGPROBS_MAX == GEN_TOP_MAX, "top log-probabilities of the header and the kernel");
+static_assert(RWKV_B200_LOGIT_BIAS_MAX == GEN_BIAS_MAX, "user bias entries of the header and the kernel");
 
 // One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
-// the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained).
+// the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained); with
+// samplers the sampled kernel (next and lp may then be NULL).
 static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
-                               const LogprobsOut * lp = nullptr) {
+                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
@@ -717,6 +761,7 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     }
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, n >= 1, "Every row has max_tokens 0");
     if (lp && !check_logprobs(sink, V, lp)) return false;
+    if (samplers && !check_samplers(sink, R, V, samplers)) return false;
     const bool constrained = next != nullptr;
     std::vector<uint8_t> live;
     if (constrained) {
@@ -764,12 +809,12 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     GenLogprobParams lpp{};
     GenLogprobRequest req{};
     const size_t cells = R * n, k = lp ? lp->top_n : 0;
-    if (lp) {       // every row unconstrained without a table; the outputs start as the caller's arrays
-        if (!constrained) {
-            const std::vector<GenMaskRow> none(R, GenMaskRow{nullptr, nullptr, 0, 0});
-            cp.mask = const_cast<GenMaskRow *>(hb.in(none.data(), R));
-            cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
-        }
+    if (!constrained && (lp || samplers)) {     // every row unconstrained without a table
+        const std::vector<GenMaskRow> none(R, GenMaskRow{nullptr, nullptr, 0, 0});
+        cp.mask = const_cast<GenMaskRow *>(hb.in(none.data(), R));
+        cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
+    }
+    if (lp) {       // the outputs start as the caller's arrays
         req.top_n = (uint32_t) k;
         req.logprobs = const_cast<float *>(hb.in(lp->logprobs, cells));
         req.sample_probs = lp->sample_probs ? const_cast<float *>(hb.in(lp->sample_probs, cells)) : static_cast<float *>(hb.alloc(cells * sizeof(float)));
@@ -778,7 +823,23 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         lpp.gen = cp;
         lpp.req = hb.in(&req, 1);
     }
-    const cudaError_t e = !hb.ok ? cudaSuccess : lp ? launch_generate_logprob_step(lpp, 0) : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
+    GenSamplerParams smp{};
+    if (samplers) {
+        std::vector<GenSamplerRow> srows(R);
+        std::vector<GenBiasEntry> pool;
+        for (size_t b = 0; b < R; b++) {
+            const SamplerIn & s = samplers[b];
+            srows[b] = GenSamplerRow{s.top_k, s.min_p, (uint32_t) pool.size(), (uint32_t) (pool.size() + s.n_bias)};
+            for (size_t k = 0; k < s.n_bias; k++) pool.push_back(GenBiasEntry{s.bias_ids[k], s.bias_values[k]});
+        }
+        const GenLogprobRequest * word = lp ? lpp.req : nullptr;
+        smp.gen = cp;
+        smp.req = hb.in(&word, 1);
+        smp.rows = hb.in(srows.data(), R);
+        smp.bias = pool.empty() ? nullptr : hb.in(pool.data(), pool.size());
+    }
+    const cudaError_t e = !hb.ok ? cudaSuccess : samplers ? launch_generate_sampled_step(smp, 0) : lp ? launch_generate_logprob_step(lpp, 0)
+                        : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
@@ -810,6 +871,29 @@ bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_
     LogprobsOut out{};
     if (!logprobs_arg(sink, lp, out)) return false;
     return generate_step_hook(a, next, n_states, states, &out);
+}
+
+bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
+                                          size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS, "Invalid generate-step arguments");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !a->temperature && !a->top_p && !a->presence_penalty && !a->frequency_penalty,
+               "temperature, top_p and the penalties come from the samplers: pass NULL");
+    LogprobsOut out{};
+    if (lp && !logprobs_arg(sink, lp, out)) return false;
+    const size_t R = a->n_rows;
+    std::vector<float> t(R), p(R), pres(R), freq(R);
+    std::vector<SamplerIn> smp(R);
+    for (size_t b = 0; b < R; b++) {
+        t[b] = samplers[b].temperature; p[b] = samplers[b].top_p;
+        pres[b] = samplers[b].presence_penalty; freq[b] = samplers[b].frequency_penalty;
+        smp[b] = sampler_in(samplers[b]);
+    }
+    struct rwkv_b200_generate_step_args args = *a;
+    args.temperature = t.data(); args.top_p = p.data(); args.presence_penalty = pres.data(); args.frequency_penalty = freq.data();
+    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data());
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

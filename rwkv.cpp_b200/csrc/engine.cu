@@ -775,6 +775,8 @@ void destroy_context(Context * ctx) {
     if (ctx->lp_req_host) cudaFreeHost(ctx->lp_req_host);
     if (ctx->lp_host) cudaFreeHost(ctx->lp_host);
     if (ctx->lp_ring_host) cudaFreeHost(ctx->lp_ring_host);
+    cudaFree(ctx->smp_dev);
+    if (ctx->smp_host) cudaFreeHost(ctx->smp_host);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
     if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
@@ -1384,6 +1386,8 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // A loop that reports log-probabilities runs the logprob step kernels instead, in graphs of their own (gen_lp_graphs); they read the
 // call's GenLogprobRequest from ctx->lp_req, and the streaming one writes each token's record into the mapped ring before it publishes
 // the token, so that stream_tokens can hand the record to the caller before on_token.
+// A loop with per-row samplers runs the sampled step kernels, in graphs of their own too (gen_smp_graphs); they read the rows, the bias
+// pool and the request word (ctx->lp_req, or NULL without log-probabilities) from ctx->smp_dev.
 namespace {
 
 size_t gen_mask_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
@@ -1434,7 +1438,10 @@ GenStreamParams generate_stream_params(Context * ctx) {
     return sp;
 }
 
-bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool logprobs) {
+size_t smp_rows_offset() { return sizeof(const GenLogprobRequest *); }
+size_t smp_bias_offset(int rows) { return smp_rows_offset() + (size_t) rows * sizeof(GenSamplerRow); }
+
+bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool logprobs, bool sampled) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     Pass p;
     if (!make_pass(ctx, rows, true, nullptr, p)) return false;
@@ -1465,7 +1472,11 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
         const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen_in + gen_mask_offset(rows)), ctx->gen_out + rows + 1};
-        CUDA_OK(ctx, logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req}, streaming, &step)
+        const GenSamplerParams smp{cp, reinterpret_cast<const GenLogprobRequest * const *>(ctx->smp_dev),
+                                   reinterpret_cast<const GenSamplerRow *>(ctx->smp_dev + smp_rows_offset()),
+                                   reinterpret_cast<const GenBiasEntry *>(ctx->smp_dev + smp_bias_offset(rows))};
+        CUDA_OK(ctx, sampled ? add_generate_sampled_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, smp, streaming, &step)
+                     : logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req}, streaming, &step)
                      : constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
                      : streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
                                  : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
@@ -1477,7 +1488,8 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
         std::swap(p.state_in, p.state_out);      // the second pass reads what the first one wrote
         prev = cond;
     }
-    CUDA_OK(ctx, cudaGraphInstantiate(logprobs ? &ctx->gen_lp_graphs[ctx->phase][streaming] : &ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
+    CUDA_OK(ctx, cudaGraphInstantiate(sampled ? &ctx->gen_smp_graphs[ctx->phase][streaming]
+                                      : logprobs ? &ctx->gen_lp_graphs[ctx->phase][streaming] : &ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
     return true;
 }
 
@@ -1528,6 +1540,15 @@ bool ensure_logprob_buffers(Context * ctx, size_t words, bool streaming) {
             CUDA_OK(ctx, cudaHostAlloc(reinterpret_cast<void **>(&ctx->lp_ring_host), (size_t) rows * 2 * GEN_LP_RECORD * sizeof(uint32_t), cudaHostAllocMapped));
         CUDA_OK(ctx, cudaHostGetDevicePointer(reinterpret_cast<void **>(&ctx->lp_ring_dev), ctx->lp_ring_host, 0));
     }
+    return true;
+}
+
+// The sampler upload at its largest (GEN_BIAS_MAX entries per row), on the device and pinned.
+bool ensure_sampler_buffers(Context * ctx) {
+    if (ctx->smp_dev) return true;
+    const size_t bytes = smp_bias_offset(ctx->batch_n ? ctx->batch_n : 1) + (size_t) (ctx->batch_n ? ctx->batch_n : 1) * GEN_BIAS_MAX * sizeof(GenBiasEntry);
+    if (!ctx->smp_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->smp_host), bytes));
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->smp_dev), bytes));
     return true;
 }
 
@@ -1583,6 +1604,8 @@ void drop_generate_graphs(Context * ctx) {
             for (auto & e : by_streaming) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
     for (auto & by_phase : ctx->gen_lp_graphs)
         for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+    for (auto & by_phase : ctx->gen_smp_graphs)
+        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
 }
 
 bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp) {
@@ -1590,6 +1613,27 @@ bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp) {
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp->top_n <= (size_t) GEN_TOP_MAX && lp->top_n <= n_vocab, "top_n (%zu) must be at most %d and n_vocab",
                lp->top_n, GEN_TOP_MAX);
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, lp->top_n == 0 || (lp->top_ids && lp->top_logprobs), "NULL top_ids or top_logprobs with top_n > 0");
+    return true;
+}
+
+bool check_samplers(ErrorSink sink, size_t n_rows, size_t n_vocab, const SamplerIn * samplers) {
+    std::vector<uint32_t> seen;       // seen[id] = 1 + the last row that listed id
+    for (size_t b = 0; b < n_rows; b++) {
+        const SamplerIn & s = samplers[b];
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, s.top_k <= n_vocab, "top_k of row %zu (%u) is above n_vocab", b, s.top_k);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, s.min_p >= 0.0f && s.min_p <= 1.0f, "min_p of row %zu must be in [0, 1]", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, s.n_bias <= (size_t) GEN_BIAS_MAX && (s.n_bias == 0 || (s.bias_ids && s.bias_values)),
+                   "Row %zu: at most %d bias entries, with ids and values not NULL", b, GEN_BIAS_MAX);
+        if (s.n_bias && seen.empty()) seen.assign(n_vocab, 0);
+        for (size_t k = 0; k < s.n_bias; k++) {
+            const uint32_t id = s.bias_ids[k];
+            const float v = s.bias_values[k];
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, id < n_vocab, "Bias id %u of row %zu is out of range", id, b);
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, seen[id] != b + 1, "Bias id %u of row %zu is listed twice", id, b);
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !std::isnan(v) && v != INFINITY, "Bias value of id %u of row %zu must be finite or -inf", id, b);
+            seen[id] = (uint32_t) b + 1;
+        }
+    }
     return true;
 }
 
@@ -1674,7 +1718,7 @@ bool check_generate_rows(ErrorSink sink, size_t n_rows, size_t n_vocab, const ui
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
               uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token, void * user, const Automaton * const * automata,
-              uint32_t * automaton_states, const LogprobsOut * lp) {
+              uint32_t * automaton_states, const LogprobsOut * lp, const SamplerIn * samplers) {
     const Model & m = *ctx->model;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     const size_t V = (size_t) m.n_vocab;
@@ -1693,6 +1737,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
         }
     }
     if (lp && !check_logprobs(ctx->sink(), V, lp)) return false;
+    if (samplers && !check_samplers(ctx->sink(), rows, V, samplers)) return false;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, V <= 65536, "On-device sampling supports n_vocab <= 65536");
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last evaluation skipped the head");
     int driver = 0;
@@ -1705,6 +1750,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     if (!ensure_generate_buffers(ctx) || (streaming && !ensure_stream_buffers(ctx)) || !ensure_capacity(ctx, rows, ctx->stream)) return false;
     const size_t lp_cells = (size_t) rows * n, lp_words = lp ? lp_cells * (2 + 2 * lp->top_n) : 0;
     if (lp && !ensure_logprob_buffers(ctx, lp_words, streaming)) return false;
+    if (samplers && !ensure_sampler_buffers(ctx)) return false;
     // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
     GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
     memset(sh, 0, sizeof(GenShared));
@@ -1734,8 +1780,21 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
                                               streaming ? ctx->lp_ring_dev : nullptr};
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_req, ctx->lp_req_host, sizeof(GenLogprobRequest), cudaMemcpyHostToDevice, ctx->stream));
     }
-    cudaGraphExec_t & graph = lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
-    if (!graph && !build_generate_graph(ctx, streaming, constrained, lp != nullptr)) return false;
+    if (samplers) {     // the request word, the rows and the bias pool in one upload
+        *reinterpret_cast<const GenLogprobRequest **>(ctx->smp_host) = lp ? ctx->lp_req : nullptr;
+        GenSamplerRow * sr = reinterpret_cast<GenSamplerRow *>(ctx->smp_host + smp_rows_offset());
+        GenBiasEntry * pool = reinterpret_cast<GenBiasEntry *>(ctx->smp_host + smp_bias_offset(rows));
+        uint32_t used = 0;
+        for (int b = 0; b < rows; b++) {
+            const SamplerIn & s = samplers[b];
+            sr[b] = GenSamplerRow{s.top_k, s.min_p, used, used + (uint32_t) s.n_bias};
+            for (size_t k = 0; k < s.n_bias; k++) pool[used++] = GenBiasEntry{s.bias_ids[k], s.bias_values[k]};
+        }
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->smp_dev, ctx->smp_host, smp_bias_offset(rows) + used * sizeof(GenBiasEntry), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    cudaGraphExec_t & graph = samplers ? ctx->gen_smp_graphs[ctx->phase][streaming]
+                            : lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
+    if (!graph && !build_generate_graph(ctx, streaming, constrained, lp != nullptr, samplers != nullptr)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));

@@ -144,6 +144,11 @@ struct Context {
     size_t lp_words = 0;
     uint32_t * lp_ring_host = nullptr, * lp_ring_dev = nullptr;
     cudaGraphExec_t gen_lp_graphs[2][2] = {};    // the logprob loops' graphs, keyed by phase and streaming
+    // Per-row samplers (generate with SamplerIn rows), allocated only by calls that use them: the call's upload at a device address
+    // the sampled graphs capture (pinned copy smp_host): the log-probability request word (lp_req or NULL), GenSamplerRow[rows], then
+    // room for rows * GEN_BIAS_MAX GenBiasEntry.
+    unsigned char * smp_dev = nullptr, * smp_host = nullptr;
+    cudaGraphExec_t gen_smp_graphs[2][2] = {};   // the sampled loops' graphs, keyed by phase and streaming
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -263,10 +268,22 @@ struct LogprobsOut {
     float * sample_probs;             // may be NULL
 };
 bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp);
+// With samplers (rwkv_b200_generate_sampled), samplers[b] adds row b's top_k, min_p and user bias entries to its draws, and lp may be
+// NULL; the loop runs the sampled kernels, which also take automata == NULL as "no row constrained". check_samplers checks the rows
+// (also for the test hook).
+struct SamplerIn {
+    uint32_t top_k;                   // 0 = off
+    float min_p;                      // 0 = off
+    size_t n_bias;
+    const uint32_t * bias_ids;
+    const float * bias_values;
+};
+bool check_samplers(ErrorSink sink, size_t n_rows, size_t n_vocab, const SamplerIn * samplers);
 bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperature, const float * top_p, const float * presence,
               const float * frequency, const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
               uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr,
-              const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr, const LogprobsOut * lp = nullptr);
+              const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr, const LogprobsOut * lp = nullptr,
+              const SamplerIn * samplers = nullptr);
 
 // A token automaton of rwkv_b200_automaton_create: the transition table next[s * n_vocab + t] (GEN_MASK_DEAD: t not allowed in s)
 // and live[s] (s allows some token) in the HBM of the model's device. It serves every context of that model.

@@ -300,6 +300,32 @@ struct GenLogprobParams {
 cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_t s);     // the blocking kernel
 cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
                                            cudaGraphNode_t * node);
+// Generation with a per-row sampler (rwkv_b200_generate_sampled / rwkv_b200_batch_generate_sampled): the constrained steps (a row with
+// a NULL table is unconstrained), with log-probabilities when *req is not NULL, where row b also has
+// - user bias entries bias[bias_begin, bias_end) (distinct ids): after the penalty / mask list is written, an id its state allows
+//   gets the entry value - (presence + count * frequency) if counted, else value;
+// - top_k (0 = off) and min_p (0 = off): a token is kept iff its probability is at least the top-p cutoff, the top_k-th largest
+//   probability (with multiplicity) and min_p * the largest probability (sample_row's KeepFilter).
+// The rows, the pool and the request word live in the per-call upload, so that one graph serves every sampler.
+constexpr int GEN_BIAS_MAX = 1024;    // user bias entries per row
+struct GenSamplerRow {                // written by the host per call
+    uint32_t top_k;
+    float min_p;
+    uint32_t bias_begin, bias_end;
+};
+struct GenBiasEntry {
+    uint32_t id;
+    float value;
+};
+struct GenSamplerParams {
+    GenConstrainedParams gen;
+    const GenLogprobRequest * const * req;    // device word: the call's log-probability request, or NULL for none
+    const GenSamplerRow * rows;               // [n_rows] device
+    const GenBiasEntry * bias;                // device, the rows' entries
+};
+cudaError_t launch_generate_sampled_step(const GenSamplerParams & p, cudaStream_t s);     // the blocking kernel
+cudaError_t add_generate_sampled_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenSamplerParams & p, bool stream,
+                                           cudaGraphNode_t * node);
 // After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);

@@ -45,10 +45,53 @@ __device__ float block_max_f(float v, float * slots) {
     return r;
 }
 
+__device__ int block_count(int v, int * slots) {                 // every thread gets the total
+    v = __reduce_add_sync(0xffffffffu, v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) slots[threadIdx.x >> 5] = v;
+    __syncthreads();
+    return __reduce_add_sync(0xffffffffu, slots[threadIdx.x & 31]);
+}
+
+// sample_row's filter of the kept set beside top-p: none.
+struct NoFilter {
+    static constexpr bool active = false;
+};
+
+// Keeps token n iff p[n] >= the top_k-th largest probability, counted with multiplicity (top_k = 0: off), and p[n] >= min_p * p_max.
+// Both come from the softmax v that also gives the top-p cutoff, so the kept set is the intersection of the three, whatever the order.
+struct KeepFilter {
+    static constexpr bool active = true;
+    uint32_t top_k;
+    float min_p;
+    // The smallest probability this filter keeps. The top_k-th largest value of v is the largest bit pattern t (non-negative floats
+    // order as their bits) with at least top_k entries >= t: a bisection over [0, bits(p_max)] with integer block counts. The pad
+    // entries past n_vocab are 0 <= every probability, so they never move it while top_k <= n_vocab. NaN probabilities (a column
+    // with a NaN or +inf) compare false everywhere, so whatever comes out keeps them as sample_row without a filter does.
+    template <int PER>
+    __device__ __forceinline__ float threshold(const float (&v)[PER], float p_max, int V) const {
+        __shared__ int islots[SAMPLE_WARPS];
+        float kth = 0.f;
+        if (top_k > 0 && top_k < (uint32_t) V) {
+            uint32_t lo = 0u, hi = __float_as_uint(p_max) + 1u;       // count(>= lo) >= top_k > count(>= hi)
+            while (hi - lo > 1u) {
+                const uint32_t mid = lo + (hi - lo) / 2u;
+                const float t = __uint_as_float(mid);
+                int c = 0;
+#pragma unroll
+                for (int j = 0; j < PER; j++) c += (v[j] >= t) ? 1 : 0;
+                if (block_count(c, islots) >= (int) top_k) lo = mid; else hi = mid;
+            }
+            kth = __uint_as_float(lo);
+        }
+        return fmaxf(kth, __fmul_rn(min_p, p_max));
+    }
+};
+
 // The whole draw for one row of logits, shared by the single-row and the batched kernel so that a row of a batch gives the bits of
-// a single launch. `p` is that row's view: its logits, parameters, bias, scratch and result words.
-template <int PER>
-__device__ __forceinline__ void sample_row(const SampleParams & p) {
+// a single launch. `p` is that row's view: its logits, parameters, bias, scratch and result words; `filter` narrows the kept set.
+template <int PER, class Filter = NoFilter>
+__device__ __forceinline__ void sample_row(const SampleParams & p, const Filter filter = Filter{}) {
     __shared__ double dslots[SAMPLE_WARPS];
     __shared__ float fslots[SAMPLE_WARPS];
     __shared__ int first_flagged, last_massive;
@@ -87,8 +130,17 @@ __device__ __forceinline__ void sample_row(const SampleParams & p) {
     const float total = (float) block_sum_dd(s, dslots);
 #pragma unroll
     for (int j = 0; j < PER; j++) v[j] = __fdiv_rn(v[j], total);
+    // the filter's threshold, from the same probabilities as the top-p cutoff below (p_max = 1 / total, as for the tempering)
+    float keep = 0.f;
+    if constexpr (Filter::active) keep = filter.template threshold<PER>(v, __fdiv_rn(1.0f, total), V);
     // top-p (:42-45)
     const float top_p = (p.top_p == 0.0f) ? 1.0f : p.top_p;
+    if constexpr (Filter::active) {
+        if (!(top_p < 1.0f) && keep > 0.f) {
+#pragma unroll
+            for (int j = 0; j < PER; j++) if (v[j] < keep) v[j] = 0.f;
+        }
+    }
     if (top_p < 1.0f) {
         auto mass_at_least = [&](float thr) {
             double m = 0;
@@ -110,6 +162,7 @@ __device__ __forceinline__ void sample_row(const SampleParams & p) {
             }
             cutoff = __uint_as_float(lo);
         }
+        if constexpr (Filter::active) cutoff = fmaxf(cutoff, keep);
 #pragma unroll
         for (int j = 0; j < PER; j++) if (v[j] < cutoff) v[j] = 0.f;
     }
@@ -359,10 +412,49 @@ struct Logprobs {
     }
 };
 
+// The sampled loops' log-probabilities: the Logprobs policy when the call asked for them (req not NULL), nothing otherwise.
+template <int PER>
+struct RequestedLogprobs {
+    const GenLogprobRequest * req;
+    bool ring;
+    __device__ __forceinline__ float * prob_slot(size_t at) const { return req ? req->sample_probs + at : nullptr; }
+    __device__ __forceinline__ void record(int b, size_t at, uint32_t step, const float * z, int V, uint32_t tok) const {
+        if (req) Logprobs<PER>{req, ring}.record(b, at, step, z, V, tok);
+    }
+};
+
+// The loops without a sampler: no user bias, no filter.
+struct NoSampler {
+    __device__ __forceinline__ void add_bias(int, int, const uint32_t *, const uint16_t *, float, float, uint32_t *, float *) const {}
+    __device__ __forceinline__ NoFilter filter(int) const { return NoFilter{}; }
+};
+
+// The per-row samplers of GenSamplerParams (ops.h).
+struct RowSampler {
+    const GenSamplerRow * rows;
+    const GenBiasEntry * bias;
+    // Every thread, once row b's penalty / mask list (ids, values, one entry per token) is written: the row's user entries over their
+    // ids. A token the state does not allow keeps its -inf; a counted one gets value - (presence + count * frequency), rounded as the
+    // penalty alone is and then once more; any other gets value.
+    __device__ __forceinline__ void add_bias(int b, int V, const uint32_t * counts, const uint16_t * allowed, float presence, float frequency,
+                                             uint32_t * ids, float * values) const {
+        const GenSamplerRow r = rows[b];
+        for (uint32_t k = r.bias_begin + threadIdx.x; k < r.bias_end; k += SAMPLE_THREADS) {
+            const GenBiasEntry e = bias[k];
+            if (e.id >= (uint32_t) V || (allowed && allowed[e.id] == GEN_MASK_DEAD)) continue;
+            const uint32_t c = counts[e.id];
+            ids[e.id] = e.id;
+            values[e.id] = c ? __fsub_rn(e.value, __fadd_rn(presence, __fmul_rn((float) c, frequency))) : e.value;
+        }
+        __syncthreads();
+    }
+    __device__ __forceinline__ KeepFilter filter(int b) const { return KeepFilter{rows[b].top_k, rows[b].min_p}; }
+};
+
 // One step of the generation loop for row blockIdx.x (ops.h: GenStepParams), gated by `gate`, its draws restricted by `mask`, every
-// draw reported by `lp`.
-template <int PER, class Gate, class Mask, class Lp = NoLogprobs>
-__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate, const Mask mask, const Lp lp = Lp{}) {
+// draw reported by `lp`, its bias list and kept set extended by `smp`.
+template <int PER, class Gate, class Mask, class Lp = NoLogprobs, class Smp = NoSampler>
+__device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate gate, const Mask mask, const Lp lp = Lp{}, const Smp smp = Smp{}) {
     __shared__ int draw, park;
     const int b = blockIdx.x, tid = threadIdx.x, V = gp.n_vocab;
     const size_t off = (size_t) b * V;
@@ -390,13 +482,14 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
             gp.bias_values[off + i] = dead ? -INFINITY : -__fadd_rn(presence, __fmul_rn((float) c, frequency));
         }
         __syncthreads();
+        smp.add_bias(b, V, gp.counts + off, allowed, presence, frequency, gp.bias_ids + off, gp.bias_values + off);
         SampleParams p;
         p.logits = gp.logits + off; p.n_vocab = V;
         p.temperature = r->temperature; p.top_p = r->top_p; p.u = gp.u[(size_t) b * sh->stride + step];
         p.bias_ids = gp.bias_ids + off; p.bias_values = gp.bias_values + off; p.n_bias = V;
         p.scratch = gp.scratch + off; p.token_out = gp.tokens + (size_t) b * sh->stride + step;
         p.prob_out = lp.prob_slot((size_t) b * sh->stride + step);
-        sample_row<PER>(p);
+        sample_row<PER>(p, smp.filter(b));
         __syncthreads();
         if (tid == 0) {
             tok = *(volatile uint32_t *) p.token_out;
@@ -477,6 +570,23 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_logprob_sam
                        Logprobs<PER>{lp.req, true});
 }
 
+// The constrained steps with a per-row sampler (GenSamplerParams) and, when the call's request word is set, log-probabilities; a row
+// with a NULL table is unconstrained, so these two serve every sampled call.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_sampled_sample_kernel(const GenSamplerParams sp) {
+    pdl_prologue();
+    generate_step<PER>(sp.gen.stream.step, NoGate{}, TableMask{sp.gen.mask, sp.gen.states_out}, RequestedLogprobs<PER>{*sp.req, false},
+                       RowSampler{sp.rows, sp.bias});
+}
+
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sampled_sample_kernel(const GenSamplerParams sp) {
+    pdl_prologue();
+    const GenStreamParams & st = sp.gen.stream;
+    generate_step<PER>(st.step, StreamGate{st.tokens, st.published, st.acked, st.timed_out}, TableMask{sp.gen.mask, sp.gen.states_out},
+                       RequestedLogprobs<PER>{*sp.req, true}, RowSampler{sp.rows, sp.bias});
+}
+
 constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
 
 __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const GenRow * rows, const float * src, float * dst, long long seq_stride, size_t n) {
@@ -505,6 +615,15 @@ void * generate_logprob_step_for(int n_vocab, bool stream) {
     const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
     return per <= 1 ? generate_logprob_step_fn<1>(stream) : per <= 4 ? generate_logprob_step_fn<4>(stream) : per <= 16 ? generate_logprob_step_fn<16>(stream)
          : per <= 50 ? generate_logprob_step_fn<50>(stream) : generate_logprob_step_fn<64>(stream);
+}
+
+template <int PER> void * generate_sampled_step_fn(bool stream) {
+    return stream ? reinterpret_cast<void *>(generate_stream_sampled_sample_kernel<PER>) : reinterpret_cast<void *>(generate_sampled_sample_kernel<PER>);
+}
+void * generate_sampled_step_for(int n_vocab, bool stream) {
+    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    return per <= 1 ? generate_sampled_step_fn<1>(stream) : per <= 4 ? generate_sampled_step_fn<4>(stream) : per <= 16 ? generate_sampled_step_fn<16>(stream)
+         : per <= 50 ? generate_sampled_step_fn<50>(stream) : generate_sampled_step_fn<64>(stream);
 }
 
 // A node of graph g after deps running step kernel `func` with the single kernel parameter `arg`.
@@ -574,6 +693,23 @@ cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_
 cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
                                            cudaGraphNode_t * node) {
     return add_step_node(g, deps, n_deps, p.gen.stream.step, p, generate_logprob_step_for(p.gen.stream.step.n_vocab, stream), node);
+}
+
+cudaError_t launch_generate_sampled_step(const GenSamplerParams & p, cudaStream_t s) {
+    const GenStepParams & gp = p.gen.stream.step;
+    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
+    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    const dim3 grid(gp.n_rows);
+    if (per <= 1) return launch_pdl(generate_sampled_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 4) return launch_pdl(generate_sampled_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 16) return launch_pdl(generate_sampled_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    if (per <= 50) return launch_pdl(generate_sampled_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return launch_pdl(generate_sampled_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+}
+
+cudaError_t add_generate_sampled_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenSamplerParams & p, bool stream,
+                                           cudaGraphNode_t * node) {
+    return add_step_node(g, deps, n_deps, p.gen.stream.step, p, generate_sampled_step_for(p.gen.stream.step.n_vocab, stream), node);
 }
 
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {

@@ -39,6 +39,12 @@ class Logprobs(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_logp
                 ("top_logprobs", ctypes.POINTER(ctypes.c_float)), ("sample_probs", ctypes.POINTER(ctypes.c_float))]
 
 
+class Sampler(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_sampler
+    _fields_ = [("temperature", ctypes.c_float), ("top_p", ctypes.c_float), ("top_k", ctypes.c_uint32), ("min_p", ctypes.c_float),
+                ("presence_penalty", ctypes.c_float), ("frequency_penalty", ctypes.c_float), ("n_bias", ctypes.c_size_t),
+                ("bias_ids", ctypes.POINTER(ctypes.c_uint32)), ("bias_values", ctypes.POINTER(ctypes.c_float))]
+
+
 class RWKVContext:
     def __init__(self, ptr: ctypes.c_void_p) -> None:
         self.ptr = ptr
@@ -218,6 +224,15 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_generate_logprobs.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_logprobs.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS]
         lib.rwkv_b200_test_generate_step_logprobs.restype = ctypes.c_bool
+        P_SAMPLER = ctypes.POINTER(Sampler)
+        lib.rwkv_b200_generate_sampled.argtypes = [vp, P_SAMPLER, vp, P_U32, ctypes.c_size_t, ctypes.c_bool, P_DOUBLE, P_U32, ctypes.c_size_t,
+                                                   RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, ctypes.POINTER(ctypes.c_size_t), P_LOGPROBS]
+        lib.rwkv_b200_generate_sampled.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_generate_sampled.argtypes = [vp, P_SAMPLER, ctypes.POINTER(vp), P_U32, P_U32, P_U8, P_DOUBLE, P_U32, ctypes.c_size_t,
+                                                         RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, P_U32, P_LOGPROBS]
+        lib.rwkv_b200_batch_generate_sampled.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step_sampled.argtypes = [ctypes.c_void_p, P_SAMPLER, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS]
+        lib.rwkv_b200_test_generate_step_sampled.restype = ctypes.c_bool
         lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
         lib.rwkv_b200_score.restype = ctypes.c_bool
         lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
