@@ -381,6 +381,26 @@ RWKV_API bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_gener
  * supplies them. next may be NULL (unconstrained) and lp may be NULL, otherwise as for rwkv_b200_test_generate_step_logprobs. */
 RWKV_API bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers,
                                                    const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp);
+/* The same step of a streaming kernel, the one the *_stream calls and the streaming generate calls run: `family` picks the twin of
+ * rwkv_b200_test_generate_step (PLAIN: samplers, next and lp NULL), _constrained (CONSTRAINED: next needed, lp NULL), _logprobs
+ * (LOGPROBS: lp needed) or _sampled (SAMPLED: samplers needed, a's temperature / top_p / penalty arrays NULL), with the arguments and
+ * outputs of that hook. It runs as the one node of a graph over pinned mapped copies of the streaming words, which are freed on return:
+ *   acked[n_rows]             in: 2 * tokens acknowledged + stop request, as the streaming loop's host thread writes it;
+ *   published[n_rows]         in / out: step + 1 for every row that drew;
+ *   stream_tokens             in / out, [n_rows][RWKV_B200_GENERATE_MAX]: the token a row drew at [b][step];
+ *   ring                      in / out, [n_rows][2][2 + 2 * RWKV_B200_TOP_LOGPROBS_MAX] words, needed with lp, else NULL: slot step % 2
+ *                             of a row that drew holds its log-probability, sample probability, top ids and their log-probabilities;
+ *   timed_out                 out: 1 if a wait ran out.
+ * A row that would draw token step > 0 with acked[b] >> 1 < step would wait for the host; the call refuses it (RWKV_ERROR_ARGS) before
+ * a device is touched, so the hook never waits. A row whose acked word has the stop bit freezes without drawing. */
+#define RWKV_B200_STEP_PLAIN 0
+#define RWKV_B200_STEP_CONSTRAINED 1
+#define RWKV_B200_STEP_LOGPROBS 2
+#define RWKV_B200_STEP_SAMPLED 3
+RWKV_API bool rwkv_b200_test_generate_step_streaming(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
+                                                     const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
+                                                     const uint32_t * acked, uint32_t * published, uint32_t * stream_tokens, uint32_t * ring,
+                                                     uint32_t * timed_out);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

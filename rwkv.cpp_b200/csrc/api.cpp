@@ -740,13 +740,22 @@ bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct 
 
 static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");
 static_assert(RWKV_B200_TOP_LOGPROBS_MAX == GEN_TOP_MAX, "top log-probabilities of the header and the kernel");
+static_assert(2 + 2 * RWKV_B200_TOP_LOGPROBS_MAX == GEN_LP_RECORD, "ring record of the header and the kernel");
 static_assert(RWKV_B200_LOGIT_BIAS_MAX == GEN_BIAS_MAX, "user bias entries of the header and the kernel");
+
+// The mapped words of the streaming step hook: acked is read, the others are written back ([n_rows], [n_rows][GENERATE_MAX],
+// [n_rows][2][GEN_LP_RECORD] or NULL without log-probabilities, one word).
+struct StreamHook {
+    const uint32_t * acked;
+    uint32_t * published, * tokens, * ring, * timed_out;
+};
 
 // One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
 // the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained); with
-// samplers the sampled kernel (next and lp may then be NULL).
+// samplers the sampled kernel (next and lp may then be NULL). With `stream` the streaming twin of that kernel runs, as the one node
+// of a graph, over pinned mapped copies of the caller's words.
 static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
-                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr) {
+                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr, const StreamHook * stream = nullptr) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
@@ -772,6 +781,16 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         live.resize(n_states);
         automaton_live(next, n_states, V, live.data());
     }
+    if (stream) {
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, stream->acked && stream->published && stream->tokens && stream->timed_out && (!lp || stream->ring),
+                   "NULL mapped word");
+        for (size_t b = 0; b < R; b++) {     // the gate of a row that draws token step > 0 waits until token step - 1 is acknowledged
+            const bool dead = constrained && states[b] != UINT32_MAX && !live[states[b]];
+            const bool draws = !a->frozen[b] && a->step[b] < a->max_tokens[b] && !dead;
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !draws || a->step[b] == 0 || (stream->acked[b] >> 1) >= a->step[b],
+                       "row %zu would wait for the acknowledgement of its token %u", b, a->step[b] - 1);
+        }
+    }
     if (!hook_device(sink)) return false;
     GenShared sh{};
     for (size_t k = 0; k < a->n_stop; k++) sh.stop[k] = a->stop_ids[k];
@@ -796,6 +815,26 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     gp.next_tokens = static_cast<int *>(hb.alloc(R * sizeof(int)));
     GenConstrainedParams cp{};
     cp.stream.step = gp;
+    // the streaming kernel's words in pinned mapped memory, as the engine keeps them: acked [R], published [R], timed_out, tokens
+    // [R][GENERATE_MAX], ring [R][2][GEN_LP_RECORD]
+    struct Pinned {
+        uint32_t * host = nullptr;
+        ~Pinned() { if (host) cudaFreeHost(host); }
+    } pinned;
+    const size_t ring_words = lp ? R * 2 * GEN_LP_RECORD : 0, tok_at = 2 * R + 1, ring_at = tok_at + R * GENERATE_MAX;
+    uint32_t * mapped = nullptr;
+    if (stream && hb.ok) {
+        hb.ok = cudaHostAlloc(reinterpret_cast<void **>(&pinned.host), (ring_at + ring_words) * sizeof(uint32_t), cudaHostAllocMapped) == cudaSuccess &&
+                cudaHostGetDevicePointer(reinterpret_cast<void **>(&mapped), pinned.host, 0) == cudaSuccess;
+        if (hb.ok) {
+            std::copy(stream->acked, stream->acked + R, pinned.host);
+            std::copy(stream->published, stream->published + R, pinned.host + R);
+            pinned.host[2 * R] = 0;
+            std::copy(stream->tokens, stream->tokens + R * GENERATE_MAX, pinned.host + tok_at);
+            if (lp) std::copy(stream->ring, stream->ring + ring_words, pinned.host + ring_at);
+            cp.stream.acked = mapped; cp.stream.published = mapped + R; cp.stream.timed_out = mapped + 2 * R; cp.stream.tokens = mapped + tok_at;
+        }
+    }
     std::vector<uint32_t> states_out(R);
     if (constrained) {
         const uint16_t * d_next = hb.in(next, n_states * V);
@@ -820,6 +859,7 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         req.sample_probs = lp->sample_probs ? const_cast<float *>(hb.in(lp->sample_probs, cells)) : static_cast<float *>(hb.alloc(cells * sizeof(float)));
         req.top_ids = k ? const_cast<uint32_t *>(hb.in(lp->top_ids, cells * k)) : nullptr;
         req.top_logprobs = k ? const_cast<float *>(hb.in(lp->top_logprobs, cells * k)) : nullptr;
+        req.ring = mapped ? mapped + ring_at : nullptr;
         lpp.gen = cp;
         lpp.req = hb.in(&req, 1);
     }
@@ -838,8 +878,24 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         smp.rows = hb.in(srows.data(), R);
         smp.bias = pool.empty() ? nullptr : hb.in(pool.data(), pool.size());
     }
-    const cudaError_t e = !hb.ok ? cudaSuccess : samplers ? launch_generate_sampled_step(smp, 0) : lp ? launch_generate_logprob_step(lpp, 0)
-                        : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
+    cudaError_t e = cudaSuccess;
+    if (hb.ok && stream) {      // the streaming kernels exist only as graph nodes
+        cudaGraph_t g = nullptr;
+        cudaGraphExec_t x = nullptr;
+        cudaGraphNode_t node = nullptr;
+        e = cudaGraphCreate(&g, 0);
+        if (e == cudaSuccess)
+            e = samplers ? add_generate_sampled_step_node(g, nullptr, 0, smp, true, &node) : lp ? add_generate_logprob_step_node(g, nullptr, 0, lpp, true, &node)
+              : constrained ? add_generate_constrained_step_node(g, nullptr, 0, cp, true, &node) : add_generate_stream_step_node(g, nullptr, 0, cp.stream, &node);
+        if (e == cudaSuccess) e = cudaGraphInstantiate(&x, g, 0);
+        if (e == cudaSuccess) e = cudaGraphLaunch(x, 0);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+        if (x) cudaGraphExecDestroy(x);
+        if (g) cudaGraphDestroy(g);
+    } else if (hb.ok) {
+        e = samplers ? launch_generate_sampled_step(smp, 0) : lp ? launch_generate_logprob_step(lpp, 0)
+          : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
+    }
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
@@ -854,6 +910,12 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     for (size_t b = 0; b < R; b++) { a->step[b] = rows[b].step; a->frozen[b] = rows[b].frozen ? 1 : 0; }
     for (size_t b = 0; constrained && b < R; b++)
         if (states[b] != UINT32_MAX) states[b] = states_out[b];
+    if (stream) {
+        std::copy(pinned.host + R, pinned.host + 2 * R, stream->published);
+        *stream->timed_out = pinned.host[2 * R];
+        std::copy(pinned.host + tok_at, pinned.host + tok_at + R * GENERATE_MAX, stream->tokens);
+        if (lp) std::copy(pinned.host + ring_at, pinned.host + ring_at + ring_words, stream->ring);
+    }
     return true;
 }
 
@@ -873,9 +935,9 @@ bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_
     return generate_step_hook(a, next, n_states, states, &out);
 }
 
-bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
-                                          size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp) {
-    g_last_error = RWKV_ERROR_NONE;
+// The sampled kernel's step: samplers[n_rows] in place of a's temperature, top_p and penalty arrays.
+static bool sampled_step_hook(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
+                              size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp, const StreamHook * stream = nullptr) {
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS, "Invalid generate-step arguments");
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
@@ -893,7 +955,31 @@ bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_a
     }
     struct rwkv_b200_generate_step_args args = *a;
     args.temperature = t.data(); args.top_p = p.data(); args.presence_penalty = pres.data(); args.frequency_penalty = freq.data();
-    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data());
+    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data(), stream);
+}
+
+bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
+                                          size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp) {
+    g_last_error = RWKV_ERROR_NONE;
+    return sampled_step_hook(a, samplers, next, n_states, states, lp);
+}
+
+bool rwkv_b200_test_generate_step_streaming(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
+                                            const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
+                                            const uint32_t * acked, uint32_t * published, uint32_t * stream_tokens, uint32_t * ring, uint32_t * timed_out) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family >= RWKV_B200_STEP_PLAIN && family <= RWKV_B200_STEP_SAMPLED, "Unknown step family %d", family);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, (family == RWKV_B200_STEP_SAMPLED) == (samplers != nullptr), "samplers go with the sampled family alone");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_CONSTRAINED ? next != nullptr : family != RWKV_B200_STEP_PLAIN || !next,
+               "The constrained family needs a table, the plain one takes none");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_LOGPROBS ? lp != nullptr : family == RWKV_B200_STEP_SAMPLED || !lp,
+               "The logprobs family needs lp, the plain and constrained ones take none");
+    const StreamHook stream{acked, published, stream_tokens, ring, timed_out};
+    if (family == RWKV_B200_STEP_SAMPLED) return sampled_step_hook(a, samplers, next, n_states, states, lp, &stream);
+    LogprobsOut out{};
+    if (lp && !logprobs_arg(sink, lp, out)) return false;
+    return generate_step_hook(a, next, n_states, states, lp ? &out : nullptr, nullptr, &stream);
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

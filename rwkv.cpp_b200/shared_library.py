@@ -233,6 +233,9 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_generate_sampled.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_sampled.argtypes = [ctypes.c_void_p, P_SAMPLER, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS]
         lib.rwkv_b200_test_generate_step_sampled.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step_streaming.argtypes = [ctypes.c_void_p, ctypes.c_int, P_SAMPLER, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS,
+                                                               P_U32, P_U32, P_U32, P_U32, P_U32]
+        lib.rwkv_b200_test_generate_step_streaming.restype = ctypes.c_bool
         lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
         lib.rwkv_b200_score.restype = ctypes.c_bool
         lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
