@@ -262,6 +262,52 @@ RWKV_API bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, 
                                                    const uint8_t * keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
                                                    rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated);
 
+/* LoRA adapters: a fine-tune of the model (RWKV-LM-LoRA / RWKV-PEFT checkpoints, python lora.py) applied on the GPU beside the base
+ * weights, which stay as loaded, at whatever type the file has (quantized included). An adapter lives in the HBM of the model's device
+ * and serves every context of that model; attached to a context, it changes what every entry point of that context computes:
+ * rwkv_eval*, the resident and ragged passes, rwkv_b200_score, sampling and every rwkv_b200_generate* family.
+ *
+ * Each entry of `t` names one tensor as the model file does ("blocks.3.att.key.weight", "blocks.0.ln0.weight", ...):
+ * - rank > 0: a low-rank delta of a layer matrix W [M][K]: a is A, [rank][K], b is B, [M][rank], both row-major host arrays. Every pass
+ *   computes y = epi(W.x + scale * B.(A.x)), where epi is that matrix's own epilogue (sigmoid, silu, relu^2, the residual add, the
+ *   gated residual add), applied once to the sum. A and B are stored as fp16 and accumulated in fp32. 1 <= rank <= 256. The matrices
+ *   that take a delta are att key / value / receptance / gate / output and ffn key / value / receptance (whichever the architecture
+ *   has); emb, head and the small LoRA matrices inside a v6 / v7 layer (time_maa_w1, time_decay_w1 / w2, w1 .. v2) are refused.
+ *   The caller's scale is lora_alpha / rank times any user scale; one scale serves every delta of the adapter.
+ * - rank == 0: a full replacement of that tensor, `values` in the file's element order and shape (the element count of the tensor).
+ *   Any tensor but emb.weight and head.weight. A replaced vector is kept in fp32; a replaced matrix is uploaded as the loader uploads
+ *   the base: at the base file's type (quantized by the library's own quantizer when the base is quantized), in the device layout, with
+ *   the tile-major copy when the base has one. A context with the adapter reads the replacement wherever it would read the base tensor.
+ *
+ * rwkv_b200_adapter_create checks every entry before it allocates anything and returns NULL with RWKV_ERROR_ARGS (read with
+ * rwkv_get_last_error(NULL)) for: an unknown name, a name listed twice, a delta on a matrix that takes none, rank above 256, NULL arrays,
+ * a non-finite scale or value. A and B, and the values of a replaced matrix whose base is not F32 (stored in fp16 or quantized with
+ * fp16 scales), must also be finite in fp16: |v| < 65520. The values are copied: the caller's arrays may be freed when it
+ * returns. A pipeline or one of its stages gives RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED.
+ * rwkv_b200_adapter_free returns false with RWKV_ERROR_ARGS, changing nothing, while any context has the adapter attached; NULL is
+ * accepted and returns true. Lifetime: the adapter holds a reference to its model's weights, as a context does, so the adapter and
+ * the contexts of that model may be freed in any order; the weights are released with the last of them.
+ * rwkv_b200_set_adapter attaches one adapter to ctx (a single-sequence or a batch context; in a batch, every sequence uses it), or
+ * detaches with adapter == NULL. It waits for the context's queued work and drops its single-token and generation graphs, which are
+ * captured again on later calls; the state, resident state and logits are untouched. A clone or a batch context made from an adapted
+ * context starts with no adapter. Refused, changing
+ * nothing: an adapter of another model (RWKV_ERROR_ARGS), a pipeline or a stage, and a call from inside that context's streaming
+ * callback (RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED).
+ * The invariants of the unadapted context hold for an adapted one: a sequence gives the bits of serial evaluation under any chunking
+ * of passes below 32 tokens, a batch row those of a single context below 16 sequences, device-side generation those of the host loop.
+ * An adapter whose every B is zero and that replaces nothing gives exactly the unadapted logits and states. */
+struct rwkv_b200_adapter;
+struct rwkv_b200_adapter_tensor {
+    const char * name;        /* tensor name as in the model file */
+    uint32_t rank;            /* > 0: low-rank delta of that matrix; 0: full replacement of that tensor */
+    const float * a;          /* rank > 0: A, [rank][K] row-major */
+    const float * b;          /* rank > 0: B, [M][rank] row-major */
+    const float * values;     /* rank == 0: the replacement, in the file's element order and shape */
+};
+RWKV_API struct rwkv_b200_adapter * rwkv_b200_adapter_create(struct rwkv_context * ctx, const struct rwkv_b200_adapter_tensor * t, size_t n, float scale);
+RWKV_API bool rwkv_b200_adapter_free(struct rwkv_b200_adapter * adapter);
+RWKV_API bool rwkv_b200_set_adapter(struct rwkv_context * ctx, const struct rwkv_b200_adapter * adapter);
+
 /* Generation with log-probabilities: the loops above that also report, for every token they draw, how likely it was, as completion
  * servers (logprobs / top_logprobs), evaluation and RL callers need, without per-token logits crossing PCIe.
  * The arguments, checks, context kinds and refusals are those of rwkv_b200_generate_constrained / rwkv_b200_batch_generate_constrained,
@@ -513,6 +559,19 @@ RWKV_API bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * 
  * emb_pitch that is a multiple of the element size. False with RWKV_ERROR_ARGS for invalid arguments, RWKV_ERROR_CTX | UNSUPPORTED
  * when the launcher refuses the shape or the device fails. */
 #define RWKV_B200_GUARD 64
+
+/* Test hook, no device needed: M rows of K values encoded in the file layout of data_type exactly as rwkv_b200_adapter_create encodes a
+ * replaced matrix before its upload (F32 copied, F16 rounded to nearest even, the quantized types by the library's quantizer, the one
+ * rwkv_quantize_model_file uses). out: M * (bytes of a row of K elements). K must be a multiple of the type's block. */
+RWKV_API bool rwkv_b200_test_encode_rows(int data_type, const float * values, size_t M, size_t K, void * out);
+
+/* The shrink and expand launches of an adapter's low-rank delta (csrc/kernels/lora.cu) on host buffers, column-major [dim, T]:
+ * u[:, t] = A . x[:, t] with A (rank x K, row-major) rounded to fp16, then y[:, t] = epi(z[:, t] + scale * B . u[:, t]) with B (M x rank,
+ * row-major) rounded to fp16. epilogue: 0 none, 1 sigmoid, 2 silu, 4 relu^2 (z is the base product W.x), 5 add and 6 gated add (z is
+ * the base's output y = res + W.x, resp. res + gate * W.x, and y = z + scale * B.u, resp. z + gate * (scale * B.u)); gate [M, T] is
+ * read by 6 only. u and y are guarded outputs. 1 <= T <= 256, 1 <= rank <= 256. */
+RWKV_API bool rwkv_b200_test_lora(int K, int M, int T, int rank, float scale, int epilogue, const float * a, const float * b, const float * x,
+                                  const float * z, const float * gate, float * u, float * y);
 
 /* x[:, t] = LN(emb[tokens[t]]; ln0). emb: n_vocab rows of emb_pitch bytes, F32 or F16 (emb_type 0 / 1). */
 RWKV_API bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, int n_vocab, const int * tokens, int T, int C,

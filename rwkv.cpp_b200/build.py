@@ -15,9 +15,9 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "librwkv.so")
 
 SOURCES = [
-    "api.cpp", "ggml_file.cpp", "quantizer.cpp", "model.cu", "engine.cu",
+    "api.cpp", "adapter.cpp", "ggml_file.cpp", "quantizer.cpp", "model.cu", "engine.cu",
     "kernels/gemv.cu", "kernels/gemv_tma.cu", "kernels/gemv_kquant.cu", "kernels/gemm_tc.cu", "kernels/pipe.cu", "kernels/glue.cu", "kernels/wkv.cu", "kernels/sampling.cu", "kernels/columns.cu",
-    "kernels/score.cu",
+    "kernels/score.cu", "kernels/lora.cu",
 ]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

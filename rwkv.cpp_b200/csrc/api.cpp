@@ -672,6 +672,8 @@ bool rwkv_b200_batch_generate_stream(struct rwkv_context * batch, const uint32_t
 
 // The opaque handle of the automaton API is the engine's Automaton.
 struct rwkv_b200_automaton : public rwkv::Automaton {};
+// ... and that of the adapter API the engine's Adapter.
+struct rwkv_b200_adapter : public rwkv::Adapter {};
 
 extern "C" {
 
@@ -686,6 +688,32 @@ struct rwkv_b200_automaton * rwkv_b200_automaton_create(struct rwkv_context * ct
 }
 
 void rwkv_b200_automaton_free(struct rwkv_b200_automaton * a) { destroy_automaton(a); }
+
+struct rwkv_b200_adapter * rwkv_b200_adapter_create(struct rwkv_context * ctx, const struct rwkv_b200_adapter_tensor * t, size_t n, float scale) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, ctx, "NULL context");
+    Model & m = *C(ctx)->model;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, !C(ctx)->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Adapters serve whole-model and batch contexts, not a pipeline or one of its stages");
+    static_assert(sizeof(rwkv_b200_adapter_tensor) == sizeof(AdapterTensor), "rwkv_b200_adapter_tensor and AdapterTensor differ");
+    return static_cast<struct rwkv_b200_adapter *>(create_adapter(&m, reinterpret_cast<const AdapterTensor *>(t), n, scale, sink));
+}
+
+bool rwkv_b200_adapter_free(struct rwkv_b200_adapter * adapter) {
+    g_last_error = RWKV_ERROR_NONE;
+    return destroy_adapter(adapter, global_sink());
+}
+
+bool rwkv_b200_set_adapter(struct rwkv_context * ctx, const struct rwkv_b200_adapter * adapter) {
+    Context * c = C(ctx);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, !c->group && c->model->layer_begin == 0 && c->model->layer_end == c->model->n_layer,
+               "Adapters serve whole-model and batch contexts, not a pipeline or one of its stages");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !adapter || adapter->model == c->model, "The adapter belongs to another model");
+    return set_adapter(c, adapter);
+}
 
 bool rwkv_b200_generate_constrained(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state, size_t max_tokens,
                                     float temperature, float top_p, float presence_penalty, float frequency_penalty, bool keep_counts, const double * u,
@@ -1271,6 +1299,53 @@ bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, 
     float * d_x = b.out(x, (size_t) C * T);
     const cudaError_t e = b.ok ? launch_embed_ln0(d_emb, emb_type, (long long) emb_pitch, d_tok, T, C, d_w, d_b, d_x, 0) : cudaSuccess;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "embed_ln0 failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_encode_rows(int data_type, const float * values, size_t M, size_t K, void * out) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, values && out && M > 0 && K > 0 && (data_type == DT_F32 || dtype_loadable(data_type)) &&
+               K % (size_t) dtype_block_elems(data_type) == 0, "Invalid encode_rows arguments");
+    encode_rows(data_type, values, M, K, static_cast<uint8_t *>(out));
+    return true;
+}
+
+bool rwkv_b200_test_lora(int K, int M, int T, int rank, float scale, int epilogue, const float * a, const float * b, const float * x,
+                         const float * z, const float * gate, float * u, float * y) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const bool epi_ok = epilogue == EPI_NONE || epilogue == EPI_SIGMOID || epilogue == EPI_SILU || epilogue == EPI_RELU_SQR || epilogue == EPI_ADD ||
+                        epilogue == EPI_MUL_ADD;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && b && x && z && u && y && K > 0 && M > 0 && T >= 1 && T <= MAX_TOKENS_PER_PASS && rank >= 1 &&
+               rank <= LORA_MAX_RANK && epi_ok && (epilogue != EPI_MUL_ADD || gate), "Invalid lora arguments");
+    if (!hook_device(sink)) return false;
+    const size_t R = (size_t) rank;
+    std::vector<uint16_t> ha(R * (size_t) K), hbt(R * (size_t) M);
+    for (size_t i = 0; i < ha.size(); i++) ha[i] = fp32_to_fp16(a[i]);
+    for (size_t r = 0; r < R; r++) for (size_t i = 0; i < (size_t) M; i++) hbt[r * M + i] = fp32_to_fp16(b[i * R + r]);
+    HookBuffers hb;
+    LoraBatch lb{};
+    lb.n = 1; lb.T = T;
+    LoraProblem & l = lb.p[0];
+    l.d.A = hb.in(ha.data(), ha.size()); l.d.Bt = hb.in(hbt.data(), hbt.size()); l.d.rank = rank; l.d.scale = scale;
+    l.K = K; l.M = M;
+    l.x = hb.in(x, (size_t) K * T); l.ldx = K;
+    l.u = hb.out(u, R * T);
+    l.P.epi = epilogue; l.P.ldy = M;
+    const bool residual = epilogue == EPI_ADD || epilogue == EPI_MUL_ADD;
+    if (residual) {
+        l.P.y = hb.inout(z, y, (size_t) M * T);
+        l.P.res = l.P.y; l.P.ldres = M;
+        if (epilogue == EPI_MUL_ADD) { l.P.gate = hb.in(gate, (size_t) M * T); l.P.ldgate = M; }
+    } else {
+        l.z = hb.in(z, (size_t) M * T); l.ldz = M;
+        l.P.y = hb.out(y, (size_t) M * T);
+    }
+    cudaError_t e = cudaSuccess;
+    if (hb.ok) e = launch_lora_shrink(lb, 0);
+    if (hb.ok && e == cudaSuccess) e = launch_lora_expand(lb, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, hb.finish(e), "lora failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

@@ -122,8 +122,10 @@ struct Pass {
 // ---- GEMV batch builder -------------------------------------------------------------------------
 struct Batch {
     GemvBatch b;
+    const LoraDelta * lora[GEMV_MAX_PROBLEMS] = {};   // the delta of each problem's matrix under the attached adapter, or NULL
     explicit Batch(int T) { memset(&b, 0, sizeof(b)); b.T = T; }
     GemvProblem & add(const DevMatrix & W, const float * x, float * y, int epi = EPI_NONE) {
+        lora[b.n] = W.lora;
         GemvProblem & p = b.p[b.n++];
         p.W = W.data; p.Wt = W.tiled; p.pitch = W.pitch; p.type = W.type; p.K = W.K; p.M = W.M;
         p.x = x; p.ldx = W.K;
@@ -168,7 +170,7 @@ bool launch_batch(Context * ctx, GemvBatch & b, cudaStream_t stream) {
     return true;
 }
 
-bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
+bool run_base(Context * ctx, const Pass & p, Batch & batch) {
     if (!ctx->profiling) return launch_batch(ctx, batch.b, p.stream);
     Context::ProfRecord rec{};
     CUDA_OK(ctx, cudaEventCreate(&rec.start));
@@ -179,6 +181,36 @@ bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
     if (!launch_batch(ctx, batch.b, p.stream)) return false;
     CUDA_OK(ctx, cudaEventRecord(rec.stop, p.stream));
     ctx->prof.push_back(rec);
+    return true;
+}
+
+// A batch with low-rank deltas (kernels/lora.h): the shrink of every adapted problem, the batch through its unchanged route with the
+// adapted problems of nonlinear epilogue retargeted to EPI_NONE into lora_z, then the expand. Problems without a delta stay as they were.
+bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
+    LoraBatch lb;
+    lb.n = 0; lb.T = batch.b.T;
+    float * u = ctx->lora_u, * z = ctx->lora_z;
+    for (int i = 0; i < batch.b.n; i++) {
+        if (!batch.lora[i]) continue;
+        GemvProblem & q = batch.b.p[i];
+        LoraProblem & l = lb.p[lb.n++];
+        l.d = *batch.lora[i];
+        l.K = q.K; l.M = q.M;
+        l.x = q.x; l.ldx = q.ldx;
+        l.u = u; u += (size_t) l.d.rank * lb.T;
+        l.P = q;
+        if (q.epi == EPI_ADD || q.epi == EPI_MUL_ADD) {      // residual epilogues: the base writes y, the expand adds to it
+            l.z = nullptr; l.ldz = 0;
+            l.P.res = q.y; l.P.ldres = q.ldy;
+        } else {
+            l.z = z; l.ldz = q.M;
+            q.y = z; q.ldy = q.M; q.epi = EPI_NONE; q.res = q.gate = q.bias = nullptr;
+            z += (size_t) q.M * lb.T;
+        }
+    }
+    if (lb.n) CUDA_OK(ctx, launch_lora_shrink(lb, p.stream));
+    if (!run_base(ctx, p, batch)) return false;
+    if (lb.n) CUDA_OK(ctx, launch_lora_expand(lb, p.stream));
     return true;
 }
 
@@ -504,6 +536,10 @@ bool make_pass(Context * ctx, int T, bool want_logits, cudaStream_t stream, Pass
     return true;
 }
 
+// The head's LayerNorm parameters: the attached adapter's replacements, or the model's.
+const float * ln_out_w(const Context * ctx) { return (ctx->adapter ? ctx->adapter->ln_out_w : ctx->model->ln_out_w).data; }
+const float * ln_out_b(const Context * ctx) { return (ctx->adapter ? ctx->adapter->ln_out_b : ctx->model->ln_out_b).data; }
+
 // The head of a scoring pass of T columns runs on the tensor cores when the layers of such a pass would (T >= 32 in a single-sequence
 // context, >= BATCH_TC_MIN in a batch context, tensor cores on) and the head's type and width have a tile-major form.
 bool score_on_tensor_cores(const Context * ctx, int T) {
@@ -521,13 +557,13 @@ bool score_head(Context * ctx, const Pass & p) {
     if (score_on_tensor_cores(ctx, T)) {
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.head_tiled && ctx->act16, "The head has no tile-major copy");
         // the columns' LayerNorm goes to mix[0], which the layers no longer need
-        CUDA_OK(ctx, launch_layer_norm_columns(p.s.x, m.ln_out_w.data, m.ln_out_b.data, C, T, p.s.mix[0], p.stream));
+        CUDA_OK(ctx, launch_layer_norm_columns(p.s.x, ln_out_w(ctx), ln_out_b(ctx), C, T, p.s.mix[0], p.stream));
         GemvProblem & q = b.add(m.head, p.s.mix[0], ctx->score_logits);
         q.Wt = m.head_tiled;
         CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, p.stream, ctx->act16, ctx->act16_bytes));
     } else {
         GemvProblem & q = b.add(m.head, p.s.x, ctx->score_logits);
-        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        q.pro = PRO_LAYERNORM; q.ln_w = ln_out_w(ctx); q.ln_b = ln_out_b(ctx);
         if (!run_batch(ctx, p, b)) return false;
     }
     ScoreParams sp{};
@@ -549,11 +585,12 @@ bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
     const int C = m.n_embed, T = p.T;
     if (l0 == 0) {
         if (!p.tokens_in_place) CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[p.phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, p.stream));
-        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, m.ln0_w.data, m.ln0_b.data, p.s.x, p.stream));
+        const DevVec & ln0_w = ctx->adapter ? ctx->adapter->ln0_w : m.ln0_w, & ln0_b = ctx->adapter ? ctx->adapter->ln0_b : m.ln0_b;
+        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, ln0_w.data, ln0_b.data, p.s.x, p.stream));
     }   // a later pipeline stage / layer group finds x (and v_first) already in place
     const size_t per_layer = m.state_floats_per_layer();
     for (int i = l0; i < l1; i++) {
-        const Layer & L = m.layers[i];
+        const Layer & L = ctx->adapter ? ctx->adapter->layers[i] : m.layers[i];
         const float * st_in = p.state_in + (size_t) i * per_layer;
         float * st_out = p.state_out + (size_t) i * per_layer;
         const LnMixParams alp = att_ln(ctx, L, p, st_in, st_out), flp = ffn_ln(ctx, L, p, st_in, st_out);
@@ -574,13 +611,13 @@ bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
         CUDA_OK(ctx, launch_copy_columns(p.s.x, p.head_col, ctx->head_x, nullptr, C, n, p.stream));
         Batch b(n);
         GemvProblem & q = b.add(m.head, ctx->head_x, ctx->head_y);
-        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        q.pro = PRO_LAYERNORM; q.ln_w = ln_out_w(ctx); q.ln_b = ln_out_b(ctx);
         if (!run_batch(ctx, p, b)) return false;
         CUDA_OK(ctx, launch_copy_columns(ctx->head_y, nullptr, p.logits, p.head_seq, m.n_vocab, n, p.stream));
     } else if (p.want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
         Batch b(ctx->batch_n ? T : 1);
         GemvProblem & q = b.add(m.head, ctx->batch_n ? p.s.x : p.s.x + (size_t) (T - 1) * C, p.logits);
-        q.pro = PRO_LAYERNORM; q.ln_w = m.ln_out_w.data; q.ln_b = m.ln_out_b.data;
+        q.pro = PRO_LAYERNORM; q.ln_w = ln_out_w(ctx); q.ln_b = ln_out_b(ctx);
         if (!run_batch(ctx, p, b)) return false;
     }
     if (ctx->trace_buf) {
@@ -743,6 +780,8 @@ void destroy_context(Context * ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     cudaFree(ctx->state_a); cudaFree(ctx->state_b); cudaFree(ctx->state_init); cudaFree(ctx->logits);
     cudaFree(ctx->tokens); cudaFree(ctx->scratch); cudaFree(ctx->trace_buf); cudaFree(ctx->act16); cudaFree(ctx->xq);
+    if (ctx->adapter) ctx->adapter->attached.fetch_sub(1);
+    cudaFree(ctx->lora_u); cudaFree(ctx->lora_z);
     for (int i = 0; i < 2; i++) {
         if (ctx->tokens_host[i]) cudaFreeHost(ctx->tokens_host[i]);
         if (ctx->ragged_host[i]) cudaFreeHost(ctx->ragged_host[i]);
@@ -1606,6 +1645,30 @@ void drop_generate_graphs(Context * ctx) {
         for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
     for (auto & by_phase : ctx->gen_smp_graphs)
         for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+}
+
+bool set_adapter(Context * ctx, const Adapter * a) {
+    if (a == ctx->adapter) return true;
+    const Model & m = *ctx->model;
+    CUDA_OK(ctx, cudaSetDevice(m.dev.device));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (a && !ctx->lora_u) {
+        const Dims d = model_dims(m);
+        const size_t z_rows = std::max(4 * d.C, d.F + d.C), T = MAX_TOKENS_PER_PASS;
+        cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), (size_t) GEMV_MAX_PROBLEMS * LORA_MAX_RANK * T * sizeof(float));
+        if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), z_rows * T * sizeof(float));
+        if (e != cudaSuccess) {
+            cudaFree(ctx->lora_u); cudaFree(ctx->lora_z); ctx->lora_u = ctx->lora_z = nullptr;
+            RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, false, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));
+        }
+    }
+    // the captured passes hold the tensors and launches of the adapter they were captured with
+    for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
+    drop_generate_graphs(ctx);
+    if (a) a->attached.fetch_add(1);
+    if (ctx->adapter) ctx->adapter->attached.fetch_sub(1);
+    ctx->adapter = a;
+    return true;
 }
 
 bool check_logprobs(ErrorSink sink, size_t n_vocab, const LogprobsOut * lp) {

@@ -28,6 +28,31 @@ struct GenLogprobRequest;               // the per-call request of the logprob g
 struct CopyPool;                        // helper threads of the pageable-buffer bounce path (engine.cu)
 void destroy_copy_pool(CopyPool * p);
 
+// A LoRA adapter of rwkv_b200_adapter_create (include/rwkv_b200.h), in the HBM of its model's device: copies of the model's layers and
+// top-level vectors in which every replaced tensor points at its replacement and every adapted matrix carries its LoraDelta. A
+// context with the adapter attached reads these instead of the model's. It serves every context of that model.
+struct Adapter {
+    Model * model = nullptr;             // holds a reference (Model::refcount), released by destroy_adapter
+    std::vector<Layer> layers;           // indexed by absolute layer id, as Model::layers
+    DevVec ln0_w, ln0_b, ln_out_w, ln_out_b;
+    std::vector<LoraDelta> deltas;       // DevMatrix::lora points into it
+    uint8_t * arena = nullptr;           // A, B and the replacements
+    mutable std::atomic<int> attached{0};   // contexts that have it attached
+};
+// M rows of K values in the file layout of `type`, as a replaced matrix is encoded before its upload: F32 copied, F16 rounded, the
+// other types by quantize_row. `out` has M * tensor_nbytes(type, K, 1, 1) bytes.
+void encode_rows(int type, const float * values, size_t M, size_t K, uint8_t * out);
+// One entry of rwkv_b200_adapter_create (the layout of struct rwkv_b200_adapter_tensor).
+struct AdapterTensor {
+    const char * name;
+    uint32_t rank;
+    const float * a, * b, * values;
+};
+// Checks every entry before it allocates anything (RWKV_ERROR_ARGS), then uploads. NULL on failure, with the flags set.
+Adapter * create_adapter(Model * model, const AdapterTensor * t, size_t n, float scale, ErrorSink sink);
+// false with RWKV_ERROR_ARGS while a context has it attached. Deletes the model when the adapter held its last reference.
+bool destroy_adapter(Adapter * a, ErrorSink sink);
+
 struct Context {
     Model * model = nullptr;
     PipeGroup * group = nullptr;           // set on the stage-0 context of an in-process pipeline
@@ -149,6 +174,12 @@ struct Context {
     // room for rows * GEN_BIAS_MAX GenBiasEntry.
     unsigned char * smp_dev = nullptr, * smp_host = nullptr;
     cudaGraphExec_t gen_smp_graphs[2][2] = {};   // the sampled loops' graphs, keyed by phase and streaming
+
+    // The attached adapter (set_adapter) or NULL, and the scratch of its deltas, allocated on the first attach for passes of up to
+    // MAX_TOKENS_PER_PASS columns so that captured graphs never see it move: u [GEMV_MAX_PROBLEMS][LORA_MAX_RANK][T] and the base
+    // outputs z of a batch's adapted problems with a nonlinear epilogue, max(4 C, F + C) rows of T.
+    const Adapter * adapter = nullptr;
+    float * lora_u = nullptr, * lora_z = nullptr;
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -303,6 +334,9 @@ Automaton * create_automaton(const Model * model, const uint16_t * next, size_t 
 void destroy_automaton(Automaton * a);
 // Drops the loop's graphs (they hold the activation buffers and the GEMM routing of the time they were captured).
 void drop_generate_graphs(Context * ctx);
+// Attaches `a` (NULL: detaches), dropping the single-token and generation graphs; the state is untouched. The caller has checked the
+// context and that `a` belongs to its model.
+bool set_adapter(Context * ctx, const Adapter * a);
 
 size_t stage_hidden_len(const Model & m, size_t T);
 

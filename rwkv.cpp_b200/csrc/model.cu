@@ -26,12 +26,7 @@ Model::~Model() {
 
 namespace {
 
-struct Request {
-    std::string name;
-    DevMatrix * mat = nullptr;   // exactly one of mat / vec is set
-    DevVec * vec = nullptr;
-    uint64_t expect_k = 0, expect_m = 0;   // matrices: 0 = unchecked
-    uint64_t expect_n = 0;                 // vectors:  0 = unchecked
+struct Request : ParamSlot {
     const TensorInfo * info = nullptr;
     size_t arena_offset = 0;
     size_t tiled_offset = 0, tiled_bytes = 0;   // matrices that get a tile-major prefill copy
@@ -125,61 +120,20 @@ cudaError_t upload_matrix(const void * host, int type, int M, int K, uint8_t * d
     return ce;
 }
 
-Model * load_model(const char * path, int device, int layer_begin, int layer_end, ErrorSink sink) {
-    ModelFile mf;
-    RWKV_PROPAGATE(sink, nullptr, scan_model_file(path, mf, sink));
-
-    std::unique_ptr<Model> model(new (std::nothrow) Model());
-    RWKV_CHECK(sink, RWKV_ERROR_MODEL | RWKV_ERROR_ALLOC, nullptr, model, "Failed to allocate the model");
-    Model & m = *model;
-    m.header = mf.header;
-    m.n_embed = (int) mf.header.n_embed;
-    m.n_vocab = (int) mf.header.n_vocab;
-    m.n_layer = (int) mf.header.n_layer;
-    if (layer_end < 0 || layer_end > m.n_layer) layer_end = m.n_layer;
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, layer_begin >= 0 && layer_begin < layer_end, "Invalid layer range [%d, %d)", layer_begin, layer_end);
-    m.layer_begin = layer_begin;
-    m.layer_end = layer_end;
-
-    // Architecture detection by key presence (rwkv_model_loading.inc:319-340).
-    m.arch_major = 4; m.arch_minor = 0;
-    if (mf.find("blocks.0.att.ln_x.weight")) { m.arch_major = 5; m.arch_minor = mf.find("blocks.0.att.gate.weight") ? 2 : 1; }
-    if (mf.find("blocks.0.att.time_maa_x")) { m.arch_major = 6; m.arch_minor = 0; }
-    if (mf.find("blocks.0.att.r_k")) { m.arch_major = 7; m.arch_minor = 0; }
-
-    const uint64_t C = mf.header.n_embed, V = mf.header.n_vocab;
-    // head geometry (rwkv_model_loading.inc:403-409)
-    uint64_t H = 0, S = 0;
-    if (m.arch_major == 7) {
-        const TensorInfo * rk = mf.find("blocks.0.att.r_k");
-        H = rk->ne[1];
-    } else if (m.arch_major >= 5) {
-        const TensorInfo * td = mf.find("blocks.0.att.time_decay");
-        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_PARAM_MISSING, nullptr, td, "Model parameter %s not found", "blocks.0.att.time_decay");
-        H = td->ne[2];
-    }
-    if (m.arch_major >= 5) {
-        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_SHAPE, nullptr, H > 0 && C % H == 0, "Head count %" PRIu64 " does not divide n_embed %" PRIu64, H, C);
-        S = C / H;
-        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_UNSUPPORTED, nullptr, S == 8 || S == 16 || S == 32 || S == 64 || S == 128,
-                   "Unsupported head size %" PRIu64, S);
-    }
-    m.head_count = (int) H;
-    m.head_size = (int) S;
-
-    // ---- parameter table (rwkv_set_params, rwkv_model_loading.inc:128-285), same key order ----
-    m.layers.resize(m.n_layer);
-    std::vector<Request> reqs;
-    auto want_vec = [&](const std::string & name, DevVec & dst, uint64_t n) { Request r; r.name = name; r.vec = &dst; r.expect_n = n; reqs.push_back(r); };
-    auto want_mat = [&](const std::string & name, DevMatrix & dst, uint64_t k, uint64_t mm) { Request r; r.name = name; r.mat = &dst; r.expect_k = k; r.expect_m = mm; reqs.push_back(r); };
+std::vector<ParamSlot> param_table(const Model & m, Layer * layers, const TopTensors & top) {
+    std::vector<ParamSlot> reqs;
+    auto want_vec = [&](const std::string & name, DevVec & dst, uint64_t n) { ParamSlot r; r.name = name; r.vec = &dst; r.expect_n = n; reqs.push_back(r); };
+    auto want_mat = [&](const std::string & name, DevMatrix & dst, uint64_t k, uint64_t mm) { ParamSlot r; r.name = name; r.mat = &dst; r.expect_k = k; r.expect_m = mm; reqs.push_back(r); };
+    const uint64_t C = (uint64_t) m.n_embed, V = (uint64_t) m.n_vocab, H = (uint64_t) m.head_count;
+    const int layer_begin = m.layer_begin, layer_end = m.layer_end;
 
     if (layer_begin == 0) {
-        want_mat("emb.weight", m.emb, C, V);
-        want_vec("blocks.0.ln0.weight", m.ln0_w, C);
-        want_vec("blocks.0.ln0.bias", m.ln0_b, C);
+        want_mat("emb.weight", *top.emb, C, V);
+        want_vec("blocks.0.ln0.weight", *top.ln0_w, C);
+        want_vec("blocks.0.ln0.bias", *top.ln0_b, C);
     }
     for (int i = layer_begin; i < layer_end; i++) {
-        Layer & L = m.layers[i];
+        Layer & L = layers[i];
         const std::string p = "blocks." + std::to_string(i) + ".";
         want_vec(p + "ln1.weight", L.ln1_w, C);
         want_vec(p + "ln1.bias", L.ln1_b, C);
@@ -270,9 +224,62 @@ Model * load_model(const char * path, int device, int layer_begin, int layer_end
         if (m.arch_major != 7) want_mat(p + "ffn.receptance.weight", L.ffn_receptance, C, C);
     }
     if (layer_end == m.n_layer) {
-        want_vec("ln_out.weight", m.ln_out_w, C);
-        want_vec("ln_out.bias", m.ln_out_b, C);
-        want_mat("head.weight", m.head, C, V);
+        want_vec("ln_out.weight", *top.ln_out_w, C);
+        want_vec("ln_out.bias", *top.ln_out_b, C);
+        want_mat("head.weight", *top.head, C, V);
+    }
+    return reqs;
+}
+
+Model * load_model(const char * path, int device, int layer_begin, int layer_end, ErrorSink sink) {
+    ModelFile mf;
+    RWKV_PROPAGATE(sink, nullptr, scan_model_file(path, mf, sink));
+
+    std::unique_ptr<Model> model(new (std::nothrow) Model());
+    RWKV_CHECK(sink, RWKV_ERROR_MODEL | RWKV_ERROR_ALLOC, nullptr, model, "Failed to allocate the model");
+    Model & m = *model;
+    m.header = mf.header;
+    m.n_embed = (int) mf.header.n_embed;
+    m.n_vocab = (int) mf.header.n_vocab;
+    m.n_layer = (int) mf.header.n_layer;
+    if (layer_end < 0 || layer_end > m.n_layer) layer_end = m.n_layer;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, layer_begin >= 0 && layer_begin < layer_end, "Invalid layer range [%d, %d)", layer_begin, layer_end);
+    m.layer_begin = layer_begin;
+    m.layer_end = layer_end;
+
+    // Architecture detection by key presence (rwkv_model_loading.inc:319-340).
+    m.arch_major = 4; m.arch_minor = 0;
+    if (mf.find("blocks.0.att.ln_x.weight")) { m.arch_major = 5; m.arch_minor = mf.find("blocks.0.att.gate.weight") ? 2 : 1; }
+    if (mf.find("blocks.0.att.time_maa_x")) { m.arch_major = 6; m.arch_minor = 0; }
+    if (mf.find("blocks.0.att.r_k")) { m.arch_major = 7; m.arch_minor = 0; }
+
+    const uint64_t C = mf.header.n_embed, V = mf.header.n_vocab;
+    // head geometry (rwkv_model_loading.inc:403-409)
+    uint64_t H = 0, S = 0;
+    if (m.arch_major == 7) {
+        const TensorInfo * rk = mf.find("blocks.0.att.r_k");
+        H = rk->ne[1];
+    } else if (m.arch_major >= 5) {
+        const TensorInfo * td = mf.find("blocks.0.att.time_decay");
+        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_PARAM_MISSING, nullptr, td, "Model parameter %s not found", "blocks.0.att.time_decay");
+        H = td->ne[2];
+    }
+    if (m.arch_major >= 5) {
+        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_SHAPE, nullptr, H > 0 && C % H == 0, "Head count %" PRIu64 " does not divide n_embed %" PRIu64, H, C);
+        S = C / H;
+        RWKV_CHECK(sink, RWKV_ERROR_MODEL_PARAMS | RWKV_ERROR_UNSUPPORTED, nullptr, S == 8 || S == 16 || S == 32 || S == 64 || S == 128,
+                   "Unsupported head size %" PRIu64, S);
+    }
+    m.head_count = (int) H;
+    m.head_size = (int) S;
+
+    // ---- parameter table (rwkv_set_params, rwkv_model_loading.inc:128-285), same key order ----
+    m.layers.resize(m.n_layer);
+    std::vector<Request> reqs;
+    for (const ParamSlot & ps : param_table(m, m.layers.data(), TopTensors{&m.emb, &m.head, &m.ln0_w, &m.ln0_b, &m.ln_out_w, &m.ln_out_b})) {
+        Request r;
+        static_cast<ParamSlot &>(r) = ps;
+        reqs.push_back(r);
     }
 
     // ---- resolve + validate + lay out the arena ----

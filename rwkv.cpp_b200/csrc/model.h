@@ -12,6 +12,7 @@
 #include "errors.h"
 #include "ggml_file.h"
 #include "kernels/gemv.h"
+#include "kernels/lora.h"
 #include "kernels/ops.h"
 
 namespace rwkv {
@@ -21,6 +22,7 @@ struct DevMatrix {          // y = W x : K = ne0 (input), M = ne1*ne2 (output ro
     const uint8_t * tiled = nullptr;   // tile-major prefill copy (gemm_tc_repack) or NULL
     int type = 0, K = 0, M = 0;
     long long pitch = 0;
+    const LoraDelta * lora = nullptr;  // the low-rank delta of an attached adapter (Adapter::layers only), or NULL
     explicit operator bool() const { return data != nullptr; }
 };
 struct DevVec {
@@ -95,6 +97,20 @@ struct Model {
     size_t state_len() const { return state_floats_per_layer() * (size_t) n_layer; }
     ~Model();
 };
+
+// One entry of a model's parameter table (rwkv_set_params, rwkv_model_loading.inc:128-285): the tensor's name in the file, the
+// matrix or vector it is loaded into (exactly one is set) and its expected shape (0 = unchecked).
+struct ParamSlot {
+    std::string name;
+    DevMatrix * mat = nullptr;
+    DevVec * vec = nullptr;
+    uint64_t expect_k = 0, expect_m = 0;
+    uint64_t expect_n = 0;
+};
+struct TopTensors { DevMatrix * emb, * head; DevVec * ln0_w, * ln0_b, * ln_out_w, * ln_out_b; };
+// The table of m's architecture, resident layers and head geometry, in the loader's key order, with the slots pointing into
+// `layers` (indexed by absolute layer id) and `top`. The loader passes m's own tensors; an adapter passes its copies of them.
+std::vector<ParamSlot> param_table(const Model & m, Layer * layers, const TopTensors & top);
 
 // Loads `path` onto CUDA device `device`. layer_end < 0 means n_layer. Returns nullptr after
 // recording the failure in `sink` (same categories/codes as rwkv_model_loading.inc:288-419).

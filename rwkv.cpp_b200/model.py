@@ -26,6 +26,8 @@ class RWKVModel:
         if not gpu_layer_count >= 0:
             raise ValueError("GPU layer count must be >= 0")
         self._library = shared_library
+        self._path = model_path
+        self._adapter = None
         self._ctx = shared_library.rwkv_init_from_file(model_path, thread_count, gpu_layer_count)
         self._state_buffer_element_count = shared_library.rwkv_get_state_buffer_element_count(self._ctx)
         self._logits_buffer_element_count = shared_library.rwkv_get_logits_buffer_element_count(self._ctx)
@@ -124,11 +126,24 @@ class RWKVModel:
         self._library.rwkv_eval_sequence_in_chunks(self._ctx, tokens, chunk_size, self._ptr(state_in), self._ptr(state_out), self._ptr(logits_out))
         return logits_out, state_out
 
+    @property
+    def arch(self) -> Tuple[int, int]:
+        """(major, minor) RWKV version of the model file."""
+        info = self._library.rwkv_b200_inspect_file(self._path)
+        return int(info.arch_major), int(info.arch_minor)
+
+    def set_adapter(self, adapter) -> None:
+        """Runs every later evaluation with `adapter` (a lora.Adapter made for this model) applied; None detaches. The state is
+        untouched. See rwkv_b200_set_adapter in include/rwkv_b200.h."""
+        self._library.rwkv_b200_set_adapter(self._ctx, adapter.handle if adapter is not None else None)
+        self._adapter = adapter
+
     def free(self) -> None:
         if not self._valid:
             raise ValueError("Already freed")
         self._valid = False
         self._library.rwkv_free(self._ctx)
+        self._adapter = None
 
     def __del__(self) -> None:
         if getattr(self, "_valid", False):

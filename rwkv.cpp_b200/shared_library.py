@@ -8,6 +8,8 @@ import ctypes
 import os
 from typing import Optional
 
+import numpy as np
+
 P_FLOAT = ctypes.POINTER(ctypes.c_float)
 P_U32 = ctypes.POINTER(ctypes.c_uint32)
 # rwkv_b200_token_fn (include/rwkv_b200.h): int (*)(void * user, size_t sequence, size_t index, uint32_t token)
@@ -43,6 +45,11 @@ class Sampler(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_sampl
     _fields_ = [("temperature", ctypes.c_float), ("top_p", ctypes.c_float), ("top_k", ctypes.c_uint32), ("min_p", ctypes.c_float),
                 ("presence_penalty", ctypes.c_float), ("frequency_penalty", ctypes.c_float), ("n_bias", ctypes.c_size_t),
                 ("bias_ids", ctypes.POINTER(ctypes.c_uint32)), ("bias_values", ctypes.POINTER(ctypes.c_float))]
+
+
+class AdapterTensor(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_adapter_tensor
+    _fields_ = [("name", ctypes.c_char_p), ("rank", ctypes.c_uint32), ("a", ctypes.POINTER(ctypes.c_float)),
+                ("b", ctypes.POINTER(ctypes.c_float)), ("values", ctypes.POINTER(ctypes.c_float))]
 
 
 class RWKVContext:
@@ -213,6 +220,16 @@ class RWKVSharedLibrary:
                                                              P_U32, ctypes.c_size_t, RWKV_TOKEN_FN, ctypes.c_void_p, P_U32, P_U32]
         lib.rwkv_b200_batch_generate_constrained.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_constrained.argtypes = [ctypes.c_void_p, P_U16, ctypes.c_size_t, P_U32]
+        lib.rwkv_b200_adapter_create.argtypes = [vp, ctypes.POINTER(AdapterTensor), ctypes.c_size_t, ctypes.c_float]
+        lib.rwkv_b200_adapter_create.restype = vp
+        lib.rwkv_b200_adapter_free.argtypes = [vp]
+        lib.rwkv_b200_adapter_free.restype = ctypes.c_bool
+        lib.rwkv_b200_set_adapter.argtypes = [vp, vp]
+        lib.rwkv_b200_set_adapter.restype = ctypes.c_bool
+        lib.rwkv_b200_test_lora.argtypes = [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int] + [P_FLOAT] * 7
+        lib.rwkv_b200_test_lora.restype = ctypes.c_bool
+        lib.rwkv_b200_test_encode_rows.argtypes = [ctypes.c_int, P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p]
+        lib.rwkv_b200_test_encode_rows.restype = ctypes.c_bool
         lib.rwkv_b200_test_generate_step_constrained.restype = ctypes.c_bool
         P_LOGPROBS = ctypes.POINTER(Logprobs)
         lib.rwkv_b200_generate_logprobs.argtypes = [vp, vp, P_U32, ctypes.c_size_t, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
@@ -329,6 +346,35 @@ class RWKVSharedLibrary:
         if not self.library.rwkv_b200_inspect_file(model_file_path.encode("utf-8"), ctypes.byref(info)):
             raise ValueError(f"rwkv_b200_inspect_file failed (error flags 0x{self.rwkv_get_last_error(None):x})")
         return info
+
+    def rwkv_b200_adapter_create(self, ctx: RWKVContext, tensors, scale: float) -> int:
+        """tensors: (name, rank, a, b, values) tuples, the arrays float32 C-contiguous numpy arrays (or None), as
+        struct rwkv_b200_adapter_tensor describes them. Returns the adapter handle."""
+        P = ctypes.POINTER(ctypes.c_float)
+        arr = (AdapterTensor * max(1, len(tensors)))()
+        keep = []
+        for i, (name, rank, a, b, values) in enumerate(tensors):
+            ptrs = []
+            for x in (a, b, values):
+                if x is None:
+                    ptrs.append(None)
+                else:
+                    x = np.ascontiguousarray(x, dtype=np.float32)
+                    keep.append(x)
+                    ptrs.append(x.ctypes.data_as(P))
+            arr[i] = AdapterTensor(name.encode("utf-8"), rank, *ptrs)
+        ptr = self.library.rwkv_b200_adapter_create(ctx.ptr, arr, len(tensors), ctypes.c_float(scale))
+        if not ptr:
+            raise ValueError(f"rwkv_b200_adapter_create failed (error flags 0x{self.rwkv_get_last_error(None):x}), check stderr")
+        return ptr
+
+    def rwkv_b200_adapter_free(self, adapter: int) -> None:
+        if not self.library.rwkv_b200_adapter_free(adapter):
+            raise ValueError("rwkv_b200_adapter_free failed: the adapter is still attached to a context")
+
+    def rwkv_b200_set_adapter(self, ctx: RWKVContext, adapter: Optional[int]) -> None:
+        if not self.library.rwkv_b200_set_adapter(ctx.ptr, adapter):
+            raise ValueError(f"rwkv_b200_set_adapter failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
 
     def rwkv_b200_init_from_file_ex(self, model_file_path: str, device: int, layer_begin: int = 0, layer_end: int = -1) -> RWKVContext:
         ptr = self.library.rwkv_b200_init_from_file_ex(model_file_path.encode("utf-8"), device, layer_begin, layer_end)

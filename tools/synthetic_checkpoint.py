@@ -76,3 +76,27 @@ def make_state_dict(kind: str, seed: int = 0):
     sd["ln_out.weight"] = 1 + n(C, scale=0.1); sd["ln_out.bias"] = n(C, scale=0.1)
     sd["head.weight"] = n(V, C, scale=C ** -0.5)
     return sd
+
+
+def make_lora_state_dict(kind: str, rank: int = 8, seed: int = 1):
+    """A seeded RWKV-PEFT-style LoRA checkpoint for make_state_dict(kind): `lora_A` [rank, in] / `lora_B` [out, rank] pairs on the
+    att and ffn layer matrices (`.lora_A.weight` naming on the ffn ones, as PEFT writes it), and trained copies of every layer's
+    ln1 / ln2, time_* (v4 .. v6: the v6 time_maa_w1 / time_decay_w1 / time_decay_w2 matrices included) or x_* / k_k and the att.w1
+    matrix (v7) parameters, moved by a small offset."""
+    base = make_state_dict(kind, seed=0)
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    for name, t in base.items():
+        if not name.startswith("blocks."):
+            continue
+        short = name.split(".", 2)[2]
+        if short in ("att.key.weight", "att.value.weight", "att.receptance.weight", "att.gate.weight", "att.output.weight",
+                     "ffn.key.weight", "ffn.value.weight", "ffn.receptance.weight"):
+            stem = name[: -len(".weight")]
+            suffix = ".weight" if short.startswith("ffn.") else ""
+            sd[stem + ".lora_A" + suffix] = torch.randn(rank, t.shape[1], generator=g) * t.shape[1] ** -0.5
+            sd[stem + ".lora_B" + suffix] = torch.randn(t.shape[0], rank, generator=g) * 0.05
+        elif short.startswith(("ln1.", "ln2.", "att.time_", "ffn.time_", "att.x_", "ffn.x_", "att.k_k")) or short == "att.w1":
+            small = short in ("att.time_maa_w1", "att.time_maa_w2", "att.time_decay_w1", "att.time_decay_w2", "att.w1")   # LoRA weights ~0.01
+            sd[name] = t + torch.randn(t.shape, generator=g) * (0.002 if small else 0.02)
+    return sd
