@@ -295,7 +295,24 @@ RWKV_API bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, 
  * callback (RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED).
  * The invariants of the unadapted context hold for an adapted one: a sequence gives the bits of serial evaluation under any chunking
  * of passes below 32 tokens, a batch row those of a single context below 16 sequences, device-side generation those of the host loop.
- * An adapter whose every B is zero and that replaces nothing gives exactly the unadapted logits and states. */
+ * An adapter whose every B is zero and that replaces nothing gives exactly the unadapted logits and states.
+ *
+ * rwkv_b200_batch_set_adapter gives sequence `sequence` of a batch context its own adapter, or puts it back on the base weights with
+ * adapter == NULL, for every pass enqueued after the call returns: rwkv_b200_batch_eval, _eval_sample, _eval_ragged,
+ * rwkv_b200_batch_score_ragged and every rwkv_b200_batch_generate* family, streaming included. Sequences may carry different adapters
+ * (of any ranks, scales and sets of adapted matrices), the same one, or none, in any mix; one pass over the base weights serves them
+ * all, and a row gives the bits of a single context with that row's adapter attached by rwkv_b200_set_adapter wherever a batch row
+ * gives those of a single context. The call waits for the context's queued work and drops its graphs, as rwkv_b200_set_adapter does;
+ * every sequence's state, logits column, penalty counts and automaton state are untouched. A batch context starts with no adapter on
+ * any sequence; rwkv_free releases its attachments, and an adapter held by any sequence is refused by rwkv_b200_adapter_free.
+ * Only an adapter made of low-rank deltas alone (every entry rank > 0) can be attached to a sequence: a replaced vector or matrix is
+ * read by kernels that take one pointer for every column of a pass (LayerNorm-mix, lerp, WKV, the head's LayerNorm, the GEMV itself).
+ * RWKV-LM-LoRA checkpoints trained with their `time` / `ln` parts carry such replacements; attach those with rwkv_b200_set_adapter.
+ * Refused, changing nothing: an ordinary context, a pipeline or a stage, and a call from inside that context's streaming callback
+ * (RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED); sequence >= n_sequences, an adapter of another model, an adapter that replaces a tensor,
+ * an adapter while the batch has one attached by rwkv_b200_set_adapter, and a 32nd distinct adapter on the batch's sequences
+ * (RWKV_ERROR_ARGS). While any sequence has its own adapter, rwkv_b200_set_adapter(batch, adapter) refuses a non-NULL adapter with
+ * RWKV_ERROR_ARGS. Detaching (NULL) is always accepted. */
 struct rwkv_b200_adapter;
 struct rwkv_b200_adapter_tensor {
     const char * name;        /* tensor name as in the model file */
@@ -307,6 +324,7 @@ struct rwkv_b200_adapter_tensor {
 RWKV_API struct rwkv_b200_adapter * rwkv_b200_adapter_create(struct rwkv_context * ctx, const struct rwkv_b200_adapter_tensor * t, size_t n, float scale);
 RWKV_API bool rwkv_b200_adapter_free(struct rwkv_b200_adapter * adapter);
 RWKV_API bool rwkv_b200_set_adapter(struct rwkv_context * ctx, const struct rwkv_b200_adapter * adapter);
+RWKV_API bool rwkv_b200_batch_set_adapter(struct rwkv_context * batch, size_t sequence, const struct rwkv_b200_adapter * adapter);
 
 /* Generation with log-probabilities: the loops above that also report, for every token they draw, how likely it was, as completion
  * servers (logprobs / top_logprobs), evaluation and RL callers need, without per-token logits crossing PCIe.
@@ -572,6 +590,13 @@ RWKV_API bool rwkv_b200_test_encode_rows(int data_type, const float * values, si
  * read by 6 only. u and y are guarded outputs. 1 <= T <= 256, 1 <= rank <= 256. */
 RWKV_API bool rwkv_b200_test_lora(int K, int M, int T, int rank, float scale, int epilogue, const float * a, const float * b, const float * x,
                                   const float * z, const float * gate, float * u, float * y);
+/* The same launches with a delta per column, as a batch context with adapters on its sequences runs them: n_adapters deltas (ranks[i],
+ * scales[i], a[i], b[i] as above), and column t takes delta col_adapter[t], or none with -1. u is [T][max rank] (column t at
+ * u + t * max rank); the rows of a column without a delta, and those past its delta's rank, are not written. A column without a delta
+ * gets y = epi(z) for the nonlinear epilogues and keeps y = z for the residual ones. 1 <= n_adapters <= 31. */
+RWKV_API bool rwkv_b200_test_lora_columns(int K, int M, int T, int n_adapters, const int * ranks, const float * scales, const float * const * a,
+                                          const float * const * b, const int * col_adapter, int epilogue, const float * x, const float * z,
+                                          const float * gate, float * u, float * y);
 
 /* x[:, t] = LN(emb[tokens[t]]; ln0). emb: n_vocab rows of emb_pitch bytes, F32 or F16 (emb_type 0 / 1). */
 RWKV_API bool rwkv_b200_test_embed_ln0(const void * emb, int emb_type, size_t emb_pitch, int n_vocab, const int * tokens, int T, int C,

@@ -105,6 +105,7 @@ Adapter * create_adapter(Model * model, const AdapterTensor * t, size_t n, float
             n_delta++;
         } else {
             RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, x.values, "Entry %zu: NULL values", e);
+            a->replaces = true;
             const size_t count = s.mat ? (size_t) s.mat->K * (size_t) s.mat->M : s.vec->n;
             // a matrix stored in fp16, or quantized with fp16 block scales, must be finite in fp16 (|v| < 65520)
             const bool f16_values = s.mat && s.mat->type != DT_F32;

@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -712,7 +713,25 @@ bool rwkv_b200_set_adapter(struct rwkv_context * ctx, const struct rwkv_b200_ada
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, !c->group && c->model->layer_begin == 0 && c->model->layer_end == c->model->n_layer,
                "Adapters serve whole-model and batch contexts, not a pipeline or one of its stages");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !adapter || adapter->model == c->model, "The adapter belongs to another model");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !adapter || c->seq_adapters.empty(),
+               "Sequences of this batch carry their own adapters; detach them with rwkv_b200_batch_set_adapter first");
     return set_adapter(c, adapter);
+}
+
+bool rwkv_b200_batch_set_adapter(struct rwkv_context * batch, size_t sequence, const struct rwkv_b200_adapter * adapter) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0 && !c->group, "Not a batch context; use rwkv_b200_set_adapter");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, sequence < (size_t) c->batch_n, "Sequence %zu is out of range (0 .. %d)", sequence, c->batch_n - 1);
+    if (adapter) {
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, adapter->model == c->model, "The adapter belongs to another model");
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !adapter->replaces,
+                   "The adapter replaces tensors, which every column of a pass shares; attach it to the whole context with rwkv_b200_set_adapter");
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !c->adapter, "The batch has an adapter of its own; detach it with rwkv_b200_set_adapter first");
+    }
+    return batch_set_adapter(c, (int) sequence, adapter);
 }
 
 bool rwkv_b200_generate_constrained(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state, size_t max_tokens,
@@ -1325,13 +1344,17 @@ bool rwkv_b200_test_lora(int K, int M, int T, int rank, float scale, int epilogu
     for (size_t i = 0; i < ha.size(); i++) ha[i] = fp32_to_fp16(a[i]);
     for (size_t r = 0; r < R; r++) for (size_t i = 0; i < (size_t) M; i++) hbt[r * M + i] = fp32_to_fp16(b[i * R + r]);
     HookBuffers hb;
-    LoraBatch lb{};
-    lb.n = 1; lb.T = T;
+    std::unique_ptr<LoraBatch> lbp(new LoraBatch());
+    LoraBatch & lb = *lbp;
+    lb.n = 1; lb.T = T; lb.n_groups = 1;
     LoraProblem & l = lb.p[0];
-    l.d.A = hb.in(ha.data(), ha.size()); l.d.Bt = hb.in(hbt.data(), hbt.size()); l.d.rank = rank; l.d.scale = scale;
+    LoraGroup & g = lb.g[0];
+    g.d.A = hb.in(ha.data(), ha.size()); g.d.Bt = hb.in(hbt.data(), hbt.size()); g.d.rank = rank; g.d.scale = scale;
+    g.problem = 0; g.col0 = 0; g.n_cols = T;
+    for (int t = 0; t < T; t++) lb.col[t] = (uint8_t) t;
     l.K = K; l.M = M;
     l.x = hb.in(x, (size_t) K * T); l.ldx = K;
-    l.u = hb.out(u, R * T);
+    l.u = hb.out(u, R * T); l.ldu = rank;
     l.P.epi = epilogue; l.P.ldy = M;
     const bool residual = epilogue == EPI_ADD || epilogue == EPI_MUL_ADD;
     if (residual) {
@@ -1346,6 +1369,65 @@ bool rwkv_b200_test_lora(int K, int M, int T, int rank, float scale, int epilogu
     if (hb.ok) e = launch_lora_shrink(lb, 0);
     if (hb.ok && e == cudaSuccess) e = launch_lora_expand(lb, 0);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, hb.finish(e), "lora failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    return true;
+}
+
+bool rwkv_b200_test_lora_columns(int K, int M, int T, int n_adapters, const int * ranks, const float * scales, const float * const * a,
+                                 const float * const * b, const int * col_adapter, int epilogue, const float * x, const float * z,
+                                 const float * gate, float * u, float * y) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    const bool epi_ok = epilogue == EPI_NONE || epilogue == EPI_SIGMOID || epilogue == EPI_SILU || epilogue == EPI_RELU_SQR || epilogue == EPI_ADD ||
+                        epilogue == EPI_MUL_ADD;
+    bool args = ranks && scales && a && b && col_adapter && x && z && u && y && K > 0 && M > 0 && T >= 1 && T <= MAX_TOKENS_PER_PASS &&
+                n_adapters >= 1 && n_adapters <= LORA_MAX_ADAPTERS && epi_ok && (epilogue != EPI_MUL_ADD || gate);
+    int max_rank = 0;
+    for (int i = 0; args && i < n_adapters; i++) {
+        args = a[i] && b[i] && ranks[i] >= 1 && ranks[i] <= LORA_MAX_RANK;
+        if (args) max_rank = std::max(max_rank, ranks[i]);
+    }
+    for (int t = 0; args && t < T; t++) args = col_adapter[t] >= -1 && col_adapter[t] < n_adapters;
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid lora_columns arguments");
+    if (!hook_device(sink)) return false;
+    HookBuffers hb;
+    std::unique_ptr<LoraBatch> lbp(new LoraBatch());
+    LoraBatch & lb = *lbp;
+    lb.n = 1; lb.T = T; lb.n_groups = 0;
+    const bool residual = epilogue == EPI_ADD || epilogue == EPI_MUL_ADD;
+    // the groups as the engine builds them: one per adapter with columns, then the columns without one (a nonlinear epilogue only)
+    int n_col = 0;
+    for (int k = 0; k <= n_adapters; k++) {
+        const int id = k < n_adapters ? k : -1;
+        int n = 0;
+        for (int t = 0; t < T; t++) n += col_adapter[t] == id;
+        if (!n || (id < 0 && residual)) continue;
+        LoraGroup & g = lb.g[lb.n_groups++];
+        g.problem = 0; g.col0 = n_col; g.n_cols = n;
+        for (int t = 0; t < T; t++) if (col_adapter[t] == id) lb.col[n_col++] = (uint8_t) t;
+        if (id < 0) continue;
+        const size_t R = (size_t) ranks[k];
+        std::vector<uint16_t> ha(R * (size_t) K), hbt(R * (size_t) M);
+        for (size_t i = 0; i < ha.size(); i++) ha[i] = fp32_to_fp16(a[k][i]);
+        for (size_t r = 0; r < R; r++) for (size_t i = 0; i < (size_t) M; i++) hbt[r * M + i] = fp32_to_fp16(b[k][i * R + r]);
+        g.d.A = hb.in(ha.data(), ha.size()); g.d.Bt = hb.in(hbt.data(), hbt.size()); g.d.rank = ranks[k]; g.d.scale = scales[k];
+    }
+    LoraProblem & l = lb.p[0];
+    l.K = K; l.M = M;
+    l.x = hb.in(x, (size_t) K * T); l.ldx = K;
+    l.u = hb.out(u, (size_t) max_rank * T); l.ldu = max_rank;
+    l.P.epi = epilogue; l.P.ldy = M;
+    if (residual) {
+        l.P.y = hb.inout(z, y, (size_t) M * T);
+        l.P.res = l.P.y; l.P.ldres = M;
+        if (epilogue == EPI_MUL_ADD) { l.P.gate = hb.in(gate, (size_t) M * T); l.P.ldgate = M; }
+    } else {
+        l.z = hb.in(z, (size_t) M * T); l.ldz = M;
+        l.P.y = hb.out(y, (size_t) M * T);
+    }
+    cudaError_t e = cudaSuccess;
+    if (hb.ok) e = launch_lora_shrink(lb, 0);
+    if (hb.ok && e == cudaSuccess) e = launch_lora_expand(lb, 0);
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, hb.finish(e), "lora_columns failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     return true;
 }
 

@@ -112,6 +112,7 @@ struct Pass {
     float * hidden_out = nullptr;
     // a ragged pass: its device map (Context::ragged_map), and how many sequences advance (the head's columns)
     const int * seq_off = nullptr, * col_seq = nullptr, * head_col = nullptr, * head_seq = nullptr;
+    const int * col_seq_host = nullptr;   // ... and the host copy of col_seq (the pinned slot it is uploaded from); NULL: column t is sequence t
     int n_active = 0;
     // a scoring pass: the targets of its columns and where their results go (greedy may be NULL)
     const uint32_t * targets = nullptr;
@@ -123,9 +124,11 @@ struct Pass {
 struct Batch {
     GemvBatch b;
     const LoraDelta * lora[GEMV_MAX_PROBLEMS] = {};   // the delta of each problem's matrix under the attached adapter, or NULL
+    const DevMatrix * mat[GEMV_MAX_PROBLEMS] = {};    // each problem's matrix, in the table the pass reads
     explicit Batch(int T) { memset(&b, 0, sizeof(b)); b.T = T; }
     GemvProblem & add(const DevMatrix & W, const float * x, float * y, int epi = EPI_NONE) {
         lora[b.n] = W.lora;
+        mat[b.n] = &W;
         GemvProblem & p = b.p[b.n++];
         p.W = W.data; p.Wt = W.tiled; p.pitch = W.pitch; p.type = W.type; p.K = W.K; p.M = W.M;
         p.x = x; p.ldx = W.K;
@@ -184,28 +187,80 @@ bool run_base(Context * ctx, const Pass & p, Batch & batch) {
     return true;
 }
 
+// The delta of matrix W of the model's layer table in adapter a's table (the same slot of a copy of that table), or NULL. Matrices outside
+// the layers (the head) take none.
+const LoraDelta * delta_in(const Model & m, const Adapter & a, const DevMatrix & W) {
+    const uintptr_t base = reinterpret_cast<uintptr_t>(m.layers.data()), w = reinterpret_cast<uintptr_t>(&W);
+    if (w < base || w - base >= m.layers.size() * sizeof(Layer)) return nullptr;
+    return reinterpret_cast<const DevMatrix *>(reinterpret_cast<const unsigned char *>(a.layers.data()) + (w - base))->lora;
+}
+
 // A batch with low-rank deltas (kernels/lora.h): the shrink of every adapted problem, the batch through its unchanged route with the
 // adapted problems of nonlinear epilogue retargeted to EPI_NONE into lora_z, then the expand. Problems without a delta stay as they were.
+// The columns of a problem are grouped by delta: all of them under the context's adapter; under per-sequence adapters (a batch context)
+// one group per distinct adapter that adapts the matrix and has columns in the pass, plus, for a retargeted problem, one group of rank 0
+// with the columns left, which the expand passes through the epilogue. A problem with no column under a delta is not adapted at all.
 bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
     LoraBatch lb;
-    lb.n = 0; lb.T = batch.b.T;
+    const int T = batch.b.T;
+    lb.n = 0; lb.T = T; lb.n_groups = 0;
     float * u = ctx->lora_u, * z = ctx->lora_z;
+    int n_col = 0;
+    const int n_ad = (int) ctx->seq_adapters.size();
     for (int i = 0; i < batch.b.n; i++) {
-        if (!batch.lora[i]) continue;
         GemvProblem & q = batch.b.p[i];
-        LoraProblem & l = lb.p[lb.n++];
-        l.d = *batch.lora[i];
+        const bool residual = q.epi == EPI_ADD || q.epi == EPI_MUL_ADD;
+        const LoraDelta * d[LORA_MAX_ADAPTERS + 1];     // the delta of each slot's adapter; slot n_ad: the columns without one
+        int slot_cols[LORA_MAX_ADAPTERS + 1] = {};
+        int slot[LORA_MAX_T];
+        if (n_ad == 0) {
+            if (!batch.lora[i]) continue;
+            d[0] = batch.lora[i];
+            for (int t = 0; t < T; t++) slot[t] = 0;
+            slot_cols[0] = T;
+        } else {
+            // only layer matrices carry deltas, and their batches have the pass's columns
+            bool any = false;
+            for (int k = 0; k < n_ad; k++) any = (d[k] = delta_in(*ctx->model, *ctx->seq_adapters[k], *batch.mat[i])) || any;
+            if (!any) continue;
+            RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, T == p.T, "A batch of %d columns in a pass of %d carries deltas", T, p.T);
+            d[n_ad] = nullptr;
+            bool adapted = false;
+            for (int t = 0; t < T; t++) {
+                const int k = ctx->seq_slot[p.col_seq_host ? p.col_seq_host[t] : t];
+                slot[t] = k >= 0 && d[k] ? k : n_ad;
+                slot_cols[slot[t]]++;
+                adapted = adapted || slot[t] < n_ad;
+            }
+            if (!adapted) continue;
+        }
+        const int n_slots = n_ad == 0 ? 1 : n_ad + 1;
+        int ldu = 0, groups = 0;
+        for (int k = 0; k < n_slots; k++)
+            if (slot_cols[k] && (d[k] || !residual)) { groups++; if (d[k]) ldu = std::max(ldu, d[k]->rank); }
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, lb.n_groups + groups <= LORA_MAX_GROUPS, "Too many delta groups in one launch");
+        const int pi = lb.n++;
+        LoraProblem & l = lb.p[pi];
+        for (int k = 0; k < n_slots; k++) {
+            if (!slot_cols[k] || (!d[k] && residual)) continue;
+            LoraGroup & g = lb.g[lb.n_groups++];
+            g.d = d[k] ? *d[k] : LoraDelta{};
+            g.problem = pi;
+            g.col0 = n_col; g.n_cols = 0;
+            for (int t = 0; t < T; t++) if (slot[t] == k) lb.col[n_col + g.n_cols++] = (uint8_t) t;
+            n_col += g.n_cols;
+        }
         l.K = q.K; l.M = q.M;
         l.x = q.x; l.ldx = q.ldx;
-        l.u = u; u += (size_t) l.d.rank * lb.T;
+        l.u = u; l.ldu = ldu; u += (size_t) ldu * T;
         l.P = q;
-        if (q.epi == EPI_ADD || q.epi == EPI_MUL_ADD) {      // residual epilogues: the base writes y, the expand adds to it
+        if (residual) {      // residual epilogues: the base writes y, the expand adds to it
             l.z = nullptr; l.ldz = 0;
             l.P.res = q.y; l.P.ldres = q.ldy;
         } else {
             l.z = z; l.ldz = q.M;
             q.y = z; q.ldy = q.M; q.epi = EPI_NONE; q.res = q.gate = q.bias = nullptr;
-            z += (size_t) q.M * lb.T;
+            z += (size_t) q.M * T;
         }
     }
     if (lb.n) CUDA_OK(ctx, launch_lora_shrink(lb, p.stream));
@@ -781,6 +836,7 @@ void destroy_context(Context * ctx) {
     cudaFree(ctx->state_a); cudaFree(ctx->state_b); cudaFree(ctx->state_init); cudaFree(ctx->logits);
     cudaFree(ctx->tokens); cudaFree(ctx->scratch); cudaFree(ctx->trace_buf); cudaFree(ctx->act16); cudaFree(ctx->xq);
     if (ctx->adapter) ctx->adapter->attached.fetch_sub(1);
+    for (const Adapter * a : ctx->seq_adapter) if (a) a->attached.fetch_sub(1);
     cudaFree(ctx->lora_u); cudaFree(ctx->lora_z);
     for (int i = 0; i < 2; i++) {
         if (ctx->tokens_host[i]) cudaFreeHost(ctx->tokens_host[i]);
@@ -1169,6 +1225,7 @@ static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t *
     }
     p.seq_off = ctx->ragged_map;
     p.col_seq = p.seq_off + B + 1;
+    p.col_seq_host = col_seq;
     p.head_col = p.col_seq + MAX_TOKENS_PER_PASS;
     p.head_seq = p.head_col + B;
     p.targets = targets; p.lp = lp; p.greedy = greedy;
@@ -1647,27 +1704,67 @@ void drop_generate_graphs(Context * ctx) {
         for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
 }
 
+namespace {
+
+// The scratch of the deltas (Context::lora_u / lora_z), allocated once for passes of up to MAX_TOKENS_PER_PASS columns.
+bool ensure_lora_scratch(Context * ctx) {
+    if (ctx->lora_u) return true;
+    const Dims d = model_dims(*ctx->model);
+    const size_t z_rows = std::max(4 * d.C, d.F + d.C), T = MAX_TOKENS_PER_PASS;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), (size_t) GEMV_MAX_PROBLEMS * LORA_MAX_RANK * T * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), z_rows * T * sizeof(float));
+    if (e != cudaSuccess) {
+        cudaFree(ctx->lora_u); cudaFree(ctx->lora_z); ctx->lora_u = ctx->lora_z = nullptr;
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, false, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));
+    }
+    return true;
+}
+
+// The captured passes hold the tensors and launches of the adapters they were captured with.
+void drop_all_graphs(Context * ctx) {
+    for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
+    drop_generate_graphs(ctx);
+}
+
+}  // namespace
+
 bool set_adapter(Context * ctx, const Adapter * a) {
     if (a == ctx->adapter) return true;
     const Model & m = *ctx->model;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    if (a && !ctx->lora_u) {
-        const Dims d = model_dims(m);
-        const size_t z_rows = std::max(4 * d.C, d.F + d.C), T = MAX_TOKENS_PER_PASS;
-        cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), (size_t) GEMV_MAX_PROBLEMS * LORA_MAX_RANK * T * sizeof(float));
-        if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), z_rows * T * sizeof(float));
-        if (e != cudaSuccess) {
-            cudaFree(ctx->lora_u); cudaFree(ctx->lora_z); ctx->lora_u = ctx->lora_z = nullptr;
-            RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, false, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));
-        }
-    }
-    // the captured passes hold the tensors and launches of the adapter they were captured with
-    for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
-    drop_generate_graphs(ctx);
+    if (a && !ensure_lora_scratch(ctx)) return false;
+    drop_all_graphs(ctx);
     if (a) a->attached.fetch_add(1);
     if (ctx->adapter) ctx->adapter->attached.fetch_sub(1);
     ctx->adapter = a;
+    return true;
+}
+
+bool batch_set_adapter(Context * ctx, int seq, const Adapter * a) {
+    const Adapter * old = ctx->seq_adapter.empty() ? nullptr : ctx->seq_adapter[seq];
+    if (a == old) return true;
+    std::vector<const Adapter *> next = ctx->seq_adapter.empty() ? std::vector<const Adapter *>(ctx->batch_n, nullptr) : ctx->seq_adapter;
+    next[seq] = a;
+    std::vector<const Adapter *> distinct;
+    std::vector<int> slot(ctx->batch_n, -1);
+    for (int b = 0; b < ctx->batch_n; b++) {
+        if (!next[b]) continue;
+        const auto it = std::find(distinct.begin(), distinct.end(), next[b]);
+        slot[b] = (int) (it - distinct.begin());
+        if (it == distinct.end()) distinct.push_back(next[b]);
+    }
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, distinct.size() <= (size_t) LORA_MAX_ADAPTERS,
+               "A batch context carries at most %d distinct adapters on its sequences", LORA_MAX_ADAPTERS);
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (a && !ensure_lora_scratch(ctx)) return false;
+    drop_all_graphs(ctx);
+    if (a) a->attached.fetch_add(1);
+    if (old) old->attached.fetch_sub(1);
+    ctx->seq_adapter = std::move(next);
+    ctx->seq_adapters = std::move(distinct);
+    ctx->seq_slot = std::move(slot);
     return true;
 }
 

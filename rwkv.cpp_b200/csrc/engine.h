@@ -37,7 +37,8 @@ struct Adapter {
     DevVec ln0_w, ln0_b, ln_out_w, ln_out_b;
     std::vector<LoraDelta> deltas;       // DevMatrix::lora points into it
     uint8_t * arena = nullptr;           // A, B and the replacements
-    mutable std::atomic<int> attached{0};   // contexts that have it attached
+    bool replaces = false;               // some entry is a replacement (rank 0): it cannot be attached to one sequence of a batch
+    mutable std::atomic<int> attached{0};   // contexts, and sequences of batch contexts, that have it attached
 };
 // M rows of K values in the file layout of `type`, as a replaced matrix is encoded before its upload: F32 copied, F16 rounded, the
 // other types by quantize_row. `out` has M * tensor_nbytes(type, K, 1, 1) bytes.
@@ -180,6 +181,10 @@ struct Context {
     // outputs z of a batch's adapted problems with a nonlinear epilogue, max(4 C, F + C) rows of T.
     const Adapter * adapter = nullptr;
     float * lora_u = nullptr, * lora_z = nullptr;
+    // A batch context's adapters per sequence (batch_set_adapter): seq_adapter [batch_n] (NULL: the base weights), empty until the first
+    // attach; the distinct adapters among them (at most LORA_MAX_ADAPTERS), and each sequence's index into that list or -1.
+    std::vector<const Adapter *> seq_adapter, seq_adapters;
+    std::vector<int> seq_slot;
 
     float last_device_ms = 0.f;      // CUDA-event time of the last forward (kernels only)
     int last_error = 0;              // rwkv_error_flags
@@ -337,6 +342,10 @@ void drop_generate_graphs(Context * ctx);
 // Attaches `a` (NULL: detaches), dropping the single-token and generation graphs; the state is untouched. The caller has checked the
 // context and that `a` belongs to its model.
 bool set_adapter(Context * ctx, const Adapter * a);
+// Gives sequence `seq` of a batch context adapter `a` (NULL: the base weights), with the same waits and dropped graphs as set_adapter.
+// The caller has checked the context, the sequence, that `a` belongs to its model, replaces nothing and that the context has no
+// adapter of its own; this checks the number of distinct adapters.
+bool batch_set_adapter(Context * ctx, int seq, const Adapter * a);
 
 size_t stage_hidden_len(const Model & m, size_t T);
 

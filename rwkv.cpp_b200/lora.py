@@ -9,6 +9,11 @@ A checkpoint holds, per adapted layer matrix `blocks.N.att.key.weight`, the pair
 such as `time_*` and `ln*`, which replace the model's. The replacements go through the converter's rewrites
 (convert_pytorch_to_ggml.transform_tensor), so they reach the library in the file's element order. Every delta gets the scale
 lora_alpha / rank * scale, so all deltas of a checkpoint must share one rank. A key that cannot be placed is an error.
+
+An adapter made of deltas alone can also be attached to single sequences of a batch context, so that one pass over the base weights
+serves several fine-tunes (rwkv_b200_batch_set_adapter). An adapter with replacements cannot: a replaced vector or matrix is read by
+kernels that take one pointer for every column of a pass. Checkpoints trained with RWKV-LM-LoRA's `time` / `ln` parts carry such
+replacements; attach those to a whole context with set_adapter.
 """
 from typing import Dict, List, Optional, Tuple
 

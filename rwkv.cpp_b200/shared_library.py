@@ -226,6 +226,12 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_adapter_free.restype = ctypes.c_bool
         lib.rwkv_b200_set_adapter.argtypes = [vp, vp]
         lib.rwkv_b200_set_adapter.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_set_adapter.argtypes = [vp, ctypes.c_size_t, vp]
+        lib.rwkv_b200_batch_set_adapter.restype = ctypes.c_bool
+        P_INT = ctypes.POINTER(ctypes.c_int)
+        lib.rwkv_b200_test_lora_columns.argtypes = [ctypes.c_int] * 4 + [P_INT, P_FLOAT, ctypes.POINTER(P_FLOAT), ctypes.POINTER(P_FLOAT), P_INT,
+                                                                          ctypes.c_int] + [P_FLOAT] * 5
+        lib.rwkv_b200_test_lora_columns.restype = ctypes.c_bool
         lib.rwkv_b200_test_lora.argtypes = [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int] + [P_FLOAT] * 7
         lib.rwkv_b200_test_lora.restype = ctypes.c_bool
         lib.rwkv_b200_test_encode_rows.argtypes = [ctypes.c_int, P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p]
@@ -375,6 +381,12 @@ class RWKVSharedLibrary:
     def rwkv_b200_set_adapter(self, ctx: RWKVContext, adapter: Optional[int]) -> None:
         if not self.library.rwkv_b200_set_adapter(ctx.ptr, adapter):
             raise ValueError(f"rwkv_b200_set_adapter failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+
+    def rwkv_b200_batch_set_adapter(self, batch: RWKVContext, sequence: int, adapter: Optional[int]) -> None:
+        """Runs sequence `sequence` of a batch context with `adapter` (None: the base weights) on every later pass. Only adapters made of
+        low-rank deltas alone can be attached to a sequence."""
+        if not self.library.rwkv_b200_batch_set_adapter(batch.ptr, sequence, adapter):
+            raise ValueError(f"rwkv_b200_batch_set_adapter failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
 
     def rwkv_b200_init_from_file_ex(self, model_file_path: str, device: int, layer_begin: int = 0, layer_end: int = -1) -> RWKVContext:
         ptr = self.library.rwkv_b200_init_from_file_ex(model_file_path.encode("utf-8"), device, layer_begin, layer_end)
