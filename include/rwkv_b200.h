@@ -413,6 +413,67 @@ RWKV_API bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, cons
                                                size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
                                                const struct rwkv_b200_logprobs * lp /* NULL = none */);
 
+/* Beam search: the most likely continuations under the model rather than a sample (translation, extraction, n-best lists for
+ * reranking), searched on the device in one graph launch: the beams are the sequences of a batch context, and moving a beam to another
+ * slot copies its state in HBM. Only the back-pointers and the finished hypotheses cross PCIe.
+ * 1. Width and root. The width W is the batch context's n_sequences, 1 <= W <= RWKV_B200_BEAM_MAX. The search starts from sequence 0:
+ *    its resident state and its logits column, which must be valid. Below 16 sequences every pass runs the multi-column GEMV, so a slot
+ *    gives the bits of a single context.
+ * 2. The log-probability of token t in a column z is lp = log_softmax(z)[t] in float32, bit for bit what rwkv_b200_score_logits
+ *    returns. A hypothesis's score is the sum of its tokens' lp in double, in token order. A token with a non-finite lp is never a
+ *    candidate, so a column with a NaN or +inf gives none.
+ * 3. Step i = 0 .. max_tokens - 1 (only the root is live at step 0):
+ *    - every live beam contributes its top 2W tokens, in the order of the logprob calls' top entries (larger logit first, the smaller id
+ *      first among equal logits), each with score = the beam's score + lp;
+ *    - all candidates are ranked by score, descending; ties go to the lower beam slot, then to the earlier top-2W position;
+ *    - the ranking is walked in order until W live beams are taken, the pool of finished hypotheses holds W, or the list ends: a stop
+ *      id goes to the pool (reported, never evaluated, as in rwkv_b200_generate), any other candidate becomes live beam k in slot k, in
+ *      the order taken. The pool never holds more than W hypotheses, and nothing is dropped from it;
+ *    - with L live beams taken, every slot k < L gets the state of its parent's slot and its token is evaluated, all in one batch pass
+ *      with logits. A step with L = 0 evaluates nothing;
+ *    - the search ends after that step if the pool holds W hypotheses, if i + 1 == max_tokens, or if L == 0.
+ * 4. The normalised score of a hypothesis is score / pow(length, length_penalty) in double; the length counts its tokens, a stop id
+ *    included.
+ * 5. Results: the pool's hypotheses in the order added, then the live beams of the last step in slot order, stably sorted by normalised
+ *    score, descending. The first n_best (1 <= n_best <= W) are written to row r of tokens_out ([n_best][max_tokens], 0 past the length),
+ *    lengths_out, scores_out (the raw sum of log-probabilities) and finished_out (1: ended on a stop id; may be NULL). Fewer than n_best
+ *    hypotheses exist only when a step took no live beam; the remaining rows get length 0, score -inf and finished 0.
+ * 6. Afterwards, for each slot k < L of the last step with L > 0, slot k holds the state after that live beam's tokens and the logits
+ *    of its last token, so rwkv_b200_batch_generate* can continue from any of them. A final step with L = 0 changes no slot. Every
+ *    other slot's state and logits column is unspecified. Penalty counts and automaton states are untouched.
+ * 7. W = 1 is greedy decoding: on finite logits it returns the tokens, state and logits of rwkv_b200_generate at temperature 0 with the
+ *    same stop ids and max_tokens.
+ * Every argument is checked before anything is enqueued, and a refused call changes nothing: an ordinary context, a pipeline or a stage,
+ * a call from inside that context's streaming callback and a driver without conditional graph nodes give RWKV_ERROR_CTX |
+ * RWKV_ERROR_UNSUPPORTED; NULL output arrays, W or n_best out of range, max_tokens 0 or above RWKV_B200_GENERATE_MAX, a non-finite
+ * length_penalty, more than RWKV_B200_GENERATE_MAX_STOP stop ids or an id >= n_vocab, invalid logits, n_vocab > 65536, and a sequence
+ * holding its own adapter from rwkv_b200_batch_set_adapter (beams move between slots; a context-wide adapter is fine) give
+ * RWKV_ERROR_ARGS. The first call allocates the search state (about 2 KB, the logits of one pass, and max_tokens * W * 8 bytes of
+ * back-pointers on the device and pinned, grown to the largest call); contexts that never search allocate nothing. */
+#define RWKV_B200_BEAM_MAX 10
+RWKV_API bool rwkv_b200_beam_search(struct rwkv_context * batch, size_t max_tokens, float length_penalty, const uint32_t * stop_ids, size_t n_stop,
+                                    size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out);
+/* Test hook: one step of the beam search kernel (rule 3 above, without the pass) on host logits, no model needed. Live beam k < n_live
+ * has logits row k of [n_live][n_vocab] and score scores[k]; the pool already holds n_pool < width hypotheses. Returns the live beams
+ * the walk took (slot k's parent beam, token and score, k < *n_live_out) and the hypotheses it added to the pool (entries n_pool ..
+ * *n_pool_out - 1 of the pool arrays). Arguments are checked before a device is touched. */
+struct rwkv_b200_beam_step_args {
+    const float * logits;                      /* [n_live][n_vocab] */
+    size_t width, n_vocab;                     /* 1 .. RWKV_B200_BEAM_MAX, 1 .. 65536 */
+    size_t n_live;                             /* 1 .. width */
+    const double * scores;                     /* [n_live], finite */
+    size_t n_pool;                             /* 0 .. width - 1 */
+    const uint32_t * stop_ids;
+    size_t n_stop;
+    uint32_t * n_live_out;
+    uint32_t * parents, * tokens;              /* [width] */
+    double * scores_out;                       /* [width] */
+    uint32_t * n_pool_out;
+    uint32_t * pool_parents, * pool_tokens;    /* [width] */
+    double * pool_scores;                      /* [width] */
+};
+RWKV_API bool rwkv_b200_test_beam_step(const struct rwkv_b200_beam_step_args * a);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each

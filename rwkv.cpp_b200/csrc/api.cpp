@@ -3,6 +3,7 @@
 // (rwkv.cpp:71-258, rwkv_eval.inc:38-241) so its C tests run unchanged against this library.
 #include <algorithm>
 #include <cinttypes>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -783,6 +784,75 @@ bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct 
     return generate_batch(batch, max_tokens, nullptr, nullptr, nullptr, nullptr, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token != nullptr,
                           on_token, user, automata != nullptr, reinterpret_cast<const Automaton * const *>(automata), automaton_states, lp != nullptr, lp,
                           true, samplers);
+}
+
+static_assert(RWKV_B200_BEAM_MAX == BEAM_MAX && 2 * BEAM_MAX <= GEN_TOP_MAX, "beam width of the header and the kernel");
+
+bool rwkv_b200_beam_search(struct rwkv_context * batch, size_t max_tokens, float length_penalty, const uint32_t * stop_ids, size_t n_stop,
+                           size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    const Model & m = *c->model;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0 && !c->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Beam search runs on a batch context, not on an ordinary context, a pipeline or one of its stages");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens_out && lengths_out && scores_out, "NULL tokens_out, lengths_out or scores_out");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->batch_n <= RWKV_B200_BEAM_MAX, "The beam width (the batch's %d sequences) must be at most %d",
+               c->batch_n, RWKV_B200_BEAM_MAX);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_best >= 1 && n_best <= (size_t) c->batch_n, "n_best must be in 1 .. %d", c->batch_n);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX, "max_tokens must be in 1 .. %d",
+               RWKV_B200_GENERATE_MAX);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, std::isfinite(length_penalty), "length_penalty must be finite");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_stop <= (size_t) RWKV_B200_GENERATE_MAX_STOP && (n_stop == 0 || stop_ids), "At most %d stop ids, not NULL",
+               RWKV_B200_GENERATE_MAX_STOP);
+    for (size_t k = 0; k < n_stop; k++)
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, stop_ids[k] < (uint32_t) m.n_vocab, "Stop id %u is out of range", stop_ids[k]);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->logits_valid, "No logits to search from: the last evaluation skipped the head");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, std::none_of(c->seq_adapter.begin(), c->seq_adapter.end(), [](const Adapter * a) { return a != nullptr; }),
+               "A sequence of this batch holds its own adapter; beams move between sequences, so only a context-wide adapter applies");
+    return beam_search(c, max_tokens, length_penalty, stop_ids, n_stop, n_best, tokens_out, lengths_out, scores_out, finished_out);
+}
+
+bool rwkv_b200_test_beam_step(const struct rwkv_b200_beam_step_args * a) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->scores && a->width >= 1 && a->width <= (size_t) RWKV_B200_BEAM_MAX && a->n_vocab >= 1 &&
+               a->n_vocab <= 65536 && a->n_live >= 1 && a->n_live <= a->width && a->n_pool < a->width && a->n_live_out && a->parents && a->tokens &&
+               a->scores_out && a->n_pool_out && a->pool_parents && a->pool_tokens && a->pool_scores, "Invalid beam-step arguments");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->n_stop <= (size_t) GENERATE_MAX_STOP && (a->n_stop == 0 || a->stop_ids), "At most %d stop ids, not NULL",
+               GENERATE_MAX_STOP);
+    for (size_t k = 0; k < a->n_live; k++) RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, std::isfinite(a->scores[k]), "Score of beam %zu is not finite", k);
+    if (!hook_device(sink)) return false;
+    const size_t W = a->width, V = a->n_vocab;
+    BeamState st{};
+    for (size_t k = 0; k < a->n_stop; k++) st.stop[k] = a->stop_ids[k];
+    st.n_stop = (uint32_t) a->n_stop; st.width = (uint32_t) W; st.max_tokens = 1;
+    st.n_live = (uint32_t) a->n_live; st.n_pool = (uint32_t) a->n_pool;
+    for (size_t k = 0; k < a->n_live; k++) st.score[k] = a->scores[k];
+    HookBuffers hb;
+    BeamStepParams p{};
+    p.logits = hb.in(a->logits, a->n_live * V); p.n_vocab = (int) V; p.width = (int) W;
+    p.st = const_cast<BeamState *>(hb.in(&st, 1));
+    p.back = static_cast<uint32_t *>(hb.alloc(W * 2 * sizeof(uint32_t)));
+    p.next_tokens = static_cast<int *>(hb.alloc(W * sizeof(int)));
+    std::vector<uint32_t> back(2 * W);
+    std::vector<int> next(W);
+    const bool ok = hb.ok && hb.finish(launch_beam_step(p, 0)) && cudaMemcpy(&st, p.st, sizeof(BeamState), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                    cudaMemcpy(back.data(), p.back, back.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                    cudaMemcpy(next.data(), p.next_tokens, W * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "beam step failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
+    *a->n_live_out = st.n_live;
+    for (size_t k = 0; k < st.n_live; k++) {
+        a->parents[k] = back[2 * k]; a->tokens[k] = back[2 * k + 1]; a->scores_out[k] = st.score[k];
+        RWKV_CHECK(sink, RWKV_ERROR_CTX, false, next[k] == (int) back[2 * k + 1], "The next input token of slot %zu is not its token", k);
+    }
+    for (size_t k = st.n_live; k < W; k++) RWKV_CHECK(sink, RWKV_ERROR_CTX, false, next[k] == 0, "The next input token of idle slot %zu is not 0", k);
+    *a->n_pool_out = st.n_pool;
+    for (size_t q = a->n_pool; q < st.n_pool; q++) {
+        a->pool_parents[q] = st.pool[q].parent; a->pool_tokens[q] = st.pool[q].token; a->pool_scores[q] = st.pool[q].score;
+    }
+    return true;
 }
 
 static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");

@@ -330,4 +330,42 @@ cudaError_t add_generate_sampled_step_node(cudaGraph_t g, const cudaGraphNode_t 
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);
 
+// Beam search (rwkv_b200_beam_search, beam.cu) over the width W sequences of a batch context, W <= BEAM_MAX. One step: CTA k < n_live
+// lists live beam k's top 2W tokens in the logprob kernels' top-N order (top_n.cuh) with their log-probabilities (score_row.cuh); the
+// last CTA ranks every candidate with a finite log-probability by score = beam score + lp (double; ties: lower beam, then earlier
+// position), walks the ranking until W live beams are taken, the pool holds W hypotheses or the list ends (a stop id goes to the pool,
+// any other token becomes live slot L in the order taken), records slot L's parent and token at back[step][L], writes the next input
+// tokens (0 past L) and, inside the loop's graph, sets run_pass = L > 0 and keep_going = L > 0 && pool < W && step + 1 < max_tokens.
+constexpr int BEAM_MAX = 10;
+constexpr int BEAM_CANDS = 2 * BEAM_MAX;
+struct BeamHyp {                      // a finished hypothesis: stop id `token` drawn at `step` from live beam `parent` of the step before
+    double score;
+    uint32_t step, parent, token, pad;
+};
+struct BeamState {                    // written by the host per call (n_live = 1, score[0] = 0: the root); then the loop's
+    uint32_t stop[GENERATE_MAX_STOP];
+    uint32_t n_stop, width, max_tokens;
+    uint32_t step;                    // steps run
+    uint32_t n_live, n_pool;          // live beams and pool entries after the last step
+    uint32_t ticket, pad;
+    double score[BEAM_MAX];           // of the live beams
+    uint32_t parent[BEAM_MAX];        // of the live beams: the gather map of the pass that evaluates them
+    BeamHyp pool[BEAM_MAX];
+    uint32_t cand_id[BEAM_MAX][BEAM_CANDS];
+    float cand_lp[BEAM_MAX][BEAM_CANDS];    // NaN: no candidate
+};
+struct BeamStepParams {
+    const float * logits;             // [width, n_vocab]: column k that of live beam k
+    int n_vocab, width;
+    BeamState * st;
+    uint32_t * back;                  // [max_tokens][width][2]: parent slot and token of every live slot of every step
+    int * next_tokens;                // [width]
+    bool set_handles;                 // inside a conditional graph: set run_pass and keep_going
+    cudaGraphConditionalHandle run_pass, keep_going;
+};
+cudaError_t launch_beam_step(const BeamStepParams & p, cudaStream_t s);
+cudaError_t add_beam_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const BeamStepParams & p, cudaGraphNode_t * node);
+// dst slice k <- src slice st->parent[k] (state_len floats, seq_stride apart) for every live slot k < st->n_live.
+cudaError_t launch_beam_gather(const BeamState * st, int width, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);
+
 }  // namespace rwkv

@@ -14,12 +14,10 @@
 #include "ops.h"
 #include "gemv.h"
 #include "score_row.cuh"
+#include "top_n.cuh"
 
 namespace rwkv {
 namespace {
-
-constexpr int SAMPLE_THREADS = 1024;
-constexpr int SAMPLE_WARPS = SAMPLE_THREADS / 32;
 
 __device__ __forceinline__ double warp_sum_dd(double v) {
 #pragma unroll
@@ -326,41 +324,10 @@ struct NoLogprobs {
     __device__ __forceinline__ void record(int, size_t, uint32_t, const float *, int, uint32_t) const {}
 };
 
-// Top-N order over (logit, id): a larger logit first, the smaller id first among equal logits. The key holds the logit's bits mapped to
-// an unsigned order in its upper half (-0 counted as +0, so that equal values differ by id alone) and ~id in its lower half, so every
-// entry of a column has its own key and the largest keys are the top entries. No entry maps to key 0 (upper half 0xFFFFFFFF and id
-// 0xFFFFFFFF together), so 0 stands for "none".
-__device__ __forceinline__ unsigned long long top_key(float v, int i) {
-    const uint32_t u = __float_as_uint(__fadd_rn(v, 0.0f));
-    return ((unsigned long long) ((u & 0x80000000u) ? ~u : (u | 0x80000000u)) << 32) | (uint32_t) ~(uint32_t) i;
-}
-// The largest key below `limit` among this thread's entries tid + k * SAMPLE_THREADS of z, or 0.
-template <int PER>
-__device__ __forceinline__ unsigned long long top_below(const float * z, int V, int tid, unsigned long long limit) {
-    unsigned long long best = 0;
-#pragma unroll 4
-    for (int k = 0; k < PER; k++) {
-        const int i = tid + k * SAMPLE_THREADS;
-        if (i < V) {
-            const unsigned long long key = top_key(z[i], i);
-            if (key < limit && key > best) best = key;
-        }
-    }
-    return best;
-}
-__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
-        v = w > v ? w : v;
-    }
-    return v;
-}
-
 // The log-probability policy of the logprob kernels (GenLogprobRequest, ops.h). After the draw of token tok from row b's raw logits z:
-// warps 0-7 run score_kernel's reduction (score_row.cuh) under named barrier 1 while every warp selects its top_n entries by
-// top_n rounds of a warp-wide key maximum (a round's winner rescans its own entries below the key it gave up). Warp 0 then merges the
-// 32 sorted lists in shared memory the same way, and its lane 0 writes the outputs at `at` (and, streaming, the ring record).
+// warps 0-7 run score_kernel's reduction (score_row.cuh) under named barrier 1 while every warp selects its top_n entries
+// (warp_top_keys, top_n.cuh). Warp 0 then merges the 32 sorted lists in shared memory (merge_top_keys), and its lane 0 writes the
+// outputs at `at` (and, streaming, the ring record).
 template <int PER>
 struct Logprobs {
     const GenLogprobRequest * req;
@@ -378,31 +345,19 @@ struct Logprobs {
         if (tid < LP_SCORE_THREADS)
             score_column(tid, z, V, s_max, s_arg, s_bad, s_sum, [] { asm volatile("bar.sync 1, %0;" :: "n"(LP_SCORE_THREADS) : "memory"); },
                          [&](float m, int, bool v, double sum) { mx = m; valid = v; if (v) log_sum = log(sum); });
-        if (top_n > 0) {
-            unsigned long long mine = top_below<PER>(z, V, tid, ~0ull);
-            for (int k = 0; k < top_n; k++) {
-                const unsigned long long w = warp_max_u64(mine);
-                if (lane == 0) s_top[warp][k] = w;
-                if (w != 0 && mine == w) mine = top_below<PER>(z, V, tid, w);
-            }
-        }
+        warp_top_keys<PER>(z, V, tid, top_n, s_top);
         __syncthreads();
         if (warp != 0) return;
         uint32_t * rec = ring ? req->ring + ((size_t) b * 2 + (step & 1u)) * GEN_LP_RECORD : nullptr;
-        int head = 0;
-        unsigned long long cur = top_n > 0 ? s_top[lane][0] : 0ull;
-        for (int k = 0; k < top_n; k++) {
-            const unsigned long long w = warp_max_u64(cur);
-            if (lane == 0) {
-                const uint32_t id = ~(uint32_t) w;
-                const uint32_t out_id = valid ? id : SCORE_NO_TARGET;
-                const float out_lp = valid ? score_logprob(z[id], mx, log_sum) : NAN;
-                req->top_ids[at * top_n + k] = out_id;
-                req->top_logprobs[at * top_n + k] = out_lp;
-                if (rec) { ((volatile uint32_t *) rec)[2 + k] = out_id; ((volatile float *) rec)[2 + GEN_TOP_MAX + k] = out_lp; }
-            }
-            if (cur == w) { head++; cur = head < top_n ? s_top[lane][head] : 0ull; }
-        }
+        merge_top_keys(lane, top_n, s_top, [&](int k, unsigned long long w) {
+            if (lane != 0) return;
+            const uint32_t id = ~(uint32_t) w;
+            const uint32_t out_id = valid ? id : SCORE_NO_TARGET;
+            const float out_lp = valid ? score_logprob(z[id], mx, log_sum) : NAN;
+            req->top_ids[at * top_n + k] = out_id;
+            req->top_logprobs[at * top_n + k] = out_lp;
+            if (rec) { ((volatile uint32_t *) rec)[2 + k] = out_id; ((volatile float *) rec)[2 + GEN_TOP_MAX + k] = out_lp; }
+        });
         if (lane == 0) {
             const float lp = valid ? score_logprob(z[tok], mx, log_sum) : NAN;
             const float prob = req->sample_probs[at];

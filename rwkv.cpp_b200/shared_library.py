@@ -52,6 +52,15 @@ class AdapterTensor(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200
                 ("b", ctypes.POINTER(ctypes.c_float)), ("values", ctypes.POINTER(ctypes.c_float))]
 
 
+class BeamStepArgs(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_beam_step_args
+    _fields_ = [("logits", ctypes.POINTER(ctypes.c_float)), ("width", ctypes.c_size_t), ("n_vocab", ctypes.c_size_t), ("n_live", ctypes.c_size_t),
+                ("scores", ctypes.POINTER(ctypes.c_double)), ("n_pool", ctypes.c_size_t), ("stop_ids", ctypes.POINTER(ctypes.c_uint32)),
+                ("n_stop", ctypes.c_size_t), ("n_live_out", ctypes.POINTER(ctypes.c_uint32)), ("parents", ctypes.POINTER(ctypes.c_uint32)),
+                ("tokens", ctypes.POINTER(ctypes.c_uint32)), ("scores_out", ctypes.POINTER(ctypes.c_double)),
+                ("n_pool_out", ctypes.POINTER(ctypes.c_uint32)), ("pool_parents", ctypes.POINTER(ctypes.c_uint32)),
+                ("pool_tokens", ctypes.POINTER(ctypes.c_uint32)), ("pool_scores", ctypes.POINTER(ctypes.c_double))]
+
+
 class RWKVContext:
     def __init__(self, ptr: ctypes.c_void_p) -> None:
         self.ptr = ptr
@@ -259,6 +268,10 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_test_generate_step_streaming.argtypes = [ctypes.c_void_p, ctypes.c_int, P_SAMPLER, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS,
                                                                P_U32, P_U32, P_U32, P_U32, P_U32]
         lib.rwkv_b200_test_generate_step_streaming.restype = ctypes.c_bool
+        lib.rwkv_b200_beam_search.argtypes = [vp, ctypes.c_size_t, ctypes.c_float, P_U32, ctypes.c_size_t, ctypes.c_size_t, P_U32, P_U32, P_DOUBLE, P_U8]
+        lib.rwkv_b200_beam_search.restype = ctypes.c_bool
+        lib.rwkv_b200_test_beam_step.argtypes = [ctypes.POINTER(BeamStepArgs)]
+        lib.rwkv_b200_test_beam_step.restype = ctypes.c_bool
         lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
         lib.rwkv_b200_score.restype = ctypes.c_bool
         lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
@@ -381,6 +394,21 @@ class RWKVSharedLibrary:
     def rwkv_b200_set_adapter(self, ctx: RWKVContext, adapter: Optional[int]) -> None:
         if not self.library.rwkv_b200_set_adapter(ctx.ptr, adapter):
             raise ValueError(f"rwkv_b200_set_adapter failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+
+    def rwkv_b200_beam_search(self, batch: RWKVContext, max_tokens: int, length_penalty: float = 1.0, stop_ids=(), n_best: int = 1):
+        """Beam search of width n_sequences from sequence 0 of a batch context. Returns the n_best hypotheses, best first, as
+        (tokens, score, finished) with score the sum of the tokens' log-probabilities; slot k keeps the state of live beam k."""
+        toks = np.zeros((n_best, max_tokens), np.uint32)
+        lengths = np.zeros(n_best, np.uint32)
+        scores = np.zeros(n_best, np.float64)
+        finished = np.zeros(n_best, np.uint8)
+        stops = (ctypes.c_uint32 * max(1, len(stop_ids)))(*stop_ids)
+        P_U32, P_U8 = ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint8)
+        if not self.library.rwkv_b200_beam_search(batch.ptr, max_tokens, ctypes.c_float(length_penalty), stops, len(stop_ids), n_best,
+                                                  toks.ctypes.data_as(P_U32), lengths.ctypes.data_as(P_U32),
+                                                  scores.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), finished.ctypes.data_as(P_U8)):
+            raise ValueError(f"rwkv_b200_beam_search failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
+        return [([int(t) for t in toks[r, :lengths[r]]], float(scores[r]), bool(finished[r])) for r in range(n_best) if lengths[r]]
 
     def rwkv_b200_batch_set_adapter(self, batch: RWKVContext, sequence: int, adapter: Optional[int]) -> None:
         """Runs sequence `sequence` of a batch context with `adapter` (None: the base weights) on every later pass. Only adapters made of
