@@ -789,6 +789,32 @@ struct rwkv_b200_gemv_batch_args {
 };
 RWKV_API bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a);
 
+/* The same batch with low-rank deltas, run as the engine runs an adapted batch (engine.cu run_batch): the LoraBatch built by the
+ * engine's own build_lora_batch, then the shrink, the base batch on base.path and the expand (csrc/kernels/lora.h). Adapter k of
+ * n_adapters (1 .. 31) carries delta delta_of[i][k] of d[] on problem i, or none with -1; column t takes adapter col_adapter[t], or none
+ * with -1. A delta (K, M, rank 1 .. 256, scale, a [rank, K] and b [M, rank] row-major, both rounded to fp16) fits every problem that
+ * carries it. The scratch u / z is what a context of n_embed / n_ffn allocates (lora_scratch_floats), followed by RWKV_B200_GUARD
+ * floats, all of it filled with 0xFF bytes before the launches. Refused (ARGS) before the device: bad arguments; after the upload and
+ * before any launch: more groups than one launch holds (CTX | UNSUPPORTED) and problems that need more scratch than that (ARGS).
+ * Results: n_groups, the floats of u / z the batch uses and allocates, and whether both guards still hold the fill. */
+struct rwkv_b200_lora_delta {
+    int K, M, rank;
+    float scale;
+    const float * a, * b;
+};
+struct rwkv_b200_lora_gemv_batch_args {
+    struct rwkv_b200_gemv_batch_args base;
+    int n_embed, n_ffn;
+    int n_deltas, n_adapters;
+    struct rwkv_b200_lora_delta d[31];
+    int delta_of[8][31];
+    int col_adapter[256];
+    int n_groups;                                /* results */
+    long long u_used, z_used, u_floats, z_floats;
+    int scratch_guards_intact;
+};
+RWKV_API bool rwkv_b200_test_lora_gemv_batch(struct rwkv_b200_lora_gemv_batch_args * a);
+
 /* The v6 fold of single-token passes of single-sequence contexts: does a layer of this shape run maa_w1 (5 * mix rows of n_embed, type
  * w1_type) inside the LayerNorm-mix launch and decay_w2 (n_embed rows of `decay`, type w2_type) inside the WKV launch? Shapes only, no
  * device. Otherwise the layer runs the two GEMV launches. */

@@ -1796,7 +1796,13 @@ bool rwkv_b200_test_wkv6_decay(const struct rwkv_b200_wkv6_decay_args * a) {
     return true;
 }
 
-bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
+}  // extern "C"
+
+namespace {
+
+// rwkv_b200_test_gemv_batch, and with la (whose base is a) rwkv_b200_test_lora_gemv_batch: the batch's LoraBatch built by
+// build_lora_batch on scratch of lora_scratch_floats, then the shrink, the base launch and the expand, as run_batch runs them.
+bool gemv_batch_hook(const rwkv_b200_gemv_batch_args * a, rwkv_b200_lora_gemv_batch_args * la) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     bool args = a && a->T >= 1 && a->T <= 256 && a->n >= 1 && a->n <= GEMV_MAX_PROBLEMS && a->path >= RWKV_B200_GEMV_ENGINE &&
@@ -1817,6 +1823,21 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
         if (args && a->path == RWKV_B200_GEMV_STREAMING) args = dtype_kquant(q.type) ? q.type == a->p[0].type : !dtype_kquant(a->p[0].type);
     }
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid gemv_batch arguments");
+    if (la) {
+        args = la->n_embed > 0 && la->n_ffn >= 0 && la->n_deltas >= 0 && la->n_deltas <= LORA_MAX_ADAPTERS && la->n_adapters >= 1 &&
+               la->n_adapters <= LORA_MAX_ADAPTERS;
+        for (int j = 0; args && j < la->n_deltas; j++) {
+            const rwkv_b200_lora_delta & d = la->d[j];
+            args = d.K > 0 && d.M > 0 && d.rank >= 1 && d.rank <= LORA_MAX_RANK && d.a && d.b;
+        }
+        for (int i = 0; args && i < GEMV_MAX_PROBLEMS; i++)
+            for (int k = 0; args && k < LORA_MAX_ADAPTERS; k++) {
+                const int j = la->delta_of[i][k];
+                args = j == -1 || (i < a->n && k < la->n_adapters && j >= 0 && j < la->n_deltas && la->d[j].K == a->p[i].K && la->d[j].M == a->p[i].M);
+            }
+        for (int t = 0; args && t < LORA_MAX_T; t++) args = la->col_adapter[t] >= -1 && la->col_adapter[t] < (t < a->T ? la->n_adapters : 0);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, args, "Invalid lora_gemv_batch arguments");
+    }
     if (!hook_device(sink)) return false;
     cudaDeviceProp prop;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceProperties(&prop, default_device()) == cudaSuccess, "cudaGetDeviceProperties failed");
@@ -1860,6 +1881,38 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
     }
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, a->path != RWKV_B200_GEMV_TENSOR_CORES || !b.ok || tc_ok,
                "A problem of the batch cannot take the tensor-core path");
+    // the deltas in the engine's layout (fp16 A and B transposed), and the scratch with a guard behind each buffer
+    LoraScratchSize scratch{};
+    float * u = nullptr, * z = nullptr;
+    std::unique_ptr<LoraBatch> lb(la ? new LoraBatch() : nullptr);
+    if (la) {
+        LoraDelta dev[LORA_MAX_ADAPTERS];
+        for (int j = 0; j < la->n_deltas; j++) {
+            const rwkv_b200_lora_delta & d = la->d[j];
+            const size_t R = (size_t) d.rank, M = (size_t) d.M;
+            std::vector<uint16_t> ha(R * (size_t) d.K), hbt(R * M);
+            for (size_t i = 0; i < ha.size(); i++) ha[i] = fp32_to_fp16(d.a[i]);
+            for (size_t r = 0; r < R; r++) for (size_t i = 0; i < M; i++) hbt[r * M + i] = fp32_to_fp16(d.b[i * R + r]);
+            dev[j].A = b.in(ha.data(), ha.size()); dev[j].Bt = b.in(hbt.data(), hbt.size()); dev[j].rank = d.rank; dev[j].scale = d.scale;
+        }
+        scratch = lora_scratch_floats((size_t) la->n_embed, (size_t) la->n_ffn);
+        const size_t guard = RWKV_B200_GUARD * sizeof(float);
+        u = static_cast<float *>(b.alloc(scratch.u * sizeof(float) + guard));
+        z = static_cast<float *>(b.alloc(scratch.z * sizeof(float) + guard));
+        if (b.ok) b.ok = cudaMemset(u, 0xFF, scratch.u * sizeof(float) + guard) == cudaSuccess && cudaMemset(z, 0xFF, scratch.z * sizeof(float) + guard) == cudaSuccess;
+        RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.ok, "lora_gemv_batch: upload failed");
+        const LoraDelta * delta[GEMV_MAX_PROBLEMS][LORA_MAX_ADAPTERS] = {};
+        for (int i = 0; i < a->n; i++)
+            for (int k = 0; k < la->n_adapters; k++) delta[i][k] = la->delta_of[i][k] >= 0 ? &dev[la->delta_of[i][k]] : nullptr;
+        size_t u_used = 0, z_used = 0;
+        if (!build_lora_batch(sink, batch, la->n_adapters, delta, la->col_adapter, u, z, *lb, u_used, z_used)) return false;
+        la->n_groups = lb->n_groups;
+        la->u_used = (long long) u_used; la->z_used = (long long) z_used;
+        la->u_floats = (long long) scratch.u; la->z_floats = (long long) scratch.z;
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, u_used <= scratch.u && z_used <= scratch.z,
+                   "The adapted problems need %zu floats of u and %zu of z; a model of n_embed %d and n_ffn %d has %zu and %zu", u_used, z_used,
+                   la->n_embed, la->n_ffn, scratch.u, scratch.z);
+    }
     void * ws = nullptr;
     size_t ws_bytes = 0;
     if (a->path == RWKV_B200_GEMV_ENGINE || a->path == RWKV_B200_GEMV_ENGINE_BATCH_CTX || a->path == RWKV_B200_GEMV_TENSOR_CORES) {
@@ -1867,7 +1920,8 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
         ws = b.alloc(ws_bytes);
     }
     cudaError_t e = cudaSuccess;
-    if (b.ok) {
+    if (b.ok && lb && lb->n) e = launch_lora_shrink(*lb, 0);
+    if (b.ok && e == cudaSuccess) {
         switch (a->path) {
             case RWKV_B200_GEMV_STREAMING: e = dtype_kquant(batch.p[0].type) ? gemv_kq_launch(batch, di, 0) : gemv_tma_launch(batch, di, 0); break;
             case RWKV_B200_GEMV_GENERIC: e = gemv_generic_launch(batch, di, 0); break;
@@ -1883,8 +1937,31 @@ bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
         }
         *a->n_launches = n;
     }
+    if (b.ok && e == cudaSuccess && lb && lb->n) e = launch_lora_expand(*lb, 0);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, b.finish(e), "gemv_batch failed: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
+    if (la) {
+        auto intact = [](const float * end) {
+            unsigned char g[RWKV_B200_GUARD * sizeof(float)];
+            if (cudaMemcpy(g, end, sizeof(g), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+            for (unsigned char c : g) if (c != 0xFF) return false;
+            return true;
+        };
+        la->scratch_guards_intact = intact(u + scratch.u) && intact(z + scratch.z);
+    }
     return true;
 }
 
+}  // namespace
+
+extern "C" {
+
+bool rwkv_b200_test_gemv_batch(const struct rwkv_b200_gemv_batch_args * a) {
+    return gemv_batch_hook(a, nullptr);
+}
+
+bool rwkv_b200_test_lora_gemv_batch(struct rwkv_b200_lora_gemv_batch_args * a) {
+    return gemv_batch_hook(a ? &a->base : nullptr, a);
+}
+
 }  // extern "C"
+

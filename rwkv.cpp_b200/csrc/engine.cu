@@ -195,74 +195,29 @@ const LoraDelta * delta_in(const Model & m, const Adapter & a, const DevMatrix &
     return reinterpret_cast<const DevMatrix *>(reinterpret_cast<const unsigned char *>(a.layers.data()) + (w - base))->lora;
 }
 
-// A batch with low-rank deltas (kernels/lora.h): the shrink of every adapted problem, the batch through its unchanged route with the
-// adapted problems of nonlinear epilogue retargeted to EPI_NONE into lora_z, then the expand. Problems without a delta stay as they were.
-// The columns of a problem are grouped by delta: all of them under the context's adapter; under per-sequence adapters (a batch context)
-// one group per distinct adapter that adapts the matrix and has columns in the pass, plus, for a retargeted problem, one group of rank 0
-// with the columns left, which the expand passes through the epilogue. A problem with no column under a delta is not adapted at all.
+// A batch with low-rank deltas (kernels/lora.h): build_lora_batch's shrink of every adapted problem, the batch through its unchanged
+// route with the adapted problems of nonlinear epilogue retargeted to EPI_NONE into lora_z, then the expand. Problems without a delta
+// stay as they were. The columns of a problem are grouped by delta: all of them under the context's adapter (one slot holding every
+// column); under per-sequence adapters (a batch context) a slot per distinct adapter, a column in the slot of its sequence's adapter.
 bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
-    LoraBatch lb;
-    const int T = batch.b.T;
-    lb.n = 0; lb.T = T; lb.n_groups = 0;
-    float * u = ctx->lora_u, * z = ctx->lora_z;
-    int n_col = 0;
-    const int n_ad = (int) ctx->seq_adapters.size();
-    for (int i = 0; i < batch.b.n; i++) {
-        GemvProblem & q = batch.b.p[i];
-        const bool residual = q.epi == EPI_ADD || q.epi == EPI_MUL_ADD;
-        const LoraDelta * d[LORA_MAX_ADAPTERS + 1];     // the delta of each slot's adapter; slot n_ad: the columns without one
-        int slot_cols[LORA_MAX_ADAPTERS + 1] = {};
-        int slot[LORA_MAX_T];
-        if (n_ad == 0) {
-            if (!batch.lora[i]) continue;
-            d[0] = batch.lora[i];
-            for (int t = 0; t < T; t++) slot[t] = 0;
-            slot_cols[0] = T;
-        } else {
-            // only layer matrices carry deltas, and their batches have the pass's columns
-            bool any = false;
-            for (int k = 0; k < n_ad; k++) any = (d[k] = delta_in(*ctx->model, *ctx->seq_adapters[k], *batch.mat[i])) || any;
-            if (!any) continue;
-            RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, T == p.T, "A batch of %d columns in a pass of %d carries deltas", T, p.T);
-            d[n_ad] = nullptr;
-            bool adapted = false;
-            for (int t = 0; t < T; t++) {
-                const int k = ctx->seq_slot[p.col_seq_host ? p.col_seq_host[t] : t];
-                slot[t] = k >= 0 && d[k] ? k : n_ad;
-                slot_cols[slot[t]]++;
-                adapted = adapted || slot[t] < n_ad;
-            }
-            if (!adapted) continue;
-        }
-        const int n_slots = n_ad == 0 ? 1 : n_ad + 1;
-        int ldu = 0, groups = 0;
+    const int T = batch.b.T, n_ad = (int) ctx->seq_adapters.size(), n_slots = n_ad ? n_ad : 1;
+    const LoraDelta * delta[GEMV_MAX_PROBLEMS][LORA_MAX_ADAPTERS];
+    bool any = false;
+    for (int i = 0; i < batch.b.n; i++)
         for (int k = 0; k < n_slots; k++)
-            if (slot_cols[k] && (d[k] || !residual)) { groups++; if (d[k]) ldu = std::max(ldu, d[k]->rank); }
-        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, lb.n_groups + groups <= LORA_MAX_GROUPS, "Too many delta groups in one launch");
-        const int pi = lb.n++;
-        LoraProblem & l = lb.p[pi];
-        for (int k = 0; k < n_slots; k++) {
-            if (!slot_cols[k] || (!d[k] && residual)) continue;
-            LoraGroup & g = lb.g[lb.n_groups++];
-            g.d = d[k] ? *d[k] : LoraDelta{};
-            g.problem = pi;
-            g.col0 = n_col; g.n_cols = 0;
-            for (int t = 0; t < T; t++) if (slot[t] == k) lb.col[n_col + g.n_cols++] = (uint8_t) t;
-            n_col += g.n_cols;
-        }
-        l.K = q.K; l.M = q.M;
-        l.x = q.x; l.ldx = q.ldx;
-        l.u = u; l.ldu = ldu; u += (size_t) ldu * T;
-        l.P = q;
-        if (residual) {      // residual epilogues: the base writes y, the expand adds to it
-            l.z = nullptr; l.ldz = 0;
-            l.P.res = q.y; l.P.ldres = q.ldy;
-        } else {
-            l.z = z; l.ldz = q.M;
-            q.y = z; q.ldy = q.M; q.epi = EPI_NONE; q.res = q.gate = q.bias = nullptr;
-            z += (size_t) q.M * T;
-        }
+            any = (delta[i][k] = n_ad ? delta_in(*ctx->model, *ctx->seq_adapters[k], *batch.mat[i]) : batch.lora[i]) || any;
+    if (!any) return run_base(ctx, p, batch);
+    int col_slot[LORA_MAX_T];
+    if (n_ad) {
+        // only layer matrices carry deltas, and their batches have the pass's columns
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, T == p.T, "A batch of %d columns in a pass of %d carries deltas", T, p.T);
+        for (int t = 0; t < T; t++) col_slot[t] = ctx->seq_slot[p.col_seq_host ? p.col_seq_host[t] : t];
+    } else {
+        for (int t = 0; t < T; t++) col_slot[t] = 0;
     }
+    LoraBatch lb;
+    size_t u_used, z_used;
+    if (!build_lora_batch(ctx->sink(), batch.b, n_slots, delta, col_slot, ctx->lora_u, ctx->lora_z, lb, u_used, z_used)) return false;
     if (lb.n) CUDA_OK(ctx, launch_lora_shrink(lb, p.stream));
     if (!run_base(ctx, p, batch)) return false;
     if (lb.n) CUDA_OK(ctx, launch_lora_expand(lb, p.stream));
@@ -405,6 +360,65 @@ bool att_v5(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
 }
 
 }  // namespace
+
+LoraScratchSize lora_scratch_floats(size_t C, size_t F) {
+    const size_t T = MAX_TOKENS_PER_PASS;
+    return LoraScratchSize{(size_t) GEMV_MAX_PROBLEMS * LORA_MAX_RANK * T, std::max(4 * C, F + C) * T};
+}
+
+bool build_lora_batch(ErrorSink sink, GemvBatch & b, int n_slots, const LoraDelta * const delta[][LORA_MAX_ADAPTERS], const int * col_slot,
+                      float * u, float * z, LoraBatch & lb, size_t & u_used, size_t & z_used) {
+    const int T = b.T;
+    lb.n = 0; lb.T = T; lb.n_groups = 0;
+    float * const u0 = u, * const z0 = z;
+    int n_col = 0;
+    for (int i = 0; i < b.n; i++) {
+        GemvProblem & q = b.p[i];
+        const bool residual = q.epi == EPI_ADD || q.epi == EPI_MUL_ADD;
+        const LoraDelta * d[LORA_MAX_ADAPTERS + 1];     // the delta of each slot; slot n_slots: the columns without one
+        int slot_cols[LORA_MAX_ADAPTERS + 1] = {};
+        int slot[LORA_MAX_T];
+        for (int k = 0; k < n_slots; k++) d[k] = delta[i][k];
+        d[n_slots] = nullptr;
+        bool adapted = false;
+        for (int t = 0; t < T; t++) {
+            const int k = col_slot[t];
+            slot[t] = k >= 0 && d[k] ? k : n_slots;
+            slot_cols[slot[t]]++;
+            adapted = adapted || slot[t] < n_slots;
+        }
+        if (!adapted) continue;
+        int ldu = 0, groups = 0;
+        for (int k = 0; k <= n_slots; k++)
+            if (slot_cols[k] && (d[k] || !residual)) { groups++; if (d[k]) ldu = std::max(ldu, d[k]->rank); }
+        RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, lb.n_groups + groups <= LORA_MAX_GROUPS, "Too many delta groups in one launch");
+        const int pi = lb.n++;
+        LoraProblem & l = lb.p[pi];
+        for (int k = 0; k <= n_slots; k++) {
+            if (!slot_cols[k] || (!d[k] && residual)) continue;
+            LoraGroup & g = lb.g[lb.n_groups++];
+            g.d = d[k] ? *d[k] : LoraDelta{};
+            g.problem = pi;
+            g.col0 = n_col; g.n_cols = 0;
+            for (int t = 0; t < T; t++) if (slot[t] == k) lb.col[n_col + g.n_cols++] = (uint8_t) t;
+            n_col += g.n_cols;
+        }
+        l.K = q.K; l.M = q.M;
+        l.x = q.x; l.ldx = q.ldx;
+        l.u = u; l.ldu = ldu; u += (size_t) ldu * T;
+        l.P = q;
+        if (residual) {      // residual epilogues: the base writes y, the expand adds to it
+            l.z = nullptr; l.ldz = 0;
+            l.P.res = q.y; l.P.ldres = q.ldy;
+        } else {
+            l.z = z; l.ldz = q.M;
+            q.y = z; q.ldy = q.M; q.epi = EPI_NONE; q.res = q.gate = q.bias = nullptr;
+            z += (size_t) q.M * T;
+        }
+    }
+    u_used = (size_t) (u - u0); z_used = (size_t) (z - z0);
+    return true;
+}
 
 bool v6_prologue_fits(int C, GemvProblem & w1) {
     if (C < 1 || C > 4096 || w1.K != C || w1.M < 1 || !dtype_supported(w1.type) || w1.K % dtype_block_elems(w1.type)) return false;
@@ -1713,9 +1727,9 @@ namespace {
 bool ensure_lora_scratch(Context * ctx) {
     if (ctx->lora_u) return true;
     const Dims d = model_dims(*ctx->model);
-    const size_t z_rows = std::max(4 * d.C, d.F + d.C), T = MAX_TOKENS_PER_PASS;
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), (size_t) GEMV_MAX_PROBLEMS * LORA_MAX_RANK * T * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), z_rows * T * sizeof(float));
+    const LoraScratchSize s = lora_scratch_floats(d.C, d.F);
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), s.u * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), s.z * sizeof(float));
     if (e != cudaSuccess) {
         cudaFree(ctx->lora_u); cudaFree(ctx->lora_z); ctx->lora_u = ctx->lora_z = nullptr;
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, false, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));

@@ -363,6 +363,18 @@ bool set_adapter(Context * ctx, const Adapter * a);
 // adapter of its own; this checks the number of distinct adapters.
 bool batch_set_adapter(Context * ctx, int seq, const Adapter * a);
 
+// Floats of a context's delta scratch (Context::lora_u / lora_z) for a model of n_embed C and largest n_ffn F.
+struct LoraScratchSize { size_t u, z; };
+LoraScratchSize lora_scratch_floats(size_t C, size_t F);
+// The LoraBatch of GEMV batch b, whose columns carry deltas through n_slots adapters (1 .. LORA_MAX_ADAPTERS): delta[i][k] is the delta
+// of problem i under adapter k or NULL, col_slot[t] the adapter of column t or -1. A problem gets one group per adapter that adapts it
+// and has columns, plus, with a nonlinear epilogue, one group of rank 0 with its other columns; a problem none of whose columns is
+// under a delta is not adapted at all. An adapted problem of nonlinear epilogue is retargeted in b to EPI_NONE into z, the next
+// M * T floats of z; u gives each adapted problem its largest rank times T floats. u_used / z_used: the floats taken. False (CTX |
+// UNSUPPORTED) past LORA_MAX_GROUPS groups. Host only: b's pointers are not read.
+bool build_lora_batch(ErrorSink sink, GemvBatch & b, int n_slots, const LoraDelta * const delta[][LORA_MAX_ADAPTERS], const int * col_slot,
+                      float * u, float * z, LoraBatch & lb, size_t & u_used, size_t & z_used);
+
 size_t stage_hidden_len(const Model & m, size_t T);
 
 // Single-token passes of a single-sequence v6 context fold the two LoRA matrices that stream almost nothing into their neighbours:

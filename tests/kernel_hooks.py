@@ -223,11 +223,7 @@ GEMV_PATHS = {"engine": 0, "engine_batch_ctx": 1, "streaming": 2, "generic": 3, 
 LAUNCH_FAMILIES = ("streaming", "generic", "tensor_cores", "convert", "expand", "kquant", "kquant_expand")
 
 
-def gemv_batch(lib, T, problems, xs, path="engine"):
-    """rwkv_b200_test_gemv_batch. problems: dicts with type, K, M, raw (file-layout bytes), input (index into xs) and optionally
-    tiled, epi, pro, res / gate ([M, T]), bias ([M]), ln_w / ln_b ([K]), xq (staged bytes), alias (y aliases res). xs: [K, T] arrays.
-    Returns (one Out of M*T floats per problem, the launches as (family, nc, only, has_ln, npad, cluster) tuples)."""
-    i = Inputs()
+def _gemv_batch_args(T, problems, xs, path, i):
     a = GemvBatchArgs(T=T, n=len(problems), path=GEMV_PATHS[path])
     for j, x in enumerate(xs):
         a.x[j] = i(x, True)
@@ -250,6 +246,55 @@ def gemv_batch(lib, T, problems, xs, path="engine"):
     rec = (GemvLaunch * 32)()
     n_rec = ctypes.c_int(0)
     a.launches, a.max_launches, a.n_launches = rec, 32, ctypes.pointer(n_rec)
+    i.keep += [rec, n_rec]
+    return a, outs, lambda: [(LAUNCH_FAMILIES[r.family], r.nc, r.only, r.has_ln, r.npad, r.cluster) for r in rec[:n_rec.value]]
+
+
+def gemv_batch(lib, T, problems, xs, path="engine"):
+    """rwkv_b200_test_gemv_batch. problems: dicts with type, K, M, raw (file-layout bytes), input (index into xs) and optionally
+    tiled, epi, pro, res / gate ([M, T]), bias ([M]), ln_w / ln_b ([K]), xq (staged bytes), alias (y aliases res). xs: [K, T] arrays.
+    Returns (one Out of M*T floats per problem, the launches as (family, nc, only, has_ln, npad, cluster) tuples)."""
+    i = Inputs()
+    a, outs, launches = _gemv_batch_args(T, problems, xs, path, i)
     _call(lib, lib.library.rwkv_b200_test_gemv_batch, a)
-    launches = [(LAUNCH_FAMILIES[r.family], r.nc, r.only, r.has_ln, r.npad, r.cluster) for r in rec[:n_rec.value]]
-    return outs, launches
+    return outs, launches()
+
+
+MAX_DELTAS = 31           # deltas / adapters of one rwkv_b200_test_lora_gemv_batch call (LORA_MAX_ADAPTERS)
+
+
+class LoraDelta(ctypes.Structure):
+    _fields_ = [("K", ctypes.c_int), ("M", ctypes.c_int), ("rank", ctypes.c_int), ("scale", ctypes.c_float), ("a", VP), ("b", VP)]
+
+
+class LoraGemvBatchArgs(ctypes.Structure):
+    _fields_ = [("base", GemvBatchArgs), ("n_embed", ctypes.c_int), ("n_ffn", ctypes.c_int), ("n_deltas", ctypes.c_int),
+                ("n_adapters", ctypes.c_int), ("d", LoraDelta * MAX_DELTAS), ("delta_of", (ctypes.c_int * MAX_DELTAS) * 8),
+                ("col_adapter", ctypes.c_int * 256), ("n_groups", ctypes.c_int), ("u_used", ctypes.c_longlong), ("z_used", ctypes.c_longlong),
+                ("u_floats", ctypes.c_longlong), ("z_floats", ctypes.c_longlong), ("scratch_guards_intact", ctypes.c_int)]
+
+
+def lora_args(T, problems, xs, path, C, F, deltas, delta_of, col_adapter, i):
+    """The argument struct of rwkv_b200_test_lora_gemv_batch (see lora_gemv_batch), and the outputs and launch record of its base."""
+    base, outs, launches = _gemv_batch_args(T, problems, xs, path, i)
+    a = LoraGemvBatchArgs(base=base, n_embed=C, n_ffn=F, n_deltas=len(deltas), n_adapters=max(1, max(len(r) for r in delta_of)))
+    for j, (A, B, scale) in enumerate(deltas):
+        a.d[j] = LoraDelta(A.shape[1], B.shape[0], A.shape[0], scale, i(A), i(B))
+    for p in range(8):
+        for k in range(MAX_DELTAS):
+            a.delta_of[p][k] = delta_of[p][k] if p < len(delta_of) and k < len(delta_of[p]) else -1
+    for t in range(256):
+        a.col_adapter[t] = col_adapter[t] if t < len(col_adapter) else -1
+    return a, outs, launches
+
+
+def lora_gemv_batch(lib, T, problems, xs, path, C, F, deltas, delta_of, col_adapter):
+    """rwkv_b200_test_lora_gemv_batch: gemv_batch's batch with low-rank deltas, on the scratch of a model of n_embed C and n_ffn F.
+    deltas: [(A [rank, K], B [M, rank], scale)]; delta_of[i][k]: the delta adapter k carries on problem i, or -1; col_adapter[t]: column
+    t's adapter, or -1. Returns (outs, launches, dict of n_groups, u_used, z_used, u_floats, z_floats, guards)."""
+    i = Inputs()
+    a, outs, launches = lora_args(T, problems, xs, path, C, F, deltas, delta_of, col_adapter, i)
+    _call(lib, lib.library.rwkv_b200_test_lora_gemv_batch, a)
+    info = dict(n_groups=a.n_groups, u_used=a.u_used, z_used=a.z_used, u_floats=a.u_floats, z_floats=a.z_floats,
+                guards=bool(a.scratch_guards_intact))
+    return outs, launches(), info

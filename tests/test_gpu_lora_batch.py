@@ -529,6 +529,14 @@ def test_a_32nd_distinct_adapter_is_refused(lib):
         assert lib.library.rwkv_b200_batch_set_adapter(bt.ptr, 31, ads[0])      # a 31st sequence on an adapter in use
         toks = prompt(32, c.n_logits, 4)
         assert bt.eval(toks)
+        # the pass with 31 distinct adapters on all 32 sequences (tensor cores; att.key in 31 groups, none without a delta): row s equals
+        # row s of the batch with its adapter attached to the whole context
+        got = [(bt.logits(s, c.n_logits), bt.state(s, c.n_state)) for s in range(32)]
+        for k in range(31):
+            want = batch_run(lib, c, ads[k], [[t] for t in toks], 1)
+            for s in (k, 31) if k == 0 else (k,):
+                assert same(got[s], want[s]), (k, s)
+        assert not same(got[1], batch_run(lib, c, None, [[t] for t in toks], 1)[1])
     finally:
         bt.free()
         free_adapters(lib, *ads)
