@@ -474,6 +474,42 @@ struct rwkv_b200_beam_step_args {
 };
 RWKV_API bool rwkv_b200_test_beam_step(const struct rwkv_b200_beam_step_args * a);
 
+/* Many beam searches at once: n_groups = G searches over the sequences of one batch context, in one graph launch, so that every pass
+ * streams the weights once for all of them.
+ * 1. Layout. G must divide the batch's n_sequences, and W = n_sequences / G, 1 <= W <= RWKV_B200_BEAM_MAX, is every group's width.
+ *    Group g owns sequences g*W .. g*W + W - 1 and starts from sequence g*W: its resident state and its logits column (one
+ *    rwkv_b200_batch_eval_ragged pass typically fills the G roots).
+ * 2. Each group runs rules 1-6 of rwkv_b200_beam_search from its own root, with its own max_tokens[g] (0 .. RWKV_B200_GENERATE_MAX)
+ *    and length_penalty[g], and the shared stop ids and n_best. Its ranking, pool and back-pointers never see another group's
+ *    candidates, and its beams move only between its own slots. n, the largest max_tokens, must be at least 1.
+ * 3. Results: rows [G][n_best] of tokens_out ([G][n_best][n], 0 past the length), lengths_out, scores_out and finished_out (may be
+ *    NULL), each group's as rule 5 gives them.
+ * 4. A group with max_tokens[g] = 0 is left as it was: the state and logits column of all W of its sequences. Its result rows get
+ *    length 0, score -inf and finished 0. A group that ends while others go on keeps rule 6: each slot k < L of its last step with
+ *    L > 0 holds the state after that beam's tokens and the logits of its last token, whatever passes the other groups still run.
+ * 5. Bits. Below 16 sequences, and at any size with rwkv_b200_set_tensor_cores(batch, false), each group returns bit for bit what
+ *    rwkv_b200_beam_search returns on a batch of W sequences whose sequence 0 holds that root, slots included. From 16 sequences with
+ *    the tensor cores on, a group's bits are those of the same search driven from the host through batch passes of the whole batch.
+ *    G = 1 is rwkv_b200_beam_search.
+ * 6. Adapters. A context-wide adapter applies as in rwkv_b200_beam_search. Adapters from rwkv_b200_batch_set_adapter are allowed when
+ *    all W sequences of a group hold the same one (or none); that group then gives the bits of a W-sequence batch with that adapter
+ *    attached to the whole context.
+ * Every argument is checked before anything is enqueued, and a refused call changes nothing. RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED:
+ * an ordinary context, a pipeline or a stage, a call from inside that context's streaming callback, a driver without conditional
+ * graph nodes. RWKV_ERROR_ARGS: NULL arrays; G = 0, a G that does not divide n_sequences, or W > RWKV_B200_BEAM_MAX; n_best outside
+ * 1 .. W; a max_tokens entry above RWKV_B200_GENERATE_MAX, or all of them 0; a non-finite length penalty; more than
+ * RWKV_B200_GENERATE_MAX_STOP stop ids or an id >= n_vocab; invalid logits; n_vocab > 65536; a group whose sequences hold different
+ * adapters. The first call allocates the search state: per group about 2 KB and max_tokens * W * 8 bytes of back-pointers, on the
+ * device and pinned, and the logits of one pass, grown to the largest call. */
+RWKV_API bool rwkv_b200_beam_search_groups(struct rwkv_context * batch, size_t n_groups, const uint32_t * max_tokens /* [G] */,
+                                           const float * length_penalty /* [G] */, const uint32_t * stop_ids, size_t n_stop, size_t n_best,
+                                           uint32_t * tokens_out /* [G][n_best][n] */, uint32_t * lengths_out /* [G][n_best] */,
+                                           double * scores_out /* [G][n_best] */, uint8_t * finished_out /* [G][n_best], may be NULL */);
+/* Test hook: n_groups groups of rwkv_b200_test_beam_step's arguments (args[g]: group g, all of one width and n_vocab) in one launch of
+ * the grouped step kernel. A group may also have n_live = 0 or n_pool = width: it does not run, and the step leaves it as it was
+ * (*n_live_out = n_live, *n_pool_out = n_pool, the other outputs untouched). Arguments are checked before a device is touched. */
+RWKV_API bool rwkv_b200_test_beam_step_groups(const struct rwkv_b200_beam_step_args * args, size_t n_groups);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each

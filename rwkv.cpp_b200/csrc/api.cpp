@@ -788,6 +788,19 @@ bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct 
 
 static_assert(RWKV_B200_BEAM_MAX == BEAM_MAX && 2 * BEAM_MAX <= GEN_TOP_MAX, "beam width of the header and the kernel");
 
+// The refusals that rwkv_b200_beam_search and rwkv_b200_beam_search_groups share: the context kind, the stop ids and the logits.
+static bool check_beam_call(Context * c, const uint32_t * stop_ids, size_t n_stop) {
+    const Model & m = *c->model;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0 && !c->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Beam search runs on a batch context, not on an ordinary context, a pipeline or one of its stages");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_stop <= (size_t) RWKV_B200_GENERATE_MAX_STOP && (n_stop == 0 || stop_ids), "At most %d stop ids, not NULL",
+               RWKV_B200_GENERATE_MAX_STOP);
+    for (size_t k = 0; k < n_stop; k++)
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, stop_ids[k] < (uint32_t) m.n_vocab, "Stop id %u is out of range", stop_ids[k]);
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->logits_valid, "No logits to search from: the last evaluation skipped the head");
+    return true;
+}
+
 bool rwkv_b200_beam_search(struct rwkv_context * batch, size_t max_tokens, float length_penalty, const uint32_t * stop_ids, size_t n_stop,
                            size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out) {
     if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
@@ -804,55 +817,117 @@ bool rwkv_b200_beam_search(struct rwkv_context * batch, size_t max_tokens, float
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX, "max_tokens must be in 1 .. %d",
                RWKV_B200_GENERATE_MAX);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, std::isfinite(length_penalty), "length_penalty must be finite");
-    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_stop <= (size_t) RWKV_B200_GENERATE_MAX_STOP && (n_stop == 0 || stop_ids), "At most %d stop ids, not NULL",
-               RWKV_B200_GENERATE_MAX_STOP);
-    for (size_t k = 0; k < n_stop; k++)
-        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, stop_ids[k] < (uint32_t) m.n_vocab, "Stop id %u is out of range", stop_ids[k]);
-    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->logits_valid, "No logits to search from: the last evaluation skipped the head");
+    if (!check_beam_call(c, stop_ids, n_stop)) return false;
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, std::none_of(c->seq_adapter.begin(), c->seq_adapter.end(), [](const Adapter * a) { return a != nullptr; }),
                "A sequence of this batch holds its own adapter; beams move between sequences, so only a context-wide adapter applies");
-    return beam_search(c, max_tokens, length_penalty, stop_ids, n_stop, n_best, tokens_out, lengths_out, scores_out, finished_out);
+    const uint32_t n = (uint32_t) max_tokens;
+    return beam_search(c, 1, &n, &length_penalty, stop_ids, n_stop, n_best, tokens_out, lengths_out, scores_out, finished_out);
+}
+
+bool rwkv_b200_beam_search_groups(struct rwkv_context * batch, size_t n_groups, const uint32_t * max_tokens, const float * length_penalty,
+                                  const uint32_t * stop_ids, size_t n_stop, size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out,
+                                  double * scores_out, uint8_t * finished_out) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    const Model & m = *c->model;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0 && !c->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Beam search runs on a batch context, not on an ordinary context, a pipeline or one of its stages");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens && length_penalty && tokens_out && lengths_out && scores_out,
+               "NULL max_tokens, length_penalty, tokens_out, lengths_out or scores_out");
+    const size_t N = (size_t) c->batch_n;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_groups >= 1 && N % n_groups == 0 && N / n_groups <= (size_t) RWKV_B200_BEAM_MAX,
+               "n_groups (%zu) must divide the batch's %zu sequences into groups of at most %d", n_groups, N, RWKV_B200_BEAM_MAX);
+    const size_t W = N / n_groups;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n_best >= 1 && n_best <= W, "n_best must be in 1 .. %zu", W);
+    uint32_t n = 0;
+    for (size_t g = 0; g < n_groups; g++) {
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens[g] <= (uint32_t) RWKV_B200_GENERATE_MAX, "max_tokens of group %zu is above %d", g,
+                   RWKV_B200_GENERATE_MAX);
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, std::isfinite(length_penalty[g]), "length_penalty of group %zu must be finite", g);
+        n = std::max(n, max_tokens[g]);
+    }
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, n >= 1, "Every group has max_tokens 0");
+    if (!check_beam_call(c, stop_ids, n_stop)) return false;
+    for (size_t g = 0; g < n_groups && !c->seq_adapter.empty(); g++)
+        for (size_t k = 1; k < W; k++)
+            RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, c->seq_adapter[g * W + k] == c->seq_adapter[g * W],
+                       "The sequences of group %zu hold different adapters; beams move between the sequences of a group", g);
+    return beam_search(c, (int) n_groups, max_tokens, length_penalty, stop_ids, n_stop, n_best, tokens_out, lengths_out, scores_out, finished_out);
+}
+
+// G groups of the step hook's arguments in one launch of the step kernel. single: the arguments of rwkv_b200_test_beam_step, where
+// every group runs; otherwise a group with n_live = 0 or n_pool = width does not run, and the step leaves it as it was.
+static bool beam_step_hook(const struct rwkv_b200_beam_step_args * a, size_t G, bool single) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && G >= 1 && G <= 1024, "Invalid beam-step arguments");
+    for (size_t g = 0; g < G; g++) {
+        const rwkv_b200_beam_step_args & e = a[g];
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, e.scores && e.width >= 1 && e.width <= (size_t) RWKV_B200_BEAM_MAX && e.width == a[0].width &&
+                   e.n_vocab >= 1 && e.n_vocab <= 65536 && e.n_vocab == a[0].n_vocab && e.n_live <= e.width && e.n_pool <= e.width &&
+                   (e.n_live == 0 || e.logits) && (!single || (e.n_live >= 1 && e.n_pool < e.width)) && e.n_live_out && e.parents && e.tokens &&
+                   e.scores_out && e.n_pool_out && e.pool_parents && e.pool_tokens && e.pool_scores, "Invalid beam-step arguments (group %zu)", g);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, e.n_stop <= (size_t) GENERATE_MAX_STOP && (e.n_stop == 0 || e.stop_ids), "At most %d stop ids, not NULL",
+                   GENERATE_MAX_STOP);
+        for (size_t k = 0; k < e.n_live; k++) RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, std::isfinite(e.scores[k]), "Score of beam %zu is not finite", k);
+    }
+    if (!hook_device(sink)) return false;
+    const size_t W = a[0].width, V = a[0].n_vocab;
+    std::vector<unsigned char> host(sizeof(BeamLoop) + G * sizeof(BeamState), 0);
+    BeamLoop * loop = reinterpret_cast<BeamLoop *>(host.data());
+    BeamState * st = reinterpret_cast<BeamState *>(loop + 1);
+    std::vector<float> z(G * W * V, 0.f);
+    for (size_t g = 0; g < G; g++) {
+        const rwkv_b200_beam_step_args & e = a[g];
+        for (size_t k = 0; k < e.n_stop; k++) st[g].stop[k] = e.stop_ids[k];
+        st[g].n_stop = (uint32_t) e.n_stop; st[g].width = (uint32_t) W; st[g].max_tokens = 1;
+        st[g].n_live = (uint32_t) e.n_live; st[g].n_pool = (uint32_t) e.n_pool;
+        for (size_t k = 0; k < e.n_live; k++) st[g].score[k] = e.scores[k];
+        if (e.n_live) std::copy(e.logits, e.logits + e.n_live * V, z.begin() + g * W * V);
+        if (e.n_live > 0 && e.n_pool < W) loop->n_active++;
+    }
+    HookBuffers hb;
+    BeamStepParams p{};
+    p.logits = hb.in(z.data(), z.size()); p.n_vocab = (int) V; p.width = (int) W; p.groups = (int) G;
+    p.loop = reinterpret_cast<BeamLoop *>(const_cast<unsigned char *>(hb.in(host.data(), host.size())));
+    p.st = reinterpret_cast<BeamState *>(p.loop + 1);
+    p.back = static_cast<uint32_t *>(hb.alloc(G * W * 2 * sizeof(uint32_t)));
+    p.next_tokens = static_cast<int *>(hb.alloc(G * W * sizeof(int)));
+    std::vector<uint32_t> back(2 * G * W);
+    std::vector<int> next(G * W, 0);
+    if (hb.ok) cudaMemset(p.next_tokens, 0, G * W * sizeof(int));
+    const bool ok = hb.ok && hb.finish(launch_beam_step(p, 0)) && cudaMemcpy(host.data(), p.loop, host.size(), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                    cudaMemcpy(back.data(), p.back, back.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                    cudaMemcpy(next.data(), p.next_tokens, G * W * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess;
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "beam step failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
+    RWKV_CHECK(sink, RWKV_ERROR_CTX, false, loop->ticket == 0 && loop->n_next == 0 && loop->any_live == 0, "The step left its loop tickets set");
+    for (size_t g = 0; g < G; g++) {
+        const rwkv_b200_beam_step_args & e = a[g];
+        const uint32_t * bk = back.data() + 2 * g * W;
+        const int * nx = next.data() + g * W;
+        *e.n_live_out = st[g].n_live;
+        *e.n_pool_out = st[g].n_pool;
+        if (!(e.n_live > 0 && e.n_pool < W)) continue;      // did not run
+        for (size_t k = 0; k < st[g].n_live; k++) {
+            e.parents[k] = bk[2 * k]; e.tokens[k] = bk[2 * k + 1]; e.scores_out[k] = st[g].score[k];
+            RWKV_CHECK(sink, RWKV_ERROR_CTX, false, nx[k] == (int) bk[2 * k + 1], "The next input token of slot %zu is not its token", k);
+        }
+        for (size_t k = st[g].n_live; k < W; k++) RWKV_CHECK(sink, RWKV_ERROR_CTX, false, nx[k] == 0, "The next input token of idle slot %zu is not 0", k);
+        for (size_t q = e.n_pool; q < st[g].n_pool; q++) {
+            e.pool_parents[q] = st[g].pool[q].parent; e.pool_tokens[q] = st[g].pool[q].token; e.pool_scores[q] = st[g].pool[q].score;
+        }
+    }
+    return true;
 }
 
 bool rwkv_b200_test_beam_step(const struct rwkv_b200_beam_step_args * a) {
-    g_last_error = RWKV_ERROR_NONE;
-    ErrorSink sink = global_sink();
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->scores && a->width >= 1 && a->width <= (size_t) RWKV_B200_BEAM_MAX && a->n_vocab >= 1 &&
-               a->n_vocab <= 65536 && a->n_live >= 1 && a->n_live <= a->width && a->n_pool < a->width && a->n_live_out && a->parents && a->tokens &&
-               a->scores_out && a->n_pool_out && a->pool_parents && a->pool_tokens && a->pool_scores, "Invalid beam-step arguments");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->n_stop <= (size_t) GENERATE_MAX_STOP && (a->n_stop == 0 || a->stop_ids), "At most %d stop ids, not NULL",
-               GENERATE_MAX_STOP);
-    for (size_t k = 0; k < a->n_live; k++) RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, std::isfinite(a->scores[k]), "Score of beam %zu is not finite", k);
-    if (!hook_device(sink)) return false;
-    const size_t W = a->width, V = a->n_vocab;
-    BeamState st{};
-    for (size_t k = 0; k < a->n_stop; k++) st.stop[k] = a->stop_ids[k];
-    st.n_stop = (uint32_t) a->n_stop; st.width = (uint32_t) W; st.max_tokens = 1;
-    st.n_live = (uint32_t) a->n_live; st.n_pool = (uint32_t) a->n_pool;
-    for (size_t k = 0; k < a->n_live; k++) st.score[k] = a->scores[k];
-    HookBuffers hb;
-    BeamStepParams p{};
-    p.logits = hb.in(a->logits, a->n_live * V); p.n_vocab = (int) V; p.width = (int) W;
-    p.st = const_cast<BeamState *>(hb.in(&st, 1));
-    p.back = static_cast<uint32_t *>(hb.alloc(W * 2 * sizeof(uint32_t)));
-    p.next_tokens = static_cast<int *>(hb.alloc(W * sizeof(int)));
-    std::vector<uint32_t> back(2 * W);
-    std::vector<int> next(W);
-    const bool ok = hb.ok && hb.finish(launch_beam_step(p, 0)) && cudaMemcpy(&st, p.st, sizeof(BeamState), cudaMemcpyDeviceToHost) == cudaSuccess &&
-                    cudaMemcpy(back.data(), p.back, back.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
-                    cudaMemcpy(next.data(), p.next_tokens, W * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess;
-    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "beam step failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
-    *a->n_live_out = st.n_live;
-    for (size_t k = 0; k < st.n_live; k++) {
-        a->parents[k] = back[2 * k]; a->tokens[k] = back[2 * k + 1]; a->scores_out[k] = st.score[k];
-        RWKV_CHECK(sink, RWKV_ERROR_CTX, false, next[k] == (int) back[2 * k + 1], "The next input token of slot %zu is not its token", k);
-    }
-    for (size_t k = st.n_live; k < W; k++) RWKV_CHECK(sink, RWKV_ERROR_CTX, false, next[k] == 0, "The next input token of idle slot %zu is not 0", k);
-    *a->n_pool_out = st.n_pool;
-    for (size_t q = a->n_pool; q < st.n_pool; q++) {
-        a->pool_parents[q] = st.pool[q].parent; a->pool_tokens[q] = st.pool[q].token; a->pool_scores[q] = st.pool[q].score;
-    }
-    return true;
+    return beam_step_hook(a, 1, true);
+}
+
+bool rwkv_b200_test_beam_step_groups(const struct rwkv_b200_beam_step_args * a, size_t n_groups) {
+    return beam_step_hook(a, n_groups, false);
 }
 
 static_assert(RWKV_B200_AUTOMATON_DEAD == GEN_MASK_DEAD, "dead transition of the header and the kernel");

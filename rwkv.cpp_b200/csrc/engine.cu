@@ -886,7 +886,7 @@ void destroy_context(Context * ctx) {
     if (ctx->lp_ring_host) cudaFreeHost(ctx->lp_ring_host);
     cudaFree(ctx->smp_dev);
     if (ctx->smp_host) cudaFreeHost(ctx->smp_host);
-    cudaFree(ctx->beam_state); cudaFree(ctx->beam_warm); cudaFree(ctx->beam_back);
+    cudaFree(ctx->beam_loop); cudaFree(ctx->beam_park); cudaFree(ctx->beam_back);
     if (ctx->beam_host) cudaFreeHost(ctx->beam_host);
     for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
@@ -2008,39 +2008,42 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     return true;
 }
 
-// Beam search: WHILE keep_going { beam step -> IF run_pass { gather ; pass } }, one pass per body. Y = state_a holds the current
-// slots: the gather copies each live slot's parent from Y into X = state_b and the pass evaluates X into Y, so the current state stays
-// in state_a and the phase does not change. The graph is keyed by the phase at entry, which decides which buffer is state_a.
+// Beam search: WHILE keep_going { beam step -> IF run_pass { gather ; pass } }, one pass per body, then (several groups) the restore
+// of the slots that groups which stopped keep. Y = state_a holds the current slots: the gather copies each live slot's parent from Y
+// into X = state_b and the pass evaluates X into Y, so the current state stays in state_a and the phase does not change. The graph is
+// keyed by the phase at entry, which decides which buffer is state_a, and by the number of groups.
 namespace {
 
-bool ensure_beam_buffers(Context * ctx, size_t max_tokens) {
-    const size_t W = (size_t) ctx->batch_n;
-    if (!ctx->beam_state) {
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_state), sizeof(BeamState)));
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_warm), W * (size_t) ctx->model->n_vocab * sizeof(float)));
-    }
-    if (max_tokens <= ctx->beam_capacity) return true;
+bool ensure_beam_buffers(Context * ctx, size_t groups, size_t max_tokens) {
+    const size_t N = (size_t) ctx->batch_n;
+    if (!ctx->beam_park) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_park), N * (size_t) ctx->model->n_vocab * sizeof(float)));
+    if (groups <= ctx->beam_groups && max_tokens <= ctx->beam_capacity) return true;
+    groups = std::max(groups, ctx->beam_groups);
+    max_tokens = std::max(max_tokens, ctx->beam_capacity);
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     for (auto & e : ctx->beam_graphs) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
-    cudaFree(ctx->beam_back);
+    cudaFree(ctx->beam_loop); cudaFree(ctx->beam_back);
     if (ctx->beam_host) cudaFreeHost(ctx->beam_host);
-    ctx->beam_back = nullptr; ctx->beam_host = nullptr; ctx->beam_capacity = 0;
-    const size_t back_bytes = max_tokens * W * 2 * sizeof(uint32_t);
+    ctx->beam_loop = nullptr; ctx->beam_state = nullptr; ctx->beam_back = nullptr; ctx->beam_host = nullptr;
+    ctx->beam_groups = 0; ctx->beam_capacity = 0;
+    const size_t state_bytes = sizeof(BeamLoop) + groups * sizeof(BeamState), back_bytes = max_tokens * N * 2 * sizeof(uint32_t);
+    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_loop), state_bytes));
+    ctx->beam_state = reinterpret_cast<BeamState *>(ctx->beam_loop + 1);
     CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_back), back_bytes));
-    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->beam_host), sizeof(BeamState) + back_bytes));
-    ctx->beam_capacity = max_tokens;
+    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->beam_host), state_bytes + back_bytes));
+    ctx->beam_groups = groups; ctx->beam_capacity = max_tokens;
     return true;
 }
 
-bool build_beam_graph(Context * ctx) {
-    const int W = ctx->batch_n;
+bool build_beam_graph(Context * ctx, int groups) {
+    const int N = ctx->batch_n, W = N / groups;
     Pass p;
-    if (!make_pass(ctx, W, true, nullptr, p)) return false;
+    if (!make_pass(ctx, N, true, nullptr, p)) return false;
     p.tokens_in_place = true;
     {   // one uncaptured pass of the loop's shape first, as build_generate_graph runs one: Y -> X with its logits set aside
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) W * sizeof(int), p.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) N * sizeof(int), p.stream));
         Pass warm = p;
-        warm.logits = ctx->beam_warm;
+        warm.logits = ctx->beam_park;
         if (!enqueue_pass(ctx, warm, 0)) return false;
     }
     p.state_in = ctx->state_b; p.state_out = ctx->state_a;
@@ -2051,24 +2054,29 @@ bool build_beam_graph(Context * ctx) {
     cudaGraphNodeParams wp = {};
     wp.type = cudaGraphNodeTypeConditional;
     wp.conditional.handle = keep_going; wp.conditional.type = cudaGraphCondTypeWhile; wp.conditional.size = 1;
-    cudaGraphNode_t loop = nullptr, step = nullptr, cond = nullptr;
+    cudaGraphNode_t loop = nullptr, step = nullptr, cond = nullptr, restore = nullptr;
     CUDA_OK(ctx, cudaGraphAddNode(&loop, top.g, nullptr, 0, &wp));
     cudaGraph_t body = wp.conditional.phGraph_out[0];
     CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&run_pass, body, 0, cudaGraphCondAssignDefault));
-    const BeamStepParams bp{ctx->logits, ctx->model->n_vocab, W, ctx->beam_state, ctx->beam_back, ctx->tokens, true, run_pass, keep_going};
+    const BeamStepParams bp{ctx->logits, ctx->model->n_vocab, W, groups, ctx->beam_loop, ctx->beam_state, ctx->beam_back, ctx->tokens, true,
+                            run_pass, keep_going};
     CUDA_OK(ctx, add_beam_step_node(body, nullptr, 0, bp, &step));
+    const BeamCopyParams cp{ctx->beam_loop, ctx->beam_state, W, groups, ctx->model->n_vocab, p.state_out, p.state_in, ctx->batch_stride,
+                            ctx->model->state_len(), ctx->logits, ctx->beam_park};
+    if (groups > 1) CUDA_OK(ctx, add_beam_restore_node(top.g, &loop, 1, cp, &restore));     // one group stops only when the loop does
     cudaGraphNodeParams ip = {};
     ip.type = cudaGraphNodeTypeConditional;
     ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
     CUDA_OK(ctx, cudaGraphAddNode(&cond, body, &step, 1, &ip));
     CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(p.stream, ip.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    cudaError_t e = launch_beam_gather(ctx->beam_state, W, p.state_out, p.state_in, ctx->batch_stride, ctx->model->state_len(), p.stream);
+    cudaError_t e = launch_beam_gather(cp, p.stream);
     const bool ok = e == cudaSuccess && enqueue_pass(ctx, p, 0);
     cudaGraph_t out = nullptr;
     const cudaError_t ec = cudaStreamEndCapture(p.stream, &out);
     if (e == cudaSuccess) e = ec;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess, "Capturing the beam search pass failed: %s", cudaGetErrorString(e));
     CUDA_OK(ctx, cudaGraphInstantiate(&ctx->beam_graphs[ctx->phase], top.g, 0));
+    ctx->beam_graph_groups[ctx->phase] = groups;
     return true;
 }
 
@@ -2080,57 +2088,75 @@ struct BeamResult {
 
 }  // namespace
 
-bool beam_search(Context * ctx, size_t max_tokens, float length_penalty, const uint32_t * stop_ids, size_t n_stop, size_t n_best,
-                 uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out) {
+bool beam_search(Context * ctx, int n_groups, const uint32_t * max_tokens, const float * length_penalty, const uint32_t * stop_ids, size_t n_stop,
+                 size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out) {
     const Model & m = *ctx->model;
-    const int W = ctx->batch_n;
+    const int N = ctx->batch_n, W = N / n_groups;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, m.n_vocab <= 65536, "Beam search supports n_vocab <= 65536");
     int driver = 0;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaDriverGetVersion(&driver) == cudaSuccess && driver >= 12040,
                "Beam search needs conditional graph nodes: a CUDA driver of 12.4 or newer (found %d)", driver);
+    size_t n = 0;
+    for (int g = 0; g < n_groups; g++) n = std::max(n, (size_t) max_tokens[g]);
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    if (!ensure_beam_buffers(ctx, max_tokens) || !ensure_capacity(ctx, W, ctx->stream)) return false;
-    BeamState * hs = reinterpret_cast<BeamState *>(ctx->beam_host);
-    memset(hs, 0, sizeof(BeamState));
-    for (size_t k = 0; k < n_stop; k++) hs->stop[k] = stop_ids[k];
-    hs->n_stop = (uint32_t) n_stop; hs->width = (uint32_t) W; hs->max_tokens = (uint32_t) max_tokens;
-    hs->n_live = 1;     // the root: sequence 0, score 0
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->beam_state, hs, sizeof(BeamState), cudaMemcpyHostToDevice, ctx->stream));
+    if (!ensure_beam_buffers(ctx, (size_t) n_groups, n) || !ensure_capacity(ctx, N, ctx->stream)) return false;
+    BeamLoop * hl = reinterpret_cast<BeamLoop *>(ctx->beam_host);
+    BeamState * hs = reinterpret_cast<BeamState *>(hl + 1);
+    memset(hl, 0, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState));
+    for (int g = 0; g < n_groups; g++) {
+        BeamState & st = hs[g];
+        for (size_t k = 0; k < n_stop; k++) st.stop[k] = stop_ids[k];
+        st.n_stop = (uint32_t) n_stop; st.width = (uint32_t) W; st.max_tokens = max_tokens[g];
+        if (max_tokens[g] > 0) {
+            st.n_live = 1;      // the root: sequence g*W, score 0
+            hl->n_active++;
+        } else {
+            st.n_keep = (uint32_t) W; st.park_at = 1;     // never runs: every slot is kept from the first pass on
+        }
+    }
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->beam_loop, hl, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyHostToDevice, ctx->stream));
+    // a group that never runs takes no token; its slots still run in the passes, on token 0
+    if (n_groups > 1) CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) N * sizeof(int), ctx->stream));
     cudaGraphExec_t & graph = ctx->beam_graphs[ctx->phase];
-    if (!graph && !build_beam_graph(ctx)) return false;
+    if (graph && ctx->beam_graph_groups[ctx->phase] != n_groups) { cudaGraphExecDestroy(graph); graph = nullptr; }
+    if (!graph && !build_beam_graph(ctx, n_groups)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
-    uint32_t * back = reinterpret_cast<uint32_t *>(ctx->beam_host + sizeof(BeamState));
-    CUDA_OK(ctx, cudaMemcpyAsync(hs, ctx->beam_state, sizeof(BeamState), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(back, ctx->beam_back, max_tokens * W * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    uint32_t * back = reinterpret_cast<uint32_t *>(hs + n_groups);
+    CUDA_OK(ctx, cudaMemcpyAsync(hl, ctx->beam_loop, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(back, ctx->beam_back, n * N * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    // the tokens of the beam in slot k after step i, from the back-pointers
-    auto history = [&](int64_t i, uint32_t k) {
-        std::vector<uint32_t> t((size_t) (i + 1));
-        for (; i >= 0; i--) {
-            const uint32_t * e = back + ((size_t) i * W + k) * 2;
-            t[(size_t) i] = e[1];
-            k = e[0];
+    memset(tokens_out, 0, (size_t) n_groups * n_best * n * sizeof(uint32_t));
+    for (int g = 0; g < n_groups; g++) {
+        const BeamState & st = hs[g];
+        // the tokens of the beam in slot k of group g after step i, from the back-pointers
+        auto history = [&](int64_t i, uint32_t k) {
+            std::vector<uint32_t> t((size_t) (i + 1));
+            for (; i >= 0; i--) {
+                const uint32_t * e = back + ((size_t) i * N + (size_t) g * W + k) * 2;
+                t[(size_t) i] = e[1];
+                k = e[0];
+            }
+            return t;
+        };
+        std::vector<BeamResult> res;
+        for (uint32_t q = 0; q < st.n_pool; q++) {
+            const BeamHyp & h = st.pool[q];
+            BeamResult r{h.score, 0.0, true, history((int64_t) h.step - 1, h.parent)};
+            r.tokens.push_back(h.token);
+            res.push_back(std::move(r));
         }
-        return t;
-    };
-    std::vector<BeamResult> res;
-    for (uint32_t q = 0; q < hs->n_pool; q++) {
-        const BeamHyp & h = hs->pool[q];
-        BeamResult r{h.score, 0.0, true, history((int64_t) h.step - 1, h.parent)};
-        r.tokens.push_back(h.token);
-        res.push_back(std::move(r));
-    }
-    for (uint32_t k = 0; k < hs->n_live; k++) res.push_back(BeamResult{hs->score[k], 0.0, false, history((int64_t) hs->step - 1, k)});
-    for (BeamResult & r : res) r.norm = r.score / std::pow((double) r.tokens.size(), (double) length_penalty);
-    std::stable_sort(res.begin(), res.end(), [](const BeamResult & a, const BeamResult & b) { return a.norm > b.norm; });
-    memset(tokens_out, 0, n_best * max_tokens * sizeof(uint32_t));
-    for (size_t r = 0; r < n_best; r++) {
-        const bool have = r < res.size();
-        if (have) std::copy(res[r].tokens.begin(), res[r].tokens.end(), tokens_out + r * max_tokens);
-        lengths_out[r] = have ? (uint32_t) res[r].tokens.size() : 0;
-        scores_out[r] = have ? res[r].score : -INFINITY;
-        if (finished_out) finished_out[r] = have && res[r].finished ? 1 : 0;
+        for (uint32_t k = 0; k < st.n_live; k++) res.push_back(BeamResult{st.score[k], 0.0, false, history((int64_t) st.step - 1, k)});
+        for (BeamResult & r : res) r.norm = r.score / std::pow((double) r.tokens.size(), (double) length_penalty[g]);
+        std::stable_sort(res.begin(), res.end(), [](const BeamResult & a, const BeamResult & b) { return a.norm > b.norm; });
+        for (size_t r = 0; r < n_best; r++) {
+            const size_t row = (size_t) g * n_best + r;
+            const bool have = r < res.size();
+            if (have) std::copy(res[r].tokens.begin(), res[r].tokens.end(), tokens_out + row * n);
+            lengths_out[row] = have ? (uint32_t) res[r].tokens.size() : 0;
+            scores_out[row] = have ? res[r].score : -INFINITY;
+            if (finished_out) finished_out[row] = have && res[r].finished ? 1 : 0;
+        }
     }
     return true;
 }

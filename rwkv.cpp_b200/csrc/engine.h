@@ -25,6 +25,7 @@ struct PipeGroup {
 
 struct SampleRow;                       // per-sequence sampling parameters (kernels/ops.h)
 struct BeamState;                       // the device state of a beam search (kernels/ops.h)
+struct BeamLoop;                        // the state its groups share (kernels/ops.h)
 struct GenLogprobRequest;               // the per-call request of the logprob generation kernels (kernels/ops.h)
 struct CopyPool;                        // helper threads of the pageable-buffer bounce path (engine.cu)
 void destroy_copy_pool(CopyPool * p);
@@ -176,15 +177,19 @@ struct Context {
     // room for rows * GEN_BIAS_MAX GenBiasEntry.
     unsigned char * smp_dev = nullptr, * smp_host = nullptr;
     cudaGraphExec_t gen_smp_graphs[2][2] = {};   // the sampled loops' graphs, keyed by phase and streaming
-    // Beam search (beam_search), allocated on the first call: the search state (kernels/ops.h: BeamState), the logits of the pass that
-    // runs before the loop is captured [batch_n, n_vocab], and the back-pointers [beam_capacity][batch_n][2], grown to the largest
-    // max_tokens (which drops beam_graphs, as they hold its address). beam_host: pinned BeamState followed by the back-pointers.
+    // Beam search (beam_search), allocated on the first call: the loop state and a search state per group (kernels/ops.h: BeamLoop,
+    // BeamState[beam_groups], one allocation), the park [batch_n, n_vocab] (the logits of the pass that runs before the loop is
+    // captured, then the logits of the slots that groups which stopped keep), and the back-pointers [beam_capacity][batch_n][2]. The
+    // states and back-pointers grow to the most groups and the largest max_tokens asked for, which drops beam_graphs, as they hold
+    // their addresses. beam_host: pinned BeamLoop, the BeamStates and the back-pointers.
+    BeamLoop * beam_loop = nullptr;
     BeamState * beam_state = nullptr;
-    float * beam_warm = nullptr;
+    float * beam_park = nullptr;
     uint32_t * beam_back = nullptr;
     unsigned char * beam_host = nullptr;
-    size_t beam_capacity = 0;
-    cudaGraphExec_t beam_graphs[2] = {};         // the search loop's graphs, keyed by phase
+    size_t beam_capacity = 0, beam_groups = 0;
+    cudaGraphExec_t beam_graphs[2] = {};         // the search loop's graphs, keyed by phase and by the groups they were built for
+    int beam_graph_groups[2] = {};
 
     // The attached adapter (set_adapter) or NULL, and the scratch of its deltas, allocated on the first attach for passes of up to
     // MAX_TOKENS_PER_PASS columns so that captured graphs never see it move: u [GEMV_MAX_PROBLEMS][LORA_MAX_RANK][T] and the base
@@ -331,11 +336,12 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
               const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr, const LogprobsOut * lp = nullptr,
               const SamplerIn * samplers = nullptr);
 
-// Beam search over the sequences of a batch context (rwkv_b200_beam_search, include/rwkv_b200.h), width batch_n, from sequence 0's
-// state and logits, as one graph launch; the context, its logits and the arguments have been checked by the caller, except n_vocab and
-// the driver, which this checks. Outputs as the C call's. Synchronises.
-bool beam_search(Context * ctx, size_t max_tokens, float length_penalty, const uint32_t * stop_ids, size_t n_stop, size_t n_best,
-                 uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out);
+// Beam search over the sequences of a batch context (rwkv_b200_beam_search_groups, include/rwkv_b200.h): n_groups searches of width
+// W = batch_n / n_groups, group g from sequence g*W's state and logits, as one graph launch; rwkv_b200_beam_search is n_groups = 1. The
+// context, its logits and the arguments have been checked by the caller, except n_vocab and the driver, which this checks. Outputs as
+// the C call's, [n_groups][n_best][n] with n the largest max_tokens. Synchronises.
+bool beam_search(Context * ctx, int n_groups, const uint32_t * max_tokens, const float * length_penalty, const uint32_t * stop_ids, size_t n_stop,
+                 size_t n_best, uint32_t * tokens_out, uint32_t * lengths_out, double * scores_out, uint8_t * finished_out);
 
 // A token automaton of rwkv_b200_automaton_create: the transition table next[s * n_vocab + t] (GEN_MASK_DEAD: t not allowed in s)
 // and live[s] (s allows some token) in the HBM of the model's device. It serves every context of that model.

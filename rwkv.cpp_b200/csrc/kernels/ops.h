@@ -336,6 +336,12 @@ cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float *
 // position), walks the ranking until W live beams are taken, the pool holds W hypotheses or the list ends (a stop id goes to the pool,
 // any other token becomes live slot L in the order taken), records slot L's parent and token at back[step][L], writes the next input
 // tokens (0 past L) and, inside the loop's graph, sets run_pass = L > 0 and keep_going = L > 0 && pool < W && step + 1 < max_tokens.
+// Grouped (rwkv_b200_beam_search_groups): G independent searches of width W over the G * W slots, group g in slots g*W .. g*W + W - 1
+// with its own BeamState. The step's grid is (W, G); a group runs while n_live > 0, n_pool < W and step < max_tokens, and the CTAs of a
+// group that does not run return at once. The last CTA of each running group walks it as above; the last walker of the step sets
+// run_pass = some group took L > 0 and keep_going = some group runs on. A group that stops, or never ran (max_tokens 0), keeps its
+// slots k < n_keep: the gather of pass park_at (BeamLoop::steps at that pass) copies them (state Y -> X, logits -> park) and the
+// restore after the loop copies them back, as every pass in between evaluates all columns.
 constexpr int BEAM_MAX = 10;
 constexpr int BEAM_CANDS = 2 * BEAM_MAX;
 struct BeamHyp {                      // a finished hypothesis: stop id `token` drawn at `step` from live beam `parent` of the step before
@@ -347,25 +353,43 @@ struct BeamState {                    // written by the host per call (n_live = 
     uint32_t n_stop, width, max_tokens;
     uint32_t step;                    // steps run
     uint32_t n_live, n_pool;          // live beams and pool entries after the last step
-    uint32_t ticket, pad;
+    uint32_t ticket;
+    uint32_t n_keep, park_at, parked;  // slots kept once the group stops; the pass that parks them (0: none); set by that pass
     double score[BEAM_MAX];           // of the live beams
     uint32_t parent[BEAM_MAX];        // of the live beams: the gather map of the pass that evaluates them
     BeamHyp pool[BEAM_MAX];
     uint32_t cand_id[BEAM_MAX][BEAM_CANDS];
     float cand_lp[BEAM_MAX][BEAM_CANDS];    // NaN: no candidate
 };
+struct BeamLoop {                     // shared by the groups of one call; written by the host per call (n_active: groups that run)
+    uint32_t n_active, ticket, n_next, any_live;    // this step's walkers, their ticket, groups that run on, groups that took L > 0
+    uint32_t steps, pad[3];                         // steps run
+};
 struct BeamStepParams {
-    const float * logits;             // [width, n_vocab]: column k that of live beam k
-    int n_vocab, width;
-    BeamState * st;
-    uint32_t * back;                  // [max_tokens][width][2]: parent slot and token of every live slot of every step
-    int * next_tokens;                // [width]
+    const float * logits;             // [groups * width, n_vocab]: column g*W + k that of live beam k of group g
+    int n_vocab, width, groups;
+    BeamLoop * loop;
+    BeamState * st;                   // [groups]
+    uint32_t * back;                  // [max_tokens][groups * width][2]: parent slot (in its group) and token of every live slot of every step
+    int * next_tokens;                // [groups * width]
     bool set_handles;                 // inside a conditional graph: set run_pass and keep_going
     cudaGraphConditionalHandle run_pass, keep_going;
 };
 cudaError_t launch_beam_step(const BeamStepParams & p, cudaStream_t s);
 cudaError_t add_beam_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const BeamStepParams & p, cudaGraphNode_t * node);
-// dst slice k <- src slice st->parent[k] (state_len floats, seq_stride apart) for every live slot k < st->n_live.
-cudaError_t launch_beam_gather(const BeamState * st, int width, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);
+struct BeamCopyParams {
+    const BeamLoop * loop;
+    BeamState * st;                   // [groups]; the gather sets `parked` of the groups it parks
+    int width, groups, n_vocab;
+    float * y, * x;                   // the current slots and the pass's input (state_len floats, seq_stride apart)
+    long long seq_stride;
+    size_t state_len;
+    float * logits, * park;           // [groups * width, n_vocab]
+};
+// Before a pass, for every group g: x slice g*W + k <- y slice g*W + parent[k] for k < n_live if it took live beams at the last step,
+// or x <- y and park <- logits for its slots k < n_keep if this pass is its park_at.
+cudaError_t launch_beam_gather(const BeamCopyParams & p, cudaStream_t s);
+// After the loop: y <- x and logits <- park for the kept slots of every parked group.
+cudaError_t add_beam_restore_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const BeamCopyParams & p, cudaGraphNode_t * node);
 
 }  // namespace rwkv

@@ -272,6 +272,11 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_beam_search.restype = ctypes.c_bool
         lib.rwkv_b200_test_beam_step.argtypes = [ctypes.POINTER(BeamStepArgs)]
         lib.rwkv_b200_test_beam_step.restype = ctypes.c_bool
+        lib.rwkv_b200_beam_search_groups.argtypes = [vp, ctypes.c_size_t, P_U32, P_FLOAT, P_U32, ctypes.c_size_t, ctypes.c_size_t, P_U32, P_U32,
+                                                     P_DOUBLE, P_U8]
+        lib.rwkv_b200_beam_search_groups.restype = ctypes.c_bool
+        lib.rwkv_b200_test_beam_step_groups.argtypes = [ctypes.POINTER(BeamStepArgs), ctypes.c_size_t]
+        lib.rwkv_b200_test_beam_step_groups.restype = ctypes.c_bool
         lib.rwkv_b200_score.argtypes = [vp, P_U32, P_U32, ctypes.c_size_t, P_FLOAT, P_U8]
         lib.rwkv_b200_score.restype = ctypes.c_bool
         lib.rwkv_b200_batch_score_ragged.argtypes = [vp, P_U32, P_U32, P_U32, P_FLOAT, P_U8]
@@ -409,6 +414,28 @@ class RWKVSharedLibrary:
                                                   scores.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), finished.ctypes.data_as(P_U8)):
             raise ValueError(f"rwkv_b200_beam_search failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
         return [([int(t) for t in toks[r, :lengths[r]]], float(scores[r]), bool(finished[r])) for r in range(n_best) if lengths[r]]
+
+    def rwkv_b200_beam_search_groups(self, batch: RWKVContext, n_groups: int, max_tokens, length_penalty, stop_ids=(), n_best: int = 1):
+        """n_groups beam searches of width n_sequences / n_groups in one call, group g from sequence g * width, with its own
+        max_tokens[g] (0: the group is left as it is) and length_penalty[g]. Returns, per group, its hypotheses as
+        rwkv_b200_beam_search does: a list of (tokens, score, finished), best first."""
+        mt = np.ascontiguousarray(max_tokens, np.uint32)
+        lp = np.ascontiguousarray(length_penalty, np.float32)
+        if mt.shape != (n_groups,) or lp.shape != (n_groups,):
+            raise ValueError("max_tokens and length_penalty need one entry per group")
+        n = max(1, int(mt.max()))
+        toks = np.zeros((n_groups, n_best, n), np.uint32)
+        lengths = np.zeros((n_groups, n_best), np.uint32)
+        scores = np.zeros((n_groups, n_best), np.float64)
+        finished = np.zeros((n_groups, n_best), np.uint8)
+        stops = (ctypes.c_uint32 * max(1, len(stop_ids)))(*stop_ids)
+        P_U32, P_U8 = ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint8)
+        if not self.library.rwkv_b200_beam_search_groups(batch.ptr, n_groups, mt.ctypes.data_as(P_U32), lp.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                                         stops, len(stop_ids), n_best, toks.ctypes.data_as(P_U32), lengths.ctypes.data_as(P_U32),
+                                                         scores.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), finished.ctypes.data_as(P_U8)):
+            raise ValueError(f"rwkv_b200_beam_search_groups failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
+        return [[([int(t) for t in toks[g, r, :lengths[g, r]]], float(scores[g, r]), bool(finished[g, r])) for r in range(n_best) if lengths[g, r]]
+                for g in range(n_groups)]
 
     def rwkv_b200_batch_set_adapter(self, batch: RWKVContext, sequence: int, adapter: Optional[int]) -> None:
         """Runs sequence `sequence` of a batch context with `adapter` (None: the base weights) on every later pass. Only adapters made of
