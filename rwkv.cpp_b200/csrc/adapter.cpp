@@ -123,7 +123,7 @@ Adapter * create_adapter(Model * model, const AdapterTensor * t, size_t n, float
     // ---- upload ----
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, cudaSetDevice(m.dev.device) == cudaSuccess, "cudaSetDevice failed");
     if (bytes) {
-        const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&a->arena), bytes);
+        const cudaError_t e = a->arena.alloc(bytes);
         RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, nullptr, e == cudaSuccess, "Failed to allocate %zu bytes for the adapter: %s", bytes, cudaGetErrorString(e));
     }
     a->deltas.reserve(n_delta);                 // DevMatrix::lora points into it
@@ -165,10 +165,7 @@ Adapter * create_adapter(Model * model, const AdapterTensor * t, size_t n, float
         }
     }
     if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) {
-        cudaFree(a->arena);
-        RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, nullptr, false, "Failed to upload the adapter: %s", cudaGetErrorString(ce));
-    }
+    RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, nullptr, ce == cudaSuccess, "Failed to upload the adapter: %s", cudaGetErrorString(ce));
     m.refcount.fetch_add(1);      // the adapter's tables point into the model's arena: it keeps the model alive
     return a.release();
 }
@@ -178,7 +175,6 @@ bool destroy_adapter(Adapter * a, ErrorSink sink) {
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a->attached.load() == 0, "The adapter is attached to %d context(s); detach it first", a->attached.load());
     Model * model = a->model;
     cudaSetDevice(model->dev.device);
-    cudaFree(a->arena);
     delete a;
     if (model->refcount.fetch_sub(1) == 1) delete model;      // the last holder of the model
     return true;

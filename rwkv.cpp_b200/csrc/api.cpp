@@ -40,15 +40,13 @@ namespace {
 // NULL on the device.
 struct HookBuffers {
     struct Out { void * dev; void * host; size_t bytes; };
-    std::vector<void *> allocs;
+    std::vector<DeviceBuffer<void>> allocs;
     std::vector<Out> outs;
     bool ok = true;
 
     void * alloc(size_t bytes) {
-        void * d = nullptr;
-        if (ok) ok = cudaMalloc(&d, bytes) == cudaSuccess;
-        if (ok) allocs.push_back(d);
-        return ok ? d : nullptr;
+        if (ok) ok = allocs.emplace_back().alloc(bytes) == cudaSuccess;
+        return ok ? allocs.back().get() : nullptr;
     }
     template <class T> const T * in(const T * host, size_t n) {
         if (!host) return nullptr;
@@ -77,7 +75,6 @@ struct HookBuffers {
             if (ok) ok = cudaMemcpy(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost) == cudaSuccess;
         return ok;
     }
-    ~HookBuffers() { for (void * d : allocs) cudaFree(d); }
 };
 
 // The device every test hook runs on; false (and the flags set) without one.
@@ -489,12 +486,11 @@ bool rwkv_b200_sample_logits(const float * logits, size_t n_vocab, float tempera
     int dev = default_device(), n_dev = 0;
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, cudaGetDeviceCount(&n_dev) == cudaSuccess && dev < n_dev && cudaSetDevice(dev) == cudaSuccess,
                "No usable CUDA device; this engine has no CPU execution path");
-    float * d_logits = nullptr, * d_scratch = nullptr, * d_bv = nullptr, * d_prob = nullptr;
-    uint32_t * d_bi = nullptr, * d_tok = nullptr;
-    bool ok = cudaMalloc((void **) &d_logits, n_vocab * 4) == cudaSuccess && cudaMalloc((void **) &d_scratch, n_vocab * 4) == cudaSuccess &&
-              cudaMalloc((void **) &d_tok, 4) == cudaSuccess && cudaMalloc((void **) &d_prob, 4) == cudaSuccess &&
-              cudaMemcpy(d_logits, logits, n_vocab * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-    if (ok && n_bias) ok = cudaMalloc((void **) &d_bi, n_bias * 4) == cudaSuccess && cudaMalloc((void **) &d_bv, n_bias * 4) == cudaSuccess &&
+    DeviceBuffer<float> d_logits, d_scratch, d_bv, d_prob;
+    DeviceBuffer<uint32_t> d_bi, d_tok;
+    bool ok = d_logits.alloc(n_vocab * 4) == cudaSuccess && d_scratch.alloc(n_vocab * 4) == cudaSuccess && d_tok.alloc(4) == cudaSuccess &&
+              d_prob.alloc(4) == cudaSuccess && cudaMemcpy(d_logits, logits, n_vocab * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (ok && n_bias) ok = d_bi.alloc(n_bias * 4) == cudaSuccess && d_bv.alloc(n_bias * 4) == cudaSuccess &&
                            cudaMemcpy(d_bi, bias_ids, n_bias * 4, cudaMemcpyHostToDevice) == cudaSuccess && cudaMemcpy(d_bv, bias_values, n_bias * 4, cudaMemcpyHostToDevice) == cudaSuccess;
     if (ok) {
         SampleParams sp{};
@@ -504,7 +500,6 @@ bool rwkv_b200_sample_logits(const float * logits, size_t n_vocab, float tempera
         if (ok && prob_out) ok = cudaMemcpy(prob_out, d_prob, 4, cudaMemcpyDeviceToHost) == cudaSuccess;
     }
     cudaError_t e = cudaGetLastError();
-    cudaFree(d_logits); cudaFree(d_scratch); cudaFree(d_tok); cudaFree(d_prob); cudaFree(d_bi); cudaFree(d_bv);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "sampling failed on the device: %s", cudaGetErrorString(e));
     return true;
 }
@@ -1009,21 +1004,18 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     cp.stream.step = gp;
     // the streaming kernel's words in pinned mapped memory, as the engine keeps them: acked [R], published [R], timed_out, tokens
     // [R][GENERATE_MAX], ring [R][2][GEN_LP_RECORD]
-    struct Pinned {
-        uint32_t * host = nullptr;
-        ~Pinned() { if (host) cudaFreeHost(host); }
-    } pinned;
+    PinnedBuffer<uint32_t> pinned;
     const size_t ring_words = lp ? R * 2 * GEN_LP_RECORD : 0, tok_at = 2 * R + 1, ring_at = tok_at + R * GENERATE_MAX;
     uint32_t * mapped = nullptr;
     if (stream && hb.ok) {
-        hb.ok = cudaHostAlloc(reinterpret_cast<void **>(&pinned.host), (ring_at + ring_words) * sizeof(uint32_t), cudaHostAllocMapped) == cudaSuccess &&
-                cudaHostGetDevicePointer(reinterpret_cast<void **>(&mapped), pinned.host, 0) == cudaSuccess;
+        hb.ok = pinned.alloc_mapped((ring_at + ring_words) * sizeof(uint32_t)) == cudaSuccess;
         if (hb.ok) {
-            std::copy(stream->acked, stream->acked + R, pinned.host);
-            std::copy(stream->published, stream->published + R, pinned.host + R);
-            pinned.host[2 * R] = 0;
-            std::copy(stream->tokens, stream->tokens + R * GENERATE_MAX, pinned.host + tok_at);
-            if (lp) std::copy(stream->ring, stream->ring + ring_words, pinned.host + ring_at);
+            mapped = pinned.device();
+            std::copy(stream->acked, stream->acked + R, pinned.get());
+            std::copy(stream->published, stream->published + R, pinned + R);
+            pinned[2 * R] = 0;
+            std::copy(stream->tokens, stream->tokens + R * GENERATE_MAX, pinned + tok_at);
+            if (lp) std::copy(stream->ring, stream->ring + ring_words, pinned + ring_at);
             cp.stream.acked = mapped; cp.stream.published = mapped + R; cp.stream.timed_out = mapped + 2 * R; cp.stream.tokens = mapped + tok_at;
         }
     }
@@ -1072,18 +1064,16 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     }
     cudaError_t e = cudaSuccess;
     if (hb.ok && stream) {      // the streaming kernels exist only as graph nodes
-        cudaGraph_t g = nullptr;
-        cudaGraphExec_t x = nullptr;
+        Graph g;
+        GraphExec x;
         cudaGraphNode_t node = nullptr;
-        e = cudaGraphCreate(&g, 0);
+        e = g.create();
         if (e == cudaSuccess)
             e = samplers ? add_generate_sampled_step_node(g, nullptr, 0, smp, true, &node) : lp ? add_generate_logprob_step_node(g, nullptr, 0, lpp, true, &node)
               : constrained ? add_generate_constrained_step_node(g, nullptr, 0, cp, true, &node) : add_generate_stream_step_node(g, nullptr, 0, cp.stream, &node);
-        if (e == cudaSuccess) e = cudaGraphInstantiate(&x, g, 0);
+        if (e == cudaSuccess) e = x.instantiate(g);
         if (e == cudaSuccess) e = cudaGraphLaunch(x, 0);
         if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-        if (x) cudaGraphExecDestroy(x);
-        if (g) cudaGraphDestroy(g);
     } else if (hb.ok) {
         e = samplers ? launch_generate_sampled_step(smp, 0) : lp ? launch_generate_logprob_step(lpp, 0)
           : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
@@ -1103,10 +1093,10 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     for (size_t b = 0; constrained && b < R; b++)
         if (states[b] != UINT32_MAX) states[b] = states_out[b];
     if (stream) {
-        std::copy(pinned.host + R, pinned.host + 2 * R, stream->published);
-        *stream->timed_out = pinned.host[2 * R];
-        std::copy(pinned.host + tok_at, pinned.host + tok_at + R * GENERATE_MAX, stream->tokens);
-        if (lp) std::copy(pinned.host + ring_at, pinned.host + ring_at + ring_words, stream->ring);
+        std::copy(pinned + R, pinned + 2 * R, stream->published);
+        *stream->timed_out = pinned[2 * R];
+        std::copy(pinned + tok_at, pinned + tok_at + R * GENERATE_MAX, stream->tokens);
+        if (lp) std::copy(pinned + ring_at, pinned + ring_at + ring_words, stream->ring);
     }
     return true;
 }
@@ -1194,7 +1184,7 @@ bool rwkv_b200_stage_eval(struct rwkv_context * ctx, const uint32_t * tokens, si
 }
 
 // ---- layer pipeline over peer memory (kernels/pipe.cu) ----
-void * rwkv_b200_stream(struct rwkv_context * ctx) { return ctx ? reinterpret_cast<void *>(C(ctx)->stream) : nullptr; }
+void * rwkv_b200_stream(struct rwkv_context * ctx) { return ctx ? reinterpret_cast<void *>(C(ctx)->stream.get()) : nullptr; }
 size_t rwkv_b200_pipe_handle_size(void) { return sizeof(cudaIpcMemHandle_t); }
 
 bool rwkv_b200_pipe_export(struct rwkv_context * ctx, void * handle_out) {
@@ -1312,11 +1302,11 @@ uint64_t rwkv_b200_bytes_per_token(const struct rwkv_context * ctx, bool with_lo
 
 float rwkv_b200_time_resident(struct rwkv_context * ctx, const uint32_t * tokens, size_t tokens_per_step, int n_steps, int warmup_steps, bool want_logits) {
     Context * c = C(ctx);
-    cudaEvent_t e0, e1;
+    Event e0, e1;
     if (!tokens || tokens_per_step == 0 || n_steps <= 0 || cudaSetDevice(c->model->dev.device) != cudaSuccess) return -1.f;
     const uint32_t * t = tokens;
     for (int i = 0; i < warmup_steps; i++, t += tokens_per_step) if (!rwkv_b200_eval_resident(ctx, t, tokens_per_step, want_logits, nullptr)) return -1.f;
-    if (cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess) return -1.f;
+    if (e0.create() != cudaSuccess || e1.create() != cudaSuccess) return -1.f;
     cudaStreamSynchronize(c->stream);
     cudaEventRecord(e0, c->stream);
     bool ok = true;
@@ -1324,7 +1314,6 @@ float rwkv_b200_time_resident(struct rwkv_context * ctx, const uint32_t * tokens
     cudaEventRecord(e1, c->stream);
     float ms = -1.f;
     if (ok && cudaEventSynchronize(e1) == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
     return ok ? ms : -1.f;
 }
 
@@ -1348,7 +1337,6 @@ bool rwkv_b200_profile_pass(struct rwkv_context * ctx, const uint32_t * tokens, 
             if (ms > out->top_ms) { out->top_ms = ms; out->top_bytes = r.bytes; }
         }
     }
-    for (auto & r : c->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
     c->prof.clear();
     return ok;
 }
@@ -1370,10 +1358,8 @@ static bool trace_rearm(Context * c) {
 bool rwkv_b200_trace_enable(struct rwkv_context * ctx) {
     Context * c = C(ctx);
     if (cudaSetDevice(c->model->dev.device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return false;
-    if (!c->trace_buf && cudaMalloc((void **) &c->trace_buf, 1024 * sizeof(TraceRec)) != cudaSuccess) return false;
-    // graphs captured so far carry no trace slots: drop them so they are re-captured
-    for (auto & g : c->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
-    drop_generate_graphs(c);
+    if (!c->trace_buf && c->trace_buf.alloc(1024 * sizeof(TraceRec)) != cudaSuccess) return false;
+    drop_all_graphs(c);      // graphs captured so far carry no trace slots: drop them so they are re-captured
     return trace_rearm(c);
 }
 
@@ -1381,10 +1367,9 @@ void rwkv_b200_trace_disable(struct rwkv_context * ctx) {
     Context * c = C(ctx);
     if (!c->trace_buf || cudaSetDevice(c->model->dev.device) != cudaSuccess) return;
     cudaStreamSynchronize(c->stream);
-    for (auto & g : c->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
-    drop_generate_graphs(c);
-    cudaFree(c->trace_buf);
-    c->trace_buf = nullptr; c->trace_count = 0;
+    drop_all_graphs(c);
+    c->trace_buf.reset();
+    c->trace_count = 0;
 }
 
 // marks_us: optional [max_records][4] intra-kernel marks of CTA 0 (-1 when absent)
@@ -1424,10 +1409,12 @@ bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, 
     // passes of >= 32 tokens go through the tensor-core kernel, which streams the tile-major copy of the matrix
     const bool tiled = T >= 32 && gemm_tc_eligible(data_type, K) && !getenv("RWKV_B200_NO_TC");
     const size_t ws_bytes = gemm_tc_batch_workspace_bytes(T, (size_t) K);
-    uint8_t * dW = nullptr, * dWt = nullptr; float * dx = nullptr, * dy = nullptr; void * ws = nullptr;
-    bool ok = cudaMalloc((void **) &dW, (size_t) matrix_pitch(data_type, (uint64_t) K) * M + 256) == cudaSuccess && cudaMalloc((void **) &dx, sizeof(float) * K * T) == cudaSuccess &&
-              cudaMalloc((void **) &dy, sizeof(float) * M * T) == cudaSuccess && cudaMemcpy(dx, x, sizeof(float) * K * T, cudaMemcpyHostToDevice) == cudaSuccess &&
-              (!tiled || (cudaMalloc((void **) &dWt, gemm_tc_tiled_bytes(data_type, M, K)) == cudaSuccess && cudaMalloc(&ws, ws_bytes) == cudaSuccess)) &&
+    DeviceBuffer<uint8_t> dW, dWt;
+    DeviceBuffer<float> dx, dy;
+    DeviceBuffer<void> ws;
+    bool ok = dW.alloc((size_t) matrix_pitch(data_type, (uint64_t) K) * M + 256) == cudaSuccess && dx.alloc(sizeof(float) * K * T) == cudaSuccess &&
+              dy.alloc(sizeof(float) * M * T) == cudaSuccess && cudaMemcpy(dx, x, sizeof(float) * K * T, cudaMemcpyHostToDevice) == cudaSuccess &&
+              (!tiled || (dWt.alloc(gemm_tc_tiled_bytes(data_type, M, K)) == cudaSuccess && ws.alloc(ws_bytes) == cudaSuccess)) &&
               upload_matrix(weights, data_type, M, K, dW, dWt) == cudaSuccess;
     if (ok) {
         GemvBatch b;
@@ -1440,7 +1427,6 @@ bool rwkv_b200_matvec(int data_type, int K, int M, int T, const void * weights, 
              cudaMemcpy(y, dy, sizeof(float) * M * T, cudaMemcpyDeviceToHost) == cudaSuccess;
     }
     cudaError_t e = cudaGetLastError();
-    cudaFree(dW); cudaFree(dWt); cudaFree(dx); cudaFree(dy); cudaFree(ws);
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "matvec failed on the device: %s", cudaGetErrorString(e));
     return true;
 }

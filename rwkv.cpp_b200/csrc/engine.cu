@@ -29,7 +29,7 @@ namespace {
 // rwkv_eval with host state buffers: pipeline the state copies against layer groups? (RWKV_B200_OVERLAP=0/1, rwkv_b200_set_overlap)
 constexpr bool OVERLAP_DEFAULT = true;
 
-struct Scratch {      // carve-up of ctx->scratch for T tokens
+struct Scratch {      // carve-up of ctx->act.scratch for T tokens
     float * x, * xx, * sx;
     float * mix[6];
     float * r, * k, * v, * g, * w, * a, * vgate, * v_first, * y;
@@ -104,8 +104,8 @@ struct Pass {
     cudaStream_t stream = nullptr;        // ctx->stream, or the stream of a pipeline stage's caller
     float * state_in = nullptr, * state_out = nullptr;   // ctx->state_a -> ctx->state_b
     float * logits = nullptr;             // where the head writes: ctx->logits
-    Scratch s{};                          // ctx->scratch carved for T tokens
-    bool tokens_in_place = false;         // ctx->tokens already holds the tokens (the generation loop's step writes them): no upload
+    Scratch s{};                          // ctx->act.scratch carved for T tokens
+    bool tokens_in_place = false;         // ctx->act.tokens already holds the tokens (the generation loop's step writes them): no upload
     // Pipeline-stage hand-off (SURVEY.md 8e): device pointers of the caller, or NULL.
     // Layout: x f32[C x T], then (v7 only) v_first f32[C x T].
     const float * hidden_in = nullptr;
@@ -168,22 +168,22 @@ void xq_bind(GemvProblem & p, const unsigned char * q, int q_type) {
 bool launch_batch(Context * ctx, GemvBatch & b, cudaStream_t stream) {
     // tensor cores: chunks of >= 32 tokens; batch contexts (one token of each of B sequences: nothing to stay bit-identical with
     // across pass sizes) from 16 sequences on, where the multi-column SIMT consumer is instruction-bound
-    void * ws = ctx->use_tensor_cores ? ctx->act16 : nullptr;
-    CUDA_OK(ctx, gemv_route(b, ctx->model->dev, stream, ws, ctx->act16_bytes, ctx->batch_n > 0 ? BATCH_TC_MIN : 32));
+    void * ws = ctx->use_tensor_cores ? ctx->act.act16.get() : nullptr;
+    CUDA_OK(ctx, gemv_route(b, ctx->model->dev, stream, ws, ctx->act.act16_bytes, ctx->batch_n > 0 ? BATCH_TC_MIN : 32));
     return true;
 }
 
 bool run_base(Context * ctx, const Pass & p, Batch & batch) {
     if (!ctx->profiling) return launch_batch(ctx, batch.b, p.stream);
-    Context::ProfRecord rec{};
-    CUDA_OK(ctx, cudaEventCreate(&rec.start));
-    CUDA_OK(ctx, cudaEventCreate(&rec.stop));
+    Context::ProfRecord rec;
+    CUDA_OK(ctx, rec.start.create());
+    CUDA_OK(ctx, rec.stop.create());
     for (int i = 0; i < batch.b.n; i++)
         rec.bytes += (double) tensor_nbytes(batch.b.p[i].type, (uint64_t) batch.b.p[i].K, (uint64_t) batch.b.p[i].M, 1);
     CUDA_OK(ctx, cudaEventRecord(rec.start, p.stream));
     if (!launch_batch(ctx, batch.b, p.stream)) return false;
     CUDA_OK(ctx, cudaEventRecord(rec.stop, p.stream));
-    ctx->prof.push_back(rec);
+    ctx->prof.push_back(std::move(rec));
     return true;
 }
 
@@ -217,7 +217,7 @@ bool run_batch(Context * ctx, const Pass & p, Batch & batch) {
     }
     LoraBatch lb;
     size_t u_used, z_used;
-    if (!build_lora_batch(ctx->sink(), batch.b, n_slots, delta, col_slot, ctx->lora_u, ctx->lora_z, lb, u_used, z_used)) return false;
+    if (!build_lora_batch(ctx->sink(), batch.b, n_slots, delta, col_slot, ctx->lora.u, ctx->lora.z, lb, u_used, z_used)) return false;
     if (lb.n) CUDA_OK(ctx, launch_lora_shrink(lb, p.stream));
     if (!run_base(ctx, p, batch)) return false;
     if (lb.n) CUDA_OK(ctx, launch_lora_expand(lb, p.stream));
@@ -557,40 +557,33 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Pass & p, const flo
 }
 
 bool ensure_capacity(Context * ctx, int T, cudaStream_t stream) {
-    if (T <= ctx->capacity_T) return true;
+    if (T <= ctx->act.capacity_T) return true;
     const Model & m = *ctx->model;
-    int cap = ctx->capacity_T ? ctx->capacity_T : 1;
+    int cap = ctx->act.capacity_T ? ctx->act.capacity_T : 1;
     while (cap < T) cap *= 2;
     if (cap > MAX_TOKENS_PER_PASS) cap = MAX_TOKENS_PER_PASS;
-    if (ctx->scratch) { cudaFree(ctx->scratch); ctx->scratch = nullptr; }
-    if (ctx->act16) { cudaFree(ctx->act16); ctx->act16 = nullptr; ctx->act16_bytes = 0; }
-    if (ctx->tokens) { cudaFree(ctx->tokens); ctx->tokens = nullptr; }
     CUDA_OK(ctx, cudaStreamSynchronize(stream));
-    for (int i = 0; i < 2; i++) {
-        if (ctx->tokens_host[i]) { cudaFreeHost(ctx->tokens_host[i]); ctx->tokens_host[i] = nullptr; }
-        ctx->slot_used[i] = false;
-    }
-    for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
-    drop_generate_graphs(ctx);
-    ctx->capacity_T = 0;
+    ctx->act = {};
+    drop_all_graphs(ctx);
+    Context::Activations a;
     const size_t n = scratch_floats_for(m, cap);
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->scratch), n * sizeof(float));
+    cudaError_t e = a.scratch.alloc(n * sizeof(float));
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes of activation memory: %s", n * sizeof(float), cudaGetErrorString(e));
-    e = cudaMalloc(reinterpret_cast<void **>(&ctx->tokens), (size_t) cap * sizeof(int));
+    e = a.tokens.alloc((size_t) cap * sizeof(int));
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate the token buffer: %s", cudaGetErrorString(e));
     for (int i = 0; i < 2; i++) {
-        e = cudaMallocHost(reinterpret_cast<void **>(&ctx->tokens_host[i]), (size_t) cap * sizeof(int));
+        e = a.tokens_host[i].alloc((size_t) cap * sizeof(int));
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate pinned token staging: %s", cudaGetErrorString(e));
     }
     if (cap >= BATCH_TC_MIN) {   // fp16 staging for the tensor-core path: up to 8 distinct inputs of max(C, F) x round16(cap)
         Dims d = model_dims(m);
         const size_t kmax = d.F > d.C ? d.F : d.C;
-        ctx->act16_bytes = gemm_tc_batch_workspace_bytes(cap, kmax);
-        e = cudaMalloc(&ctx->act16, ctx->act16_bytes);
+        a.act16_bytes = gemm_tc_batch_workspace_bytes(cap, kmax);
+        e = a.act16.alloc(a.act16_bytes);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate fp16 staging: %s", cudaGetErrorString(e));
     }
-    ctx->scratch_floats = n;
-    ctx->capacity_T = cap;
+    a.capacity_T = cap;
+    ctx->act = std::move(a);
     return true;
 }
 
@@ -601,7 +594,7 @@ bool make_pass(Context * ctx, int T, bool want_logits, cudaStream_t stream, Pass
     if (!ensure_capacity(ctx, T, p.stream)) return false;
     p.T = T; p.want_logits = want_logits; p.phase = ctx->phase;
     p.state_in = ctx->state_a; p.state_out = ctx->state_b; p.logits = ctx->logits;
-    p.s = carve(*ctx->model, ctx->scratch, T);
+    p.s = carve(*ctx->model, ctx->act.scratch, T);
     return true;
 }
 
@@ -624,12 +617,12 @@ bool score_head(Context * ctx, const Pass & p) {
     const int C = m.n_embed, V = m.n_vocab, T = p.T;
     Batch b(T);
     if (score_on_tensor_cores(ctx, T)) {
-        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.head_tiled && ctx->act16, "The head has no tile-major copy");
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.head_tiled && ctx->act.act16, "The head has no tile-major copy");
         // the columns' LayerNorm goes to mix[0], which the layers no longer need
         CUDA_OK(ctx, launch_layer_norm_columns(p.s.x, ln_out_w(ctx), ln_out_b(ctx), C, T, p.s.mix[0], p.stream));
         GemvProblem & q = b.add(m.head, p.s.mix[0], ctx->score_logits);
         q.Wt = m.head_tiled;
-        CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, p.stream, ctx->act16, ctx->act16_bytes));
+        CUDA_OK(ctx, gemm_tc_launch(b.b, m.dev, p.stream, ctx->act.act16, ctx->act.act16_bytes));
     } else {
         GemvProblem & q = b.add(m.head, p.s.x, ctx->score_logits);
         q.pro = PRO_LAYERNORM; q.ln_w = ln_out_w(ctx); q.ln_b = ln_out_b(ctx);
@@ -653,9 +646,9 @@ bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
     g_trace_next = 0;
     const int C = m.n_embed, T = p.T;
     if (l0 == 0) {
-        if (!p.tokens_in_place) CUDA_OK(ctx, cudaMemcpyAsync(ctx->tokens, ctx->tokens_host[p.phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, p.stream));
+        if (!p.tokens_in_place) CUDA_OK(ctx, cudaMemcpyAsync(ctx->act.tokens, ctx->act.tokens_host[p.phase], (size_t) T * sizeof(int), cudaMemcpyHostToDevice, p.stream));
         const DevVec & ln0_w = ctx->adapter ? ctx->adapter->ln0_w : m.ln0_w, & ln0_b = ctx->adapter ? ctx->adapter->ln0_b : m.ln0_b;
-        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->tokens, T, C, ln0_w.data, ln0_b.data, p.s.x, p.stream));
+        CUDA_OK(ctx, launch_embed_ln0(m.emb.data, m.emb.type, m.emb.pitch, ctx->act.tokens, T, C, ln0_w.data, ln0_b.data, p.s.x, p.stream));
     }   // a later pipeline stage / layer group finds x (and v_first) already in place
     const size_t per_layer = m.state_floats_per_layer();
     for (int i = l0; i < l1; i++) {
@@ -677,12 +670,12 @@ bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
     } else if (p.want_logits && l1 == m.n_layer && p.seq_off) {
         // ragged: the head on the last column of every advancing sequence, gathered; its columns go to those sequences' logits
         const int n = p.n_active;
-        CUDA_OK(ctx, launch_copy_columns(p.s.x, p.head_col, ctx->head_x, nullptr, C, n, p.stream));
+        CUDA_OK(ctx, launch_copy_columns(p.s.x, p.head_col, ctx->ragged.head_x, nullptr, C, n, p.stream));
         Batch b(n);
-        GemvProblem & q = b.add(m.head, ctx->head_x, ctx->head_y);
+        GemvProblem & q = b.add(m.head, ctx->ragged.head_x, ctx->ragged.head_y);
         q.pro = PRO_LAYERNORM; q.ln_w = ln_out_w(ctx); q.ln_b = ln_out_b(ctx);
         if (!run_batch(ctx, p, b)) return false;
-        CUDA_OK(ctx, launch_copy_columns(ctx->head_y, nullptr, p.logits, p.head_seq, m.n_vocab, n, p.stream));
+        CUDA_OK(ctx, launch_copy_columns(ctx->ragged.head_y, nullptr, p.logits, p.head_seq, m.n_vocab, n, p.stream));
     } else if (p.want_logits && l1 == m.n_layer) {   // :705-708 / :851-854  head . LN(x_last; ln_out); a batch context wants every column
         Batch b(ctx->batch_n ? T : 1);
         GemvProblem & q = b.add(m.head, ctx->batch_n ? p.s.x : p.s.x + (size_t) (T - 1) * C, p.logits);
@@ -701,9 +694,9 @@ bool enqueue_pass(Context * ctx, const Pass & p, int seg) {
 // put copies between the layer groups: begin_pass (token staging, hand-off in), run_layers per segment, end_pass.
 bool begin_pass(Context * ctx, const uint32_t * tokens, const Pass & p) {
     const int phase = p.phase, T = p.T;
-    if (ctx->slot_used[phase]) CUDA_OK(ctx, cudaEventSynchronize(ctx->slot_free[phase]));   // pass n-2 has consumed this slot
+    if (ctx->act.slot_used[phase]) CUDA_OK(ctx, cudaEventSynchronize(ctx->slot_free[phase]));   // pass n-2 has consumed this slot
     const Model & m = *ctx->model;
-    if (m.layer_begin == 0) for (int t = 0; t < T; t++) ctx->tokens_host[phase][t] = (int) tokens[t];
+    if (m.layer_begin == 0) for (int t = 0; t < T; t++) ctx->act.tokens_host[phase][t] = (int) tokens[t];
     const size_t ct = (size_t) m.n_embed * (size_t) T * sizeof(float);
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_start, p.stream));
     if (p.hidden_in) {    // outside the captured graph: the caller's pointers may change from call to call
@@ -730,12 +723,11 @@ bool run_layers(Context * ctx, const Pass & p, int seg) {
         const unsigned long long before = g_kernel_launches;
         CUDA_OK(ctx, cudaStreamBeginCapture(p.stream, cudaStreamCaptureModeThreadLocal));
         const bool ok = enqueue_pass(ctx, p, seg);
-        cudaGraph_t graph = nullptr;
-        cudaError_t e = cudaStreamEndCapture(p.stream, &graph);
+        Graph graph;
+        cudaError_t e = graph.end_capture(p.stream);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess && graph, "CUDA graph capture failed: %s", cudaGetErrorString(e));
         g->launches = g_kernel_launches - before;
-        e = cudaGraphInstantiate(&g->exec, graph, 0);
-        cudaGraphDestroy(graph);
+        e = g->exec.instantiate(graph);
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, e == cudaSuccess, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
         CUDA_OK(ctx, cudaGraphLaunch(g->exec, p.stream));
         g_graph_launches++;
@@ -755,8 +747,8 @@ bool end_pass(Context * ctx, const Pass & p) {
     }
     CUDA_OK(ctx, cudaEventRecord(ctx->ev_stop, p.stream));
     CUDA_OK(ctx, cudaEventRecord(ctx->slot_free[p.phase], p.stream));
-    ctx->slot_used[p.phase] = true;
-    float * tmp = ctx->state_a; ctx->state_a = ctx->state_b; ctx->state_b = tmp;
+    ctx->act.slot_used[p.phase] = true;
+    std::swap(ctx->state_a, ctx->state_b);
     ctx->phase ^= 1;
     ctx->logits_valid = p.want_logits && m.layer_end == m.n_layer;
     return true;
@@ -767,14 +759,16 @@ bool forward_pass(Context * ctx, const uint32_t * tokens, const Pass & p) {
 }
 
 bool ensure_copy_streams(Context * ctx) {
-    if (ctx->copy_in) return true;
-    CUDA_OK(ctx, cudaStreamCreateWithFlags(&ctx->copy_in, cudaStreamNonBlocking));
-    CUDA_OK(ctx, cudaStreamCreateWithFlags(&ctx->copy_out, cudaStreamNonBlocking));
-    CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->pass_begin, cudaEventDisableTiming));
+    if (ctx->copies.in) return true;
+    Context::CopyStreams c;
+    CUDA_OK(ctx, c.in.create());
+    CUDA_OK(ctx, c.out.create());
+    CUDA_OK(ctx, c.pass_begin.create(cudaEventDisableTiming));
     for (int i = 0; i < Context::MAX_SEGMENTS; i++) {
-        CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->seg_in[i], cudaEventDisableTiming));
-        CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->seg_out[i], cudaEventDisableTiming));
+        CUDA_OK(ctx, c.seg_in[i].create(cudaEventDisableTiming));
+        CUDA_OK(ctx, c.seg_out[i].create(cudaEventDisableTiming));
     }
+    ctx->copies = std::move(c);
     return true;
 }
 
@@ -804,17 +798,17 @@ Context * create_context(Model * model, ErrorSink sink, int batch_n) {
     const size_t seqs = batch_n > 0 ? (size_t) batch_n : 1;
     if (batch_n > 0) { ctx->batch_n = batch_n; ctx->batch_stride = (long long) n; ctx->overlap_copies = false; }
     bool ok = cudaSetDevice(model->dev.device) == cudaSuccess
-        && cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) == cudaSuccess
-        && cudaEventCreate(&ctx->ev_start) == cudaSuccess && cudaEventCreate(&ctx->ev_stop) == cudaSuccess
-        && cudaEventCreateWithFlags(&ctx->slot_free[0], cudaEventDisableTiming) == cudaSuccess
-        && cudaEventCreateWithFlags(&ctx->slot_free[1], cudaEventDisableTiming) == cudaSuccess
-        && cudaMalloc(reinterpret_cast<void **>(&ctx->state_a), seqs * n * sizeof(float)) == cudaSuccess
-        && cudaMalloc(reinterpret_cast<void **>(&ctx->state_b), seqs * n * sizeof(float)) == cudaSuccess
-        && cudaMalloc(reinterpret_cast<void **>(&ctx->state_init), n * sizeof(float)) == cudaSuccess
-        && cudaMalloc(reinterpret_cast<void **>(&ctx->logits), seqs * (size_t) model->n_vocab * sizeof(float)) == cudaSuccess;
+        && ctx->stream.create() == cudaSuccess
+        && ctx->ev_start.create() == cudaSuccess && ctx->ev_stop.create() == cudaSuccess
+        && ctx->slot_free[0].create(cudaEventDisableTiming) == cudaSuccess
+        && ctx->slot_free[1].create(cudaEventDisableTiming) == cudaSuccess
+        && ctx->state_a.alloc(seqs * n * sizeof(float)) == cudaSuccess
+        && ctx->state_b.alloc(seqs * n * sizeof(float)) == cudaSuccess
+        && ctx->state_init.alloc(n * sizeof(float)) == cudaSuccess
+        && ctx->logits.alloc(seqs * (size_t) model->n_vocab * sizeof(float)) == cudaSuccess;
     if (ok && batch_n == 0) {      // staged-column hand-off slots (every handed-off vector has n_embed elements, at most 2 bytes each) 
         ctx->xq_slot_bytes = ((size_t) 2 * model->n_embed + 64 + 255) / 256 * 256;
-        ok = cudaMalloc(reinterpret_cast<void **>(&ctx->xq), (size_t) XQ_SLOTS * ctx->xq_slot_bytes) == cudaSuccess;
+        ok = ctx->xq.alloc((size_t) XQ_SLOTS * ctx->xq_slot_bytes) == cudaSuccess;
     }
     // a batch context's logits start as zeros: after ragged passes a column that was never computed is a uniform draw, not garbage
     if (ok && batch_n > 0) ok = cudaMemset(ctx->logits, 0, seqs * (size_t) model->n_vocab * sizeof(float)) == cudaSuccess;
@@ -846,54 +840,11 @@ void destroy_context(Context * ctx) {
     }
     Model * model = ctx->model;
     if (model) cudaSetDevice(model->dev.device);
-    if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->state_a); cudaFree(ctx->state_b); cudaFree(ctx->state_init); cudaFree(ctx->logits);
-    cudaFree(ctx->tokens); cudaFree(ctx->scratch); cudaFree(ctx->trace_buf); cudaFree(ctx->act16); cudaFree(ctx->xq);
+    for (cudaStream_t s : {ctx->stream.get(), ctx->copies.in.get(), ctx->copies.out.get()}) if (s) cudaStreamSynchronize(s);
     if (ctx->adapter) ctx->adapter->attached.fetch_sub(1);
     for (const Adapter * a : ctx->seq_adapter) if (a) a->attached.fetch_sub(1);
-    cudaFree(ctx->lora_u); cudaFree(ctx->lora_z);
-    for (int i = 0; i < 2; i++) {
-        if (ctx->tokens_host[i]) cudaFreeHost(ctx->tokens_host[i]);
-        if (ctx->ragged_host[i]) cudaFreeHost(ctx->ragged_host[i]);
-        if (ctx->slot_free[i]) cudaEventDestroy(ctx->slot_free[i]);
-    }
-    cudaFree(ctx->ragged_map); cudaFree(ctx->head_x); cudaFree(ctx->head_y);
-    cudaFree(ctx->score_logits); cudaFree(ctx->score_targets); cudaFree(ctx->score_lp); cudaFree(ctx->score_greedy);
-    for (auto & g : ctx->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (ctx->copy_pool) destroy_copy_pool(ctx->copy_pool);
-    if (ctx->bounce_in) { cudaFreeHost(ctx->bounce_in); cudaFreeHost(ctx->bounce_out); cudaFreeHost(ctx->bounce_logits); }
-    for (int i = 0; i < Context::MAX_SEGMENTS; i++) if (ctx->seg_d2h[i]) cudaEventDestroy(ctx->seg_d2h[i]);
-    if (ctx->copy_in) { cudaStreamSynchronize(ctx->copy_in); cudaStreamDestroy(ctx->copy_in); }
-    if (ctx->copy_out) { cudaStreamSynchronize(ctx->copy_out); cudaStreamDestroy(ctx->copy_out); }
-    if (ctx->pass_begin) cudaEventDestroy(ctx->pass_begin);
-    if (ctx->pipe_done) cudaEventDestroy(ctx->pipe_done);
-    for (int i = 0; i < Context::MAX_SEGMENTS; i++) { if (ctx->seg_in[i]) cudaEventDestroy(ctx->seg_in[i]); if (ctx->seg_out[i]) cudaEventDestroy(ctx->seg_out[i]); }
-    cudaFree(ctx->sample_token); cudaFree(ctx->sample_scratch); cudaFree(ctx->bias_ids); cudaFree(ctx->bias_values);
-    if (ctx->sample_token_host) cudaFreeHost(ctx->sample_token_host);
-    cudaFree(ctx->sample_rows); cudaFree(ctx->sample_tokens);
-    if (ctx->sample_rows_host) cudaFreeHost(ctx->sample_rows_host);
-    if (ctx->sample_tokens_host) cudaFreeHost(ctx->sample_tokens_host);
-    drop_generate_graphs(ctx);
-    cudaFree(ctx->gen_in); cudaFree(ctx->gen_out); cudaFree(ctx->gen_counts); cudaFree(ctx->gen_bias_ids); cudaFree(ctx->gen_bias_values);
-    cudaFree(ctx->gen_scratch); cudaFree(ctx->gen_park);
-    if (ctx->gen_in_host) cudaFreeHost(ctx->gen_in_host);
-    if (ctx->gen_out_host) cudaFreeHost(ctx->gen_out_host);
-    if (ctx->stream_host) cudaFreeHost(ctx->stream_host);
-    if (ctx->stream_done) cudaEventDestroy(ctx->stream_done);
-    cudaFree(ctx->lp_req); cudaFree(ctx->lp_dev);
-    if (ctx->lp_req_host) cudaFreeHost(ctx->lp_req_host);
-    if (ctx->lp_host) cudaFreeHost(ctx->lp_host);
-    if (ctx->lp_ring_host) cudaFreeHost(ctx->lp_ring_host);
-    cudaFree(ctx->smp_dev);
-    if (ctx->smp_host) cudaFreeHost(ctx->smp_host);
-    cudaFree(ctx->beam_loop); cudaFree(ctx->beam_park); cudaFree(ctx->beam_back);
-    if (ctx->beam_host) cudaFreeHost(ctx->beam_host);
-    for (auto & r : ctx->prof) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
-    if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
-    if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
+    delete ctx;      // the members' owners release every buffer, event, stream and graph, on the model's device
     if (model && model->refcount.fetch_sub(1) == 1) delete model;
-    delete ctx;
 }
 
 bool upload_state(Context * ctx, const float * state_in) {
@@ -931,26 +882,6 @@ static bool bounce_enabled() {
 // states below this size go the plain way (two helper threads cost ~0.1 ms); rwkv_b200_set_bounce_min_bytes moves the bar (tests)
 std::atomic<size_t> g_bounce_min_bytes{(size_t) 4 << 20};
 std::atomic<unsigned long long> g_graph_launches{0};
-CopyPool * new_copy_pool();
-static bool ensure_bounce(Context * ctx) {
-    if (ctx->bounce_in) return true;
-    const size_t bytes = ctx->model->state_len() * sizeof(float);
-    if (cudaMallocHost(reinterpret_cast<void **>(&ctx->bounce_in), bytes) != cudaSuccess ||
-        cudaMallocHost(reinterpret_cast<void **>(&ctx->bounce_out), bytes) != cudaSuccess ||
-        cudaMallocHost(reinterpret_cast<void **>(&ctx->bounce_logits), (size_t) ctx->model->n_vocab * sizeof(float)) != cudaSuccess) {
-        cudaGetLastError();
-        if (ctx->bounce_in) cudaFreeHost(ctx->bounce_in);
-        if (ctx->bounce_out) cudaFreeHost(ctx->bounce_out);
-        ctx->bounce_in = ctx->bounce_out = ctx->bounce_logits = nullptr;
-        return false;                      // not an error: the caller falls back to plain copies
-    }
-    for (int i = 0; i < Context::MAX_SEGMENTS; i++)
-        if (cudaEventCreateWithFlags(&ctx->seg_d2h[i], cudaEventDisableTiming) != cudaSuccess) return false;
-    ctx->copy_pool = new_copy_pool();
-    return ctx->copy_pool != nullptr;
-}
-}  // namespace rwkv (the pool type is named in engine.h)
-namespace rwkv {
 
 // The helper threads of the bounce path: COPY_LANES per direction, created with the bounce buffers and parked on a condition variable
 // between passes (spawning eight threads per token would cost more than the copies). One job = one pass: lane k of a direction copies
@@ -994,8 +925,23 @@ struct CopyPool {
         for (auto & t : th) if (t.joinable()) t.join();
     }
 };
-void destroy_copy_pool(CopyPool * p) { delete p; }
-CopyPool * new_copy_pool() { return new (std::nothrow) CopyPool(); }
+void CopyPoolDelete::operator()(CopyPool * p) const { delete p; }
+
+static bool ensure_bounce(Context * ctx) {
+    if (ctx->bounce.in) return true;
+    const size_t bytes = ctx->model->state_len() * sizeof(float);
+    Context::Bounce b;
+    bool ok = b.in.alloc(bytes) == cudaSuccess && b.out.alloc(bytes) == cudaSuccess &&
+              b.logits.alloc((size_t) ctx->model->n_vocab * sizeof(float)) == cudaSuccess;
+    for (int i = 0; ok && i < Context::MAX_SEGMENTS; i++) ok = b.seg_d2h[i].create(cudaEventDisableTiming) == cudaSuccess;
+    if (ok) b.pool.reset(new (std::nothrow) CopyPool());
+    if (!ok || !b.pool) {
+        cudaGetLastError();
+        return false;                      // not an error: the caller falls back to plain copies
+    }
+    ctx->bounce = std::move(b);
+    return true;
+}
 
 namespace {
 // Progress of one pass's copies; waits for the lanes whatever way the pass ends.
@@ -1036,7 +982,7 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
     };
     BouncePass bp;
     if (b_in || b_out) {
-        bp.pool = ctx->copy_pool;
+        bp.pool = ctx->bounce.pool.get();
         bp.pool->start([&, G, dev, b_in, b_out](int k) {
             const bool inward = k < LANES;
             const int lane = inward ? k : k - LANES;
@@ -1044,7 +990,7 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
                 if (!b_in) return;
                 for (int g = 1; g <= G && !bp.abort.load(); g++) {
                     size_t off, cnt; part(g, lane, off, cnt);
-                    if (cnt) memcpy(ctx->bounce_in + off, state_in + off, cnt * sizeof(float));
+                    if (cnt) memcpy(ctx->bounce.in + off, state_in + off, cnt * sizeof(float));
                     bp.in_parts[g - 1].fetch_add(1, std::memory_order_release);
                 }
             } else {
@@ -1053,25 +999,25 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
                 for (int g = 1; g <= G; g++) {
                     if (lane == 0) {      // one lane waits for the DMA, the others for that lane
                         while (bp.out_posted.load(std::memory_order_acquire) < g) { if (bp.abort.load()) return; std::this_thread::yield(); }
-                        if (cudaEventSynchronize(ctx->seg_d2h[g - 1]) != cudaSuccess) { bp.abort.store(true); return; }
+                        if (cudaEventSynchronize(ctx->bounce.seg_d2h[g - 1]) != cudaSuccess) { bp.abort.store(true); return; }
                         bp.out_arrived.store(g, std::memory_order_release);
                     } else {
                         while (bp.out_arrived.load(std::memory_order_acquire) < g) { if (bp.abort.load()) return; std::this_thread::yield(); }
                     }
                     size_t off, cnt; part(g, lane, off, cnt);
-                    if (cnt) memcpy(state_out + off, ctx->bounce_out + off, cnt * sizeof(float));
+                    if (cnt) memcpy(state_out + off, ctx->bounce.out + off, cnt * sizeof(float));
                 }
             }
         });
     }
     // nothing of this pass may start before everything enqueued earlier on the context's stream has finished with the state
-    CUDA_OK(ctx, cudaEventRecord(ctx->pass_begin, ctx->stream));
-    CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->pass_begin, 0));
+    CUDA_OK(ctx, cudaEventRecord(ctx->copies.pass_begin, ctx->stream));
+    CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copies.in, ctx->copies.pass_begin, 0));
     if (state_in && !b_in) {
         for (int g = 1; g <= G; g++) {
             size_t off, cnt; slice(g, off, cnt);
-            CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a + off, state_in + off, cnt * sizeof(float), cudaMemcpyDefault, ctx->copy_in));
-            CUDA_OK(ctx, cudaEventRecord(ctx->seg_in[g - 1], ctx->copy_in));
+            CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a + off, state_in + off, cnt * sizeof(float), cudaMemcpyDefault, ctx->copies.in));
+            CUDA_OK(ctx, cudaEventRecord(ctx->copies.seg_in[g - 1], ctx->copies.in));
         }
     } else if (!state_in && !resident_in) {
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a, ctx->state_init, m.state_len() * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -1082,39 +1028,39 @@ static bool eval_host_overlapped(Context * ctx, const uint32_t * tokens, int T, 
         if (b_in) {      // the slice is in pinned memory once every lane has delivered its part
             while (bp.in_parts[g - 1].load(std::memory_order_acquire) < LANES) std::this_thread::yield();
             size_t off, cnt; slice(g, off, cnt);
-            CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a + off, ctx->bounce_in + off, cnt * sizeof(float), cudaMemcpyHostToDevice, ctx->copy_in));
-            CUDA_OK(ctx, cudaEventRecord(ctx->seg_in[g - 1], ctx->copy_in));
+            CUDA_OK(ctx, cudaMemcpyAsync(ctx->state_a + off, ctx->bounce.in + off, cnt * sizeof(float), cudaMemcpyHostToDevice, ctx->copies.in));
+            CUDA_OK(ctx, cudaEventRecord(ctx->copies.seg_in[g - 1], ctx->copies.in));
         }
-        if (state_in) CUDA_OK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->seg_in[g - 1], 0));
+        if (state_in) CUDA_OK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->copies.seg_in[g - 1], 0));
         if (!run_layers(ctx, p, g)) return false;
-        CUDA_OK(ctx, cudaEventRecord(ctx->seg_out[g - 1], ctx->stream));
+        CUDA_OK(ctx, cudaEventRecord(ctx->copies.seg_out[g - 1], ctx->stream));
         if (b_out && g > 1) {      // one group behind: the copy-out stream never waits for something that has not been enqueued
             size_t off, cnt; slice(g - 1, off, cnt);
             // the new state of group g-1 is in state_b until end_pass swaps the buffers
-            CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->seg_out[g - 2], 0));
-            CUDA_OK(ctx, cudaMemcpyAsync(ctx->bounce_out + off, ctx->state_b + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, ctx->copy_out));
-            CUDA_OK(ctx, cudaEventRecord(ctx->seg_d2h[g - 2], ctx->copy_out));
+            CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copies.out, ctx->copies.seg_out[g - 2], 0));
+            CUDA_OK(ctx, cudaMemcpyAsync(ctx->bounce.out + off, ctx->state_b + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, ctx->copies.out));
+            CUDA_OK(ctx, cudaEventRecord(ctx->bounce.seg_d2h[g - 2], ctx->copies.out));
             bp.out_posted.store(g - 1, std::memory_order_release);
         }
     }
     if (!end_pass(ctx, p)) return false;      // the new state is ctx->state_a from here on
-    if (logits_out) CUDA_OK(ctx, cudaMemcpyAsync(b_log ? ctx->bounce_logits : logits_out, ctx->logits, (size_t) m.n_vocab * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    if (logits_out) CUDA_OK(ctx, cudaMemcpyAsync(b_log ? ctx->bounce.logits : logits_out, ctx->logits, (size_t) m.n_vocab * sizeof(float), cudaMemcpyDefault, ctx->stream));
     if (state_out && b_out) {
         size_t off, cnt; slice(G, off, cnt);
-        CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->seg_out[G - 1], 0));
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->bounce_out + off, ctx->state_a + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, ctx->copy_out));
-        CUDA_OK(ctx, cudaEventRecord(ctx->seg_d2h[G - 1], ctx->copy_out));
+        CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copies.out, ctx->copies.seg_out[G - 1], 0));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->bounce.out + off, ctx->state_a + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, ctx->copies.out));
+        CUDA_OK(ctx, cudaEventRecord(ctx->bounce.seg_d2h[G - 1], ctx->copies.out));
         bp.out_posted.store(G, std::memory_order_release);
     } else if (state_out) {
         for (int g = 1; g <= G; g++) {
             size_t off, cnt; slice(g, off, cnt);
-            CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->seg_out[g - 1], 0));
-            CUDA_OK(ctx, cudaMemcpyAsync(state_out + off, ctx->state_a + off, cnt * sizeof(float), cudaMemcpyDefault, ctx->copy_out));
+            CUDA_OK(ctx, cudaStreamWaitEvent(ctx->copies.out, ctx->copies.seg_out[g - 1], 0));
+            CUDA_OK(ctx, cudaMemcpyAsync(state_out + off, ctx->state_a + off, cnt * sizeof(float), cudaMemcpyDefault, ctx->copies.out));
         }
     }
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    if (b_log) memcpy(logits_out, ctx->bounce_logits, (size_t) m.n_vocab * sizeof(float));
-    if (state_out) CUDA_OK(ctx, cudaStreamSynchronize(ctx->copy_out));
+    if (b_log) memcpy(logits_out, ctx->bounce.logits, (size_t) m.n_vocab * sizeof(float));
+    if (state_out) CUDA_OK(ctx, cudaStreamSynchronize(ctx->copies.out));
     if (bp.pool) { bp.pool->wait(); bp.pool = nullptr; }      // the last slices have been copied to the caller
     return !bp.abort.load();
 }
@@ -1214,22 +1160,24 @@ static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t *
     const int B = ctx->batch_n;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     const size_t map_bytes = ragged_map_ints(B) * sizeof(int);
-    if (!ctx->ragged_map) {
-        for (int i = 0; i < 2; i++) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->ragged_host[i]), map_bytes));
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->head_x), (size_t) B * m.n_embed * sizeof(float)));
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->head_y), (size_t) B * m.n_vocab * sizeof(float)));
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->ragged_map), map_bytes));
+    if (!ctx->ragged.map) {
+        Context::Ragged r;
+        for (int i = 0; i < 2; i++) CUDA_OK(ctx, r.host[i].alloc(map_bytes));
+        CUDA_OK(ctx, r.head_x.alloc((size_t) B * m.n_embed * sizeof(float)));
+        CUDA_OK(ctx, r.head_y.alloc((size_t) B * m.n_vocab * sizeof(float)));
+        CUDA_OK(ctx, r.map.alloc(map_bytes));
+        ctx->ragged = std::move(r);
     }
     Pass p;
     if (!make_pass(ctx, T, want_logits, nullptr, p) || !begin_pass(ctx, tokens, p)) return false;   // waits until the pass that last used this phase's slots has read them
-    int * off = ctx->ragged_host[p.phase], * col_seq = off + B + 1, * head_col = col_seq + MAX_TOKENS_PER_PASS, * head_seq = head_col + B;
+    int * off = ctx->ragged.host[p.phase], * col_seq = off + B + 1, * head_col = col_seq + MAX_TOKENS_PER_PASS, * head_seq = head_col + B;
     off[0] = 0;
     for (int b = 0; b < B; b++) {
         off[b + 1] = off[b] + (int) counts[b];
         for (int t = off[b]; t < off[b + 1]; t++) col_seq[t] = b;
         if (counts[b]) { head_col[p.n_active] = off[b + 1] - 1; head_seq[p.n_active] = b; p.n_active++; }
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->ragged_map, off, map_bytes, cudaMemcpyHostToDevice, p.stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->ragged.map, off, map_bytes, cudaMemcpyHostToDevice, p.stream));
     // the state of every idle sequence (runs of them are contiguous) goes to state_b as it is: end_pass swaps the whole buffers
     const size_t n = m.state_len();
     for (int b = 0; b < B;) {
@@ -1239,7 +1187,7 @@ static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t *
         CUDA_OK(ctx, cudaMemcpyAsync(p.state_out + (size_t) b * n, p.state_in + (size_t) b * n, (size_t) (e - b) * n * sizeof(float), cudaMemcpyDeviceToDevice, p.stream));
         b = e;
     }
-    p.seq_off = ctx->ragged_map;
+    p.seq_off = ctx->ragged.map;
     p.col_seq = p.seq_off + B + 1;
     p.col_seq_host = col_seq;
     p.head_col = p.col_seq + MAX_TOKENS_PER_PASS;
@@ -1276,15 +1224,14 @@ bool ensure_head_tiled(Context * ctx) {
     std::lock_guard<std::mutex> lk(m.head_tiled_lock);
     if (m.head_tiled) return true;
     const size_t bytes = gemm_tc_tiled_bytes(m.head.type, m.head.M, m.head.K);
-    void * p = nullptr;
-    cudaError_t e = cudaMalloc(&p, bytes);
+    DeviceBuffer<uint8_t> p;
+    cudaError_t e = p.alloc(bytes);
     if (e != cudaSuccess) cudaGetLastError();
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes for the head's tile-major copy: %s", bytes, cudaGetErrorString(e));
     e = gemm_tc_repack(m.head.data, m.head.pitch, m.head.type, m.head.M, m.head.K, p, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // other contexts' streams use it from now on
-    if (e != cudaSuccess) cudaFree(p);
     CUDA_OK(ctx, e);
-    m.head_tiled = static_cast<uint8_t *>(p);
+    m.head_tiled = std::move(p);
     return true;
 }
 
@@ -1293,37 +1240,36 @@ bool ensure_head_tiled(Context * ctx) {
 bool prepare_score(Context * ctx, size_t n, bool any_tc) {
     const Model & m = *ctx->model;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    auto alloc = [&](void ** p, size_t bytes) {
-        const cudaError_t e = cudaMalloc(p, bytes);
-        if (e != cudaSuccess) { cudaGetLastError(); *p = nullptr; }
+    auto alloc = [&](auto & buf, size_t bytes) {
+        const cudaError_t e = buf.alloc(bytes);
+        if (e != cudaSuccess) cudaGetLastError();
         RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes of scoring buffers: %s", bytes, cudaGetErrorString(e));
         return true;
     };
-    if (!ctx->score_logits && !alloc(reinterpret_cast<void **>(&ctx->score_logits), (size_t) MAX_TOKENS_PER_PASS * m.n_vocab * sizeof(float))) return false;
-    if (n > ctx->score_capacity) {
+    if (!ctx->score_logits && !alloc(ctx->score_logits, (size_t) MAX_TOKENS_PER_PASS * m.n_vocab * sizeof(float))) return false;
+    if (n > ctx->score.capacity) {
         CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->score_targets); cudaFree(ctx->score_lp); cudaFree(ctx->score_greedy);
-        ctx->score_targets = nullptr; ctx->score_lp = nullptr; ctx->score_greedy = nullptr; ctx->score_capacity = 0;
-        size_t cap = 256;
-        while (cap < n) cap *= 2;
-        if (!alloc(reinterpret_cast<void **>(&ctx->score_targets), cap * sizeof(uint32_t)) || !alloc(reinterpret_cast<void **>(&ctx->score_lp), cap * sizeof(float)) ||
-            !alloc(reinterpret_cast<void **>(&ctx->score_greedy), cap)) return false;
-        ctx->score_capacity = cap;
+        ctx->score = {};
+        Context::ScoreIo io;
+        io.capacity = 256;
+        while (io.capacity < n) io.capacity *= 2;
+        if (!alloc(io.targets, io.capacity * sizeof(uint32_t)) || !alloc(io.lp, io.capacity * sizeof(float)) || !alloc(io.greedy, io.capacity)) return false;
+        ctx->score = std::move(io);
     }
     return !any_tc || ensure_head_tiled(ctx);
 }
 
 // Targets in, and the caller's outputs too, so that positions without a target come back as they were.
 bool score_copy_in(Context * ctx, const uint32_t * targets, size_t n, const float * logprobs_out, const uint8_t * greedy_out) {
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_targets, targets, n * sizeof(uint32_t), cudaMemcpyDefault, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_lp, logprobs_out, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
-    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(ctx->score_greedy, greedy_out, n, cudaMemcpyDefault, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score.targets, targets, n * sizeof(uint32_t), cudaMemcpyDefault, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->score.lp, logprobs_out, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(ctx->score.greedy, greedy_out, n, cudaMemcpyDefault, ctx->stream));
     return true;
 }
 
 bool score_copy_out(Context * ctx, size_t n, float * logprobs_out, uint8_t * greedy_out) {
-    CUDA_OK(ctx, cudaMemcpyAsync(logprobs_out, ctx->score_lp, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
-    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(greedy_out, ctx->score_greedy, n, cudaMemcpyDefault, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(logprobs_out, ctx->score.lp, n * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    if (greedy_out) CUDA_OK(ctx, cudaMemcpyAsync(greedy_out, ctx->score.greedy, n, cudaMemcpyDefault, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return true;
 }
@@ -1339,9 +1285,9 @@ bool score(Context * ctx, const uint32_t * tokens, const uint32_t * targets, siz
         const int T = (int) std::min(n - done, (size_t) MAX_TOKENS_PER_PASS);
         Pass p;
         if (!make_pass(ctx, T, true, nullptr, p)) return false;
-        p.targets = ctx->score_targets + done;
-        p.lp = ctx->score_lp + done;
-        p.greedy = greedy_out ? ctx->score_greedy + done : nullptr;
+        p.targets = ctx->score.targets + done;
+        p.lp = ctx->score.lp + done;
+        p.greedy = greedy_out ? ctx->score.greedy + done : nullptr;
         // enqueue_pass directly: a scoring pass is never captured into a graph or replayed from one
         if (!begin_pass(ctx, tokens + done, p) || !enqueue_pass(ctx, p, 0) || !end_pass(ctx, p)) return false;
         done += (size_t) T;
@@ -1354,7 +1300,7 @@ bool batch_score_ragged(Context * ctx, const uint32_t * tokens, const uint32_t *
     if (!check_ragged(ctx, tokens, counts, total)) return false;
     if (!prepare_score(ctx, total, score_on_tensor_cores(ctx, (int) total))) return false;
     if (!score_copy_in(ctx, targets, total, logprobs_out, greedy_out)) return false;
-    return ragged_pass(ctx, tokens, counts, (int) total, true, ctx->score_targets, ctx->score_lp, greedy_out ? ctx->score_greedy : nullptr) &&
+    return ragged_pass(ctx, tokens, counts, (int) total, true, ctx->score.targets, ctx->score.lp, greedy_out ? ctx->score.greedy.get() : nullptr) &&
            score_copy_out(ctx, total, logprobs_out, greedy_out);
 }
 
@@ -1362,17 +1308,18 @@ namespace {
 
 // Device copy of a logit bias list (the buffers grow as needed) and the scratch of scratch_floats floats the biased logits go to.
 bool upload_bias(Context * ctx, const uint32_t * bias_ids, const float * bias_values, size_t n_bias, size_t scratch_floats) {
-    if (!ctx->sample_scratch) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_scratch), scratch_floats * sizeof(float)));
-    if (n_bias > ctx->bias_capacity) {
+    if (!ctx->sample_scratch) CUDA_OK(ctx, ctx->sample_scratch.alloc(scratch_floats * sizeof(float)));
+    if (n_bias > ctx->bias.capacity) {
         CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->bias_ids); cudaFree(ctx->bias_values);
-        ctx->bias_ids = nullptr; ctx->bias_values = nullptr; ctx->bias_capacity = 0;
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_ids), n_bias * sizeof(uint32_t)));
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->bias_values), n_bias * sizeof(float)));
-        ctx->bias_capacity = n_bias;
+        ctx->bias = {};
+        Context::Bias b;
+        CUDA_OK(ctx, b.ids.alloc(n_bias * sizeof(uint32_t)));
+        CUDA_OK(ctx, b.values.alloc(n_bias * sizeof(float)));
+        b.capacity = n_bias;
+        ctx->bias = std::move(b);
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_ids, bias_ids, n_bias * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias_values, bias_values, n_bias * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias.ids, bias_ids, n_bias * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->bias.values, bias_values, n_bias * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     return true;
 }
 
@@ -1389,21 +1336,23 @@ bool sample_token(Context * ctx, float temperature, float top_p, double u, const
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, ctx->logits_valid, "No logits to sample from: the last evaluation skipped the head");
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.n_vocab <= 65536, "On-device sampling supports n_vocab <= 65536");
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    if (!ctx->sample_token) {
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_token), 2 * sizeof(uint32_t)));
-        CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_token_host), 2 * sizeof(uint32_t)));
+    if (!ctx->sample_out.token) {
+        Context::SampleOut o;
+        CUDA_OK(ctx, o.token.alloc(2 * sizeof(uint32_t)));
+        CUDA_OK(ctx, o.token_host.alloc(2 * sizeof(uint32_t)));
+        ctx->sample_out = std::move(o);
     }
     std::vector<uint64_t> seen;
     if (!check_bias_ids(ctx->sink(), bias_ids, n_bias, (size_t) m.n_vocab, seen)) return false;
     if (n_bias > 0 && !upload_bias(ctx, bias_ids, bias_values, n_bias, (size_t) m.n_vocab)) return false;
     SampleParams sp{};
     sp.logits = ctx->logits; sp.n_vocab = m.n_vocab; sp.temperature = temperature; sp.top_p = top_p; sp.u = u;
-    sp.bias_ids = ctx->bias_ids; sp.bias_values = ctx->bias_values; sp.n_bias = (int) n_bias;
-    sp.scratch = ctx->sample_scratch; sp.token_out = ctx->sample_token; sp.prob_out = nullptr;
+    sp.bias_ids = ctx->bias.ids; sp.bias_values = ctx->bias.values; sp.n_bias = (int) n_bias;
+    sp.scratch = ctx->sample_scratch; sp.token_out = ctx->sample_out.token; sp.prob_out = nullptr;
     CUDA_OK(ctx, launch_sample(sp, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_token_host, ctx->sample_token, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_out.token_host, ctx->sample_out.token, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    *token_out = ctx->sample_token_host[0];
+    *token_out = ctx->sample_out.token_host[0];
     return true;
 }
 
@@ -1459,22 +1408,26 @@ bool batch_sample(Context * ctx, const float * temperature, const float * top_p,
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, m.n_vocab <= 65536, "On-device sampling supports n_vocab <= 65536");
     const size_t n_bias = bias_offsets ? bias_offsets[B] : 0;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    if (!ctx->sample_rows) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_rows), (size_t) B * sizeof(SampleRow)));
-    if (!ctx->sample_rows_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_rows_host), (size_t) B * sizeof(SampleRow)));
-    if (!ctx->sample_tokens) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->sample_tokens), (size_t) B * sizeof(uint32_t)));
-    if (!ctx->sample_tokens_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->sample_tokens_host), (size_t) B * sizeof(uint32_t)));
+    if (!ctx->sample_rows.rows) {
+        Context::SampleRows r;
+        CUDA_OK(ctx, r.rows.alloc((size_t) B * sizeof(SampleRow)));
+        CUDA_OK(ctx, r.rows_host.alloc((size_t) B * sizeof(SampleRow)));
+        CUDA_OK(ctx, r.tokens.alloc((size_t) B * sizeof(uint32_t)));
+        CUDA_OK(ctx, r.tokens_host.alloc((size_t) B * sizeof(uint32_t)));
+        ctx->sample_rows = std::move(r);
+    }
     if (n_bias > 0 && !upload_bias(ctx, bias_ids, bias_values, n_bias, (size_t) B * m.n_vocab)) return false;
     // every call ends with a stream synchronisation, so the previous copy out of the pinned rows has completed
-    fill_sample_rows(ctx->sample_rows_host, B, temperature, top_p, u, bias_offsets);
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_rows, ctx->sample_rows_host, (size_t) B * sizeof(SampleRow), cudaMemcpyHostToDevice, ctx->stream));
+    fill_sample_rows(ctx->sample_rows.rows_host, B, temperature, top_p, u, bias_offsets);
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_rows.rows, ctx->sample_rows.rows_host, (size_t) B * sizeof(SampleRow), cudaMemcpyHostToDevice, ctx->stream));
     SampleBatchParams bp{};
-    bp.logits = ctx->logits; bp.n_vocab = m.n_vocab; bp.n_rows = B; bp.rows = ctx->sample_rows;
-    bp.bias_ids = n_bias ? ctx->bias_ids : nullptr; bp.bias_values = n_bias ? ctx->bias_values : nullptr;
-    bp.scratch = n_bias ? ctx->sample_scratch : nullptr; bp.token_out = ctx->sample_tokens; bp.prob_out = nullptr;
+    bp.logits = ctx->logits; bp.n_vocab = m.n_vocab; bp.n_rows = B; bp.rows = ctx->sample_rows.rows;
+    bp.bias_ids = n_bias ? ctx->bias.ids.get() : nullptr; bp.bias_values = n_bias ? ctx->bias.values.get() : nullptr;
+    bp.scratch = n_bias ? ctx->sample_scratch.get() : nullptr; bp.token_out = ctx->sample_rows.tokens; bp.prob_out = nullptr;
     CUDA_OK(ctx, launch_sample_batch(bp, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_tokens_host, ctx->sample_tokens, (size_t) B * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->sample_rows.tokens_host, ctx->sample_rows.tokens, (size_t) B * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(tokens_out, ctx->sample_tokens_host, (size_t) B * sizeof(uint32_t));
+    memcpy(tokens_out, ctx->sample_rows.tokens_host, (size_t) B * sizeof(uint32_t));
     return true;
 }
 
@@ -1488,7 +1441,7 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 
 // ---- device-side generation -----------------------------------------------------------------------------------------------------
 // The loop of a generate call is one graph launch: WHILE { step -> IF { pass X -> Y } -> step -> IF { pass Y -> X } }. Each step
-// (generate_sample_kernel) draws every active row's next token and writes it into ctx->tokens, then sets both conditions to "a row is
+// (generate_sample_kernel) draws every active row's next token and writes it into ctx->act.tokens, then sets both conditions to "a row is
 // still active". A body holds two passes because the passes double-buffer the state. In a batch context every pass computes all
 // columns, so its shape and graph stay fixed; a frozen row's state is copied back over its output after each pass and its logits,
 // parked by the step that froze it, come back after the loop.
@@ -1496,10 +1449,10 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // before the next draw of that row it waits for the calling thread to acknowledge it (stream_tokens), so that the pass evaluating
 // token j overlaps the callback of token j, and a callback can end its row before token j + 1 is drawn.
 // A loop that reports log-probabilities runs the logprob step kernels instead, in graphs of their own (gen_lp_graphs); they read the
-// call's GenLogprobRequest from ctx->lp_req, and the streaming one writes each token's record into the mapped ring before it publishes
+// call's GenLogprobRequest from ctx->lp_req.dev, and the streaming one writes each token's record into the mapped ring before it publishes
 // the token, so that stream_tokens can hand the record to the caller before on_token.
 // A loop with per-row samplers runs the sampled step kernels, in graphs of their own too (gen_smp_graphs); they read the rows, the bias
-// pool and the request word (ctx->lp_req, or NULL without log-probabilities) from ctx->smp_dev.
+// pool and the request word (ctx->lp_req.dev, or NULL without log-probabilities) from ctx->smp.dev.
 namespace {
 
 size_t gen_mask_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
@@ -1511,16 +1464,16 @@ GenStepParams generate_step_params(Context * ctx) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     GenStepParams gp{};
     gp.logits = ctx->logits; gp.n_vocab = ctx->model->n_vocab; gp.n_rows = rows;
-    gp.shared = reinterpret_cast<GenShared *>(ctx->gen_in);
-    gp.rows = reinterpret_cast<GenRow *>(ctx->gen_in + sizeof(GenShared));
-    gp.u = reinterpret_cast<const double *>(ctx->gen_in + gen_u_offset(rows));
-    gp.counts = ctx->gen_counts; gp.bias_ids = ctx->gen_bias_ids; gp.bias_values = ctx->gen_bias_values; gp.scratch = ctx->gen_scratch;
-    gp.n_generated = ctx->gen_out; gp.passes = ctx->gen_out + rows; gp.tokens = ctx->gen_out + gen_tokens_word(rows);
-    gp.next_tokens = ctx->tokens; gp.park = ctx->batch_n ? ctx->gen_park : nullptr;
+    gp.shared = reinterpret_cast<GenShared *>(ctx->gen.in.get());
+    gp.rows = reinterpret_cast<GenRow *>(ctx->gen.in + sizeof(GenShared));
+    gp.u = reinterpret_cast<const double *>(ctx->gen.in + gen_u_offset(rows));
+    gp.counts = ctx->gen.counts; gp.bias_ids = ctx->gen.bias_ids; gp.bias_values = ctx->gen.bias_values; gp.scratch = ctx->gen.scratch;
+    gp.n_generated = ctx->gen.out; gp.passes = ctx->gen.out + rows; gp.tokens = ctx->gen.out + gen_tokens_word(rows);
+    gp.next_tokens = ctx->act.tokens; gp.park = ctx->batch_n ? ctx->gen.park.get() : nullptr;
     return gp;
 }
 
-// Pass p of the loop (input tokens already in ctx->tokens) captured into `body`.
+// Pass p of the loop (input tokens already in ctx->act.tokens) captured into `body`.
 bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p) {
     CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(p.stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
     bool ok = enqueue_pass(ctx, p, 0);
@@ -1534,19 +1487,14 @@ bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p) {
     return true;
 }
 
-struct GraphHolder {
-    cudaGraph_t g = nullptr;
-    ~GraphHolder() { if (g) cudaGraphDestroy(g); }
-};
-
 size_t stream_token_offset(int rows) { return 2 * (size_t) rows + 1; }
 
 GenStreamParams generate_stream_params(Context * ctx) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     GenStreamParams sp{};
     sp.step = generate_step_params(ctx);
-    sp.published = ctx->stream_dev; sp.acked = ctx->stream_dev + rows; sp.timed_out = ctx->stream_dev + 2 * rows;
-    sp.tokens = ctx->stream_dev + stream_token_offset(rows);
+    sp.published = ctx->streamed.words.device(); sp.acked = ctx->streamed.words.device() + rows; sp.timed_out = ctx->streamed.words.device() + 2 * rows;
+    sp.tokens = ctx->streamed.words.device() + stream_token_offset(rows);
     return sp;
 }
 
@@ -1560,20 +1508,20 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
     p.tokens_in_place = true;
     {   // one uncaptured pass of the loop's shape first, as run_layers does before it captures; its logits go to the step's scratch
         // and its state to state_b, which holds nothing between passes
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) rows * sizeof(int), p.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->act.tokens, 0, (size_t) rows * sizeof(int), p.stream));
         Pass warm = p;
-        warm.logits = ctx->gen_scratch;
+        warm.logits = ctx->gen.scratch;
         if (!enqueue_pass(ctx, warm, 0)) return false;
     }
-    GraphHolder top;
-    CUDA_OK(ctx, cudaGraphCreate(&top.g, 0));
+    Graph top;
+    CUDA_OK(ctx, top.create());
     cudaGraphConditionalHandle keep_going;
-    CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&keep_going, top.g, 1, cudaGraphCondAssignDefault));
+    CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&keep_going, top, 1, cudaGraphCondAssignDefault));
     cudaGraphNodeParams wp = {};
     wp.type = cudaGraphNodeTypeConditional;
     wp.conditional.handle = keep_going; wp.conditional.type = cudaGraphCondTypeWhile; wp.conditional.size = 1;
     cudaGraphNode_t loop = nullptr;
-    CUDA_OK(ctx, cudaGraphAddNode(&loop, top.g, nullptr, 0, &wp));
+    CUDA_OK(ctx, cudaGraphAddNode(&loop, top, nullptr, 0, &wp));
     cudaGraph_t body = wp.conditional.phGraph_out[0];
     cudaGraphNode_t prev = nullptr;
     for (int half = 0; half < 2; half++) {
@@ -1583,12 +1531,12 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
         GenStepParams & gp = sp.step;
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
-        const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen_in + gen_mask_offset(rows)), ctx->gen_out + rows + 1};
-        const GenSamplerParams smp{cp, reinterpret_cast<const GenLogprobRequest * const *>(ctx->smp_dev),
-                                   reinterpret_cast<const GenSamplerRow *>(ctx->smp_dev + smp_rows_offset()),
-                                   reinterpret_cast<const GenBiasEntry *>(ctx->smp_dev + smp_bias_offset(rows))};
+        const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen.in + gen_mask_offset(rows)), ctx->gen.out + rows + 1};
+        const GenSamplerParams smp{cp, reinterpret_cast<const GenLogprobRequest * const *>(ctx->smp.dev.get()),
+                                   reinterpret_cast<const GenSamplerRow *>(ctx->smp.dev + smp_rows_offset()),
+                                   reinterpret_cast<const GenBiasEntry *>(ctx->smp.dev + smp_bias_offset(rows))};
         CUDA_OK(ctx, sampled ? add_generate_sampled_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, smp, streaming, &step)
-                     : logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req}, streaming, &step)
+                     : logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req.dev}, streaming, &step)
                      : constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
                      : streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
                                  : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
@@ -1600,67 +1548,71 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
         std::swap(p.state_in, p.state_out);      // the second pass reads what the first one wrote
         prev = cond;
     }
-    CUDA_OK(ctx, cudaGraphInstantiate(sampled ? &ctx->gen_smp_graphs[ctx->phase][streaming]
-                                      : logprobs ? &ctx->gen_lp_graphs[ctx->phase][streaming] : &ctx->gen_graphs[ctx->phase][streaming][constrained], top.g, 0));
+    GraphExec & exec = sampled ? ctx->gen_smp_graphs[ctx->phase][streaming]
+                       : logprobs ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
+    CUDA_OK(ctx, exec.instantiate(top));
     return true;
 }
 
 bool ensure_generate_buffers(Context * ctx) {
-    if (ctx->gen_in) return true;
+    if (ctx->gen.in) return true;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     const size_t V = (size_t) ctx->model->n_vocab, in_bytes = gen_u_offset(rows) + (size_t) rows * GENERATE_MAX * sizeof(double);
     const size_t out_bytes = gen_out_words(rows, GENERATE_MAX) * sizeof(uint32_t), table = (size_t) rows * V;
-    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->gen_in_host), in_bytes));
-    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->gen_out_host), out_bytes));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_out), out_bytes));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_counts), table * sizeof(uint32_t)));
-    CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_counts, 0, table * sizeof(uint32_t), ctx->stream));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_bias_ids), table * sizeof(uint32_t)));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_bias_values), table * sizeof(float)));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_scratch), table * sizeof(float)));
-    if (ctx->batch_n) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_park), table * sizeof(float)));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->gen_in), in_bytes));      // last: it marks the set as complete
+    Context::Generate g;
+    CUDA_OK(ctx, g.in_host.alloc(in_bytes));
+    CUDA_OK(ctx, g.out_host.alloc(out_bytes));
+    CUDA_OK(ctx, g.out.alloc(out_bytes));
+    CUDA_OK(ctx, g.counts.alloc(table * sizeof(uint32_t)));
+    CUDA_OK(ctx, cudaMemsetAsync(g.counts, 0, table * sizeof(uint32_t), ctx->stream));
+    CUDA_OK(ctx, g.bias_ids.alloc(table * sizeof(uint32_t)));
+    CUDA_OK(ctx, g.bias_values.alloc(table * sizeof(float)));
+    CUDA_OK(ctx, g.scratch.alloc(table * sizeof(float)));
+    if (ctx->batch_n) CUDA_OK(ctx, g.park.alloc(table * sizeof(float)));
+    CUDA_OK(ctx, g.in.alloc(in_bytes));
+    ctx->gen = std::move(g);
     return true;
 }
 
 bool ensure_stream_buffers(Context * ctx) {
-    if (ctx->stream_dev) return true;
+    if (ctx->streamed.words) return true;
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
-    const size_t bytes = (stream_token_offset(rows) + (size_t) rows * GENERATE_MAX) * sizeof(uint32_t);
-    if (!ctx->stream_done) CUDA_OK(ctx, cudaEventCreateWithFlags(&ctx->stream_done, cudaEventDisableTiming));
-    if (!ctx->stream_host) CUDA_OK(ctx, cudaHostAlloc(reinterpret_cast<void **>(&ctx->stream_host), bytes, cudaHostAllocMapped));
-    CUDA_OK(ctx, cudaHostGetDevicePointer(reinterpret_cast<void **>(&ctx->stream_dev), ctx->stream_host, 0));
+    Context::Streaming st;
+    CUDA_OK(ctx, st.done.create(cudaEventDisableTiming));
+    CUDA_OK(ctx, st.words.alloc_mapped((stream_token_offset(rows) + (size_t) rows * GENERATE_MAX) * sizeof(uint32_t)));
+    ctx->streamed = std::move(st);
     return true;
 }
 
 // The request and output buffers of a logprob call whose outputs take `words` 32-bit words, and for a streaming one the ring.
 bool ensure_logprob_buffers(Context * ctx, size_t words, bool streaming) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
-    if (!ctx->lp_req_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->lp_req_host), sizeof(GenLogprobRequest)));
-    if (!ctx->lp_req) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->lp_req), sizeof(GenLogprobRequest)));
-    if (words > ctx->lp_words) {      // no graph holds these addresses: they travel in the request
-        cudaFree(ctx->lp_dev);
-        if (ctx->lp_host) cudaFreeHost(ctx->lp_host);
-        ctx->lp_dev = ctx->lp_host = nullptr;
-        ctx->lp_words = 0;
-        CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->lp_dev), words * sizeof(uint32_t)));
-        CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->lp_host), words * sizeof(uint32_t)));
-        ctx->lp_words = words;
+    if (!ctx->lp_req.dev) {
+        Context::LogprobRequest r;
+        CUDA_OK(ctx, r.host.alloc(sizeof(GenLogprobRequest)));
+        CUDA_OK(ctx, r.dev.alloc(sizeof(GenLogprobRequest)));
+        ctx->lp_req = std::move(r);
     }
-    if (streaming && !ctx->lp_ring_dev) {
-        if (!ctx->lp_ring_host)
-            CUDA_OK(ctx, cudaHostAlloc(reinterpret_cast<void **>(&ctx->lp_ring_host), (size_t) rows * 2 * GEN_LP_RECORD * sizeof(uint32_t), cudaHostAllocMapped));
-        CUDA_OK(ctx, cudaHostGetDevicePointer(reinterpret_cast<void **>(&ctx->lp_ring_dev), ctx->lp_ring_host, 0));
+    if (words > ctx->lp_out.words) {      // no graph holds these addresses: they travel in the request
+        ctx->lp_out = {};
+        Context::LogprobOut o;
+        CUDA_OK(ctx, o.dev.alloc(words * sizeof(uint32_t)));
+        CUDA_OK(ctx, o.host.alloc(words * sizeof(uint32_t)));
+        o.words = words;
+        ctx->lp_out = std::move(o);
     }
+    if (streaming && !ctx->lp_ring) CUDA_OK(ctx, ctx->lp_ring.alloc_mapped((size_t) rows * 2 * GEN_LP_RECORD * sizeof(uint32_t)));
     return true;
 }
 
 // The sampler upload at its largest (GEN_BIAS_MAX entries per row), on the device and pinned.
 bool ensure_sampler_buffers(Context * ctx) {
-    if (ctx->smp_dev) return true;
+    if (ctx->smp.dev) return true;
     const size_t bytes = smp_bias_offset(ctx->batch_n ? ctx->batch_n : 1) + (size_t) (ctx->batch_n ? ctx->batch_n : 1) * GEN_BIAS_MAX * sizeof(GenBiasEntry);
-    if (!ctx->smp_host) CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->smp_host), bytes));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->smp_dev), bytes));
+    Context::Samplers smp;
+    CUDA_OK(ctx, smp.host.alloc(bytes));
+    CUDA_OK(ctx, smp.dev.alloc(bytes));
+    ctx->smp = std::move(smp);
     return true;
 }
 
@@ -1671,17 +1623,17 @@ void put_logprob_entry(const LogprobsOut & lp, size_t at, float logprob, float s
     for (size_t k = 0; k < lp.top_n; k++) { lp.top_ids[at * lp.top_n + k] = ids[k]; lp.top_logprobs[at * lp.top_n + k] = top_lps[k]; }
 }
 
-// The calling thread's side of a streaming loop that has been enqueued up to ctx->stream_done: calls on_token for every token the
+// The calling thread's side of a streaming loop that has been enqueued up to ctx->streamed.done: calls on_token for every token the
 // step kernel publishes, in order per row, and acknowledges each one (the stop bit set when on_token returned nonzero), until the
 // stream has passed the event and every published token is delivered. Busy-polls, yielding between empty sweeps. Returns false when
 // a wait of the device for an acknowledgement ran out. With lp, token j's ring record goes to entry j of lp's arrays (`stride` entries per row) first.
 bool stream_tokens(Context * ctx, TokenFn on_token, void * user, const LogprobsOut * lp, size_t stride) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
-    uint32_t * published = ctx->stream_host, * acked = published + rows, * tokens = published + stream_token_offset(rows);
+    uint32_t * published = ctx->streamed.words, * acked = published + rows, * tokens = published + stream_token_offset(rows);
     std::vector<uint32_t> delivered((size_t) rows, 0);
     ctx->in_stream = true;
     for (bool done = false; !done;) {
-        done = cudaEventQuery(ctx->stream_done) != cudaErrorNotReady;      // before the sweep, so that the last sweep sees every token
+        done = cudaEventQuery(ctx->streamed.done) != cudaErrorNotReady;      // before the sweep, so that the last sweep sees every token
         bool any = false;
         for (int b = 0; b < rows; b++) {
             const uint32_t n = __atomic_load_n(published + b, __ATOMIC_ACQUIRE);
@@ -1689,7 +1641,7 @@ bool stream_tokens(Context * ctx, TokenFn on_token, void * user, const LogprobsO
                 const uint32_t tok = __atomic_load_n(tokens + (size_t) b * GENERATE_MAX + j, __ATOMIC_RELAXED);
                 if (lp) {
                     uint32_t rec[GEN_LP_RECORD];
-                    const uint32_t * src = ctx->lp_ring_host + ((size_t) b * 2 + (j & 1u)) * GEN_LP_RECORD;
+                    const uint32_t * src = ctx->lp_ring + ((size_t) b * 2 + (j & 1u)) * GEN_LP_RECORD;
                     for (int w = 0; w < GEN_LP_RECORD; w++) rec[w] = __atomic_load_n(src + w, __ATOMIC_RELAXED);
                     float f[2 + GEN_TOP_MAX];
                     memcpy(f, rec, 2 * sizeof(float));
@@ -1713,34 +1665,33 @@ bool stream_tokens(Context * ctx, TokenFn on_token, void * user, const LogprobsO
 void drop_generate_graphs(Context * ctx) {
     for (auto & by_phase : ctx->gen_graphs)
         for (auto & by_streaming : by_phase)
-            for (auto & e : by_streaming) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+            for (auto & e : by_streaming) e.reset();
     for (auto & by_phase : ctx->gen_lp_graphs)
-        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+        for (auto & e : by_phase) e.reset();
     for (auto & by_phase : ctx->gen_smp_graphs)
-        for (auto & e : by_phase) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
-    for (auto & e : ctx->beam_graphs) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
+        for (auto & e : by_phase) e.reset();
+    for (auto & e : ctx->beam_graphs) e.reset();
+}
+
+// The captured passes hold the adapters, the trace buffer and the activation buffers of the time they were captured.
+void drop_all_graphs(Context * ctx) {
+    for (auto & g : ctx->graphs) g = Context::GraphSlot();
+    drop_generate_graphs(ctx);
 }
 
 namespace {
 
-// The scratch of the deltas (Context::lora_u / lora_z), allocated once for passes of up to MAX_TOKENS_PER_PASS columns.
+// The scratch of the deltas (Context::lora), allocated once for passes of up to MAX_TOKENS_PER_PASS columns.
 bool ensure_lora_scratch(Context * ctx) {
-    if (ctx->lora_u) return true;
+    if (ctx->lora.u) return true;
     const Dims d = model_dims(*ctx->model);
     const LoraScratchSize s = lora_scratch_floats(d.C, d.F);
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_u), s.u * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ctx->lora_z), s.z * sizeof(float));
-    if (e != cudaSuccess) {
-        cudaFree(ctx->lora_u); cudaFree(ctx->lora_z); ctx->lora_u = ctx->lora_z = nullptr;
-        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, false, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));
-    }
+    Context::LoraScratch l;
+    cudaError_t e = l.u.alloc(s.u * sizeof(float));
+    if (e == cudaSuccess) e = l.z.alloc(s.z * sizeof(float));
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate the adapter's scratch: %s", cudaGetErrorString(e));
+    ctx->lora = std::move(l);
     return true;
-}
-
-// The captured passes hold the tensors and launches of the adapters they were captured with.
-void drop_all_graphs(Context * ctx) {
-    for (auto & g : ctx->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = Context::GraphSlot(); }
-    drop_generate_graphs(ctx);
 }
 
 }  // namespace
@@ -1849,8 +1800,7 @@ Automaton * create_automaton(const Model * model, const uint16_t * next, size_t 
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, cudaSetDevice(model->dev.device) == cudaSuccess, "Cannot select the model's device");
     Automaton * a = new Automaton;
     a->model = model; a->device = model->dev.device; a->n_vocab = V; a->n_states = (uint32_t) n_states;
-    const bool ok = cudaMalloc(reinterpret_cast<void **>(&a->next), n_states * V * sizeof(uint16_t)) == cudaSuccess &&
-                    cudaMalloc(reinterpret_cast<void **>(&a->live), n_states) == cudaSuccess &&
+    const bool ok = a->next.alloc(n_states * V * sizeof(uint16_t)) == cudaSuccess && a->live.alloc(n_states) == cudaSuccess &&
                     cudaMemcpy(a->next, next, n_states * V * sizeof(uint16_t), cudaMemcpyDefault) == cudaSuccess &&
                     cudaMemcpy(a->live, live.data(), n_states, cudaMemcpyHostToDevice) == cudaSuccess;
     if (!ok) {
@@ -1864,8 +1814,6 @@ Automaton * create_automaton(const Model * model, const uint16_t * next, size_t 
 void destroy_automaton(Automaton * a) {
     if (!a) return;
     cudaSetDevice(a->device);
-    if (a->next) cudaFree(a->next);
-    if (a->live) cudaFree(a->live);
     delete a;
 }
 
@@ -1929,73 +1877,73 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     if (lp && !ensure_logprob_buffers(ctx, lp_words, streaming)) return false;
     if (samplers && !ensure_sampler_buffers(ctx)) return false;
     // the call's parameters, loop state and u in one upload (every call ends with a synchronisation, so the pinned buffer is free)
-    GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen_in_host);
+    GenShared * sh = reinterpret_cast<GenShared *>(ctx->gen.in_host.get());
     memset(sh, 0, sizeof(GenShared));
     for (size_t k = 0; k < n_stop; k++) sh->stop[k] = stop_ids[k];
     sh->n_stop = (uint32_t) n_stop; sh->stride = (uint32_t) n;
-    GenRow * gr = reinterpret_cast<GenRow *>(ctx->gen_in_host + sizeof(GenShared));
+    GenRow * gr = reinterpret_cast<GenRow *>(ctx->gen.in_host + sizeof(GenShared));
     for (int b = 0; b < rows; b++) gr[b] = GenRow{temperature[b], top_p[b], presence[b], frequency[b], max_tokens[b], 0, 0, 0};
-    GenMaskRow * mr = reinterpret_cast<GenMaskRow *>(ctx->gen_in_host + gen_mask_offset(rows));
+    GenMaskRow * mr = reinterpret_cast<GenMaskRow *>(ctx->gen.in_host + gen_mask_offset(rows));
     for (int b = 0; b < rows; b++)
         mr[b] = constrained && automata[b] ? GenMaskRow{automata[b]->next, automata[b]->live, automaton_states[b], 0} : GenMaskRow{nullptr, nullptr, 0, 0};
     const size_t u_off = gen_u_offset(rows);
-    memcpy(ctx->gen_in_host + u_off, u, (size_t) rows * n * sizeof(double));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_in, ctx->gen_in_host, u_off + (size_t) rows * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    memcpy(ctx->gen.in_host + u_off, u, (size_t) rows * n * sizeof(double));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen.in, ctx->gen.in_host, u_off + (size_t) rows * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     for (int b = 0; b < rows;) {      // counts of the rows that start from zero (runs of them are contiguous)
         if (keep_counts && keep_counts[b]) { b++; continue; }
         int e = b;
         while (e < rows && !(keep_counts && keep_counts[e])) e++;
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_counts + (size_t) b * V, 0, (size_t) (e - b) * V * sizeof(uint32_t), ctx->stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->gen.counts + (size_t) b * V, 0, (size_t) (e - b) * V * sizeof(uint32_t), ctx->stream));
         b = e;
     }
     const size_t out_words = gen_out_words(rows, n);
-    CUDA_OK(ctx, cudaMemsetAsync(ctx->gen_out, 0, out_words * sizeof(uint32_t), ctx->stream));
-    if (streaming) memset(ctx->stream_host, 0, stream_token_offset(rows) * sizeof(uint32_t));     // published, acked, timed_out
+    CUDA_OK(ctx, cudaMemsetAsync(ctx->gen.out, 0, out_words * sizeof(uint32_t), ctx->stream));
+    if (streaming) memset(ctx->streamed.words, 0, stream_token_offset(rows) * sizeof(uint32_t));     // published, acked, timed_out
     if (lp) {
-        float * f = reinterpret_cast<float *>(ctx->lp_dev);
-        *ctx->lp_req_host = GenLogprobRequest{(uint32_t) lp->top_n, 0, f, f + lp_cells, ctx->lp_dev + 2 * lp_cells, f + 2 * lp_cells + lp_cells * lp->top_n,
-                                              streaming ? ctx->lp_ring_dev : nullptr};
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_req, ctx->lp_req_host, sizeof(GenLogprobRequest), cudaMemcpyHostToDevice, ctx->stream));
+        float * f = reinterpret_cast<float *>(ctx->lp_out.dev.get());
+        *ctx->lp_req.host = GenLogprobRequest{(uint32_t) lp->top_n, 0, f, f + lp_cells, ctx->lp_out.dev + 2 * lp_cells, f + 2 * lp_cells + lp_cells * lp->top_n,
+                                              streaming ? ctx->lp_ring.device() : nullptr};
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_req.dev, ctx->lp_req.host, sizeof(GenLogprobRequest), cudaMemcpyHostToDevice, ctx->stream));
     }
     if (samplers) {     // the request word, the rows and the bias pool in one upload
-        *reinterpret_cast<const GenLogprobRequest **>(ctx->smp_host) = lp ? ctx->lp_req : nullptr;
-        GenSamplerRow * sr = reinterpret_cast<GenSamplerRow *>(ctx->smp_host + smp_rows_offset());
-        GenBiasEntry * pool = reinterpret_cast<GenBiasEntry *>(ctx->smp_host + smp_bias_offset(rows));
+        *reinterpret_cast<const GenLogprobRequest **>(ctx->smp.host.get()) = lp ? ctx->lp_req.dev.get() : nullptr;
+        GenSamplerRow * sr = reinterpret_cast<GenSamplerRow *>(ctx->smp.host + smp_rows_offset());
+        GenBiasEntry * pool = reinterpret_cast<GenBiasEntry *>(ctx->smp.host + smp_bias_offset(rows));
         uint32_t used = 0;
         for (int b = 0; b < rows; b++) {
             const SamplerIn & s = samplers[b];
             sr[b] = GenSamplerRow{s.top_k, s.min_p, used, used + (uint32_t) s.n_bias};
             for (size_t k = 0; k < s.n_bias; k++) pool[used++] = GenBiasEntry{s.bias_ids[k], s.bias_values[k]};
         }
-        CUDA_OK(ctx, cudaMemcpyAsync(ctx->smp_dev, ctx->smp_host, smp_bias_offset(rows) + used * sizeof(GenBiasEntry), cudaMemcpyHostToDevice, ctx->stream));
+        CUDA_OK(ctx, cudaMemcpyAsync(ctx->smp.dev, ctx->smp.host, smp_bias_offset(rows) + used * sizeof(GenBiasEntry), cudaMemcpyHostToDevice, ctx->stream));
     }
-    cudaGraphExec_t & graph = samplers ? ctx->gen_smp_graphs[ctx->phase][streaming]
-                            : lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
+    GraphExec & graph = samplers ? ctx->gen_smp_graphs[ctx->phase][streaming]
+                      : lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
     if (!graph && !build_generate_graph(ctx, streaming, constrained, lp != nullptr, samplers != nullptr)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
-    if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen_park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen_out_host, ctx->gen_out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (lp_words) CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_host, ctx->lp_dev, lp_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen.park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen.out_host, ctx->gen.out, out_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (lp_words) CUDA_OK(ctx, cudaMemcpyAsync(ctx->lp_out.host, ctx->lp_out.dev, lp_words * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     bool in_time = true;
     if (streaming) {
-        CUDA_OK(ctx, cudaEventRecord(ctx->stream_done, ctx->stream));
+        CUDA_OK(ctx, cudaEventRecord(ctx->streamed.done, ctx->stream));
         in_time = stream_tokens(ctx, on_token, user, lp, n);
     }
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    const uint32_t * res = ctx->gen_out_host;
+    const uint32_t * res = ctx->gen.out_host;
     memcpy(n_generated, res, (size_t) rows * sizeof(uint32_t));
     memcpy(tokens_out, res + gen_tokens_word(rows), (size_t) rows * n * sizeof(uint32_t));
     for (int b = 0; constrained && b < rows; b++)
         if (automata[b]) automaton_states[b] = res[rows + 1 + b];
     if (lp) {       // drawn entries from the device, the rest NaN / SCORE_NO_TARGET
-        const float * f = reinterpret_cast<const float *>(ctx->lp_host);
+        const float * f = reinterpret_cast<const float *>(ctx->lp_out.host.get());
         const std::vector<uint32_t> none(lp->top_n, SCORE_NO_TARGET);
         const std::vector<float> nans(lp->top_n, NAN);
         for (int b = 0; b < rows; b++)
             for (size_t i = 0; i < n; i++) {
                 const size_t at = (size_t) b * n + i, k = lp->top_n;
-                if (i < res[b]) put_logprob_entry(*lp, at, f[at], f[lp_cells + at], ctx->lp_host + 2 * lp_cells + at * k, f + 2 * lp_cells + lp_cells * k + at * k);
+                if (i < res[b]) put_logprob_entry(*lp, at, f[at], f[lp_cells + at], ctx->lp_out.host + 2 * lp_cells + at * k, f + 2 * lp_cells + lp_cells * k + at * k);
                 else put_logprob_entry(*lp, at, NAN, NAN, none.data(), nans.data());
             }
     }
@@ -2016,22 +1964,20 @@ namespace {
 
 bool ensure_beam_buffers(Context * ctx, size_t groups, size_t max_tokens) {
     const size_t N = (size_t) ctx->batch_n;
-    if (!ctx->beam_park) CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_park), N * (size_t) ctx->model->n_vocab * sizeof(float)));
-    if (groups <= ctx->beam_groups && max_tokens <= ctx->beam_capacity) return true;
-    groups = std::max(groups, ctx->beam_groups);
-    max_tokens = std::max(max_tokens, ctx->beam_capacity);
+    if (!ctx->beam_park) CUDA_OK(ctx, ctx->beam_park.alloc(N * (size_t) ctx->model->n_vocab * sizeof(float)));
+    if (groups <= ctx->beam.groups && max_tokens <= ctx->beam.capacity) return true;
+    groups = std::max(groups, ctx->beam.groups);
+    max_tokens = std::max(max_tokens, ctx->beam.capacity);
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
-    for (auto & e : ctx->beam_graphs) if (e) { cudaGraphExecDestroy(e); e = nullptr; }
-    cudaFree(ctx->beam_loop); cudaFree(ctx->beam_back);
-    if (ctx->beam_host) cudaFreeHost(ctx->beam_host);
-    ctx->beam_loop = nullptr; ctx->beam_state = nullptr; ctx->beam_back = nullptr; ctx->beam_host = nullptr;
-    ctx->beam_groups = 0; ctx->beam_capacity = 0;
+    for (auto & e : ctx->beam_graphs) e.reset();
+    ctx->beam = {};
     const size_t state_bytes = sizeof(BeamLoop) + groups * sizeof(BeamState), back_bytes = max_tokens * N * 2 * sizeof(uint32_t);
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_loop), state_bytes));
-    ctx->beam_state = reinterpret_cast<BeamState *>(ctx->beam_loop + 1);
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&ctx->beam_back), back_bytes));
-    CUDA_OK(ctx, cudaMallocHost(reinterpret_cast<void **>(&ctx->beam_host), state_bytes + back_bytes));
-    ctx->beam_groups = groups; ctx->beam_capacity = max_tokens;
+    Context::Beam b;
+    CUDA_OK(ctx, b.loop.alloc(state_bytes));
+    CUDA_OK(ctx, b.back.alloc(back_bytes));
+    CUDA_OK(ctx, b.host.alloc(state_bytes + back_bytes));
+    b.groups = groups; b.capacity = max_tokens;
+    ctx->beam = std::move(b);
     return true;
 }
 
@@ -2041,29 +1987,29 @@ bool build_beam_graph(Context * ctx, int groups) {
     if (!make_pass(ctx, N, true, nullptr, p)) return false;
     p.tokens_in_place = true;
     {   // one uncaptured pass of the loop's shape first, as build_generate_graph runs one: Y -> X with its logits set aside
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) N * sizeof(int), p.stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->act.tokens, 0, (size_t) N * sizeof(int), p.stream));
         Pass warm = p;
         warm.logits = ctx->beam_park;
         if (!enqueue_pass(ctx, warm, 0)) return false;
     }
     p.state_in = ctx->state_b; p.state_out = ctx->state_a;
-    GraphHolder top;
-    CUDA_OK(ctx, cudaGraphCreate(&top.g, 0));
+    Graph top;
+    CUDA_OK(ctx, top.create());
     cudaGraphConditionalHandle keep_going, run_pass;
-    CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&keep_going, top.g, 1, cudaGraphCondAssignDefault));
+    CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&keep_going, top, 1, cudaGraphCondAssignDefault));
     cudaGraphNodeParams wp = {};
     wp.type = cudaGraphNodeTypeConditional;
     wp.conditional.handle = keep_going; wp.conditional.type = cudaGraphCondTypeWhile; wp.conditional.size = 1;
     cudaGraphNode_t loop = nullptr, step = nullptr, cond = nullptr, restore = nullptr;
-    CUDA_OK(ctx, cudaGraphAddNode(&loop, top.g, nullptr, 0, &wp));
+    CUDA_OK(ctx, cudaGraphAddNode(&loop, top, nullptr, 0, &wp));
     cudaGraph_t body = wp.conditional.phGraph_out[0];
     CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&run_pass, body, 0, cudaGraphCondAssignDefault));
-    const BeamStepParams bp{ctx->logits, ctx->model->n_vocab, W, groups, ctx->beam_loop, ctx->beam_state, ctx->beam_back, ctx->tokens, true,
+    const BeamStepParams bp{ctx->logits, ctx->model->n_vocab, W, groups, ctx->beam.loop, ctx->beam.states(), ctx->beam.back, ctx->act.tokens, true,
                             run_pass, keep_going};
     CUDA_OK(ctx, add_beam_step_node(body, nullptr, 0, bp, &step));
-    const BeamCopyParams cp{ctx->beam_loop, ctx->beam_state, W, groups, ctx->model->n_vocab, p.state_out, p.state_in, ctx->batch_stride,
+    const BeamCopyParams cp{ctx->beam.loop, ctx->beam.states(), W, groups, ctx->model->n_vocab, p.state_out, p.state_in, ctx->batch_stride,
                             ctx->model->state_len(), ctx->logits, ctx->beam_park};
-    if (groups > 1) CUDA_OK(ctx, add_beam_restore_node(top.g, &loop, 1, cp, &restore));     // one group stops only when the loop does
+    if (groups > 1) CUDA_OK(ctx, add_beam_restore_node(top, &loop, 1, cp, &restore));     // one group stops only when the loop does
     cudaGraphNodeParams ip = {};
     ip.type = cudaGraphNodeTypeConditional;
     ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
@@ -2075,7 +2021,7 @@ bool build_beam_graph(Context * ctx, int groups) {
     const cudaError_t ec = cudaStreamEndCapture(p.stream, &out);
     if (e == cudaSuccess) e = ec;
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok && e == cudaSuccess, "Capturing the beam search pass failed: %s", cudaGetErrorString(e));
-    CUDA_OK(ctx, cudaGraphInstantiate(&ctx->beam_graphs[ctx->phase], top.g, 0));
+    CUDA_OK(ctx, ctx->beam_graphs[ctx->phase].instantiate(top));
     ctx->beam_graph_groups[ctx->phase] = groups;
     return true;
 }
@@ -2100,7 +2046,7 @@ bool beam_search(Context * ctx, int n_groups, const uint32_t * max_tokens, const
     for (int g = 0; g < n_groups; g++) n = std::max(n, (size_t) max_tokens[g]);
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
     if (!ensure_beam_buffers(ctx, (size_t) n_groups, n) || !ensure_capacity(ctx, N, ctx->stream)) return false;
-    BeamLoop * hl = reinterpret_cast<BeamLoop *>(ctx->beam_host);
+    BeamLoop * hl = reinterpret_cast<BeamLoop *>(ctx->beam.host.get());
     BeamState * hs = reinterpret_cast<BeamState *>(hl + 1);
     memset(hl, 0, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState));
     for (int g = 0; g < n_groups; g++) {
@@ -2114,17 +2060,17 @@ bool beam_search(Context * ctx, int n_groups, const uint32_t * max_tokens, const
             st.n_keep = (uint32_t) W; st.park_at = 1;     // never runs: every slot is kept from the first pass on
         }
     }
-    CUDA_OK(ctx, cudaMemcpyAsync(ctx->beam_loop, hl, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->beam.loop, hl, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyHostToDevice, ctx->stream));
     // a group that never runs takes no token; its slots still run in the passes, on token 0
-    if (n_groups > 1) CUDA_OK(ctx, cudaMemsetAsync(ctx->tokens, 0, (size_t) N * sizeof(int), ctx->stream));
-    cudaGraphExec_t & graph = ctx->beam_graphs[ctx->phase];
-    if (graph && ctx->beam_graph_groups[ctx->phase] != n_groups) { cudaGraphExecDestroy(graph); graph = nullptr; }
+    if (n_groups > 1) CUDA_OK(ctx, cudaMemsetAsync(ctx->act.tokens, 0, (size_t) N * sizeof(int), ctx->stream));
+    GraphExec & graph = ctx->beam_graphs[ctx->phase];
+    if (ctx->beam_graph_groups[ctx->phase] != n_groups) graph.reset();
     if (!graph && !build_beam_graph(ctx, n_groups)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
     uint32_t * back = reinterpret_cast<uint32_t *>(hs + n_groups);
-    CUDA_OK(ctx, cudaMemcpyAsync(hl, ctx->beam_loop, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_OK(ctx, cudaMemcpyAsync(back, ctx->beam_back, n * N * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(hl, ctx->beam.loop, sizeof(BeamLoop) + (size_t) n_groups * sizeof(BeamState), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_OK(ctx, cudaMemcpyAsync(back, ctx->beam.back, n * N * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     memset(tokens_out, 0, (size_t) n_groups * n_best * n * sizeof(uint32_t));
     for (int g = 0; g < n_groups; g++) {
@@ -2163,15 +2109,17 @@ bool beam_search(Context * ctx, int n_groups, const uint32_t * max_tokens, const
 
 bool pipe_ensure_box(Context * ctx) {
     Model & m = *ctx->model;
-    if (m.link.box) return true;
+    if (m.link.box) return true;      // a link without a box has no neighbours yet: the connect calls make the box first
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
-    m.link.slot_floats = stage_hidden_len(m, (size_t) MAX_TOKENS_PER_PASS);
-    m.link.bytes = sizeof(PipeBox) + (size_t) PIPE_SLOTS * m.link.slot_floats * sizeof(float);
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&m.link.box), m.link.bytes));
-    CUDA_OK(ctx, cudaMemset(m.link.box, 0, sizeof(PipeBox)));
-    CUDA_OK(ctx, cudaMalloc(reinterpret_cast<void **>(&m.link.counters), 8 * sizeof(unsigned long long)));
-    CUDA_OK(ctx, cudaMemset(m.link.counters, 0, 8 * sizeof(unsigned long long)));
+    PipeLink link;
+    link.slot_floats = stage_hidden_len(m, (size_t) MAX_TOKENS_PER_PASS);
+    link.bytes = sizeof(PipeBox) + (size_t) PIPE_SLOTS * link.slot_floats * sizeof(float);
+    CUDA_OK(ctx, link.box.alloc(link.bytes));
+    CUDA_OK(ctx, cudaMemset(link.box, 0, sizeof(PipeBox)));
+    CUDA_OK(ctx, link.counters.alloc(8 * sizeof(unsigned long long)));
+    CUDA_OK(ctx, cudaMemset(link.counters, 0, 8 * sizeof(unsigned long long)));
     CUDA_OK(ctx, cudaDeviceSynchronize());
+    m.link = std::move(link);
     return true;
 }
 
@@ -2332,7 +2280,7 @@ bool pipeline_eval_host(Context * head, const uint32_t * tokens, size_t T, size_
             // completion marker of THIS evaluation on stage r. Waiting on the stream itself (cudaStreamSynchronize) outside the lock
             // would be illegal whenever another host thread is capturing its stage graph on the same stream at that moment (found by
             // compute-sanitizer's slower timing: cudaErrorStreamCaptureInvalidated); an event recorded before that capture began is fine.
-            if (!c->pipe_done) CUDA_OK(head, cudaEventCreateWithFlags(&c->pipe_done, cudaEventDisableTiming));
+            if (!c->pipe_done) CUDA_OK(head, c->pipe_done.create(cudaEventDisableTiming));
             CUDA_OK(head, cudaEventRecord(c->pipe_done, g.streams[r]));
         }
     }

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <atomic>
 #include <cstdint>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -23,12 +24,8 @@ struct PipeGroup {
     std::atomic<int> refs{0};
 };
 
-struct SampleRow;                       // per-sequence sampling parameters (kernels/ops.h)
-struct BeamState;                       // the device state of a beam search (kernels/ops.h)
-struct BeamLoop;                        // the state its groups share (kernels/ops.h)
-struct GenLogprobRequest;               // the per-call request of the logprob generation kernels (kernels/ops.h)
 struct CopyPool;                        // helper threads of the pageable-buffer bounce path (engine.cu)
-void destroy_copy_pool(CopyPool * p);
+struct CopyPoolDelete { void operator()(CopyPool * p) const; };
 
 // A LoRA adapter of rwkv_b200_adapter_create (include/rwkv_b200.h), in the HBM of its model's device: copies of the model's layers and
 // top-level vectors in which every replaced tensor points at its replacement and every adapted matrix carries its LoraDelta. A
@@ -38,7 +35,7 @@ struct Adapter {
     std::vector<Layer> layers;           // indexed by absolute layer id, as Model::layers
     DevVec ln0_w, ln0_b, ln_out_w, ln_out_b;
     std::vector<LoraDelta> deltas;       // DevMatrix::lora points into it
-    uint8_t * arena = nullptr;           // A, B and the replacements
+    DeviceBuffer<uint8_t> arena;         // A, B and the replacements
     bool replaces = false;               // some entry is a replacement (rank 0): it cannot be attached to one sequence of a batch
     mutable std::atomic<int> attached{0};   // contexts, and sequences of batch contexts, that have it attached
 };
@@ -56,32 +53,35 @@ Adapter * create_adapter(Model * model, const AdapterTensor * t, size_t n, float
 // false with RWKV_ERROR_ARGS while a context has it attached. Deletes the model when the adapter held its last reference.
 bool destroy_adapter(Adapter * a, ErrorSink sink);
 
+// Every CUDA resource of a context is a member owner (cuda_handles.h), released when the context is deleted, in the reverse order of
+// declaration. A lazily allocated set is a member struct built by one ensure function in engine.cu: complete or empty, never partial.
 struct Context {
+    Stream stream;                         // declared first, so destroyed last: the other members' work is enqueued on it
     Model * model = nullptr;
     PipeGroup * group = nullptr;           // set on the stage-0 context of an in-process pipeline
     std::vector<Context *> stages;         // ... which owns the contexts of stages 1 .. N-1
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
+    Event ev_start, ev_stop;
 
     // device buffers
-    float * state_a = nullptr;       // current input state
-    float * state_b = nullptr;       // output state of the running evaluation
-    float * state_init = nullptr;    // rwkv_init_state image, copied when state_in == NULL
-    float * logits = nullptr;        // [n_vocab]
-    int * tokens = nullptr;          // [capacity_T]
-    float * scratch = nullptr;       // activation arena for capacity_T tokens
-    unsigned char * xq = nullptr;    // staged activation columns handed from producer kernels to single-token GEMVs (act_stage.cuh)
+    DeviceBuffer<float> state_a;           // current input state
+    DeviceBuffer<float> state_b;           // output state of the running evaluation
+    DeviceBuffer<float> state_init;        // rwkv_init_state image, copied when state_in == NULL
+    DeviceBuffer<float> logits;            // [n_vocab]
+    DeviceBuffer<unsigned char> xq;        // staged activation columns handed from producer kernels to single-token GEMVs (act_stage.cuh)
     size_t xq_slot_bytes = 0;
-    cudaEvent_t pipe_done = nullptr; // in-process pipeline: end of this context's latest evaluation on its stage's stream
-    void * act16 = nullptr;          // fp16 copies of GEMM inputs for the tensor-core prefill path
-    size_t act16_bytes = 0;
+    Event pipe_done;                 // in-process pipeline: end of this context's latest evaluation on its stage's stream
     bool use_tensor_cores = true;
-    size_t scratch_floats = 0;
-    int capacity_T = 0;
-    // Two pinned token slots, used alternately (`phase`): the host may prepare pass n+1 while pass n runs.
-    int * tokens_host[2] = {nullptr, nullptr};
-    cudaEvent_t slot_free[2] = {nullptr, nullptr};   // recorded after the pass that last read the slot
-    bool slot_used[2] = {false, false};
+    // The buffers of passes of up to capacity_T tokens (ensure_capacity): the tokens, the activation arena, fp16 copies of GEMM inputs
+    // for the tensor-core path, and two pinned token slots, used alternately (`phase`): the host may prepare pass n+1 while pass n runs.
+    struct Activations {
+        DeviceBuffer<int> tokens;          // [capacity_T]
+        DeviceBuffer<float> scratch;
+        DeviceBuffer<void> act16; size_t act16_bytes = 0;
+        PinnedBuffer<int> tokens_host[2];
+        bool slot_used[2] = {false, false};   // slot_free has been recorded since the slot was allocated
+        int capacity_T = 0;
+    } act;
+    Event slot_free[2];                    // recorded after the pass that last read the slot
     int phase = 0;                   // flips every pass together with the state_a/state_b swap
 
     // A single-token pass runs either over all resident layers at once (segment 0) or, when the caller's host state is copied in
@@ -92,25 +92,25 @@ struct Context {
     static int slot_index(bool want_logits, int phase, int segment) { return ((want_logits ? 1 : 0) * 2 + phase) * (1 + MAX_SEGMENTS) + segment; }
     int n_segments = 1;              // layer groups of the overlapped path (1 = no overlap)
     bool overlap_copies = false;     // rwkv_eval with host state: pipeline the state copies against the layer groups
-    cudaStream_t copy_in = nullptr, copy_out = nullptr;
-    cudaEvent_t seg_in[MAX_SEGMENTS] = {}, seg_out[MAX_SEGMENTS] = {};
-    cudaEvent_t pass_begin = nullptr;
+    struct CopyStreams { Stream in, out; Event pass_begin, seg_in[MAX_SEGMENTS], seg_out[MAX_SEGMENTS]; } copies;
     // pinned bounce buffers for pageable caller memory (engine.cu: eval_host_overlapped), allocated on first need
-    float * bounce_in = nullptr, * bounce_out = nullptr, * bounce_logits = nullptr;
-    cudaEvent_t seg_d2h[MAX_SEGMENTS] = {};          // slice g has arrived in bounce_out
-    CopyPool * copy_pool = nullptr;
+    struct Bounce {
+        PinnedBuffer<float> in, out, logits;
+        Event seg_d2h[MAX_SEGMENTS];       // slice g has arrived in `out`
+        std::unique_ptr<CopyPool, CopyPoolDelete> pool;   // declared after the buffers, so its threads are joined before they are freed
+    } bounce;
 
     // CUDA graphs for single-token passes; captured on the second use of a slot.
-    struct GraphSlot { cudaGraphExec_t exec = nullptr; int uses = 0; unsigned long long launches = 0; };
+    struct GraphSlot { GraphExec exec; int uses = 0; unsigned long long launches = 0; };
     GraphSlot graphs[N_SLOTS];
     bool use_graphs = true;
 
     // Profiling mode (bench.py roofline leg): CUDA events around every GEMV launch, graphs off.
     bool profiling = false;
-    struct ProfRecord { cudaEvent_t start, stop; double bytes; };
+    struct ProfRecord { Event start, stop; double bytes = 0; };
     std::vector<ProfRecord> prof;
 
-    TraceRec * trace_buf = nullptr;  // in-kernel timeline records (rwkv_b200_trace_*), 1024 slots
+    DeviceBuffer<TraceRec> trace_buf;  // in-kernel timeline records (rwkv_b200_trace_*), 1024 slots
     int trace_count = 0;             // slots used by the last enqueued / captured pass
     const char * trace_names[1024] = {};   // kernel name per slot (string literals)
 
@@ -121,81 +121,77 @@ struct Context {
     long long batch_stride = 0;
     // Ragged passes of a batch context (batch_eval_ragged), allocated on the first one. The host writes each pass's map into a pinned
     // slot that follows the tokens_host / slot_free rule: column offsets [batch_n + 1], the sequence of every column
-    // [MAX_TOKENS_PER_PASS], then the last column and the index of every advancing sequence [batch_n each]; ragged_map is its device
+    // [MAX_TOKENS_PER_PASS], then the last column and the index of every advancing sequence [batch_n each]; map is its device
     // copy. The head runs on the gathered last columns (head_x [C, batch_n]) into head_y [n_vocab, batch_n].
-    int * ragged_host[2] = {nullptr, nullptr};
-    int * ragged_map = nullptr;
-    float * head_x = nullptr, * head_y = nullptr;
-    // Scoring passes (score, batch_score_ragged), allocated on the first: the head's output for every column of a pass
-    // ([MAX_TOKENS_PER_PASS, n_vocab]), and the targets and results of a call's tokens (score_capacity entries each).
-    float * score_logits = nullptr;
-    uint32_t * score_targets = nullptr;
-    float * score_lp = nullptr;
-    uint8_t * score_greedy = nullptr;
-    size_t score_capacity = 0;
+    struct Ragged { PinnedBuffer<int> host[2]; DeviceBuffer<int> map; DeviceBuffer<float> head_x, head_y; } ragged;
+    // Scoring passes (score, batch_score_ragged): the head's output for every column of a pass ([MAX_TOKENS_PER_PASS, n_vocab]),
+    // allocated on the first, and the targets and results of a call's tokens (capacity entries each), grown to the largest call.
+    DeviceBuffer<float> score_logits;
+    struct ScoreIo { DeviceBuffer<uint32_t> targets; DeviceBuffer<float> lp; DeviceBuffer<uint8_t> greedy; size_t capacity = 0; } score;
 
     // On-device sampling (kernels/sampling.cu): result word, scratch for biased logits, device copy of the caller's logit bias.
     bool logits_valid = false;       // ctx->logits holds the head output of the most recent pass
-    uint32_t * sample_token = nullptr;   // device
-    uint32_t * sample_token_host = nullptr;   // pinned
-    float * sample_scratch = nullptr;    // [n_vocab] device ([batch_n, n_vocab] in a batch context)
-    uint32_t * bias_ids = nullptr; float * bias_values = nullptr; size_t bias_capacity = 0;   // device (a batch: all rows' lists back to back)
+    struct SampleOut { DeviceBuffer<uint32_t> token; PinnedBuffer<uint32_t> token_host; } sample_out;
+    DeviceBuffer<float> sample_scratch;    // [n_vocab] ([batch_n, n_vocab] in a batch context)
+    struct Bias { DeviceBuffer<uint32_t> ids; DeviceBuffer<float> values; size_t capacity = 0; } bias;   // a batch: all rows' lists back to back
     // ... and in a batch context the per-sequence parameters and results, [batch_n] each, allocated on the first batch_sample
-    SampleRow * sample_rows = nullptr, * sample_rows_host = nullptr;          // device / pinned
-    uint32_t * sample_tokens = nullptr, * sample_tokens_host = nullptr;       // device / pinned
+    struct SampleRows {
+        DeviceBuffer<SampleRow> rows; PinnedBuffer<SampleRow> rows_host;
+        DeviceBuffer<uint32_t> tokens; PinnedBuffer<uint32_t> tokens_host;
+    } sample_rows;
 
     // Device-side generation (generate), allocated on the first call at GENERATE_MAX tokens per row so that the pointers captured in
-    // the loop's graph never change. gen_in: GenShared, GenRow [rows], GenMaskRow [rows], u [rows][GENERATE_MAX]; gen_out:
-    // n_generated [rows], the number of passes that ran, automaton states [rows], tokens [rows][GENERATE_MAX]. Both are packed with
-    // the call's row stride, so each crosses PCIe once.
-    unsigned char * gen_in = nullptr, * gen_in_host = nullptr;        // device / pinned
-    uint32_t * gen_out = nullptr, * gen_out_host = nullptr;           // device / pinned
-    uint32_t * gen_counts = nullptr;                                  // [rows, n_vocab] penalty counts
-    uint32_t * gen_bias_ids = nullptr;                                // [rows, n_vocab]
-    float * gen_bias_values = nullptr, * gen_scratch = nullptr;       // [rows, n_vocab] each
-    float * gen_park = nullptr;                                       // batch contexts: [rows, n_vocab] logits of frozen rows
+    // the loop's graph never change. in: GenShared, GenRow [rows], GenMaskRow [rows], u [rows][GENERATE_MAX]; out: n_generated
+    // [rows], the number of passes that ran, automaton states [rows], tokens [rows][GENERATE_MAX]. Both are packed with the call's
+    // row stride, so each crosses PCIe once.
+    struct Generate {
+        DeviceBuffer<unsigned char> in; PinnedBuffer<unsigned char> in_host;
+        DeviceBuffer<uint32_t> out; PinnedBuffer<uint32_t> out_host;
+        DeviceBuffer<uint32_t> counts;     // [rows, n_vocab] penalty counts
+        DeviceBuffer<uint32_t> bias_ids;   // [rows, n_vocab]
+        DeviceBuffer<float> bias_values, scratch;   // [rows, n_vocab] each
+        DeviceBuffer<float> park;          // batch contexts: [rows, n_vocab] logits of frozen rows
+    } gen;
     // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by whether
     // the loop streams its tokens to a callback, and by whether its draws are constrained by automata
-    cudaGraphExec_t gen_graphs[2][2][2] = {};
+    GraphExec gen_graphs[2][2][2];
     // Streaming generation, allocated on the first streaming call: mapped pinned words shared by the step kernel and the calling
     // thread (GenStreamParams), at device addresses the streaming graph captures. Layout: published [rows], acked [rows], timed_out,
     // then tokens [rows][GENERATE_MAX].
-    uint32_t * stream_host = nullptr, * stream_dev = nullptr;
-    cudaEvent_t stream_done = nullptr;   // recorded after the streaming loop's copies
+    struct Streaming { PinnedBuffer<uint32_t> words; Event done; } streamed;   // done: recorded after the streaming loop's copies
     bool in_stream = false;          // the calling thread is inside a streaming call's callbacks: this context's stream is busy
     // Log-probabilities of generated tokens (generate with a LogprobsOut), allocated only by calls that ask for them. lp_req: the
-    // call's GenLogprobRequest, at a device address the logprob graphs capture (pinned copy lp_req_host). lp_dev / lp_host: the call's
-    // outputs [rows][n] logprobs, sample probs, then [rows][n][top_n] ids and log-probabilities, lp_words 32-bit words each, grown to
-    // the largest rows * n * (2 + 2 * top_n) asked for. lp_ring: mapped [rows][2][GEN_LP_RECORD] records of the streaming loop.
-    GenLogprobRequest * lp_req = nullptr, * lp_req_host = nullptr;
-    uint32_t * lp_dev = nullptr, * lp_host = nullptr;
-    size_t lp_words = 0;
-    uint32_t * lp_ring_host = nullptr, * lp_ring_dev = nullptr;
-    cudaGraphExec_t gen_lp_graphs[2][2] = {};    // the logprob loops' graphs, keyed by phase and streaming
+    // call's GenLogprobRequest, at a device address the logprob graphs capture, and its pinned copy. lp_out: the call's outputs
+    // [rows][n] logprobs, sample probs, then [rows][n][top_n] ids and log-probabilities, `words` 32-bit words each, grown to the
+    // largest rows * n * (2 + 2 * top_n) asked for. lp_ring: mapped [rows][2][GEN_LP_RECORD] records of the streaming loop.
+    struct LogprobRequest { DeviceBuffer<GenLogprobRequest> dev; PinnedBuffer<GenLogprobRequest> host; } lp_req;
+    struct LogprobOut { DeviceBuffer<uint32_t> dev; PinnedBuffer<uint32_t> host; size_t words = 0; } lp_out;
+    PinnedBuffer<uint32_t> lp_ring;
+    GraphExec gen_lp_graphs[2][2];         // the logprob loops' graphs, keyed by phase and streaming
     // Per-row samplers (generate with SamplerIn rows), allocated only by calls that use them: the call's upload at a device address
-    // the sampled graphs capture (pinned copy smp_host): the log-probability request word (lp_req or NULL), GenSamplerRow[rows], then
+    // the sampled graphs capture, and its pinned copy: the log-probability request word (lp_req or NULL), GenSamplerRow[rows], then
     // room for rows * GEN_BIAS_MAX GenBiasEntry.
-    unsigned char * smp_dev = nullptr, * smp_host = nullptr;
-    cudaGraphExec_t gen_smp_graphs[2][2] = {};   // the sampled loops' graphs, keyed by phase and streaming
-    // Beam search (beam_search), allocated on the first call: the loop state and a search state per group (kernels/ops.h: BeamLoop,
-    // BeamState[beam_groups], one allocation), the park [batch_n, n_vocab] (the logits of the pass that runs before the loop is
-    // captured, then the logits of the slots that groups which stopped keep), and the back-pointers [beam_capacity][batch_n][2]. The
-    // states and back-pointers grow to the most groups and the largest max_tokens asked for, which drops beam_graphs, as they hold
-    // their addresses. beam_host: pinned BeamLoop, the BeamStates and the back-pointers.
-    BeamLoop * beam_loop = nullptr;
-    BeamState * beam_state = nullptr;
-    float * beam_park = nullptr;
-    uint32_t * beam_back = nullptr;
-    unsigned char * beam_host = nullptr;
-    size_t beam_capacity = 0, beam_groups = 0;
-    cudaGraphExec_t beam_graphs[2] = {};         // the search loop's graphs, keyed by phase and by the groups they were built for
+    struct Samplers { DeviceBuffer<unsigned char> dev; PinnedBuffer<unsigned char> host; } smp;
+    GraphExec gen_smp_graphs[2][2];        // the sampled loops' graphs, keyed by phase and streaming
+    // Beam search (beam_search): the park [batch_n, n_vocab] (the logits of the pass that runs before the loop is captured, then the
+    // logits of the slots that groups which stopped keep), allocated on the first call; the loop state and a search state per group
+    // (kernels/ops.h: BeamLoop, BeamState[groups], one allocation) and the back-pointers [capacity][batch_n][2], grown to the most
+    // groups and the largest max_tokens asked for, which drops beam_graphs, as they hold their addresses. host: pinned BeamLoop, the
+    // BeamStates and the back-pointers.
+    DeviceBuffer<float> beam_park;
+    struct Beam {
+        DeviceBuffer<BeamLoop> loop; DeviceBuffer<uint32_t> back; PinnedBuffer<unsigned char> host;
+        size_t capacity = 0, groups = 0;
+        BeamState * states() const { return reinterpret_cast<BeamState *>(loop.get() + 1); }
+    } beam;
+    GraphExec beam_graphs[2];              // the search loop's graphs, keyed by phase and by the groups they were built for
     int beam_graph_groups[2] = {};
 
     // The attached adapter (set_adapter) or NULL, and the scratch of its deltas, allocated on the first attach for passes of up to
     // MAX_TOKENS_PER_PASS columns so that captured graphs never see it move: u [GEMV_MAX_PROBLEMS][LORA_MAX_RANK][T] and the base
     // outputs z of a batch's adapted problems with a nonlinear epilogue, max(4 C, F + C) rows of T.
     const Adapter * adapter = nullptr;
-    float * lora_u = nullptr, * lora_z = nullptr;
+    struct LoraScratch { DeviceBuffer<float> u, z; } lora;
     // A batch context's adapters per sequence (batch_set_adapter): seq_adapter [batch_n] (NULL: the base weights), empty until the first
     // attach; the distinct adapters among them (at most LORA_MAX_ADAPTERS), and each sequence's index into that list or -1.
     std::vector<const Adapter *> seq_adapter, seq_adapters;
@@ -350,8 +346,8 @@ struct Automaton {
     int device = 0;
     size_t n_vocab = 0;
     uint32_t n_states = 0;
-    uint16_t * next = nullptr;
-    uint8_t * live = nullptr;
+    DeviceBuffer<uint16_t> next;
+    DeviceBuffer<uint8_t> live;
 };
 // Host checks of a table (1 <= n_states <= 65535, every entry below n_states or dead) and its live flags, [n_states].
 bool check_automaton_table(ErrorSink sink, const uint16_t * next, size_t n_states, size_t n_vocab);
@@ -361,6 +357,8 @@ Automaton * create_automaton(const Model * model, const uint16_t * next, size_t 
 void destroy_automaton(Automaton * a);
 // Drops the loop's graphs (they hold the activation buffers and the GEMM routing of the time they were captured).
 void drop_generate_graphs(Context * ctx);
+// Drops the single-token graphs as well: every graph the context holds.
+void drop_all_graphs(Context * ctx);
 // Attaches `a` (NULL: detaches), dropping the single-token and generation graphs; the state is untouched. The caller has checked the
 // context and that `a` belongs to its model.
 bool set_adapter(Context * ctx, const Adapter * a);

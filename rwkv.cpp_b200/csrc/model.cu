@@ -14,14 +14,11 @@
 
 namespace rwkv {
 
+// The owners free the rest on this device, as the members are destroyed; IPC-opened mappings are not allocations.
 Model::~Model() {
     if (arena || link.box || head_tiled) cudaSetDevice(dev.device);
-    cudaFree(head_tiled);
     if (link.prev && link.prev_ipc) cudaIpcCloseMemHandle(link.prev);
     if (link.next && link.next_ipc) cudaIpcCloseMemHandle(link.next);
-    cudaFree(link.box);
-    cudaFree(link.counters);
-    if (arena) cudaFree(arena);
 }
 
 namespace {
@@ -343,7 +340,7 @@ Model * load_model(const char * path, int device, int layer_begin, int layer_end
     m.dev.max_smem_optin = (int) prop.sharedMemPerBlockOptin;
     m.device_name = prop.name;
 
-    ce = cudaMalloc(reinterpret_cast<void **>(&m.arena), arena_bytes);
+    ce = m.arena.alloc(arena_bytes);
     RWKV_CHECK(sink, RWKV_ERROR_MODEL | RWKV_ERROR_ALLOC, nullptr, ce == cudaSuccess, "Failed to allocate %zu bytes of device memory: %s", arena_bytes, cudaGetErrorString(ce));
     m.arena_bytes = arena_bytes;
 

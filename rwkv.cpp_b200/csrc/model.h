@@ -9,6 +9,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_handles.h"
 #include "errors.h"
 #include "ggml_file.h"
 #include "kernels/gemv.h"
@@ -56,11 +57,11 @@ struct Layer {
 // IPC or shared inside the process) and the mappings of its neighbours'. One per model: every context (in-flight sequence) of a
 // stage sends and receives through the same link, in item order, on one stream.
 struct PipeLink {
-    PipeBox * box = nullptr;               // my mailbox allocation: PipeBox + PIPE_SLOTS x slot_floats floats
+    DeviceBuffer<PipeBox> box;             // my mailbox allocation: PipeBox + PIPE_SLOTS x slot_floats floats
     size_t slot_floats = 0, bytes = 0;
     PipeBox * prev = nullptr, * next = nullptr;
     bool prev_ipc = false, next_ipc = false;
-    unsigned long long * counters = nullptr;   // device: tickets / completions of the hand-off kernels
+    DeviceBuffer<unsigned long long> counters;   // device: tickets / completions of the hand-off kernels
 };
 
 struct Model {
@@ -76,7 +77,7 @@ struct Model {
     std::vector<Layer> layers;      // indexed by absolute layer id; non-resident entries are empty
 
     DeviceInfo dev{};
-    uint8_t * arena = nullptr;
+    DeviceBuffer<uint8_t> arena;
     size_t arena_bytes = 0;
     size_t tiled_bytes = 0;              // of which: tile-major prefill copies of the layer matrices
     size_t weight_bytes_per_token = 0;   // byte model of SURVEY.md 8(d), resident layers, with head
@@ -85,7 +86,7 @@ struct Model {
     size_t head_matrix_bytes = 0;
     // The head's tile-major copy for the tensor-core head of scoring passes (engine.cu: ensure_head_tiled), built by the first one
     // that needs it, under head_tiled_lock, and freed with the model. Every other pass streams the head with the GEMV.
-    uint8_t * head_tiled = nullptr;
+    DeviceBuffer<uint8_t> head_tiled;
     std::mutex head_tiled_lock;
     std::atomic<int> refcount{0};
     PipeLink link;
