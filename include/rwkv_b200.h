@@ -510,6 +510,48 @@ RWKV_API bool rwkv_b200_beam_search_groups(struct rwkv_context * batch, size_t n
  * (*n_live_out = n_live, *n_pool_out = n_pool, the other outputs untouched). Arguments are checked before a device is touched. */
 RWKV_API bool rwkv_b200_test_beam_step_groups(const struct rwkv_b200_beam_step_args * args, size_t n_groups);
 
+/* Checkpoints: the recurrent state after chosen tokens of a pass, the RNN form of a prefix cache (the end of a system prompt, of each
+ * chat turn, a branch point), written by the same launches that run the pass.
+ * 1. The call. rwkv_b200_eval_checkpoints is rwkv_b200_eval_resident(ctx, tokens, n_tokens, want_logits, logits_out) and
+ *    rwkv_b200_batch_eval_ragged_checkpoints is rwkv_b200_batch_eval_ragged(batch, tokens, counts, want_logits): the same passes (any
+ *    n_tokens, cut at 256), routes and argument checks, and the same rules for state, logits and their validity. Asking for checkpoints
+ *    changes none of these, bit for bit, nor the number of kernel launches (rwkv_b200_kernel_launch_count). n_cp = 0 is the plain call.
+ * 2. Order. Entries are strictly increasing in position (single context; sequence must be 0) or in (sequence, position) (ragged), with
+ *    position < n_tokens or position < counts[sequence].
+ * 3. Contents. cp[i].state_out receives rwkv_get_state_len() floats: the state after tokens[0 .. position] of that sequence's tokens of
+ *    this call, in the ABI layout, so rwkv_b200_state_load, the state_in of rwkv_eval* and rwkv_b200_batch_set_state take it as it is.
+ *    A checkpoint at a sequence's last token of the call equals what rwkv_b200_state_store / rwkv_b200_batch_get_state return after the
+ *    call, bit for bit. Where passes are bit-identical to serial evaluation (fewer than 32 tokens per pass, a ragged sum below 16, or
+ *    rwkv_b200_set_tensor_cores(ctx, false) at any length), a checkpoint at position i equals the state after rwkv_eval of tokens[0 .. i]
+ *    one at a time, bit for bit; elsewhere it carries the rounding of the tensor-core pass it came from. A checkpoint holds no logits.
+ * 4. Adapters. A context-wide adapter and adapters per sequence apply as in the plain call: the checkpoint is the adapted state.
+ * 5. Destinations are host memory (pageable or pinned) or device memory of the context's device, at any float alignment. The call
+ *    synchronises before it returns, so every checkpoint has been written by then.
+ * 6. Cost. A checkpoint at the last column of a pass (every 256th token, or the last of the call) is a copy after the pass; the other
+ *    ones are written by the pass's LayerNorm and WKV kernels, straight into device destinations that are 16-byte aligned. The first
+ *    call with such a checkpoint allocates 3 KB of maps on the device and twice that pinned. Host destinations and device ones at
+ *    another alignment go through device staging of state_len floats per checkpoint, grown to the most of them in one pass of a
+ *    call, and are copied after the pass.
+ * Every refusal is decided before anything is enqueued and changes no state, logits or validity. RWKV_ERROR_ARGS: cp == NULL with
+ * n_cp > 0, a NULL state_out, entries out of order or repeated, a position or sequence out of range, destinations that overlap, a
+ * device pointer of another device, and the plain call's own refusals. RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED: the wrong kind of
+ * context (a batch context for the first, an ordinary one for the second), a pipeline handle or stage, a call from inside that
+ * context's streaming callback. RWKV_ERROR_CTX | RWKV_ERROR_ALLOC: the maps or the staging cannot be allocated. */
+struct rwkv_b200_checkpoint {
+    uint32_t sequence;   /* batch contexts: the sequence; 0 for a single-sequence context */
+    uint32_t position;   /* index into that sequence's tokens of this call: the state after tokens[0 .. position] */
+    float * state_out;   /* rwkv_get_state_len() floats: host memory or device memory of the context's device */
+};
+RWKV_API bool rwkv_b200_eval_checkpoints(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, bool want_logits, float * logits_out,
+                                         const struct rwkv_b200_checkpoint * cp, size_t n_cp);
+RWKV_API bool rwkv_b200_batch_eval_ragged_checkpoints(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits,
+                                                      const struct rwkv_b200_checkpoint * cp, size_t n_cp);
+/* Test hook: the checks rule 2 and the RWKV_ERROR_ARGS refusals make of the entries alone, without a context or a device: n_sequences
+ * sequences of counts[s] tokens (a single context: 1 and {n_tokens}), destinations of state_len floats. Device pointers are not
+ * examined. */
+RWKV_API bool rwkv_b200_test_checkpoint_args(size_t n_sequences, const uint32_t * counts, size_t state_len, const struct rwkv_b200_checkpoint * cp,
+                                             size_t n_cp);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each

@@ -403,6 +403,48 @@ bool rwkv_b200_batch_eval_ragged(struct rwkv_context * batch, const uint32_t * t
     RWKV_NOT_STREAMING(c);
     return batch_eval_ragged(c, tokens, counts, want_logits);
 }
+static_assert(sizeof(rwkv_b200_checkpoint) == sizeof(CheckpointReq) && offsetof(rwkv_b200_checkpoint, position) == offsetof(CheckpointReq, position) &&
+              offsetof(rwkv_b200_checkpoint, state_out) == offsetof(CheckpointReq, state_out), "struct rwkv_b200_checkpoint is CheckpointReq");
+static const CheckpointReq * checkpoint_reqs(const rwkv_b200_checkpoint * cp) { return reinterpret_cast<const CheckpointReq *>(cp); }
+
+bool rwkv_b200_eval_checkpoints(struct rwkv_context * ctx, const uint32_t * tokens, size_t n_tokens, bool want_logits, float * logits_out,
+                                const struct rwkv_b200_checkpoint * cp, size_t n_cp) {
+    if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(ctx);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    const Model & m = *c->model;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0 && !c->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Checkpoints run on an ordinary context, not on a batch context, a pipeline or one of its stages");
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens && n_tokens > 0, "No tokens");
+    const size_t n_vocab = (size_t) m.n_vocab;
+    for (size_t i = 0; i < n_tokens; i++)
+        RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, tokens[i] < n_vocab, "Token at index %zu (%" PRIu32 ") is out of range (0 .. %zu)", i, tokens[i], n_vocab - 1);
+    const uint32_t count = n_tokens > UINT32_MAX ? UINT32_MAX : (uint32_t) n_tokens;
+    if (!check_checkpoints(c->sink(), 1, &count, m.state_len(), m.dev.device, checkpoint_reqs(cp), n_cp)) return false;
+    if (n_cp == 0) return rwkv_b200_eval_resident(ctx, tokens, n_tokens, want_logits, logits_out);
+    if (!forward_checkpoints(c, tokens, n_tokens, want_logits || logits_out, checkpoint_reqs(cp), n_cp)) return false;
+    if (logits_out) return download_outputs(c, nullptr, logits_out);
+    return true;
+}
+bool rwkv_b200_batch_eval_ragged_checkpoints(struct rwkv_context * batch, const uint32_t * tokens, const uint32_t * counts, bool want_logits,
+                                             const struct rwkv_b200_checkpoint * cp, size_t n_cp) {
+    if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
+    Context * c = C(batch);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_NOT_STREAMING(c);
+    size_t total = 0;
+    if (!check_ragged(c, tokens, counts, total)) return false;
+    if (!check_checkpoints(c->sink(), (size_t) c->batch_n, counts, c->model->state_len(), c->model->dev.device, checkpoint_reqs(cp), n_cp)) return false;
+    if (n_cp == 0) return batch_eval_ragged(c, tokens, counts, want_logits);
+    return batch_eval_ragged_checkpoints(c, tokens, counts, total, want_logits, checkpoint_reqs(cp), n_cp);
+}
+bool rwkv_b200_test_checkpoint_args(size_t n_sequences, const uint32_t * counts, size_t state_len, const struct rwkv_b200_checkpoint * cp, size_t n_cp) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, counts && n_sequences > 0 && state_len > 0, "NULL counts, no sequences or an empty state");
+    return check_checkpoints(sink, n_sequences, counts, state_len, -1, checkpoint_reqs(cp), n_cp);
+}
 bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(C(batch));

@@ -118,7 +118,17 @@ struct Pass {
     const uint32_t * targets = nullptr;
     float * lp = nullptr;
     uint8_t * greedy = nullptr;
+    // a pass with checkpoints inside it (Context::cps): the device map of its columns' slots and of the slots' destinations
+    const int * cp_slot = nullptr;
+    float * const * cp_dst = nullptr;
 };
+
+// The checkpoint map of a launch whose state slice starts at `slice` of the pass's output (kernels/ops.h: CheckpointMap), or none.
+CheckpointMap checkpoints_at(const Pass & p, const float * slice) {
+    CheckpointMap cp;
+    if (p.cp_slot) { cp.slot = p.cp_slot; cp.dst = p.cp_dst; cp.at = slice - p.state_out; }
+    return cp;
+}
 
 // ---- GEMV batch builder -------------------------------------------------------------------------
 struct Batch {
@@ -264,7 +274,7 @@ LnMixParams ffn_ln(const Context * ctx, const Layer & L, const Pass & p, const f
 bool ffn(Context * ctx, const Layer & L, const Pass & p, const LnMixParams & lp) {
     const Model & m = *ctx->model;
     const int C = m.n_embed;
-    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream, checkpoints_at(p, lp.state_out)));
     {
         Batch b(p.T);
         b.add(L.ffn_key, p.s.mix[0], p.s.ffn_k, EPI_RELU_SQR);
@@ -317,7 +327,7 @@ LnMixParams att_ln(const Context * ctx, const Layer & L, const Pass & p, const f
 
 bool att_v4(Context * ctx, const Layer & L, const Pass & p, const float * st_in, float * st_out, const LnMixParams & lp) {
     const int C = ctx->model->n_embed;
-    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream, checkpoints_at(p, lp.state_out)));
     Batch b(p.T);
     b.add(L.att_receptance, p.s.mix[2], p.s.r, EPI_SIGMOID);
     b.add(L.att_key, p.s.mix[0], p.s.k);
@@ -330,6 +340,7 @@ bool att_v4(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
     wp.aa_out = st_out + 2 * C; wp.bb_out = st_out + 3 * C; wp.pp_out = st_out + 4 * C;
     wp.y = p.s.y; wp.C = C; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (C % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    wp.cp = checkpoints_at(p, wp.aa_out);
     CUDA_OK(ctx, launch_wkv4(wp, p.stream));
     return att_output(ctx, L, p, wp.q_out);
 }
@@ -338,7 +349,7 @@ bool att_v5(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
     const Model & m = *ctx->model;
     const int C = m.n_embed;
     const bool v52 = m.arch_minor >= 2;
-    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream, checkpoints_at(p, lp.state_out)));
     Batch b(p.T);
     b.add(L.att_receptance, p.s.mix[2], p.s.r);
     b.add(L.att_key, p.s.mix[0], p.s.k);
@@ -355,6 +366,7 @@ bool att_v5(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
     wp.g = v52 ? p.s.g : nullptr;
     wp.y = p.s.y; wp.eps = 1e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    wp.cp = checkpoints_at(p, wp.state_out);
     CUDA_OK(ctx, launch_wkv6(wp, p.stream));
     return att_output(ctx, L, p, wp.q_out);
 }
@@ -474,7 +486,7 @@ bool att_v6(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
         dw2.x = p.s.lora[1]; dw2.bias = L.att_time_decay.data;     // dw2's output is the WKV kernel's decay row in shared memory
         CUDA_OK(ctx, launch_v6_prologue(lp, w1, p.stream));
     } else {
-        CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+        CUDA_OK(ctx, launch_ln_mix(lp, p.stream, checkpoints_at(p, lp.state_out)));
         Batch b(p.T);   // :313-321  tanh(W1 . xxx)
         b.add(L.att_maa_w1, p.s.mix[0], p.s.lora[0], EPI_TANH);
         if (!run_batch(ctx, p, b)) return false;
@@ -515,6 +527,7 @@ bool att_v6(Context * ctx, const Layer & L, const Pass & p, const float * st_in,
     wp.lnx_w = L.att_ln_x_w.data; wp.lnx_b = L.att_ln_x_b.data;
     wp.g = p.s.g; wp.y = p.s.y; wp.eps = 64e-5f; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    wp.cp = checkpoints_at(p, wp.state_out);
     CUDA_OK(ctx, launch_wkv6(wp, p.stream));
     return att_output(ctx, L, p, wp.q_out);
 }
@@ -524,7 +537,7 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Pass & p, const flo
     const int C = m.n_embed;
     const bool first = layer == 0;
     float * v_dst = first ? p.s.v_first : p.s.v;
-    CUDA_OK(ctx, launch_ln_mix(lp, p.stream));
+    CUDA_OK(ctx, launch_ln_mix(lp, p.stream, checkpoints_at(p, lp.state_out)));
     {   // :415-432, 439, 447 -- first halves of the LoRA pairs
         Batch b(p.T);
         b.add(L.att_receptance, p.s.mix[0], p.s.r);
@@ -552,6 +565,7 @@ bool att_v7(Context * ctx, const Layer & L, int layer, const Pass & p, const flo
     wp.state_in = st_in + 2 * C; wp.state_out = st_out + 2 * C;
     wp.y = p.s.y; wp.H = m.head_count; wp.S = m.head_size; wp.T = p.T; wp.seq_stride = ctx->batch_stride; wp.seq_off = p.seq_off; wp.n_seq = ctx->batch_n;
     wp.q_out = (m.head_size % 32 == 0) ? xq_slot(ctx, p.T, XQ_WKV, L.att_output) : nullptr; wp.q_type = L.att_output.type;
+    wp.cp = checkpoints_at(p, wp.state_out);
     CUDA_OK(ctx, launch_wkv7(wp, p.stream));
     return att_output(ctx, L, p, wp.q_out);
 }
@@ -1137,6 +1151,137 @@ bool batch_eval(Context * ctx, const uint32_t * tokens, bool want_logits) {
     return make_pass(ctx, ctx->batch_n, want_logits, nullptr, p) && forward_pass(ctx, tokens, p);
 }
 
+// ---- checkpoints ---------------------------------------------------------------------------------------------------------------
+// The checkpoints of one pass: those at a column inside it, which the kernels write, and those at the last column of their sequence,
+// copies of that sequence's state after the pass.
+struct PassCheckpoints {
+    struct Inner { int col; float * dst; };
+    struct AtEnd { int seq; float * dst; };
+    std::vector<Inner> inner;
+    std::vector<AtEnd> at_end;
+};
+
+static bool on_device(const void * p, int * device = nullptr) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (device) *device = a.device;
+    return a.type == cudaMemoryTypeDevice;
+}
+
+// The kernels write a checkpoint straight into device memory that is 16-byte aligned (wkv6_kernel stores float4s); every other
+// destination (host memory, or a device pointer at another offset) is written to Context::cp_staging and copied after the pass.
+static bool written_in_place(const float * p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0 && on_device(p); }
+
+bool check_checkpoints(ErrorSink sink, size_t n_seq, const uint32_t * counts, size_t state_len, int device, const CheckpointReq * cp, size_t n_cp) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, cp || n_cp == 0, "NULL checkpoints");
+    std::vector<uintptr_t> at(n_cp);
+    for (size_t i = 0; i < n_cp; i++) {
+        const CheckpointReq & c = cp[i];
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, c.state_out, "Checkpoint %zu has a NULL state_out", i);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, c.sequence < n_seq && c.position < counts[c.sequence],
+                   "Checkpoint %zu (sequence %u, position %u) is out of range", i, c.sequence, c.position);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, i == 0 || c.sequence > cp[i - 1].sequence || (c.sequence == cp[i - 1].sequence && c.position > cp[i - 1].position),
+                   "Checkpoint %zu is not after checkpoint %zu", i, i - 1);
+        int dev = -1;
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, device < 0 || !on_device(c.state_out, &dev) || dev == device,
+                   "Checkpoint %zu's state_out is memory of device %d, not of the context's device %d", i, dev, device);
+        at[i] = reinterpret_cast<uintptr_t>(c.state_out);
+    }
+    std::sort(at.begin(), at.end());
+    for (size_t i = 1; i < n_cp; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, at[i] - at[i - 1] >= state_len * sizeof(float), "Two checkpoints' state_out ranges overlap");
+    return true;
+}
+
+// The maps and the staging for the passes of a call (plan), built before the call enqueues anything; a grown staging replaces the old
+// one after a synchronise, as the other sets grow.
+static bool ensure_checkpoint_buffers(Context * ctx, const std::vector<PassCheckpoints> & plan) {
+    size_t inner = 0, host = 0;
+    for (const PassCheckpoints & pc : plan) {
+        inner += pc.inner.size();
+        size_t h = 0;
+        for (const PassCheckpoints::Inner & c : pc.inner) h += !written_in_place(c.dst);
+        host = std::max(host, h);
+    }
+    if (inner && !ctx->cps.map) {
+        Context::CheckpointMaps m;
+        const size_t bytes = (size_t) MAX_TOKENS_PER_PASS * (sizeof(int) + sizeof(float *));
+        cudaError_t e = m.map.alloc(bytes);
+        for (int i = 0; i < 2 && e == cudaSuccess; i++) e = m.host[i].alloc(bytes);
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate the checkpoint maps: %s", cudaGetErrorString(e));
+        ctx->cps = std::move(m);
+    }
+    if (host > ctx->cp_staging.count) {
+        CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+        ctx->cp_staging = {};
+        Context::CheckpointStaging st;
+        const size_t bytes = host * ctx->model->state_len() * sizeof(float);
+        const cudaError_t e = st.states.alloc(bytes);
+        RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX | RWKV_ERROR_ALLOC, false, e == cudaSuccess, "Failed to allocate %zu bytes of checkpoint staging: %s", bytes, cudaGetErrorString(e));
+        st.count = host;
+        ctx->cp_staging = std::move(st);
+    }
+    return true;
+}
+
+// After begin_pass (which waited for the pass that last read this phase's slot): the map of the pass's inner checkpoints, uploaded, and
+// the copies of staged states that follow the pass.
+struct StagedCopy { float * dst; const float * src; };
+static bool stage_checkpoints(Context * ctx, Pass & p, const PassCheckpoints & pc, std::vector<StagedCopy> & staged) {
+    staged.clear();
+    if (pc.inner.empty()) return true;
+    unsigned char * host = ctx->cps.host[p.phase];
+    int * slot = reinterpret_cast<int *>(host);
+    float ** dst = reinterpret_cast<float **>(host + MAX_TOKENS_PER_PASS * sizeof(int));
+    for (int t = 0; t < p.T; t++) slot[t] = -1;
+    const size_t n = ctx->model->state_len();
+    for (size_t k = 0; k < pc.inner.size(); k++) {
+        slot[pc.inner[k].col] = (int) k;
+        dst[k] = pc.inner[k].dst;
+        if (!written_in_place(dst[k])) {
+            dst[k] = ctx->cp_staging.states + staged.size() * n;
+            staged.push_back({pc.inner[k].dst, dst[k]});
+        }
+    }
+    const size_t bytes = (size_t) MAX_TOKENS_PER_PASS * (sizeof(int) + sizeof(float *));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->cps.map, host, bytes, cudaMemcpyHostToDevice, p.stream));
+    p.cp_slot = reinterpret_cast<const int *>(ctx->cps.map.get());
+    p.cp_dst = reinterpret_cast<float * const *>(ctx->cps.map.get() + MAX_TOKENS_PER_PASS * sizeof(int));
+    return true;
+}
+
+// After end_pass: the staged states to their host destinations, and the checkpoints at the pass's end from the new state (state_a).
+static bool finish_checkpoints(Context * ctx, const Pass & p, const PassCheckpoints & pc, const std::vector<StagedCopy> & staged) {
+    const size_t n = ctx->model->state_len();
+    for (const StagedCopy & c : staged) CUDA_OK(ctx, cudaMemcpyAsync(c.dst, c.src, n * sizeof(float), cudaMemcpyDefault, p.stream));
+    for (const PassCheckpoints::AtEnd & c : pc.at_end)
+        CUDA_OK(ctx, cudaMemcpyAsync(c.dst, ctx->state_a + (size_t) c.seq * n, n * sizeof(float), cudaMemcpyDefault, p.stream));
+    return true;
+}
+
+bool forward_checkpoints(Context * ctx, const uint32_t * tokens, size_t T, bool want_logits, const CheckpointReq * cp, size_t n_cp) {
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    const size_t P = MAX_TOKENS_PER_PASS;
+    std::vector<PassCheckpoints> plan((T + P - 1) / P);
+    for (size_t i = 0; i < n_cp; i++) {
+        const size_t pass = cp[i].position / P, col = cp[i].position % P, n = std::min(P, T - pass * P);
+        if (col + 1 == n) plan[pass].at_end.push_back({0, cp[i].state_out});
+        else plan[pass].inner.push_back({(int) col, cp[i].state_out});
+    }
+    if (!ensure_checkpoint_buffers(ctx, plan)) return false;
+    std::vector<StagedCopy> staged;
+    for (size_t k = 0, done = 0; done < T; k++) {
+        const size_t n = std::min(P, T - done);
+        Pass p;
+        if (!make_pass(ctx, (int) n, want_logits && done + n == T, nullptr, p) || !begin_pass(ctx, tokens + done, p) ||
+            !stage_checkpoints(ctx, p, plan[k], staged) || !run_layers(ctx, p, 0) || !end_pass(ctx, p) || !finish_checkpoints(ctx, p, plan[k], staged))
+            return false;
+        done += n;
+    }
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return true;
+}
+
 // Ints of one ragged map (Context::ragged_host): offsets [B + 1], column sequences [MAX_TOKENS_PER_PASS], head columns and sequences [B each].
 static size_t ragged_map_ints(int B) { return (size_t) 3 * B + 1 + MAX_TOKENS_PER_PASS; }
 
@@ -1155,7 +1300,7 @@ bool check_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * count
 // batch_eval_ragged on arguments that passed check_ragged (T tokens in all); with targets, a scoring pass whose results go to lp and
 // greedy (greedy may be NULL).
 static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t * counts, int T, bool want_logits, const uint32_t * targets,
-                        float * lp, uint8_t * greedy) {
+                        float * lp, uint8_t * greedy, const PassCheckpoints * pc = nullptr) {
     const Model & m = *ctx->model;
     const int B = ctx->batch_n;
     CUDA_OK(ctx, cudaSetDevice(m.dev.device));
@@ -1193,16 +1338,34 @@ static bool ragged_pass(Context * ctx, const uint32_t * tokens, const uint32_t *
     p.head_col = p.col_seq + MAX_TOKENS_PER_PASS;
     p.head_seq = p.head_col + B;
     p.targets = targets; p.lp = lp; p.greedy = greedy;
+    std::vector<StagedCopy> staged;
+    if (pc && !stage_checkpoints(ctx, p, *pc, staged)) return false;
     if (!enqueue_pass(ctx, p, 0)) return false;     // never a graph: the map changes from call to call
     const bool had_logits = ctx->logits_valid;
     if (!end_pass(ctx, p)) return false;
     ctx->logits_valid = had_logits || want_logits;     // idle columns keep what they held
-    return true;
+    return !pc || finish_checkpoints(ctx, p, *pc, staged);
 }
 
 bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits) {
     size_t total = 0;
     return check_ragged(ctx, tokens, counts, total) && ragged_pass(ctx, tokens, counts, (int) total, want_logits, nullptr, nullptr, nullptr);
+}
+
+bool batch_eval_ragged_checkpoints(Context * ctx, const uint32_t * tokens, const uint32_t * counts, size_t total, bool want_logits, const CheckpointReq * cp,
+                                   size_t n_cp) {
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    std::vector<PassCheckpoints> plan(1);
+    std::vector<uint32_t> off(ctx->batch_n + 1, 0);
+    for (int b = 0; b < ctx->batch_n; b++) off[b + 1] = off[b] + counts[b];
+    for (size_t i = 0; i < n_cp; i++) {
+        const uint32_t s = cp[i].sequence, pos = cp[i].position;
+        if (pos + 1 == counts[s]) plan[0].at_end.push_back({(int) s, cp[i].state_out});
+        else plan[0].inner.push_back({(int) (off[s] + pos), cp[i].state_out});
+    }
+    if (!ensure_checkpoint_buffers(ctx, plan) || !ragged_pass(ctx, tokens, counts, (int) total, want_logits, nullptr, nullptr, nullptr, &plan[0])) return false;
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return true;
 }
 
 bool batch_get_logits(Context * ctx, int seq, float * logits_out) {

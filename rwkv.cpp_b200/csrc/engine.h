@@ -127,6 +127,12 @@ struct Context {
     // Scoring passes (score, batch_score_ragged): the head's output for every column of a pass ([MAX_TOKENS_PER_PASS, n_vocab]),
     // allocated on the first, and the targets and results of a call's tokens (capacity entries each), grown to the largest call.
     DeviceBuffer<float> score_logits;
+    // Checkpoints inside passes (eval_checkpoints), allocated on the first pass that has one: a pinned map per phase, which follows the
+    // tokens_host / slot_free rule, and its device copy: the slot of every column [MAX_TOKENS_PER_PASS] (-1: none), then the state each
+    // slot writes [MAX_TOKENS_PER_PASS]. Host destinations, and device ones that are not 16-byte aligned, are written to `staging`
+    // (count states) and copied out after the pass; it grows to the most such checkpoints inside one pass of a call.
+    struct CheckpointMaps { PinnedBuffer<unsigned char> host[2]; DeviceBuffer<unsigned char> map; } cps;
+    struct CheckpointStaging { DeviceBuffer<float> states; size_t count = 0; } cp_staging;
     struct ScoreIo { DeviceBuffer<uint32_t> targets; DeviceBuffer<float> lp; DeviceBuffer<uint8_t> greedy; size_t capacity = 0; } score;
 
     // On-device sampling (kernels/sampling.cu): result word, scratch for biased logits, device copy of the caller's logit bias.
@@ -264,6 +270,24 @@ bool batch_score_ragged(Context * ctx, const uint32_t * tokens, const uint32_t *
 // pass over the weights. Checks every argument before it enqueues anything. want_logits: the logits column of every sequence with
 // counts[b] > 0 receives the logits of its last token, the other columns keep what they held. Never replays a CUDA graph.
 bool batch_eval_ragged(Context * ctx, const uint32_t * tokens, const uint32_t * counts, bool want_logits);
+
+// Checkpoints (rwkv_b200_eval_checkpoints / rwkv_b200_batch_eval_ragged_checkpoints, include/rwkv_b200.h): the state after token
+// `position` of sequence `sequence`'s tokens of the call, into state_out (host or device memory). The layout of struct rwkv_b200_checkpoint.
+struct CheckpointReq {
+    uint32_t sequence, position;
+    float * state_out;
+};
+// The entries' own rules (RWKV_ERROR_ARGS): cp not NULL when n_cp > 0, strictly increasing (sequence, position), sequence < n_seq,
+// position < counts[sequence], no NULL destination, no two destinations of state_len floats that overlap and, when device >= 0, no
+// device pointer of another device than `device`.
+bool check_checkpoints(ErrorSink sink, size_t n_seq, const uint32_t * counts, size_t state_len, int device, const CheckpointReq * cp, size_t n_cp);
+// forward(tokens, T, want_logits) / batch_eval_ragged(tokens, counts, want_logits) with the same passes and launches, which also write
+// the checkpoints: one at the last column of its sequence in a pass is a copy of that state after the pass; the kernels write the others
+// (16-byte aligned device destinations directly, the others through Context::cp_staging). The arguments have been checked (check_checkpoints, and
+// check_ragged, which gave `total`, for the ragged call); nothing is enqueued before the staging is allocated. Synchronises.
+bool forward_checkpoints(Context * ctx, const uint32_t * tokens, size_t T, bool want_logits, const CheckpointReq * cp, size_t n_cp);
+bool batch_eval_ragged_checkpoints(Context * ctx, const uint32_t * tokens, const uint32_t * counts, size_t total, bool want_logits, const CheckpointReq * cp,
+                                   size_t n_cp);
 
 // Samples the next token from ctx->logits on the device (reference python/sampling.py:10-52 with the caller's uniform number u in
 // [0, 1) in place of numpy's RandomState draw); only the token id is copied back. Requires a preceding pass that computed logits.

@@ -87,9 +87,11 @@ __device__ __forceinline__ double block_sum_ln(double v, double * slots) {
 // column and LN(x[:, t-1]) on the others; the sequence's last column writes its new carry.
 // The body is shared with v6_prologue_kernel: token t of the launch; out0, if not NULL, takes the place of p.out[0] (t == 0);
 // write_carry = false skips out_sx, out_xx and state_out.
+// MODE | SEQ_SNAP: a column with a checkpoint slot in *cp also writes its LN(x), the carry it would leave as the last column, into the slot.
 template <int PER, int PRE_N, int MODE>
-__device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float * out0, bool write_carry, double (&slots)[4][LN_WARPS]) {
-    constexpr bool BATCH = MODE == SEQ_BATCH, RAGGED = MODE == SEQ_RAGGED;
+__device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float * out0, bool write_carry, double (&slots)[4][LN_WARPS],
+                                            const CheckpointMap * cp = nullptr) {
+    constexpr bool BATCH = (MODE & ~SEQ_SNAP) == SEQ_BATCH, RAGGED = (MODE & ~SEQ_SNAP) == SEQ_RAGGED;
     const int C = p.C, tid = threadIdx.x;
     // ragged: the sequence's first and last column and its state's offset. The column map is written by the host: safe before the
     // dependency wait. (The other modes keep their expressions below as they were: they are what their code was compiled from.)
@@ -204,6 +206,16 @@ __device__ __forceinline__ void ln_mix_body(const LnMixParams & p, int t, float 
         if (p.out_xx) p.out_xx[o0 + i * LN_THREADS] = xa[i];
         if (BATCH || (RAGGED ? t == r_last : t == p.T - 1)) p.state_out[BATCH ? t * p.seq_stride + c : RAGGED ? r_so + c : c] = xa[i];
     }
+    if constexpr ((MODE & SEQ_SNAP) != 0) {
+        const int slot = cp->slot[t];
+        if (slot < 0) return;
+        float * dst = cp->dst[slot] + cp->at;
+#pragma unroll
+        for (int i = 0; i < PER; i++) {
+            const int c = tid + i * LN_THREADS;
+            if (c < C) dst[c] = xa[i];
+        }
+    }
 }
 
 template <int PER, int PRE_N, int MODE>
@@ -212,6 +224,16 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const LnMixParams p)
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     ln_mix_body<PER, PRE_N, MODE>(p, blockIdx.x, nullptr, true, slots);
+    trace_end(p.trace);
+}
+
+// ln_mix_kernel with checkpoints (MODE SEQ_ONE or SEQ_RAGGED).
+template <int PER, int PRE_N, int MODE>
+__global__ void __launch_bounds__(LN_THREADS) ln_mix_snap_kernel(const LnMixParams p, const CheckpointMap cp) {
+    __shared__ double slots[4][LN_WARPS];
+    trace_begin(p.trace);
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    ln_mix_body<PER, PRE_N, MODE | SEQ_SNAP>(p, blockIdx.x, nullptr, true, slots, &cp);
     trace_end(p.trace);
 }
 
@@ -419,18 +441,23 @@ cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch
 
 // Grid row t is token t, sequence t in batch mode, or column t in ragged mode. The single-sequence instantiation comes first: with
 // the batch one first, nvcc emitted different code for the untouched v6_lerp_kernel<8, 16> of this file. The ragged one comes last.
+// The checkpoint instantiations come after all of these.
 template <int PER, int PRE_N>
-cudaError_t launch_ln_mix_kernel(const LnMixParams & p, cudaStream_t s) {
-    return !p.seq_stride ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_ONE>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
-         : !p.seq_off    ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_BATCH>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
-                         : launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_RAGGED>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
+cudaError_t launch_ln_mix_kernel(const LnMixParams & p, cudaStream_t s, const CheckpointMap & cp) {
+    if (!cp.slot)
+        return !p.seq_stride ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_ONE>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
+             : !p.seq_off    ? launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_BATCH>, dim3(p.T), dim3(LN_THREADS), 0, s, p)
+                             : launch_pdl(ln_mix_kernel<PER, PRE_N, SEQ_RAGGED>, dim3(p.T), dim3(LN_THREADS), 0, s, p);
+    if (p.seq_stride && !p.seq_off) return cudaErrorInvalidValue;
+    return !p.seq_stride ? launch_pdl(ln_mix_snap_kernel<PER, PRE_N, SEQ_ONE>, dim3(p.T), dim3(LN_THREADS), 0, s, p, cp)
+                         : launch_pdl(ln_mix_snap_kernel<PER, PRE_N, SEQ_RAGGED>, dim3(p.T), dim3(LN_THREADS), 0, s, p, cp);
 }
 
-cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s) {
+cudaError_t launch_ln_mix(const LnMixParams & p_in, cudaStream_t s, const CheckpointMap & cp) {
     LnMixParams p = p_in;
     p.trace = trace_slot("ln_mix");
     const int per = (p.C + LN_THREADS - 1) / LN_THREADS;
-#define RWKV_LN(PER_) return p.n_out > 3 ? launch_ln_mix_kernel<PER_, 6>(p, s) : launch_ln_mix_kernel<PER_, 3>(p, s);
+#define RWKV_LN(PER_) return p.n_out > 3 ? launch_ln_mix_kernel<PER_, 6>(p, s, cp) : launch_ln_mix_kernel<PER_, 3>(p, s, cp);
     if (per <= 1) { RWKV_LN(1) }
     if (per <= 2) { RWKV_LN(2) }
     if (per <= 4) { RWKV_LN(4) }

@@ -19,6 +19,16 @@ namespace rwkv {
 
 // The MODE template argument of the state-carrying kernels: T tokens of one sequence, one token of each of T sequences, ragged.
 constexpr int SEQ_ONE = 0, SEQ_BATCH = 1, SEQ_RAGGED = 2;
+// Checkpoints (rwkv_b200_eval_checkpoints): the SEQ_SNAP | SEQ_ONE and SEQ_SNAP | SEQ_RAGGED instantiations run exactly the arithmetic
+// of the plain mode and also write the state after every column t with slot[t] >= 0 into the state that starts at dst[slot[t]], in the
+// ABI layout: the launch's slice sits `at` floats into it. A launch takes them whenever slot is set. (A batch pass needs none: each
+// sequence advances one token, so its checkpoint is the state after the pass.)
+constexpr int SEQ_SNAP = 4;
+struct CheckpointMap {
+    const int * slot = nullptr;       // [T] the checkpoint slot of each column, -1: none
+    float * const * dst = nullptr;    // device array: the state each slot writes
+    long long at = 0;
+};
 
 // x[:, t] = LN(emb[tokens[t]]; ln0)     (rwkv_graph.inc:655-658, 787-790)
 cudaError_t launch_embed_ln0(const void * emb, int emb_type, long long emb_pitch, const int * tokens, int T, int C,
@@ -44,7 +54,8 @@ struct LnMixParams {
     const int * seq_off = nullptr;   // ragged mode: [n_seq + 1] column offsets of the sequences
     const int * col_seq = nullptr;   // ragged mode: [T] the sequence of each column
 };
-cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s);
+// cp.slot set: the checkpoint kernel (a kernel argument of its own: v6_prologue_kernel takes LnMixParams by value before another struct)
+cudaError_t launch_ln_mix(const LnMixParams & p, cudaStream_t s, const CheckpointMap & cp = {});
 
 // v6 time-mixing prologue of a single-token pass, ln_mix (one token, n_out == 1) and the first LoRA matrix in one launch:
 // w1.y = tanh(W1 . mix[0]) with w1 = {maa_w1, EPI_TANH} planned by gemv_tma_plan. Every CTA runs the LayerNorm of ln_mix_kernel on
@@ -82,6 +93,7 @@ struct Wkv4Params {
     unsigned char * q_out; int q_type;  // T == 1, C % 32 == 0 only: y as a staged column (act_stage.cuh)
     long long seq_stride = 0;
     const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
+    CheckpointMap cp;                 // appended last: the other members keep their offsets
 };
 cudaError_t launch_wkv4(const Wkv4Params & p, cudaStream_t s);
 
@@ -106,6 +118,7 @@ struct Wkv6Params {
     // dw2 = {decay_w2, x = lora1, bias = time_decay, EPI_BIAS_EXPNEGEXP} planned by gemv_tma_plan, instead of read from td.
     GemvProblem dw2 = {};
     const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
+    CheckpointMap cp;                 // appended last: the other members keep their offsets
 };
 cudaError_t launch_wkv6(const Wkv6Params & p, cudaStream_t s);
 // Dynamic shared memory of a wkv6 launch that computes the decay (head size 64): the head's rows of dw2 and the staged lora1.
@@ -130,6 +143,7 @@ struct Wkv7Params {
     unsigned char * q_out; int q_type;  // T == 1, S % 32 == 0 only: y as a staged column (act_stage.cuh)
     long long seq_stride = 0;
     const int * seq_off = nullptr; int n_seq = 0;   // ragged mode: [n_seq + 1] column offsets of the sequences
+    CheckpointMap cp;                 // appended last: the other members keep their offsets
 };
 cudaError_t launch_wkv7(const Wkv7Params & p, cudaStream_t s);
 

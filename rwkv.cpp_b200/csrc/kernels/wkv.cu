@@ -17,17 +17,19 @@ namespace {
 // Every ggml node is its own rounding, so no FMA contraction here.
 // MODE SEQ_BATCH: one token, column blockIdx.y, on the state of sequence blockIdx.y.
 // MODE SEQ_RAGGED: the columns [seq_off[y], seq_off[y + 1]) of sequence y = blockIdx.y on its state.
+// MODE | SEQ_SNAP: aa, bb, pp after every column with a checkpoint slot also go to the slot (aa at cp.at, bb and pp C and 2 C after it).
 // ---------------------------------------------------------------------------------------------
 template <int MODE>
 __global__ void wkv4_kernel(const Wkv4Params p) {
-    constexpr bool BATCH = MODE == SEQ_BATCH;
+    constexpr int M = MODE & ~SEQ_SNAP;
+    constexpr bool BATCH = M == SEQ_BATCH;
     trace_begin(p.trace);
     pdl_prologue();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= p.C) return;
-    const long long so = MODE != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
+    const long long so = M != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
     int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
-    if constexpr (MODE == SEQ_RAGGED) {
+    if constexpr (M == SEQ_RAGGED) {
         t_begin = p.seq_off[blockIdx.y]; t_end = p.seq_off[blockIdx.y + 1];
         if (t_begin == t_end) return;
     }
@@ -48,6 +50,13 @@ __global__ void wkv4_kernel(const Wkv4Params p) {
         aa = __fadd_rn(__fmul_rn(e1, aa), __fmul_rn(e2, v));
         bb = __fadd_rn(__fmul_rn(e1, bb), e2);
         pp = qq;
+        if constexpr ((MODE & SEQ_SNAP) != 0) {
+            const int slot = p.cp.slot[t];
+            if (slot >= 0) {
+                float * dst = p.cp.dst[slot] + p.cp.at + c;
+                dst[0] = aa; dst[p.C] = bb; dst[2 * p.C] = pp;
+            }
+        }
         const float yv = __fmul_rn(p.r[o], __fdiv_rn(a, b));
         p.y[o] = yv;
         if (p.q_out) act::warp_emit_block(act::StagedOut{p.q_out, p.q_type, p.C}, c >> 5, yv);      // T == 1, C % 32 == 0: whole warps only
@@ -120,11 +129,14 @@ __device__ __forceinline__ void wkv_bar_arrive(int id, int count) { asm volatile
 // stages a column, and rows_dot writes exp(-exp(..)) straight into the decay row the recurrence reads.
 // DW2 == WKV6_RAGGED (with BATCH_OR_RAGGED = true): the ragged mode. (A value of the third argument rather than a MODE argument of its own, so
 // that the names of the other instantiations stay what they were.)
-constexpr int WKV6_RAGGED = -2;
+// DW2 == WKV6_SNAP (BATCH_OR_RAGGED = false) / WKV6_RAGGED_SNAP (true): the single-sequence / ragged mode with checkpoints: after every
+// column with a checkpoint slot, each worker also writes its 8 x 4 state patch into the slot.
+constexpr int WKV6_RAGGED = -2, WKV6_SNAP = -3, WKV6_RAGGED_SNAP = -4;
 template <int S, bool BATCH_OR_RAGGED, int DW2 = -1>
 __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Params p) {
     using LY = Wkv6Layout<S>;
-    constexpr int MODE = DW2 == WKV6_RAGGED ? SEQ_RAGGED : BATCH_OR_RAGGED ? SEQ_BATCH : SEQ_ONE;
+    constexpr bool SNAP = DW2 == WKV6_SNAP || DW2 == WKV6_RAGGED_SNAP;
+    constexpr int MODE = (DW2 == WKV6_RAGGED || DW2 == WKV6_RAGGED_SNAP) ? SEQ_RAGGED : BATCH_OR_RAGGED ? SEQ_BATCH : SEQ_ONE;
     constexpr bool BATCH = MODE == SEQ_BATCH;
     constexpr int TB = WKV6_TB, NOCT = LY::NOCT, NT = LY::NT, WORK = LY::WORK, BLOCK = LY::BLOCK, NNW = LY::NORM_WARPS, CPL = (S + 31) / 32;
     constexpr int BAR_FULL = 1, BAR_EMPTY = 3, BAR_WORK = 5;        // named barriers: FULL / EMPTY + (chunk & 1), the workers' own
@@ -234,6 +246,10 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
             const Wkv6Chunk<S> & B = buf[c & 1];
             float (* yb)[S] = ybuf[c & 1];
             const int t0 = c * TB, nt = BATCH ? 1 : min(TB, (RAGGED ? r_T : p.T) - t0);
+            unsigned snap = 0;     // SNAP: bit tt = token tt of the chunk has a checkpoint slot
+            if constexpr (SNAP) {
+                for (int tt = 0; tt < nt; tt++) snap |= (p.cp.slot[col0 + t0 + tt] >= 0 ? 1u : 0u) << tt;
+            }
             // recurrence (kv = v_j*k_i;  y_j += (kv*tf_i + S_ij) * r_i;  S_ij = S_ij*td_i + kv), 8 + 8 + 8 + 4 operands per token from
             // shared memory
             float kk[8], rr[8], dv[8], vv[4];
@@ -272,6 +288,14 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
                     for (int jj = 0; jj < 4; jj++) y[jj] += __shfl_xor_sync(0xffffffffu, y[jj], o);
                 }
                 if (worker && oct == 0) *reinterpret_cast<float4 *>(&yb[tt][j0]) = make_float4(y[0], y[1], y[2], y[3]);
+                if constexpr (SNAP) {
+                    if (worker && ((snap >> tt) & 1u)) {
+                        float * dst = p.cp.dst[p.cp.slot[col0 + t0 + tt]] + p.cp.at + ((size_t) h * S + i0) * S + j0;
+#pragma unroll
+                        for (int ii = 0; ii < 8; ii++)
+                            *reinterpret_cast<float4 *>(dst + (size_t) ii * S) = make_float4(st[ii][0], st[ii][1], st[ii][2], st[ii][3]);
+                    }
+                }
             }
             tick(a1);
             wkv_bar_arrive(BAR_FULL + (c & 1), BLOCK);     // the chunk's output rows are complete: over to the normalising warps
@@ -352,16 +376,18 @@ __global__ void __launch_bounds__(Wkv6Layout<S>::BLOCK) wkv6_kernel(const Wkv6Pa
 // ---------------------------------------------------------------------------------------------
 // MODE SEQ_BATCH: the block handles ONE token, column blockIdx.y, on the state of sequence blockIdx.y.
 // MODE SEQ_RAGGED: the columns [seq_off[y], seq_off[y + 1]) of sequence y = blockIdx.y on its state; none: the block leaves at once.
+// MODE | SEQ_SNAP: after every column with a checkpoint slot, thread i also writes its state row into the slot.
 template <int S, int MODE>
 __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
-    constexpr bool BATCH = MODE == SEQ_BATCH;
+    constexpr int M = MODE & ~SEQ_SNAP;
+    constexpr bool BATCH = M == SEQ_BATCH;
     __shared__ float sr[S], sw[S], sk[S], sa[S], sb[S], red[S];
     trace_begin(p.trace);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int h = blockIdx.x, i = threadIdx.x, C = p.H * S, c = h * S + i;
-    const long long so = MODE != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
+    const long long so = M != SEQ_ONE ? blockIdx.y * p.seq_stride : 0;
     int t_begin = BATCH ? blockIdx.y : 0, t_end = BATCH ? blockIdx.y + 1 : p.T;
-    if constexpr (MODE == SEQ_RAGGED) {
+    if constexpr (M == SEQ_RAGGED) {
         t_begin = p.seq_off[blockIdx.y]; t_end = p.seq_off[blockIdx.y + 1];
         if (t_begin == t_end) return;
     }
@@ -403,6 +429,14 @@ __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
             st[j] = __fmaf_rn(dot_a, sb[j], __fmaf_rn(st[j], sw[j], kv));
             y = __fmaf_rn(st[j], sr[j], y);
         }
+        if constexpr ((MODE & SEQ_SNAP) != 0) {
+            const int slot = p.cp.slot[t];
+            if (slot >= 0) {
+                float * dst = p.cp.dst[slot] + p.cp.at + ((size_t) h * S + i) * S;
+#pragma unroll
+                for (int j = 0; j < S; j++) dst[j] = st[j];
+            }
+        }
         float n = head_norm<S>(y, 64e-5f, red);
         n = __fadd_rn(__fmul_rn(n, lw), lb);
         // + v * sum_head(k*r*r_k)   (rwkv_graph.inc:472-477; ggml_sum_rows accumulates in double)
@@ -426,20 +460,29 @@ __global__ void __launch_bounds__(S) wkv7_kernel(const Wkv7Params p) {
 
 // Grid row y is sequence y in batch mode (seq_stride > 0) and in ragged mode (seq_off set: n_seq rows); one sequence has a single
 // row. The ragged instantiations come after the two others.
+// The checkpoint instantiations (cp.slot set: single-sequence or ragged passes) come last.
 cudaError_t launch_wkv4(const Wkv4Params & p_in, cudaStream_t s) {
     Wkv4Params p = p_in;
     p.trace = trace_slot("wkv4");
     const int threads = 128;
-    return !p.seq_stride ? launch_pdl(wkv4_kernel<SEQ_ONE>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
-         : !p.seq_off    ? launch_pdl(wkv4_kernel<SEQ_BATCH>, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p)
-                         : launch_pdl(wkv4_kernel<SEQ_RAGGED>, dim3((p.C + threads - 1) / threads, p.n_seq), dim3(threads), 0, s, p);
+    if (!p.cp.slot)
+        return !p.seq_stride ? launch_pdl(wkv4_kernel<SEQ_ONE>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
+             : !p.seq_off    ? launch_pdl(wkv4_kernel<SEQ_BATCH>, dim3((p.C + threads - 1) / threads, p.T), dim3(threads), 0, s, p)
+                             : launch_pdl(wkv4_kernel<SEQ_RAGGED>, dim3((p.C + threads - 1) / threads, p.n_seq), dim3(threads), 0, s, p);
+    if (p.seq_stride && !p.seq_off) return cudaErrorInvalidValue;
+    return !p.seq_stride ? launch_pdl(wkv4_kernel<SEQ_SNAP | SEQ_ONE>, dim3((p.C + threads - 1) / threads), dim3(threads), 0, s, p)
+                         : launch_pdl(wkv4_kernel<SEQ_SNAP | SEQ_RAGGED>, dim3((p.C + threads - 1) / threads, p.n_seq), dim3(threads), 0, s, p);
 }
 
 template <int S>
 cudaError_t launch_wkv6_kernel(const Wkv6Params & p, cudaStream_t s) {
-    return !p.seq_stride ? launch_pdl(wkv6_kernel<S, false>, dim3(p.H), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
-         : !p.seq_off    ? launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
-                         : launch_pdl(wkv6_kernel<S, true, WKV6_RAGGED>, dim3(p.H, p.n_seq), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
+    if (!p.cp.slot)
+        return !p.seq_stride ? launch_pdl(wkv6_kernel<S, false>, dim3(p.H), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
+             : !p.seq_off    ? launch_pdl(wkv6_kernel<S, true>, dim3(p.H, p.T), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
+                             : launch_pdl(wkv6_kernel<S, true, WKV6_RAGGED>, dim3(p.H, p.n_seq), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
+    if (p.seq_stride && !p.seq_off) return cudaErrorInvalidValue;
+    return !p.seq_stride ? launch_pdl(wkv6_kernel<S, false, WKV6_SNAP>, dim3(p.H), dim3(Wkv6Layout<S>::BLOCK), 0, s, p)
+                         : launch_pdl(wkv6_kernel<S, true, WKV6_RAGGED_SNAP>, dim3(p.H, p.n_seq), dim3(Wkv6Layout<S>::BLOCK), 0, s, p);
 }
 
 template <int DW2>
@@ -459,7 +502,7 @@ cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
     Wkv6Params p = p_in;
     p.trace = trace_slot("wkv6");
     if (p.dw2.W) {      // v6_lora_fold has checked the shape: S == 64, one token of one sequence, a WK == 1 plan
-        if (p.S != 64 || p.T != 1 || p.seq_stride || wkv6_decay_smem_bytes(p.dw2) > WKV6_DECAY_MAX_SMEM) return cudaErrorInvalidValue;
+        if (p.S != 64 || p.T != 1 || p.seq_stride || p.cp.slot || wkv6_decay_smem_bytes(p.dw2) > WKV6_DECAY_MAX_SMEM) return cudaErrorInvalidValue;
         switch (p.dw2.type) {
             case DT_Q4_0: return launch_wkv6_decay<DT_Q4_0>(p, s);
             case DT_Q4_1: return launch_wkv6_decay<DT_Q4_1>(p, s);
@@ -483,9 +526,13 @@ cudaError_t launch_wkv6(const Wkv6Params & p_in, cudaStream_t s) {
 
 template <int S>
 cudaError_t launch_wkv7_kernel(const Wkv7Params & p, cudaStream_t s) {
-    return !p.seq_stride ? launch_pdl(wkv7_kernel<S, SEQ_ONE>, dim3(p.H), dim3(S), 0, s, p)
-         : !p.seq_off    ? launch_pdl(wkv7_kernel<S, SEQ_BATCH>, dim3(p.H, p.T), dim3(S), 0, s, p)
-                         : launch_pdl(wkv7_kernel<S, SEQ_RAGGED>, dim3(p.H, p.n_seq), dim3(S), 0, s, p);
+    if (!p.cp.slot)
+        return !p.seq_stride ? launch_pdl(wkv7_kernel<S, SEQ_ONE>, dim3(p.H), dim3(S), 0, s, p)
+             : !p.seq_off    ? launch_pdl(wkv7_kernel<S, SEQ_BATCH>, dim3(p.H, p.T), dim3(S), 0, s, p)
+                             : launch_pdl(wkv7_kernel<S, SEQ_RAGGED>, dim3(p.H, p.n_seq), dim3(S), 0, s, p);
+    if (p.seq_stride && !p.seq_off) return cudaErrorInvalidValue;
+    return !p.seq_stride ? launch_pdl(wkv7_kernel<S, SEQ_SNAP | SEQ_ONE>, dim3(p.H), dim3(S), 0, s, p)
+                         : launch_pdl(wkv7_kernel<S, SEQ_SNAP | SEQ_RAGGED>, dim3(p.H, p.n_seq), dim3(S), 0, s, p);
 }
 
 cudaError_t launch_wkv7(const Wkv7Params & p_in, cudaStream_t s) {

@@ -61,6 +61,25 @@ class BeamStepArgs(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_
                 ("pool_tokens", ctypes.POINTER(ctypes.c_uint32)), ("pool_scores", ctypes.POINTER(ctypes.c_double))]
 
 
+class Checkpoint(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_checkpoint
+    _fields_ = [("sequence", ctypes.c_uint32), ("position", ctypes.c_uint32), ("state_out", ctypes.POINTER(ctypes.c_float))]
+
+
+def _state_address(buf, n: int) -> int:
+    """Address of a buffer that can take one state of n floats: a C-contiguous float32 numpy array or torch tensor (host or CUDA) of
+    at least n elements. Anything else is refused before the library could write past it."""
+    if hasattr(buf, "data_ptr"):
+        import torch
+        ok = buf.dtype == torch.float32 and buf.is_contiguous() and buf.numel() >= n
+        addr = buf.data_ptr()
+    else:
+        ok = isinstance(buf, np.ndarray) and buf.dtype == np.float32 and buf.flags.c_contiguous and buf.size >= n
+        addr = buf.ctypes.data if ok else 0
+    if not ok:
+        raise ValueError(f"a checkpoint buffer must be a contiguous float32 array or tensor of at least {n} elements")
+    return addr
+
+
 class RWKVContext:
     def __init__(self, ptr: ctypes.c_void_p) -> None:
         self.ptr = ptr
@@ -283,6 +302,13 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_score_ragged.restype = ctypes.c_bool
         lib.rwkv_b200_score_logits.argtypes = [P_FLOAT, ctypes.c_size_t, ctypes.c_size_t, P_U32, P_FLOAT, P_U8]
         lib.rwkv_b200_score_logits.restype = ctypes.c_bool
+        P_CP = ctypes.POINTER(Checkpoint)
+        lib.rwkv_b200_eval_checkpoints.argtypes = [vp, P_U32, ctypes.c_size_t, ctypes.c_bool, P_FLOAT, P_CP, ctypes.c_size_t]
+        lib.rwkv_b200_eval_checkpoints.restype = ctypes.c_bool
+        lib.rwkv_b200_batch_eval_ragged_checkpoints.argtypes = [vp, P_U32, P_U32, ctypes.c_bool, P_CP, ctypes.c_size_t]
+        lib.rwkv_b200_batch_eval_ragged_checkpoints.restype = ctypes.c_bool
+        lib.rwkv_b200_test_checkpoint_args.argtypes = [ctypes.c_size_t, P_U32, ctypes.c_size_t, P_CP, ctypes.c_size_t]
+        lib.rwkv_b200_test_checkpoint_args.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
@@ -442,6 +468,39 @@ class RWKVSharedLibrary:
         low-rank deltas alone can be attached to a sequence."""
         if not self.library.rwkv_b200_batch_set_adapter(batch.ptr, sequence, adapter):
             raise ValueError(f"rwkv_b200_batch_set_adapter failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
+
+    def _checkpoints(self, ctx: RWKVContext, entries, out):
+        """The rwkv_b200_checkpoint array of (sequence, position) entries, into out (one float32 buffer of state_len per entry:
+        numpy arrays or torch tensors, CUDA ones included) or into a new [n, state_len] numpy array, which is returned."""
+        n = self.rwkv_get_state_len(ctx)
+        if out is None:
+            out = np.empty((len(entries), n), np.float32)
+        if len(out) != len(entries):
+            raise ValueError("one output buffer per checkpoint")
+        arr = (Checkpoint * max(1, len(entries)))()
+        for i, (seq, pos) in enumerate(entries):
+            arr[i] = Checkpoint(seq, pos, ctypes.cast(_state_address(out[i], n), P_FLOAT))
+        return arr, out
+
+    def rwkv_b200_eval_checkpoints(self, ctx: RWKVContext, tokens, positions, want_logits: bool = False, out=None, logits_out_address: int = 0):
+        """rwkv_b200_eval_resident(tokens) that also returns the state after tokens[0 .. p] for every p of positions (increasing), as
+        rows of a new numpy array, or written into out (one buffer per position)."""
+        toks = (ctypes.c_uint32 * len(tokens))(*tokens)
+        arr, out = self._checkpoints(ctx, [(0, p) for p in positions], out)
+        if not self.library.rwkv_b200_eval_checkpoints(ctx.ptr, toks, len(tokens), want_logits, ctypes.cast(logits_out_address or 0, P_FLOAT),
+                                                       arr, len(positions)):
+            raise ValueError(f"rwkv_b200_eval_checkpoints failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+        return out
+
+    def rwkv_b200_batch_eval_ragged_checkpoints(self, batch: RWKVContext, tokens, counts, checkpoints, want_logits: bool = False, out=None):
+        """rwkv_b200_batch_eval_ragged(tokens, counts) that also returns the state of each (sequence, position) of checkpoints (increasing)
+        after that sequence's tokens[0 .. position] of this call, as rows of a new numpy array, or written into out."""
+        toks = (ctypes.c_uint32 * max(1, len(tokens)))(*tokens)
+        cnt = (ctypes.c_uint32 * len(counts))(*counts)
+        arr, out = self._checkpoints(batch, checkpoints, out)
+        if not self.library.rwkv_b200_batch_eval_ragged_checkpoints(batch.ptr, toks, cnt, want_logits, arr, len(checkpoints)):
+            raise ValueError(f"rwkv_b200_batch_eval_ragged_checkpoints failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
+        return out
 
     def rwkv_b200_init_from_file_ex(self, model_file_path: str, device: int, layer_begin: int = 0, layer_end: int = -1) -> RWKVContext:
         ptr = self.library.rwkv_b200_init_from_file_ex(model_file_path.encode("utf-8"), device, layer_begin, layer_end)
