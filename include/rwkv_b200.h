@@ -159,7 +159,9 @@ RWKV_API bool rwkv_b200_sample_logits_batch(const float * logits, size_t n_rows,
  * python/chat_with_bot.py:244-260 and python/generate_completions.py:60-67. Afterwards the state has consumed every evaluated token,
  * the logits are those of the last evaluated token (the row the last token was drawn from), and n_generated counts the tokens written,
  * a stop token included.
- * The penalty counts are a per-sequence table in HBM, allocated on first use. keep_counts false starts the sequence from zero counts;
+ * The penalty counts are a per-sequence table in HBM, allocated on first use; rwkv_b200_set_penalty_decay, rwkv_b200_set_penalty_weights
+ * and rwkv_b200_get_penalty_counts / rwkv_b200_set_penalty_counts decay, weight, read and write them (step 5 with the defaults: decay
+ * 1, every weight 1). keep_counts false starts the sequence from zero counts;
  * true continues from its previous generate call, so that a server can generate in short windows (between ragged admissions in a
  * batch) without losing its penalties. keep_counts applies to every sequence of an accepted call, also one that generates nothing
  * (max_tokens[b] = 0, or a constrained sequence that starts in a state that allows no token): its state and logits are left as they
@@ -552,6 +554,44 @@ RWKV_API bool rwkv_b200_batch_eval_ragged_checkpoints(struct rwkv_context * batc
 RWKV_API bool rwkv_b200_test_checkpoint_args(size_t n_sequences, const uint32_t * counts, size_t state_len, const struct rwkv_b200_checkpoint * cp,
                                              size_t n_cp);
 
+/* Penalty decay, penalty weights and the penalty counts of device-side generation (every rwkv_b200_generate* and
+ * rwkv_b200_batch_generate* call). The penalty count table c of a sequence holds n_vocab float32 values. One step of a sequence that
+ * draws, with decay d of that sequence and weight table w of the context (all 1 when none is set):
+ * 1. Bias. A token n with c[n] != 0 is counted. Its bias is -(presence_penalty + c[n] * frequency_penalty) in float32, the multiply
+ *    and the add rounded separately; a token an automaton state does not allow takes -inf instead, and a sampler's bias entry of a
+ *    counted token is value - (presence_penalty + c[n] * frequency_penalty), as before.
+ * 2. Draw. Bit for bit rwkv_b200_sample with that bias list.
+ * 3. Update, after the draw of a token that is evaluated (a stop id is reported and changes no count): first c[n] = c[n] * d for
+ *    every n, then c[tok] = c[tok] + w[tok], each rounded to float32. This is the order of the RWKV runtimes' penalty decay
+ *    (alpha_decay): decay everything, then add the new token.
+ * 4. A sequence that does not draw (its budget is spent, a stop id or an automaton state ended it, its callback asked it to stop)
+ *    does not decay. So a sequence that ends after token j has the counts of the same call with max_tokens = j + 1.
+ * 5. A token of weight 0 is never counted and takes no penalty at all, while the rwkv pip package gives such tokens the presence
+ *    penalty. Decay is plain float32 arithmetic with denormals; a count that decays to 0 is no longer counted.
+ * 6. With d = 1 and no weights, generation gives the tokens, counts, state, logits and log-probabilities of integer counts, except
+ *    that a count stops growing at 2^24 = 16777216 (float32 has no integer above it that + 1 changes), which takes more than 4096
+ *    full-length calls with keep_counts on one token.
+ * rwkv_b200_set_penalty_decay: d of one sequence for every later generate call of any family; 0 < decay <= 1. A new context, a clone
+ *   and every sequence of a new batch context start at 1. It takes effect at the next call and never re-captures a graph.
+ * rwkv_b200_set_penalty_weights: w for every sequence of the context, n_vocab finite values >= 0 in host or device memory; NULL goes
+ *   back to all 1. The first table allocates n_vocab floats on the device, kept until the context is freed.
+ * rwkv_b200_get_penalty_counts: c of one sequence into counts_out, n_vocab floats of host memory or device memory of the context's
+ *   device. A sequence of a context that has never generated reads as zeros, and nothing is allocated for it.
+ * rwkv_b200_set_penalty_counts: c of one sequence from counts_in, n_vocab finite values >= 0 in host or device memory; the next
+ *   generate call of that sequence starts from them when it passes keep_counts. This is how a server counts a prompt's tokens, or
+ *   moves a conversation's counts with its state (rwkv_b200_checkpoint, rwkv_b200_batch_get_state / _set_state) to another slot or
+ *   context. It allocates the generation buffers if there are none, all or nothing.
+ * `sequence` is 0 for a single-sequence context. The calls synchronise before they return. Every refusal is decided before anything
+ * is enqueued, and a refused call changes nothing: RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED for a pipeline or a stage of one, and for a
+ * call from inside that context's streaming callback; RWKV_ERROR_ARGS for a NULL context or table pointer (except the weights' NULL),
+ * a sequence out of range, a decay outside (0, 1] or NaN, a negative, NaN or infinite weight or count, and a device pointer of another
+ * device. RWKV_ERROR_CTX | RWKV_ERROR_ALLOC: the weight table or the generation buffers cannot be allocated. Beam search reads and
+ * writes no counts. */
+RWKV_API bool rwkv_b200_set_penalty_decay(struct rwkv_context * ctx, size_t sequence, float decay);
+RWKV_API bool rwkv_b200_set_penalty_weights(struct rwkv_context * ctx, const float * weights);
+RWKV_API bool rwkv_b200_get_penalty_counts(struct rwkv_context * ctx, size_t sequence, float * counts_out);
+RWKV_API bool rwkv_b200_set_penalty_counts(struct rwkv_context * ctx, size_t sequence, const float * counts_in);
+
 /* Test hook: one step of the generation loop's kernel on n_rows x n_vocab host logits, no model needed. n is the largest max_tokens
  * (>= 1); u and tokens are [n_rows][n]. A row that is not frozen freezes once step == max_tokens, otherwise draws with u[b * n + step],
  * writes tokens[b * n + step], increments step, and freezes on a stop id or else increments counts[b][tok]. next_tokens receives each
@@ -604,6 +644,13 @@ RWKV_API bool rwkv_b200_test_generate_step_streaming(const struct rwkv_b200_gene
                                                      const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
                                                      const uint32_t * acked, uint32_t * published, uint32_t * stream_tokens, uint32_t * ring,
                                                      uint32_t * timed_out);
+/* The same step of a blocking kernel of `family` (as for rwkv_b200_test_generate_step_streaming, without the streaming words) with the
+ * penalty rules of rwkv_b200_set_penalty_decay: a->counts must be NULL; counts [n_rows, n_vocab] (in / out, finite, >= 0) is the
+ * float count table, decay [n_rows] each row's decay in (0, 1], weights [n_vocab] (finite, >= 0) the weight table or NULL for all 1.
+ * The other hooks run with decay 1 and no weights, their integer counts converted to the float table and back. */
+RWKV_API bool rwkv_b200_test_generate_step_penalty(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
+                                                   const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
+                                                   float * counts, const float * decay, const float * weights);
 
 /* Layer pipeline across GPUs (SURVEY.md 8e; the reference has no equivalent: ggml offloads layers of ONE context,
  * rwkv.cpp:97-116). A context created with rwkv_b200_init_from_file_ex(path, device, begin, end) is one stage; its slice

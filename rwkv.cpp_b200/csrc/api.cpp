@@ -445,6 +445,40 @@ bool rwkv_b200_test_checkpoint_args(size_t n_sequences, const uint32_t * counts,
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, counts && n_sequences > 0 && state_len > 0, "NULL counts, no sequences or an empty state");
     return check_checkpoints(sink, n_sequences, counts, state_len, -1, checkpoint_reqs(cp), n_cp);
 }
+// The context and sequence of the penalty calls: a whole-model context or batch context that is not inside its streaming callback,
+// and a sequence below its number of sequences (0 for a single-sequence context).
+static Context * penalty_context(struct rwkv_context * ctx, size_t sequence) {
+    if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, nullptr, false, "NULL context"); }
+    Context * c = C(ctx);
+    c->last_error = RWKV_ERROR_NONE;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, !c->in_stream,
+               "This context is inside a streaming generation; use another context from its callback");
+    const Model & m = *c->model;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, nullptr, !c->group && m.layer_begin == 0 && m.layer_end == m.n_layer,
+               "Penalties belong to generation, which runs on a whole-model context or batch context, not on a pipeline or one of its stages");
+    const size_t rows = c->batch_n ? (size_t) c->batch_n : 1;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, nullptr, sequence < rows, "Sequence %zu is out of range (0 .. %zu)", sequence, rows - 1);
+    return c;
+}
+bool rwkv_b200_set_penalty_decay(struct rwkv_context * ctx, size_t sequence, float decay) {
+    Context * c = penalty_context(ctx, sequence);
+    if (!c) return false;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, decay > 0.0f && decay <= 1.0f, "The penalty decay must be in (0, 1], not %g", decay);
+    c->penalty_decay[sequence] = decay;
+    return true;
+}
+bool rwkv_b200_set_penalty_weights(struct rwkv_context * ctx, const float * weights) {
+    Context * c = penalty_context(ctx, 0);
+    return c && set_penalty_weights(c, weights);
+}
+bool rwkv_b200_get_penalty_counts(struct rwkv_context * ctx, size_t sequence, float * counts_out) {
+    Context * c = penalty_context(ctx, sequence);
+    return c && get_penalty_counts(c, (int) sequence, counts_out);
+}
+bool rwkv_b200_set_penalty_counts(struct rwkv_context * ctx, size_t sequence, const float * counts_in) {
+    Context * c = penalty_context(ctx, sequence);
+    return c && set_penalty_counts(c, (int) sequence, counts_in);
+}
 bool rwkv_b200_batch_get_logits(struct rwkv_context * batch, size_t sequence, float * logits_out) {
     C(batch)->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(C(batch));
@@ -979,17 +1013,39 @@ struct StreamHook {
     uint32_t * published, * tokens, * ring, * timed_out;
 };
 
+// The penalty tables of rwkv_b200_test_generate_step_penalty: float counts [n_rows, n_vocab] in / out, decay [n_rows], weights
+// [n_vocab] or NULL.
+struct PenaltyHook {
+    float * counts;
+    const float * decay, * weights;
+};
+
+static bool finite_nonneg(const float * p, size_t n) {
+    for (size_t i = 0; i < n; i++)
+        if (!(std::isfinite(p[i]) && p[i] >= 0.0f)) return false;
+    return true;
+}
+
 // One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
 // the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained); with
 // samplers the sampled kernel (next and lp may then be NULL). With `stream` the streaming twin of that kernel runs, as the one node
-// of a graph, over pinned mapped copies of the caller's words.
+// of a graph, over pinned mapped copies of the caller's words. Without `pen` the rows take a->counts (integers, converted to the
+// kernel's float table and back), decay 1 and no weights; with it, a->counts must be NULL and pen's tables are used.
 static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
-                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr, const StreamHook * stream = nullptr) {
+                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr, const StreamHook * stream = nullptr,
+                               const PenaltyHook * pen = nullptr) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
-               a->step && a->frozen && a->counts && a->next_tokens && a->any_active, "Invalid generate-step arguments");
+               a->step && a->frozen && (pen ? !a->counts && pen->counts && pen->decay : a->counts != nullptr) && a->next_tokens && a->any_active,
+               "Invalid generate-step arguments");
     const size_t R = a->n_rows, V = a->n_vocab;
+    if (pen) {
+        for (size_t b = 0; b < R; b++)
+            RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, pen->decay[b] > 0.0f && pen->decay[b] <= 1.0f, "decay of row %zu must be in (0, 1]", b);
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, finite_nonneg(pen->counts, R * V), "The penalty counts must be finite and >= 0");
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !pen->weights || finite_nonneg(pen->weights, V), "The penalty weights must be finite and >= 0");
+    }
     if (!check_generate_rows(sink, R, V, a->max_tokens, a->temperature, a->top_p, a->presence_penalty, a->frequency_penalty, a->u, a->stop_ids, a->n_stop,
                              a->tokens, a->step)) return false;
     uint32_t n = 0;
@@ -1021,20 +1077,24 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         }
     }
     if (!hook_device(sink)) return false;
+    HookBuffers hb;
     GenShared sh{};
     for (size_t k = 0; k < a->n_stop; k++) sh.stop[k] = a->stop_ids[k];
     sh.n_stop = (uint32_t) a->n_stop; sh.stride = n;
+    sh.weights = pen ? hb.in(pen->weights, V) : nullptr;
     std::vector<GenRow> rows(R);
     for (size_t b = 0; b < R; b++)
-        rows[b] = GenRow{a->temperature[b], a->top_p[b], a->presence_penalty[b], a->frequency_penalty[b], a->max_tokens[b], a->step[b], a->frozen[b] ? 1u : 0u, 0};
+        rows[b] = GenRow{a->temperature[b], a->top_p[b], a->presence_penalty[b], a->frequency_penalty[b], a->max_tokens[b], a->step[b], a->frozen[b] ? 1u : 0u,
+                         pen ? pen->decay[b] : 1.0f};
+    std::vector<float> counts(pen ? 0 : R * V);
+    for (size_t i = 0; i < counts.size(); i++) counts[i] = (float) a->counts[i];
     const uint32_t zero = 0;
-    HookBuffers hb;
     GenStepParams gp{};
     gp.logits = hb.in(a->logits, R * V); gp.n_vocab = (int) V; gp.n_rows = (int) R;
     gp.rows = const_cast<GenRow *>(hb.in(rows.data(), R));
     gp.shared = const_cast<GenShared *>(hb.in(&sh, 1));
     gp.u = hb.in(a->u, R * n);
-    gp.counts = const_cast<uint32_t *>(hb.in(a->counts, R * V));
+    gp.counts = const_cast<float *>(hb.in(pen ? pen->counts : counts.data(), R * V));
     gp.bias_ids = static_cast<uint32_t *>(hb.alloc(R * V * sizeof(uint32_t)));
     gp.bias_values = static_cast<float *>(hb.alloc(R * V * sizeof(float)));
     gp.scratch = static_cast<float *>(hb.alloc(R * V * sizeof(float)));
@@ -1121,7 +1181,7 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
           : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
     }
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
-              cudaMemcpy(a->counts, gp.counts, R * V * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(pen ? pen->counts : counts.data(), gp.counts, R * V * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->next_tokens, gp.next_tokens, R * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
@@ -1132,6 +1192,7 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
                       cudaMemcpy(lp->top_logprobs, req.top_logprobs, cells * k * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess));
     RWKV_CHECK(sink, RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, ok, "generate step failed on the device: %s", cudaGetErrorString(e != cudaSuccess ? e : cudaGetLastError()));
     for (size_t b = 0; b < R; b++) { a->step[b] = rows[b].step; a->frozen[b] = rows[b].frozen ? 1 : 0; }
+    for (size_t i = 0; i < counts.size(); i++) a->counts[i] = (uint32_t) counts[i];
     for (size_t b = 0; constrained && b < R; b++)
         if (states[b] != UINT32_MAX) states[b] = states_out[b];
     if (stream) {
@@ -1161,7 +1222,8 @@ bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_
 
 // The sampled kernel's step: samplers[n_rows] in place of a's temperature, top_p and penalty arrays.
 static bool sampled_step_hook(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
-                              size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp, const StreamHook * stream = nullptr) {
+                              size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp, const StreamHook * stream = nullptr,
+                              const PenaltyHook * pen = nullptr) {
     ErrorSink sink = global_sink();
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS, "Invalid generate-step arguments");
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
@@ -1179,7 +1241,7 @@ static bool sampled_step_hook(const struct rwkv_b200_generate_step_args * a, con
     }
     struct rwkv_b200_generate_step_args args = *a;
     args.temperature = t.data(); args.top_p = p.data(); args.presence_penalty = pres.data(); args.frequency_penalty = freq.data();
-    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data(), stream);
+    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data(), stream, pen);
 }
 
 bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
@@ -1204,6 +1266,24 @@ bool rwkv_b200_test_generate_step_streaming(const struct rwkv_b200_generate_step
     LogprobsOut out{};
     if (lp && !logprobs_arg(sink, lp, out)) return false;
     return generate_step_hook(a, next, n_states, states, lp ? &out : nullptr, nullptr, &stream);
+}
+
+bool rwkv_b200_test_generate_step_penalty(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
+                                          const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
+                                          float * counts, const float * decay, const float * weights) {
+    g_last_error = RWKV_ERROR_NONE;
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family >= RWKV_B200_STEP_PLAIN && family <= RWKV_B200_STEP_SAMPLED, "Unknown step family %d", family);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, (family == RWKV_B200_STEP_SAMPLED) == (samplers != nullptr), "samplers go with the sampled family alone");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_CONSTRAINED ? next != nullptr : family != RWKV_B200_STEP_PLAIN || !next,
+               "The constrained family needs a table, the plain one takes none");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_LOGPROBS ? lp != nullptr : family == RWKV_B200_STEP_SAMPLED || !lp,
+               "The logprobs family needs lp, the plain and constrained ones take none");
+    const PenaltyHook pen{counts, decay, weights};
+    if (family == RWKV_B200_STEP_SAMPLED) return sampled_step_hook(a, samplers, next, n_states, states, lp, nullptr, &pen);
+    LogprobsOut out{};
+    if (lp && !logprobs_arg(sink, lp, out)) return false;
+    return generate_step_hook(a, next, n_states, states, lp ? &out : nullptr, nullptr, nullptr, &pen);
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

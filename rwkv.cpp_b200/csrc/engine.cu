@@ -811,6 +811,7 @@ Context * create_context(Model * model, ErrorSink sink, int batch_n) {
     const size_t n = model->state_len();
     const size_t seqs = batch_n > 0 ? (size_t) batch_n : 1;
     if (batch_n > 0) { ctx->batch_n = batch_n; ctx->batch_stride = (long long) n; ctx->overlap_copies = false; }
+    ctx->penalty_decay.assign(seqs, 1.0f);
     bool ok = cudaSetDevice(model->dev.device) == cudaSuccess
         && ctx->stream.create() == cudaSuccess
         && ctx->ev_start.create() == cudaSuccess && ctx->ev_stop.create() == cudaSuccess
@@ -1726,8 +1727,8 @@ bool ensure_generate_buffers(Context * ctx) {
     CUDA_OK(ctx, g.in_host.alloc(in_bytes));
     CUDA_OK(ctx, g.out_host.alloc(out_bytes));
     CUDA_OK(ctx, g.out.alloc(out_bytes));
-    CUDA_OK(ctx, g.counts.alloc(table * sizeof(uint32_t)));
-    CUDA_OK(ctx, cudaMemsetAsync(g.counts, 0, table * sizeof(uint32_t), ctx->stream));
+    CUDA_OK(ctx, g.counts.alloc(table * sizeof(float)));
+    CUDA_OK(ctx, cudaMemsetAsync(g.counts, 0, table * sizeof(float), ctx->stream));
     CUDA_OK(ctx, g.bias_ids.alloc(table * sizeof(uint32_t)));
     CUDA_OK(ctx, g.bias_values.alloc(table * sizeof(float)));
     CUDA_OK(ctx, g.scratch.alloc(table * sizeof(float)));
@@ -2044,8 +2045,9 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     memset(sh, 0, sizeof(GenShared));
     for (size_t k = 0; k < n_stop; k++) sh->stop[k] = stop_ids[k];
     sh->n_stop = (uint32_t) n_stop; sh->stride = (uint32_t) n;
+    sh->weights = ctx->pen_weights.set ? ctx->pen_weights.table.get() : nullptr;
     GenRow * gr = reinterpret_cast<GenRow *>(ctx->gen.in_host + sizeof(GenShared));
-    for (int b = 0; b < rows; b++) gr[b] = GenRow{temperature[b], top_p[b], presence[b], frequency[b], max_tokens[b], 0, 0, 0};
+    for (int b = 0; b < rows; b++) gr[b] = GenRow{temperature[b], top_p[b], presence[b], frequency[b], max_tokens[b], 0, 0, ctx->penalty_decay[b]};
     GenMaskRow * mr = reinterpret_cast<GenMaskRow *>(ctx->gen.in_host + gen_mask_offset(rows));
     for (int b = 0; b < rows; b++)
         mr[b] = constrained && automata[b] ? GenMaskRow{automata[b]->next, automata[b]->live, automaton_states[b], 0} : GenMaskRow{nullptr, nullptr, 0, 0};
@@ -2056,7 +2058,7 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
         if (keep_counts && keep_counts[b]) { b++; continue; }
         int e = b;
         while (e < rows && !(keep_counts && keep_counts[e])) e++;
-        CUDA_OK(ctx, cudaMemsetAsync(ctx->gen.counts + (size_t) b * V, 0, (size_t) (e - b) * V * sizeof(uint32_t), ctx->stream));
+        CUDA_OK(ctx, cudaMemsetAsync(ctx->gen.counts + (size_t) b * V, 0, (size_t) (e - b) * V * sizeof(float), ctx->stream));
         b = e;
     }
     const size_t out_words = gen_out_words(rows, n);
@@ -2116,6 +2118,59 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
     }
     RWKV_CHECK(ctx->sink(), RWKV_ERROR_CTX, false, in_time, "A token callback kept the device waiting for more than %d ms; its sequence was ended there",
                STREAM_TIMEOUT_MS);
+    return true;
+}
+
+bool read_penalty_table(ErrorSink sink, const float * p, size_t n, int device, std::vector<float> & host, const char * what) {
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, p, "NULL %s", what);
+    int dev = -1;
+    const bool in_hbm = on_device(p, &dev);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !in_hbm || dev == device, "The %s are in the memory of device %d, not of the context's device %d", what, dev, device);
+    host.resize(n);
+    if (in_hbm) RWKV_CHECK(sink, RWKV_ERROR_CTX, false, cudaMemcpy(host.data(), p, n * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess,
+                           "Reading the %s failed", what);
+    else memcpy(host.data(), p, n * sizeof(float));
+    for (size_t i = 0; i < n; i++)
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, std::isfinite(host[i]) && host[i] >= 0.0f, "The %s must be finite and >= 0 (entry %zu is %g)", what, i, host[i]);
+    return true;
+}
+
+bool set_penalty_weights(Context * ctx, const float * weights) {
+    if (!weights) { ctx->pen_weights.set = false; return true; }
+    const size_t V = (size_t) ctx->model->n_vocab;
+    std::vector<float> host;
+    if (!read_penalty_table(ctx->sink(), weights, V, ctx->model->dev.device, host, "penalty weights")) return false;
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    if (!ctx->pen_weights.table) CUDA_OK(ctx, ctx->pen_weights.table.alloc(V * sizeof(float)));
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->pen_weights.table, host.data(), V * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->pen_weights.set = true;
+    return true;
+}
+
+bool get_penalty_counts(Context * ctx, int seq, float * counts_out) {
+    const size_t V = (size_t) ctx->model->n_vocab;
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, counts_out, "NULL counts_out");
+    int dev = -1;
+    const bool in_hbm = on_device(counts_out, &dev);
+    RWKV_CHECK(ctx->sink(), RWKV_ERROR_ARGS, false, !in_hbm || dev == ctx->model->dev.device, "counts_out is in the memory of device %d, not of the context's device %d",
+               dev, ctx->model->dev.device);
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    if (ctx->gen.counts) CUDA_OK(ctx, cudaMemcpyAsync(counts_out, ctx->gen.counts + (size_t) seq * V, V * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    else if (in_hbm) CUDA_OK(ctx, cudaMemsetAsync(counts_out, 0, V * sizeof(float), ctx->stream));      // never generated: zeros, nothing allocated
+    else memset(counts_out, 0, V * sizeof(float));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
+    return true;
+}
+
+bool set_penalty_counts(Context * ctx, int seq, const float * counts_in) {
+    const size_t V = (size_t) ctx->model->n_vocab;
+    std::vector<float> host;
+    if (!read_penalty_table(ctx->sink(), counts_in, V, ctx->model->dev.device, host, "penalty counts")) return false;
+    CUDA_OK(ctx, cudaSetDevice(ctx->model->dev.device));
+    if (!ensure_generate_buffers(ctx)) return false;
+    CUDA_OK(ctx, cudaMemcpyAsync(ctx->gen.counts + (size_t) seq * V, host.data(), V * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_OK(ctx, cudaStreamSynchronize(ctx->stream));
     return true;
 }
 

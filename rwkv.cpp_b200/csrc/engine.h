@@ -153,11 +153,16 @@ struct Context {
     struct Generate {
         DeviceBuffer<unsigned char> in; PinnedBuffer<unsigned char> in_host;
         DeviceBuffer<uint32_t> out; PinnedBuffer<uint32_t> out_host;
-        DeviceBuffer<uint32_t> counts;     // [rows, n_vocab] penalty counts
+        DeviceBuffer<float> counts;        // [rows, n_vocab] penalty counts
         DeviceBuffer<uint32_t> bias_ids;   // [rows, n_vocab]
         DeviceBuffer<float> bias_values, scratch;   // [rows, n_vocab] each
         DeviceBuffer<float> park;          // batch contexts: [rows, n_vocab] logits of frozen rows
     } gen;
+    // The penalty decay of every row (set_penalty_decay), 1 until set; it travels in the call's GenRow. The penalty weights
+    // (set_penalty_weights): n_vocab floats, allocated by the first call that sets a table and kept at that address; `set` false
+    // means all 1. The call's GenShared carries the table's address, so no graph holds it.
+    std::vector<float> penalty_decay;
+    struct PenaltyWeights { DeviceBuffer<float> table; bool set = false; } pen_weights;
     // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by whether
     // the loop streams its tokens to a callback, and by whether its draws are constrained by automata
     GraphExec gen_graphs[2][2][2];
@@ -355,6 +360,14 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
               uint32_t * tokens_out, uint32_t * n_generated, TokenFn on_token = nullptr, void * user = nullptr,
               const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr, const LogprobsOut * lp = nullptr,
               const SamplerIn * samplers = nullptr);
+// The penalty tables of generation (rwkv_b200_set_penalty_weights, rwkv_b200_get_penalty_counts / rwkv_b200_set_penalty_counts,
+// include/rwkv_b200.h). read_penalty_table copies n floats from host memory or device memory of `device` into `host` and checks that
+// each is finite and >= 0 (RWKV_ERROR_ARGS, also for a device pointer of another device). The others have their context and sequence
+// checked by the caller, check their table, allocate what they need all or nothing, and synchronise. weights NULL: all 1.
+bool read_penalty_table(ErrorSink sink, const float * p, size_t n, int device, std::vector<float> & host, const char * what);
+bool set_penalty_weights(Context * ctx, const float * weights);
+bool get_penalty_counts(Context * ctx, int seq, float * counts_out);
+bool set_penalty_counts(Context * ctx, int seq, const float * counts_in);
 
 // Beam search over the sequences of a batch context (rwkv_b200_beam_search_groups, include/rwkv_b200.h): n_groups searches of width
 // W = batch_n / n_groups, group g from sequence g*W's state and logits, as one graph launch; rwkv_b200_beam_search is n_groups = 1. The

@@ -219,18 +219,21 @@ cudaError_t launch_sample_batch(const SampleBatchParams & p, cudaStream_t s);
 
 // Device-side generation (rwkv_b200_generate / rwkv_b200_batch_generate): one step of the sample-and-evaluate loop per launch, CTA b
 // for row b. A row that is not frozen freezes when it has drawn max_tokens tokens; otherwise it draws with u[b * stride + step] from
-// its logits with the bias -(presence + count[n] * frequency) on every token n it has counted (sample_row's bias path), writes the
-// token to tokens[b * stride + step], and freezes on a stop token or else counts it and makes it the row's next input token. The
-// last CTA of the step sets both conditional handles to "some row is still active" and, if so, counts one more pass.
+// its logits with the bias -(presence + c[n] * frequency) on every token n with penalty count c[n] != 0 (sample_row's bias path),
+// writes the token to tokens[b * stride + step], and freezes on a stop token; any other token is evaluated: every count of the row
+// becomes c[n] * decay, then c[tok] += weights[tok] (1 without a table), and tok is the row's next input token. The last CTA of the
+// step sets both conditional handles to "some row is still active" and, if so, counts one more pass.
 struct GenRow {                       // written by the host per call; step and frozen are then the loop's state
     float temperature, top_p, presence, frequency;
-    uint32_t max_tokens, step, frozen, pad;
+    uint32_t max_tokens, step, frozen;
+    float decay;                      // penalty decay, 0 < decay <= 1 (1: the counts only grow)
 };
 constexpr int GENERATE_MAX_STOP = 16;
 struct GenShared {                    // written by the host per call (ticket = active = 0)
     uint32_t stop[GENERATE_MAX_STOP];
     uint32_t n_stop, stride;
     uint32_t ticket, active;          // CTAs done with this step / rows active after it; reset by the step's last CTA
+    const float * weights;            // [n_vocab] penalty weights, or NULL for all 1; in the upload so that no graph holds it
 };
 struct GenStepParams {
     const float * logits;             // [n_rows, n_vocab]
@@ -238,7 +241,7 @@ struct GenStepParams {
     GenRow * rows;                    // [n_rows]
     GenShared * shared;
     const double * u;                 // [n_rows][stride]
-    uint32_t * counts;                // [n_rows, n_vocab]
+    float * counts;                   // [n_rows, n_vocab] penalty counts
     uint32_t * bias_ids;              // [n_rows, n_vocab] scratch: the bias list of a row, one entry per token (id n_vocab = none)
     float * bias_values;
     float * scratch;                  // [n_rows, n_vocab]: the biased logits
@@ -317,7 +320,7 @@ cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t 
 // Generation with a per-row sampler (rwkv_b200_generate_sampled / rwkv_b200_batch_generate_sampled): the constrained steps (a row with
 // a NULL table is unconstrained), with log-probabilities when *req is not NULL, where row b also has
 // - user bias entries bias[bias_begin, bias_end) (distinct ids): after the penalty / mask list is written, an id its state allows
-//   gets the entry value - (presence + count * frequency) if counted, else value;
+//   gets the entry value - (presence + c * frequency) if its penalty count c is not 0, else value;
 // - top_k (0 = off) and min_p (0 = off): a token is kept iff its probability is at least the top-p cutoff, the top_k-th largest
 //   probability (with multiplicity) and min_p * the largest probability (sample_row's KeepFilter).
 // The rows, the pool and the request word live in the per-call upload, so that one graph serves every sampler.

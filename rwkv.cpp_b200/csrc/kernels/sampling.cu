@@ -380,7 +380,7 @@ struct RequestedLogprobs {
 
 // The loops without a sampler: no user bias, no filter.
 struct NoSampler {
-    __device__ __forceinline__ void add_bias(int, int, const uint32_t *, const uint16_t *, float, float, uint32_t *, float *) const {}
+    __device__ __forceinline__ void add_bias(int, int, const float *, const uint16_t *, float, float, uint32_t *, float *) const {}
     __device__ __forceinline__ NoFilter filter(int) const { return NoFilter{}; }
 };
 
@@ -389,17 +389,17 @@ struct RowSampler {
     const GenSamplerRow * rows;
     const GenBiasEntry * bias;
     // Every thread, once row b's penalty / mask list (ids, values, one entry per token) is written: the row's user entries over their
-    // ids. A token the state does not allow keeps its -inf; a counted one gets value - (presence + count * frequency), rounded as the
-    // penalty alone is and then once more; any other gets value.
-    __device__ __forceinline__ void add_bias(int b, int V, const uint32_t * counts, const uint16_t * allowed, float presence, float frequency,
+    // ids. A token the state does not allow keeps its -inf; a counted one (count c != 0) gets value - (presence + c * frequency),
+    // rounded as the penalty alone is and then once more; any other gets value.
+    __device__ __forceinline__ void add_bias(int b, int V, const float * counts, const uint16_t * allowed, float presence, float frequency,
                                              uint32_t * ids, float * values) const {
         const GenSamplerRow r = rows[b];
         for (uint32_t k = r.bias_begin + threadIdx.x; k < r.bias_end; k += SAMPLE_THREADS) {
             const GenBiasEntry e = bias[k];
             if (e.id >= (uint32_t) V || (allowed && allowed[e.id] == GEN_MASK_DEAD)) continue;
-            const uint32_t c = counts[e.id];
+            const float c = counts[e.id];
             ids[e.id] = e.id;
-            values[e.id] = c ? __fsub_rn(e.value, __fadd_rn(presence, __fmul_rn((float) c, frequency))) : e.value;
+            values[e.id] = c != 0.f ? __fsub_rn(e.value, __fadd_rn(presence, __fmul_rn(c, frequency))) : e.value;
         }
         __syncthreads();
     }
@@ -428,13 +428,13 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
     uint32_t tok = 0;
     if (draw) {
         const uint32_t step = r->step;
-        const float presence = r->presence, frequency = r->frequency;
+        const float presence = r->presence, frequency = r->frequency, decay = r->decay;
         const uint16_t * allowed = mask.table_row(b, V);
         for (int i = tid; i < V; i += SAMPLE_THREADS) {      // chat_with_bot.py:244-247, as a bias list over every token
-            const uint32_t c = gp.counts[off + i];
+            const float c = gp.counts[off + i];
             const bool dead = allowed && allowed[i] == GEN_MASK_DEAD;     // a token the state does not allow: -inf, whatever its count
-            gp.bias_ids[off + i] = (c || dead) ? (uint32_t) i : (uint32_t) V;
-            gp.bias_values[off + i] = dead ? -INFINITY : -__fadd_rn(presence, __fmul_rn((float) c, frequency));
+            gp.bias_ids[off + i] = (c != 0.f || dead) ? (uint32_t) i : (uint32_t) V;
+            gp.bias_values[off + i] = dead ? -INFINITY : -__fadd_rn(presence, __fmul_rn(c, frequency));
         }
         __syncthreads();
         smp.add_bias(b, V, gp.counts + off, allowed, presence, frequency, gp.bias_ids + off, gp.bias_values + off);
@@ -452,9 +452,25 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
             bool stop = false;
             for (uint32_t k = 0; k < sh->n_stop; k++) stop = stop || sh->stop[k] == tok;
             if (stop) { r->frozen = 1; park = 1; }      // reported, not evaluated, not counted (chat_with_bot.py:249-252)
-            else { gp.counts[off + tok] += 1; mask.advance(b, V, tok); }
+            else {
+                if (decay == 1.0f) gp.counts[off + tok] = __fadd_rn(gp.counts[off + tok], sh->weights ? sh->weights[tok] : 1.0f);
+                mask.advance(b, V, tok);
+            }
         }
         __syncthreads();
+        // The decay of an evaluated token: every count becomes c * decay, then the drawn token's own count adds its weight, both in
+        // the thread that owns it, so that no barrier orders them. It cannot share the bias loop above: that runs before the draw,
+        // and a drawn stop id leaves the counts as they were. The row was read by that loop, so this pass reads it from L2.
+        if (decay != 1.0f && !park) {
+            const uint32_t t = *(volatile uint32_t *) p.token_out;
+            const float w = sh->weights ? sh->weights[t] : 1.0f;
+            for (int i = tid; i < V; i += SAMPLE_THREADS) {
+                const float c = gp.counts[off + i];
+                if (c == 0.f && i != (int) t) continue;         // 0 * decay is 0: most of a row is never written
+                const float d = __fmul_rn(c, decay);
+                gp.counts[off + i] = i == (int) t ? __fadd_rn(d, w) : d;
+            }
+        }
         lp.record(b, (size_t) b * sh->stride + step, step, gp.logits + off, V, tok);
     }
     if (park && gp.park)

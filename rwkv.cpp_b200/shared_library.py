@@ -65,9 +65,9 @@ class Checkpoint(ctypes.Structure):   # include/rwkv_b200.h: struct rwkv_b200_ch
     _fields_ = [("sequence", ctypes.c_uint32), ("position", ctypes.c_uint32), ("state_out", ctypes.POINTER(ctypes.c_float))]
 
 
-def _state_address(buf, n: int) -> int:
-    """Address of a buffer that can take one state of n floats: a C-contiguous float32 numpy array or torch tensor (host or CUDA) of
-    at least n elements. Anything else is refused before the library could write past it."""
+def _state_address(buf, n: int, what: str = "a checkpoint buffer") -> int:
+    """Address of a buffer that can take one state (or penalty table) of n floats: a C-contiguous float32 numpy array or torch tensor
+    (host or CUDA) of at least n elements. Anything else is refused before the library could read or write past it."""
     if hasattr(buf, "data_ptr"):
         import torch
         ok = buf.dtype == torch.float32 and buf.is_contiguous() and buf.numel() >= n
@@ -76,7 +76,7 @@ def _state_address(buf, n: int) -> int:
         ok = isinstance(buf, np.ndarray) and buf.dtype == np.float32 and buf.flags.c_contiguous and buf.size >= n
         addr = buf.ctypes.data if ok else 0
     if not ok:
-        raise ValueError(f"a checkpoint buffer must be a contiguous float32 array or tensor of at least {n} elements")
+        raise ValueError(f"{what} must be a contiguous float32 array or tensor of at least {n} elements")
     return addr
 
 
@@ -309,6 +309,17 @@ class RWKVSharedLibrary:
         lib.rwkv_b200_batch_eval_ragged_checkpoints.restype = ctypes.c_bool
         lib.rwkv_b200_test_checkpoint_args.argtypes = [ctypes.c_size_t, P_U32, ctypes.c_size_t, P_CP, ctypes.c_size_t]
         lib.rwkv_b200_test_checkpoint_args.restype = ctypes.c_bool
+        lib.rwkv_b200_set_penalty_decay.argtypes = [vp, ctypes.c_size_t, ctypes.c_float]
+        lib.rwkv_b200_set_penalty_decay.restype = ctypes.c_bool
+        lib.rwkv_b200_set_penalty_weights.argtypes = [vp, P_FLOAT]
+        lib.rwkv_b200_set_penalty_weights.restype = ctypes.c_bool
+        lib.rwkv_b200_get_penalty_counts.argtypes = [vp, ctypes.c_size_t, P_FLOAT]
+        lib.rwkv_b200_get_penalty_counts.restype = ctypes.c_bool
+        lib.rwkv_b200_set_penalty_counts.argtypes = [vp, ctypes.c_size_t, P_FLOAT]
+        lib.rwkv_b200_set_penalty_counts.restype = ctypes.c_bool
+        lib.rwkv_b200_test_generate_step_penalty.argtypes = [ctypes.c_void_p, ctypes.c_int, P_SAMPLER, P_U16, ctypes.c_size_t, P_U32, P_LOGPROBS,
+                                                             P_FLOAT, P_FLOAT, P_FLOAT]
+        lib.rwkv_b200_test_generate_step_penalty.restype = ctypes.c_bool
         lib.rwkv_b200_matvec.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, P_FLOAT, P_FLOAT, ctypes.c_int]
         lib.rwkv_b200_matvec.restype = ctypes.c_bool
 
@@ -501,6 +512,37 @@ class RWKVSharedLibrary:
         if not self.library.rwkv_b200_batch_eval_ragged_checkpoints(batch.ptr, toks, cnt, want_logits, arr, len(checkpoints)):
             raise ValueError(f"rwkv_b200_batch_eval_ragged_checkpoints failed (error flags 0x{self.rwkv_get_last_error(batch):x})")
         return out
+
+    def rwkv_b200_set_penalty_decay(self, ctx: RWKVContext, sequence: int, decay: float) -> None:
+        """Every later generate call of `sequence` (0 for a single-sequence context) multiplies all of its penalty counts by decay
+        (0 < decay <= 1) after each evaluated token, before that token's count grows."""
+        if not self.library.rwkv_b200_set_penalty_decay(ctx.ptr, sequence, ctypes.c_float(decay)):
+            raise ValueError(f"rwkv_b200_set_penalty_decay failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+
+    def rwkv_b200_set_penalty_weights(self, ctx: RWKVContext, weights=None) -> None:
+        """What an evaluated token adds to its own penalty count, per token (n_vocab floats >= 0, a numpy array or a torch tensor, CUDA
+        ones included), for every sequence of the context; None goes back to 1 for every token."""
+        addr = 0 if weights is None else _state_address(weights, self.rwkv_get_logits_len(ctx), "a penalty table")
+        if not self.library.rwkv_b200_set_penalty_weights(ctx.ptr, ctypes.cast(addr, P_FLOAT)):
+            raise ValueError(f"rwkv_b200_set_penalty_weights failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+
+    def rwkv_b200_get_penalty_counts(self, ctx: RWKVContext, sequence: int = 0, out=None):
+        """The penalty counts of `sequence` as a new float32 numpy array of n_vocab, or written into out (a numpy array or a torch
+        tensor, CUDA ones included), which is returned."""
+        n = self.rwkv_get_logits_len(ctx)
+        if out is None:
+            out = np.empty(n, np.float32)
+        addr = _state_address(out, n, "a penalty table")
+        if not self.library.rwkv_b200_get_penalty_counts(ctx.ptr, sequence, ctypes.cast(addr, P_FLOAT)):
+            raise ValueError(f"rwkv_b200_get_penalty_counts failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
+        return out
+
+    def rwkv_b200_set_penalty_counts(self, ctx: RWKVContext, sequence: int, counts) -> None:
+        """Replaces the penalty counts of `sequence` (n_vocab floats >= 0, a numpy array or a torch tensor, CUDA ones included); the next
+        generate call of that sequence with keep_counts starts from them."""
+        addr = _state_address(counts, self.rwkv_get_logits_len(ctx), "a penalty table")
+        if not self.library.rwkv_b200_set_penalty_counts(ctx.ptr, sequence, ctypes.cast(addr, P_FLOAT)):
+            raise ValueError(f"rwkv_b200_set_penalty_counts failed (error flags 0x{self.rwkv_get_last_error(ctx):x})")
 
     def rwkv_b200_init_from_file_ex(self, model_file_path: str, device: int, layer_begin: int = 0, layer_end: int = -1) -> RWKVContext:
         ptr = self.library.rwkv_b200_init_from_file_ex(model_file_path.encode("utf-8"), device, layer_begin, layer_end)
