@@ -643,20 +643,27 @@ static bool logprobs_arg(ErrorSink sink, const struct rwkv_b200_logprobs * lp, L
 // The engine's part of a public sampler (temperature, top_p and the penalties travel in GenRow).
 static SamplerIn sampler_in(const struct rwkv_b200_sampler & s) { return SamplerIn{s.top_k, s.min_p, s.n_bias, s.bias_ids, s.bias_values}; }
 
-// The single-sequence generate calls; on_token NULL is the blocking loop. `constrained`: the row follows *automaton from
-// *automaton_state (both checked here, the rest by generate). `sampled`: *sampler (checked here) replaces temperature, top_p and the
-// penalties, and lp may be NULL.
+// The name suffix of a family's generate calls.
+static const char * generate_suffix(GenFamily family, bool streaming) {
+    static const char * const suffix[] = {"", "_constrained", "_logprobs", "_sampled"};
+    return family == GEN_PLAIN && streaming ? "_stream" : suffix[family];
+}
+
+// The single-sequence generate calls of `family`; on_token NULL is the blocking loop. GEN_CONSTRAINED, or a logprobs or sampled call
+// with an automaton: the row follows *automaton from *automaton_state (both checked here, the rest by generate). GEN_LOGPROBS: lp is
+// checked here. GEN_SAMPLED: *sampler (checked here) replaces temperature, top_p and the penalties, and lp may be NULL.
 static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float temperature, float top_p, float presence_penalty, float frequency_penalty,
                             bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, size_t * n_generated,
-                            bool streaming, TokenFn on_token, void * user, bool constrained = false, const Automaton * automaton = nullptr,
-                            uint32_t * automaton_state = nullptr, bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr,
-                            bool sampled = false, const struct rwkv_b200_sampler * sampler = nullptr) {
+                            bool streaming, TokenFn on_token, void * user, GenFamily family = GEN_PLAIN, const Automaton * automaton = nullptr,
+                            uint32_t * automaton_state = nullptr, const struct rwkv_b200_logprobs * lp = nullptr,
+                            const struct rwkv_b200_sampler * sampler = nullptr) {
     if (!ctx) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(ctx);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
-    const char * suffix = sampled ? "_sampled" : logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "";
-    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s", suffix);
+    const bool constrained = family == GEN_CONSTRAINED || automaton, logprobs = family == GEN_LOGPROBS || lp, sampled = family == GEN_SAMPLED;
+    RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n == 0, "This is a batch context; use rwkv_b200_batch_generate%s",
+               generate_suffix(family, streaming));
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, max_tokens >= 1 && max_tokens <= (size_t) RWKV_B200_GENERATE_MAX && n_generated,
                "max_tokens must be in 1 .. %d and n_generated not NULL", RWKV_B200_GENERATE_MAX);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
@@ -679,25 +686,25 @@ static bool generate_single(struct rwkv_context * ctx, size_t max_tokens, float 
     return ok;
 }
 
-// The batch generate calls; on_token NULL is the blocking loop. `sampled`: samplers[n_sequences] (checked here) replace the
-// temperature, top_p and penalty arrays.
+// The batch generate calls of `family`; on_token NULL is the blocking loop. The automata and lp as for generate_single; GEN_SAMPLED:
+// samplers[n_sequences] (checked here) replace the temperature, top_p and penalty arrays.
 static bool generate_batch(struct rwkv_context * batch, const uint32_t * max_tokens, const float * temperature, const float * top_p,
                            const float * presence_penalty, const float * frequency_penalty, const uint8_t * keep_counts, const double * u,
                            const uint32_t * stop_ids, size_t n_stop, uint32_t * tokens_out, uint32_t * n_generated, bool streaming, TokenFn on_token, void * user,
-                           bool constrained = false, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr,
-                           bool logprobs = false, const struct rwkv_b200_logprobs * lp = nullptr, bool sampled = false,
-                           const struct rwkv_b200_sampler * samplers = nullptr) {
+                           GenFamily family = GEN_PLAIN, const Automaton * const * automata = nullptr, uint32_t * automaton_states = nullptr,
+                           const struct rwkv_b200_logprobs * lp = nullptr, const struct rwkv_b200_sampler * samplers = nullptr) {
     if (!batch) { ErrorSink sink = global_sink(); g_last_error = RWKV_ERROR_NONE; RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL context"); }
     Context * c = C(batch);
     c->last_error = RWKV_ERROR_NONE;
     RWKV_NOT_STREAMING(c);
+    const bool constrained = family == GEN_CONSTRAINED || automata, logprobs = family == GEN_LOGPROBS || lp;
     RWKV_CHECK(c->sink(), RWKV_ERROR_CTX | RWKV_ERROR_UNSUPPORTED, false, c->batch_n > 0, "Not a batch context; use rwkv_b200_generate%s",
-               sampled ? "_sampled" : logprobs ? "_logprobs" : constrained ? "_constrained" : streaming ? "_stream" : "");
+               generate_suffix(family, streaming));
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !streaming || on_token, "NULL on_token");
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, !constrained || (automata && automaton_states), "NULL automata or automaton_states");
     LogprobsOut out{};
     if (logprobs && !logprobs_arg(c->sink(), lp, out)) return false;
-    if (!sampled)
+    if (family != GEN_SAMPLED)
         return generate(c, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
                         on_token, user, automata, automaton_states, logprobs ? &out : nullptr);
     RWKV_CHECK(c->sink(), RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
@@ -811,7 +818,7 @@ bool rwkv_b200_generate_constrained(struct rwkv_context * ctx, const struct rwkv
                                     const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
                                     size_t * n_generated) {
     return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
-                           false, on_token, user, true, automaton, automaton_state);
+                           false, on_token, user, GEN_CONSTRAINED, automaton, automaton_state);
 }
 
 bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata, uint32_t * automaton_states,
@@ -820,7 +827,7 @@ bool rwkv_b200_batch_generate_constrained(struct rwkv_context * batch, const str
                                           size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated) {
     static_assert(sizeof(struct rwkv_b200_automaton) == sizeof(Automaton), "the handle is the engine's automaton");
     return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
-                          false, on_token, user, true, reinterpret_cast<const Automaton * const *>(automata), automaton_states);
+                          false, on_token, user, GEN_CONSTRAINED, reinterpret_cast<const Automaton * const *>(automata), automaton_states);
 }
 
 bool rwkv_b200_generate_logprobs(struct rwkv_context * ctx, const struct rwkv_b200_automaton * automaton, uint32_t * automaton_state, size_t max_tokens,
@@ -828,7 +835,7 @@ bool rwkv_b200_generate_logprobs(struct rwkv_context * ctx, const struct rwkv_b2
                                  const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
                                  size_t * n_generated, const struct rwkv_b200_logprobs * lp) {
     return generate_single(ctx, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
-                           on_token != nullptr, on_token, user, automaton != nullptr, automaton, automaton_state, true, lp);
+                           on_token != nullptr, on_token, user, GEN_LOGPROBS, automaton, automaton_state, lp);
 }
 
 bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, const struct rwkv_b200_automaton * const * automata, uint32_t * automaton_states,
@@ -837,15 +844,14 @@ bool rwkv_b200_batch_generate_logprobs(struct rwkv_context * batch, const struct
                                        size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, uint32_t * n_generated,
                                        const struct rwkv_b200_logprobs * lp) {
     return generate_batch(batch, max_tokens, temperature, top_p, presence_penalty, frequency_penalty, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated,
-                          on_token != nullptr, on_token, user, automata != nullptr, reinterpret_cast<const Automaton * const *>(automata), automaton_states,
-                          true, lp);
+                          on_token != nullptr, on_token, user, GEN_LOGPROBS, reinterpret_cast<const Automaton * const *>(automata), automaton_states, lp);
 }
 
 bool rwkv_b200_generate_sampled(struct rwkv_context * ctx, const struct rwkv_b200_sampler * sampler, const struct rwkv_b200_automaton * automaton,
                                 uint32_t * automaton_state, size_t max_tokens, bool keep_counts, const double * u, const uint32_t * stop_ids, size_t n_stop,
                                 rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out, size_t * n_generated, const struct rwkv_b200_logprobs * lp) {
     return generate_single(ctx, max_tokens, 0.0f, 0.0f, 0.0f, 0.0f, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token != nullptr, on_token, user,
-                           automaton != nullptr, automaton, automaton_state, lp != nullptr, lp, true, sampler);
+                           GEN_SAMPLED, automaton, automaton_state, lp, sampler);
 }
 
 bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct rwkv_b200_sampler * samplers, const struct rwkv_b200_automaton * const * automata,
@@ -853,8 +859,7 @@ bool rwkv_b200_batch_generate_sampled(struct rwkv_context * batch, const struct 
                                       const uint32_t * stop_ids, size_t n_stop, rwkv_b200_token_fn on_token, void * user, uint32_t * tokens_out,
                                       uint32_t * n_generated, const struct rwkv_b200_logprobs * lp) {
     return generate_batch(batch, max_tokens, nullptr, nullptr, nullptr, nullptr, keep_counts, u, stop_ids, n_stop, tokens_out, n_generated, on_token != nullptr,
-                          on_token, user, automata != nullptr, reinterpret_cast<const Automaton * const *>(automata), automaton_states, lp != nullptr, lp,
-                          true, samplers);
+                          on_token, user, GEN_SAMPLED, reinterpret_cast<const Automaton * const *>(automata), automaton_states, lp, samplers);
 }
 
 static_assert(RWKV_B200_BEAM_MAX == BEAM_MAX && 2 * BEAM_MAX <= GEN_TOP_MAX, "beam width of the header and the kernel");
@@ -1026,16 +1031,39 @@ static bool finite_nonneg(const float * p, size_t n) {
     return true;
 }
 
-// One step of the generation kernel on host logits: the unconstrained kernel, or with `next` the constrained one, row b following
-// the table from states[b] (UINT32_MAX: unconstrained); with lp the logprob kernel (next may then be NULL: no row constrained); with
-// samplers the sampled kernel (next and lp may then be NULL). With `stream` the streaming twin of that kernel runs, as the one node
-// of a graph, over pinned mapped copies of the caller's words. Without `pen` the rows take a->counts (integers, converted to the
-// kernel's float table and back), decay 1 and no weights; with it, a->counts must be NULL and pen's tables are used.
-static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
-                               const LogprobsOut * lp = nullptr, const SamplerIn * samplers = nullptr, const StreamHook * stream = nullptr,
-                               const PenaltyHook * pen = nullptr) {
+// One step of the `family` kernel (ops.h: GenFamily) on host logits. With `next`, row b follows the table from states[b] (UINT32_MAX:
+// unconstrained); the logprobs and sampled kernels also run without one (no row constrained). The logprobs kernel reports into *lp_in;
+// the sampled kernel draws with samplers[n_rows] in place of a's temperature, top_p and penalty arrays, and reports into *lp_in when it
+// is not NULL. With `stream` the streaming twin of that kernel runs, as the one node of a graph, over pinned mapped copies of the
+// caller's words. Without `pen` the rows take a->counts (integers, converted to the kernel's float table and back), decay 1 and no
+// weights; with it, a->counts must be NULL and pen's tables are used.
+static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, GenFamily family, const struct rwkv_b200_sampler * sampler_args,
+                               const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp_in,
+                               const StreamHook * stream = nullptr, const PenaltyHook * pen = nullptr) {
     g_last_error = RWKV_ERROR_NONE;
     ErrorSink sink = global_sink();
+    LogprobsOut out{};
+    if ((family == GEN_LOGPROBS || lp_in) && !logprobs_arg(sink, lp_in, out)) return false;
+    const LogprobsOut * lp = family == GEN_LOGPROBS || lp_in ? &out : nullptr;
+    struct rwkv_b200_generate_step_args sampled_args;
+    std::vector<float> temperature, top_p, presence, frequency;
+    std::vector<SamplerIn> sampler_in_rows;
+    if (family == GEN_SAMPLED) {
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS, "Invalid generate-step arguments");
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, sampler_args, "NULL samplers");
+        RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !a->temperature && !a->top_p && !a->presence_penalty && !a->frequency_penalty,
+                   "temperature, top_p and the penalties come from the samplers: pass NULL");
+        for (size_t b = 0; b < a->n_rows; b++) {
+            temperature.push_back(sampler_args[b].temperature); top_p.push_back(sampler_args[b].top_p);
+            presence.push_back(sampler_args[b].presence_penalty); frequency.push_back(sampler_args[b].frequency_penalty);
+            sampler_in_rows.push_back(sampler_in(sampler_args[b]));
+        }
+        sampled_args = *a;
+        sampled_args.temperature = temperature.data(); sampled_args.top_p = top_p.data();
+        sampled_args.presence_penalty = presence.data(); sampled_args.frequency_penalty = frequency.data();
+        a = &sampled_args;
+    }
+    const SamplerIn * samplers = family == GEN_SAMPLED ? sampler_in_rows.data() : nullptr;
     RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->logits && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS && a->n_vocab >= 1 && a->n_vocab <= 65536 &&
                a->step && a->frozen && (pen ? !a->counts && pen->counts && pen->decay : a->counts != nullptr) && a->next_tokens && a->any_active,
                "Invalid generate-step arguments");
@@ -1102,8 +1130,6 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     gp.n_generated = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
     gp.passes = const_cast<uint32_t *>(hb.in(&zero, 1));
     gp.next_tokens = static_cast<int *>(hb.alloc(R * sizeof(int)));
-    GenConstrainedParams cp{};
-    cp.stream.step = gp;
     // the streaming kernel's words in pinned mapped memory, as the engine keeps them: acked [R], published [R], timed_out, tokens
     // [R][GENERATE_MAX], ring [R][2][GEN_LP_RECORD]
     PinnedBuffer<uint32_t> pinned;
@@ -1118,27 +1144,22 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
             pinned[2 * R] = 0;
             std::copy(stream->tokens, stream->tokens + R * GENERATE_MAX, pinned + tok_at);
             if (lp) std::copy(stream->ring, stream->ring + ring_words, pinned + ring_at);
-            cp.stream.acked = mapped; cp.stream.published = mapped + R; cp.stream.timed_out = mapped + 2 * R; cp.stream.tokens = mapped + tok_at;
+            gp.acked = mapped; gp.published = mapped + R; gp.timed_out = mapped + 2 * R; gp.stream_tokens = mapped + tok_at;
         }
     }
     std::vector<uint32_t> states_out(R);
-    if (constrained) {
-        const uint16_t * d_next = hb.in(next, n_states * V);
-        const uint8_t * d_live = hb.in(live.data(), n_states);
+    if (family != GEN_PLAIN) {      // without a table every row is unconstrained
+        const uint16_t * d_next = constrained ? hb.in(next, n_states * V) : nullptr;
+        const uint8_t * d_live = constrained ? hb.in(live.data(), n_states) : nullptr;
         std::vector<GenMaskRow> mask(R);
         for (size_t b = 0; b < R; b++)
-            mask[b] = states[b] == UINT32_MAX ? GenMaskRow{nullptr, nullptr, 0, 0} : GenMaskRow{d_next, d_live, states[b], 0};
-        cp.mask = const_cast<GenMaskRow *>(hb.in(mask.data(), R));
-        cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
+            mask[b] = !constrained || states[b] == UINT32_MAX ? GenMaskRow{nullptr, nullptr, 0, 0} : GenMaskRow{d_next, d_live, states[b], 0};
+        gp.mask = const_cast<GenMaskRow *>(hb.in(mask.data(), R));
+        gp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
     }
-    GenLogprobParams lpp{};
     GenLogprobRequest req{};
+    const GenLogprobRequest * d_req = nullptr;
     const size_t cells = R * n, k = lp ? lp->top_n : 0;
-    if (!constrained && (lp || samplers)) {     // every row unconstrained without a table
-        const std::vector<GenMaskRow> none(R, GenMaskRow{nullptr, nullptr, 0, 0});
-        cp.mask = const_cast<GenMaskRow *>(hb.in(none.data(), R));
-        cp.states_out = static_cast<uint32_t *>(hb.alloc(R * sizeof(uint32_t)));
-    }
     if (lp) {       // the outputs start as the caller's arrays
         req.top_n = (uint32_t) k;
         req.logprobs = const_cast<float *>(hb.in(lp->logprobs, cells));
@@ -1146,10 +1167,9 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         req.top_ids = k ? const_cast<uint32_t *>(hb.in(lp->top_ids, cells * k)) : nullptr;
         req.top_logprobs = k ? const_cast<float *>(hb.in(lp->top_logprobs, cells * k)) : nullptr;
         req.ring = mapped ? mapped + ring_at : nullptr;
-        lpp.gen = cp;
-        lpp.req = hb.in(&req, 1);
+        d_req = hb.in(&req, 1);
     }
-    GenSamplerParams smp{};
+    if (family == GEN_LOGPROBS) gp.lp = d_req;
     if (samplers) {
         std::vector<GenSamplerRow> srows(R);
         std::vector<GenBiasEntry> pool;
@@ -1158,11 +1178,9 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
             srows[b] = GenSamplerRow{s.top_k, s.min_p, (uint32_t) pool.size(), (uint32_t) (pool.size() + s.n_bias)};
             for (size_t k = 0; k < s.n_bias; k++) pool.push_back(GenBiasEntry{s.bias_ids[k], s.bias_values[k]});
         }
-        const GenLogprobRequest * word = lp ? lpp.req : nullptr;
-        smp.gen = cp;
-        smp.req = hb.in(&word, 1);
-        smp.rows = hb.in(srows.data(), R);
-        smp.bias = pool.empty() ? nullptr : hb.in(pool.data(), pool.size());
+        gp.lp_word = hb.in(&d_req, 1);
+        gp.samplers = hb.in(srows.data(), R);
+        gp.user_bias = pool.empty() ? nullptr : hb.in(pool.data(), pool.size());
     }
     cudaError_t e = cudaSuccess;
     if (hb.ok && stream) {      // the streaming kernels exist only as graph nodes
@@ -1170,22 +1188,19 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
         GraphExec x;
         cudaGraphNode_t node = nullptr;
         e = g.create();
-        if (e == cudaSuccess)
-            e = samplers ? add_generate_sampled_step_node(g, nullptr, 0, smp, true, &node) : lp ? add_generate_logprob_step_node(g, nullptr, 0, lpp, true, &node)
-              : constrained ? add_generate_constrained_step_node(g, nullptr, 0, cp, true, &node) : add_generate_stream_step_node(g, nullptr, 0, cp.stream, &node);
+        if (e == cudaSuccess) e = add_generate_step_node(g, nullptr, 0, gp, family, true, &node);
         if (e == cudaSuccess) e = x.instantiate(g);
         if (e == cudaSuccess) e = cudaGraphLaunch(x, 0);
         if (e == cudaSuccess) e = cudaStreamSynchronize(0);
     } else if (hb.ok) {
-        e = samplers ? launch_generate_sampled_step(smp, 0) : lp ? launch_generate_logprob_step(lpp, 0)
-          : constrained ? launch_generate_constrained_step(cp, 0) : launch_generate_step(gp, 0);
+        e = launch_generate_step(gp, family, 0);
     }
     bool ok = hb.finish(e) && cudaMemcpy(rows.data(), gp.rows, R * sizeof(GenRow), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(pen ? pen->counts : counts.data(), gp.counts, R * V * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->tokens, gp.tokens, R * n * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->next_tokens, gp.next_tokens, R * sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess &&
               cudaMemcpy(a->any_active, gp.passes, sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
-              (!constrained || cudaMemcpy(states_out.data(), cp.states_out, R * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess) &&
+              (!constrained || cudaMemcpy(states_out.data(), gp.states_out, R * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess) &&
               (!lp || cudaMemcpy(lp->logprobs, req.logprobs, cells * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess) &&
               (!lp || !lp->sample_probs || cudaMemcpy(lp->sample_probs, req.sample_probs, cells * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess) &&
               (!k || (cudaMemcpy(lp->top_ids, req.top_ids, cells * k * sizeof(uint32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
@@ -1204,86 +1219,55 @@ static bool generate_step_hook(const struct rwkv_b200_generate_step_args * a, co
     return true;
 }
 
-bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) { return generate_step_hook(a, nullptr, 0, nullptr); }
+bool rwkv_b200_test_generate_step(const struct rwkv_b200_generate_step_args * a) {
+    return generate_step_hook(a, GEN_PLAIN, nullptr, nullptr, 0, nullptr, nullptr);
+}
 
 bool rwkv_b200_test_generate_step_constrained(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states) {
     if (!next) { g_last_error = RWKV_ERROR_NONE; ErrorSink sink = global_sink(); RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, false, "NULL table"); }
-    return generate_step_hook(a, next, n_states, states);
+    return generate_step_hook(a, GEN_CONSTRAINED, nullptr, next, n_states, states, nullptr);
 }
 
 bool rwkv_b200_test_generate_step_logprobs(const struct rwkv_b200_generate_step_args * a, const uint16_t * next, size_t n_states, uint32_t * states,
                                            const struct rwkv_b200_logprobs * lp) {
-    g_last_error = RWKV_ERROR_NONE;
-    ErrorSink sink = global_sink();
-    LogprobsOut out{};
-    if (!logprobs_arg(sink, lp, out)) return false;
-    return generate_step_hook(a, next, n_states, states, &out);
-}
-
-// The sampled kernel's step: samplers[n_rows] in place of a's temperature, top_p and penalty arrays.
-static bool sampled_step_hook(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
-                              size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp, const StreamHook * stream = nullptr,
-                              const PenaltyHook * pen = nullptr) {
-    ErrorSink sink = global_sink();
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, a && a->n_rows >= 1 && a->n_rows <= (size_t) SAMPLE_MAX_ROWS, "Invalid generate-step arguments");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, samplers, "NULL samplers");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, !a->temperature && !a->top_p && !a->presence_penalty && !a->frequency_penalty,
-               "temperature, top_p and the penalties come from the samplers: pass NULL");
-    LogprobsOut out{};
-    if (lp && !logprobs_arg(sink, lp, out)) return false;
-    const size_t R = a->n_rows;
-    std::vector<float> t(R), p(R), pres(R), freq(R);
-    std::vector<SamplerIn> smp(R);
-    for (size_t b = 0; b < R; b++) {
-        t[b] = samplers[b].temperature; p[b] = samplers[b].top_p;
-        pres[b] = samplers[b].presence_penalty; freq[b] = samplers[b].frequency_penalty;
-        smp[b] = sampler_in(samplers[b]);
-    }
-    struct rwkv_b200_generate_step_args args = *a;
-    args.temperature = t.data(); args.top_p = p.data(); args.presence_penalty = pres.data(); args.frequency_penalty = freq.data();
-    return generate_step_hook(&args, next, n_states, states, lp ? &out : nullptr, smp.data(), stream, pen);
+    return generate_step_hook(a, GEN_LOGPROBS, nullptr, next, n_states, states, lp);
 }
 
 bool rwkv_b200_test_generate_step_sampled(const struct rwkv_b200_generate_step_args * a, const struct rwkv_b200_sampler * samplers, const uint16_t * next,
                                           size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp) {
+    return generate_step_hook(a, GEN_SAMPLED, samplers, next, n_states, states, lp);
+}
+
+static_assert(RWKV_B200_STEP_PLAIN == GEN_PLAIN && RWKV_B200_STEP_CONSTRAINED == GEN_CONSTRAINED && RWKV_B200_STEP_LOGPROBS == GEN_LOGPROBS &&
+              RWKV_B200_STEP_SAMPLED == GEN_SAMPLED, "step families of the header and the kernels");
+
+// The family of the streaming and penalty step hooks, and the arguments that go with it.
+static bool step_family_arg(int family, const struct rwkv_b200_sampler * samplers, const uint16_t * next, const struct rwkv_b200_logprobs * lp) {
     g_last_error = RWKV_ERROR_NONE;
-    return sampled_step_hook(a, samplers, next, n_states, states, lp);
+    ErrorSink sink = global_sink();
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family >= RWKV_B200_STEP_PLAIN && family <= RWKV_B200_STEP_SAMPLED, "Unknown step family %d", family);
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, (family == RWKV_B200_STEP_SAMPLED) == (samplers != nullptr), "samplers go with the sampled family alone");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_CONSTRAINED ? next != nullptr : family != RWKV_B200_STEP_PLAIN || !next,
+               "The constrained family needs a table, the plain one takes none");
+    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_LOGPROBS ? lp != nullptr : family == RWKV_B200_STEP_SAMPLED || !lp,
+               "The logprobs family needs lp, the plain and constrained ones take none");
+    return true;
 }
 
 bool rwkv_b200_test_generate_step_streaming(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
                                             const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
                                             const uint32_t * acked, uint32_t * published, uint32_t * stream_tokens, uint32_t * ring, uint32_t * timed_out) {
-    g_last_error = RWKV_ERROR_NONE;
-    ErrorSink sink = global_sink();
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family >= RWKV_B200_STEP_PLAIN && family <= RWKV_B200_STEP_SAMPLED, "Unknown step family %d", family);
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, (family == RWKV_B200_STEP_SAMPLED) == (samplers != nullptr), "samplers go with the sampled family alone");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_CONSTRAINED ? next != nullptr : family != RWKV_B200_STEP_PLAIN || !next,
-               "The constrained family needs a table, the plain one takes none");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_LOGPROBS ? lp != nullptr : family == RWKV_B200_STEP_SAMPLED || !lp,
-               "The logprobs family needs lp, the plain and constrained ones take none");
+    if (!step_family_arg(family, samplers, next, lp)) return false;
     const StreamHook stream{acked, published, stream_tokens, ring, timed_out};
-    if (family == RWKV_B200_STEP_SAMPLED) return sampled_step_hook(a, samplers, next, n_states, states, lp, &stream);
-    LogprobsOut out{};
-    if (lp && !logprobs_arg(sink, lp, out)) return false;
-    return generate_step_hook(a, next, n_states, states, lp ? &out : nullptr, nullptr, &stream);
+    return generate_step_hook(a, (GenFamily) family, samplers, next, n_states, states, lp, &stream);
 }
 
 bool rwkv_b200_test_generate_step_penalty(const struct rwkv_b200_generate_step_args * a, int family, const struct rwkv_b200_sampler * samplers,
                                           const uint16_t * next, size_t n_states, uint32_t * states, const struct rwkv_b200_logprobs * lp,
                                           float * counts, const float * decay, const float * weights) {
-    g_last_error = RWKV_ERROR_NONE;
-    ErrorSink sink = global_sink();
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family >= RWKV_B200_STEP_PLAIN && family <= RWKV_B200_STEP_SAMPLED, "Unknown step family %d", family);
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, (family == RWKV_B200_STEP_SAMPLED) == (samplers != nullptr), "samplers go with the sampled family alone");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_CONSTRAINED ? next != nullptr : family != RWKV_B200_STEP_PLAIN || !next,
-               "The constrained family needs a table, the plain one takes none");
-    RWKV_CHECK(sink, RWKV_ERROR_ARGS, false, family == RWKV_B200_STEP_LOGPROBS ? lp != nullptr : family == RWKV_B200_STEP_SAMPLED || !lp,
-               "The logprobs family needs lp, the plain and constrained ones take none");
+    if (!step_family_arg(family, samplers, next, lp)) return false;
     const PenaltyHook pen{counts, decay, weights};
-    if (family == RWKV_B200_STEP_SAMPLED) return sampled_step_hook(a, samplers, next, n_states, states, lp, nullptr, &pen);
-    LogprobsOut out{};
-    if (lp && !logprobs_arg(sink, lp, out)) return false;
-    return generate_step_hook(a, next, n_states, states, lp ? &out : nullptr, nullptr, nullptr, &pen);
+    return generate_step_hook(a, (GenFamily) family, samplers, next, n_states, states, lp, nullptr, &pen);
 }
 
 size_t rwkv_b200_stage_hidden_len(const struct rwkv_context * ctx, size_t n_tokens) { return stage_hidden_len(*C(ctx)->model, n_tokens); }

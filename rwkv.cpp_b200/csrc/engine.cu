@@ -1612,11 +1612,11 @@ bool batch_eval_sample(Context * ctx, const uint32_t * tokens, const float * tem
 // A streaming loop runs generate_stream_sample_kernel instead: after each draw it publishes the token to mapped host memory, and
 // before the next draw of that row it waits for the calling thread to acknowledge it (stream_tokens), so that the pass evaluating
 // token j overlaps the callback of token j, and a callback can end its row before token j + 1 is drawn.
-// A loop that reports log-probabilities runs the logprob step kernels instead, in graphs of their own (gen_lp_graphs); they read the
-// call's GenLogprobRequest from ctx->lp_req.dev, and the streaming one writes each token's record into the mapped ring before it publishes
-// the token, so that stream_tokens can hand the record to the caller before on_token.
-// A loop with per-row samplers runs the sampled step kernels, in graphs of their own too (gen_smp_graphs); they read the rows, the bias
-// pool and the request word (ctx->lp_req.dev, or NULL without log-probabilities) from ctx->smp.dev.
+// A loop that reports log-probabilities runs the logprob step kernels instead, in graphs of their own (gen_graphs[..][GEN_LOGPROBS]);
+// they read the call's GenLogprobRequest from ctx->lp_req.dev, and the streaming one writes each token's record into the mapped ring
+// before it publishes the token, so that stream_tokens can hand the record to the caller before on_token.
+// A loop with per-row samplers runs the sampled step kernels, in graphs of their own too (gen_graphs[..][GEN_SAMPLED]); they read the
+// rows, the bias pool and the request word (ctx->lp_req.dev, or NULL without log-probabilities) from ctx->smp.dev.
 namespace {
 
 size_t gen_mask_offset(int rows) { return (sizeof(GenShared) + (size_t) rows * sizeof(GenRow) + 7) / 8 * 8; }
@@ -1624,7 +1624,12 @@ size_t gen_u_offset(int rows) { return gen_mask_offset(rows) + (size_t) rows * s
 size_t gen_tokens_word(int rows) { return 2 * (size_t) rows + 1; }
 size_t gen_out_words(int rows, size_t n) { return gen_tokens_word(rows) + (size_t) rows * n; }
 
-GenStepParams generate_step_params(Context * ctx) {
+size_t stream_token_offset(int rows) { return 2 * (size_t) rows + 1; }
+size_t smp_rows_offset() { return sizeof(const GenLogprobRequest *); }
+size_t smp_bias_offset(int rows) { return smp_rows_offset() + (size_t) rows * sizeof(GenSamplerRow); }
+
+// The step kernel's parameters over the context's buffers, with the fields that `family` and `streaming` read.
+GenStepParams generate_step_params(Context * ctx, GenFamily family, bool streaming) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     GenStepParams gp{};
     gp.logits = ctx->logits; gp.n_vocab = ctx->model->n_vocab; gp.n_rows = rows;
@@ -1634,16 +1639,31 @@ GenStepParams generate_step_params(Context * ctx) {
     gp.counts = ctx->gen.counts; gp.bias_ids = ctx->gen.bias_ids; gp.bias_values = ctx->gen.bias_values; gp.scratch = ctx->gen.scratch;
     gp.n_generated = ctx->gen.out; gp.passes = ctx->gen.out + rows; gp.tokens = ctx->gen.out + gen_tokens_word(rows);
     gp.next_tokens = ctx->act.tokens; gp.park = ctx->batch_n ? ctx->gen.park.get() : nullptr;
+    if (streaming) {
+        uint32_t * words = ctx->streamed.words.device();
+        gp.published = words; gp.acked = words + rows; gp.timed_out = words + 2 * rows; gp.stream_tokens = words + stream_token_offset(rows);
+    }
+    if (family != GEN_PLAIN) {
+        gp.mask = reinterpret_cast<GenMaskRow *>(ctx->gen.in + gen_mask_offset(rows));
+        gp.states_out = ctx->gen.out + rows + 1;
+    }
+    if (family == GEN_LOGPROBS) gp.lp = ctx->lp_req.dev;
+    if (family == GEN_SAMPLED) {
+        gp.lp_word = reinterpret_cast<const GenLogprobRequest * const *>(ctx->smp.dev.get());
+        gp.samplers = reinterpret_cast<const GenSamplerRow *>(ctx->smp.dev + smp_rows_offset());
+        gp.user_bias = reinterpret_cast<const GenBiasEntry *>(ctx->smp.dev + smp_bias_offset(rows));
+    }
     return gp;
 }
 
-// Pass p of the loop (input tokens already in ctx->act.tokens) captured into `body`.
-bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p) {
+// Pass p of the loop (input tokens already in ctx->act.tokens) captured into `body`; in a batch context the frozen rows of `rows`
+// keep their state.
+bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p, const GenRow * rows) {
     CUDA_OK(ctx, cudaStreamBeginCaptureToGraph(p.stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
     bool ok = enqueue_pass(ctx, p, 0);
     cudaError_t e = cudaSuccess;
     if (ok && ctx->batch_n)
-        e = launch_restore_frozen(generate_step_params(ctx).rows, p.T, p.state_in, p.state_out, ctx->batch_stride, ctx->model->state_len(), p.stream);
+        e = launch_restore_frozen(rows, p.T, p.state_in, p.state_out, ctx->batch_stride, ctx->model->state_len(), p.stream);
     cudaGraph_t out = nullptr;
     const cudaError_t ec = cudaStreamEndCapture(p.stream, &out);
     if (e == cudaSuccess) e = ec;
@@ -1651,21 +1671,7 @@ bool capture_generate_pass(Context * ctx, cudaGraph_t body, const Pass & p) {
     return true;
 }
 
-size_t stream_token_offset(int rows) { return 2 * (size_t) rows + 1; }
-
-GenStreamParams generate_stream_params(Context * ctx) {
-    const int rows = ctx->batch_n ? ctx->batch_n : 1;
-    GenStreamParams sp{};
-    sp.step = generate_step_params(ctx);
-    sp.published = ctx->streamed.words.device(); sp.acked = ctx->streamed.words.device() + rows; sp.timed_out = ctx->streamed.words.device() + 2 * rows;
-    sp.tokens = ctx->streamed.words.device() + stream_token_offset(rows);
-    return sp;
-}
-
-size_t smp_rows_offset() { return sizeof(const GenLogprobRequest *); }
-size_t smp_bias_offset(int rows) { return smp_rows_offset() + (size_t) rows * sizeof(GenSamplerRow); }
-
-bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool logprobs, bool sampled) {
+bool build_generate_graph(Context * ctx, GenFamily family, bool streaming) {
     const int rows = ctx->batch_n ? ctx->batch_n : 1;
     Pass p;
     if (!make_pass(ctx, rows, true, nullptr, p)) return false;
@@ -1691,30 +1697,19 @@ bool build_generate_graph(Context * ctx, bool streaming, bool constrained, bool 
     for (int half = 0; half < 2; half++) {
         cudaGraphConditionalHandle run_pass;
         CUDA_OK(ctx, cudaGraphConditionalHandleCreate(&run_pass, body, 0, cudaGraphCondAssignDefault));
-        GenStreamParams sp = generate_stream_params(ctx);
-        GenStepParams & gp = sp.step;
+        GenStepParams gp = generate_step_params(ctx, family, streaming);
         gp.set_handles = true; gp.run_pass = run_pass; gp.keep_going = keep_going;
         cudaGraphNode_t step = nullptr, cond = nullptr;
-        const GenConstrainedParams cp{sp, reinterpret_cast<GenMaskRow *>(ctx->gen.in + gen_mask_offset(rows)), ctx->gen.out + rows + 1};
-        const GenSamplerParams smp{cp, reinterpret_cast<const GenLogprobRequest * const *>(ctx->smp.dev.get()),
-                                   reinterpret_cast<const GenSamplerRow *>(ctx->smp.dev + smp_rows_offset()),
-                                   reinterpret_cast<const GenBiasEntry *>(ctx->smp.dev + smp_bias_offset(rows))};
-        CUDA_OK(ctx, sampled ? add_generate_sampled_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, smp, streaming, &step)
-                     : logprobs ? add_generate_logprob_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, GenLogprobParams{cp, ctx->lp_req.dev}, streaming, &step)
-                     : constrained ? add_generate_constrained_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, cp, streaming, &step)
-                     : streaming ? add_generate_stream_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, sp, &step)
-                                 : add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, &step));
+        CUDA_OK(ctx, add_generate_step_node(body, prev ? &prev : nullptr, prev ? 1 : 0, gp, family, streaming, &step));
         cudaGraphNodeParams ip = {};
         ip.type = cudaGraphNodeTypeConditional;
         ip.conditional.handle = run_pass; ip.conditional.type = cudaGraphCondTypeIf; ip.conditional.size = 1;
         CUDA_OK(ctx, cudaGraphAddNode(&cond, body, &step, 1, &ip));
-        if (!capture_generate_pass(ctx, ip.conditional.phGraph_out[0], p)) return false;
+        if (!capture_generate_pass(ctx, ip.conditional.phGraph_out[0], p, gp.rows)) return false;
         std::swap(p.state_in, p.state_out);      // the second pass reads what the first one wrote
         prev = cond;
     }
-    GraphExec & exec = sampled ? ctx->gen_smp_graphs[ctx->phase][streaming]
-                       : logprobs ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
-    CUDA_OK(ctx, exec.instantiate(top));
+    CUDA_OK(ctx, ctx->gen_graphs[ctx->phase][family][streaming].instantiate(top));
     return true;
 }
 
@@ -1828,12 +1823,8 @@ bool stream_tokens(Context * ctx, TokenFn on_token, void * user, const LogprobsO
 
 void drop_generate_graphs(Context * ctx) {
     for (auto & by_phase : ctx->gen_graphs)
-        for (auto & by_streaming : by_phase)
-            for (auto & e : by_streaming) e.reset();
-    for (auto & by_phase : ctx->gen_lp_graphs)
-        for (auto & e : by_phase) e.reset();
-    for (auto & by_phase : ctx->gen_smp_graphs)
-        for (auto & e : by_phase) e.reset();
+        for (auto & by_family : by_phase)
+            for (auto & e : by_family) e.reset();
     for (auto & e : ctx->beam_graphs) e.reset();
 }
 
@@ -2082,9 +2073,9 @@ bool generate(Context * ctx, const uint32_t * max_tokens, const float * temperat
         }
         CUDA_OK(ctx, cudaMemcpyAsync(ctx->smp.dev, ctx->smp.host, smp_bias_offset(rows) + used * sizeof(GenBiasEntry), cudaMemcpyHostToDevice, ctx->stream));
     }
-    GraphExec & graph = samplers ? ctx->gen_smp_graphs[ctx->phase][streaming]
-                      : lp ? ctx->gen_lp_graphs[ctx->phase][streaming] : ctx->gen_graphs[ctx->phase][streaming][constrained];
-    if (!graph && !build_generate_graph(ctx, streaming, constrained, lp != nullptr, samplers != nullptr)) return false;
+    const GenFamily family = samplers ? GEN_SAMPLED : lp ? GEN_LOGPROBS : constrained ? GEN_CONSTRAINED : GEN_PLAIN;
+    GraphExec & graph = ctx->gen_graphs[ctx->phase][family][streaming];
+    if (!graph && !build_generate_graph(ctx, family, streaming)) return false;
     CUDA_OK(ctx, cudaGraphLaunch(graph, ctx->stream));
     g_graph_launches++;
     if (ctx->batch_n) CUDA_OK(ctx, cudaMemcpyAsync(ctx->logits, ctx->gen.park, (size_t) rows * V * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));

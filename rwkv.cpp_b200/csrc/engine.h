@@ -163,11 +163,11 @@ struct Context {
     // means all 1. The call's GenShared carries the table's address, so no graph holds it.
     std::vector<float> penalty_decay;
     struct PenaltyWeights { DeviceBuffer<float> table; bool set = false; } pen_weights;
-    // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by whether
-    // the loop streams its tokens to a callback, and by whether its draws are constrained by automata
-    GraphExec gen_graphs[2][2][2];
+    // the loop's graphs, keyed by phase (which state buffer holds the current state), as the single-token slots are, by the family
+    // of its step kernel (GenFamily) and by whether the loop streams its tokens to a callback
+    GraphExec gen_graphs[2][4][2];
     // Streaming generation, allocated on the first streaming call: mapped pinned words shared by the step kernel and the calling
-    // thread (GenStreamParams), at device addresses the streaming graph captures. Layout: published [rows], acked [rows], timed_out,
+    // thread (GenStepParams), at device addresses the streaming graphs capture. Layout: published [rows], acked [rows], timed_out,
     // then tokens [rows][GENERATE_MAX].
     struct Streaming { PinnedBuffer<uint32_t> words; Event done; } streamed;   // done: recorded after the streaming loop's copies
     bool in_stream = false;          // the calling thread is inside a streaming call's callbacks: this context's stream is busy
@@ -178,12 +178,10 @@ struct Context {
     struct LogprobRequest { DeviceBuffer<GenLogprobRequest> dev; PinnedBuffer<GenLogprobRequest> host; } lp_req;
     struct LogprobOut { DeviceBuffer<uint32_t> dev; PinnedBuffer<uint32_t> host; size_t words = 0; } lp_out;
     PinnedBuffer<uint32_t> lp_ring;
-    GraphExec gen_lp_graphs[2][2];         // the logprob loops' graphs, keyed by phase and streaming
     // Per-row samplers (generate with SamplerIn rows), allocated only by calls that use them: the call's upload at a device address
     // the sampled graphs capture, and its pinned copy: the log-probability request word (lp_req or NULL), GenSamplerRow[rows], then
     // room for rows * GEN_BIAS_MAX GenBiasEntry.
     struct Samplers { DeviceBuffer<unsigned char> dev; PinnedBuffer<unsigned char> host; } smp;
-    GraphExec gen_smp_graphs[2][2];        // the sampled loops' graphs, keyed by phase and streaming
     // Beam search (beam_search): the park [batch_n, n_vocab] (the logits of the pass that runs before the loop is captured, then the
     // logits of the slots that groups which stopped keep), allocated on the first call; the loop state and a search state per group
     // (kernels/ops.h: BeamLoop, BeamState[groups], one allocation) and the back-pointers [capacity][batch_n][2], grown to the most

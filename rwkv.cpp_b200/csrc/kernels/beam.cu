@@ -173,10 +173,7 @@ __global__ void __launch_bounds__(GATHER_THREADS) beam_restore_kernel(const Beam
 }
 
 void * beam_step_for(int n_vocab) {
-    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? reinterpret_cast<void *>(beam_step_kernel<1>) : per <= 4 ? reinterpret_cast<void *>(beam_step_kernel<4>)
-         : per <= 16 ? reinterpret_cast<void *>(beam_step_kernel<16>) : per <= 50 ? reinterpret_cast<void *>(beam_step_kernel<50>)
-         : reinterpret_cast<void *>(beam_step_kernel<64>);
+    return with_sample_per(n_vocab, [](auto per) { return reinterpret_cast<void *>(beam_step_kernel<decltype(per)::value>); });
 }
 
 bool beam_args_ok(const BeamStepParams & p) {

@@ -235,43 +235,13 @@ struct GenShared {                    // written by the host per call (ticket = 
     uint32_t ticket, active;          // CTAs done with this step / rows active after it; reset by the step's last CTA
     const float * weights;            // [n_vocab] penalty weights, or NULL for all 1; in the upload so that no graph holds it
 };
-struct GenStepParams {
-    const float * logits;             // [n_rows, n_vocab]
-    int n_vocab, n_rows;
-    GenRow * rows;                    // [n_rows]
-    GenShared * shared;
-    const double * u;                 // [n_rows][stride]
-    float * counts;                   // [n_rows, n_vocab] penalty counts
-    uint32_t * bias_ids;              // [n_rows, n_vocab] scratch: the bias list of a row, one entry per token (id n_vocab = none)
-    float * bias_values;
-    float * scratch;                  // [n_rows, n_vocab]: the biased logits
-    uint32_t * tokens;                // [n_rows][stride]
-    uint32_t * n_generated;           // [n_rows]: the row's step after this launch
-    uint32_t * passes;                // +1 for every step after which a row is active
-    int * next_tokens;                // [n_rows]: input tokens of the next pass (0 for a frozen row)
-    float * park;                     // [n_rows, n_vocab] or NULL: a row's logits are copied here when it freezes (batch contexts)
-    bool set_handles;                 // inside a conditional graph: set run_pass and keep_going
-    cudaGraphConditionalHandle run_pass, keep_going;
-};
-cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s);
-// The same step as a kernel node of graph g after deps (the body of the generation loop).
-cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node);
-
 // Streaming generation (rwkv_b200_generate_stream / rwkv_b200_batch_generate_stream): the same step with a gate and a publisher over
 // words in mapped pinned host memory. Gate: before a row that is not frozen draws token step (0 < step < max_tokens), thread 0 waits
 // until acked[b] >> 1 == step, i.e. the host has acknowledged token step - 1; acked bit 0 asks the row to stop, which freezes it as an
 // exhausted budget does. A wait longer than STREAM_TIMEOUT_MS freezes the row the same way and sets *timed_out. Publisher: after a
-// draw, tokens[b * GENERATE_MAX + step] = token, then (release, system scope) published[b] = step + 1.
+// draw, stream_tokens[b * GENERATE_MAX + step] = token, then (release, system scope) published[b] = step + 1.
 constexpr int GENERATE_MAX = 4096;
 constexpr int STREAM_TIMEOUT_MS = 10000;
-struct GenStreamParams {
-    GenStepParams step;
-    uint32_t * tokens;                // mapped [n_rows][GENERATE_MAX]
-    uint32_t * published;             // mapped [n_rows]: tokens published this call
-    const uint32_t * acked;           // mapped [n_rows]: 2 * tokens acknowledged + stop request
-    uint32_t * timed_out;             // mapped: set when a wait ran out
-};
-cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node);
 // Constrained generation (rwkv_b200_generate_constrained / rwkv_b200_batch_generate_constrained): the same steps, blocking or streaming,
 // with row b restricted by a token automaton, next[s * n_vocab + t] the state after token t in state s or GEN_MASK_DEAD. A row in a
 // state s with !live[s] freezes before it draws, as an exhausted budget freezes it; otherwise every token t with next[s][t] dead
@@ -284,14 +254,6 @@ struct GenMaskRow {                   // written by the host per call; state is 
     const uint8_t * live;             // [n_states]: the state allows some token
     uint32_t state, pad;
 };
-struct GenConstrainedParams {
-    GenStreamParams stream;           // the step's parameters; the mapped words are used by the streaming kernel only
-    GenMaskRow * mask;                // [n_rows]
-    uint32_t * states_out;            // [n_rows]
-};
-cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s);     // the blocking kernel
-cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
-                                               cudaGraphNode_t * node);
 // Generation with log-probabilities (rwkv_b200_generate_logprobs / rwkv_b200_batch_generate_logprobs): the constrained steps (a row
 // with a NULL table is unconstrained) that also report, for every token they draw at [b][step] of the request's [n_rows][stride]
 // arrays: logprobs = log_softmax(z)[tok] of the raw logits z the token was drawn from, in the arithmetic and order of score_kernel;
@@ -310,16 +272,9 @@ struct GenLogprobRequest {            // written by the host per call
     float * top_logprobs;             // [n_rows][stride][top_n] device
     uint32_t * ring;                  // mapped [n_rows][2][GEN_LP_RECORD], streaming only
 };
-struct GenLogprobParams {
-    GenConstrainedParams gen;
-    const GenLogprobRequest * req;    // device
-};
-cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_t s);     // the blocking kernel
-cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
-                                           cudaGraphNode_t * node);
 // Generation with a per-row sampler (rwkv_b200_generate_sampled / rwkv_b200_batch_generate_sampled): the constrained steps (a row with
-// a NULL table is unconstrained), with log-probabilities when *req is not NULL, where row b also has
-// - user bias entries bias[bias_begin, bias_end) (distinct ids): after the penalty / mask list is written, an id its state allows
+// a NULL table is unconstrained), with log-probabilities when *lp_word is not NULL, where row b also has
+// - user bias entries user_bias[bias_begin, bias_end) (distinct ids): after the penalty / mask list is written, an id its state allows
 //   gets the entry value - (presence + c * frequency) if its penalty count c is not 0, else value;
 // - top_k (0 = off) and min_p (0 = off): a token is kept iff its probability is at least the top-p cutoff, the top_k-th largest
 //   probability (with multiplicity) and min_p * the largest probability (sample_row's KeepFilter).
@@ -334,15 +289,47 @@ struct GenBiasEntry {
     uint32_t id;
     float value;
 };
-struct GenSamplerParams {
-    GenConstrainedParams gen;
-    const GenLogprobRequest * const * req;    // device word: the call's log-probability request, or NULL for none
-    const GenSamplerRow * rows;               // [n_rows] device
-    const GenBiasEntry * bias;                // device, the rows' entries
+// The step kernels come in four families, each blocking or streaming: plain, constrained, logprobs and sampled as described above.
+enum GenFamily { GEN_PLAIN, GEN_CONSTRAINED, GEN_LOGPROBS, GEN_SAMPLED };
+// The parameters of every step kernel. A family reads the step fields, the mapped words when it streams and the fields marked with its
+// name; it leaves the others NULL.
+struct GenStepParams {
+    const float * logits;             // [n_rows, n_vocab]
+    int n_vocab, n_rows;
+    GenRow * rows;                    // [n_rows]
+    GenShared * shared;
+    const double * u;                 // [n_rows][stride]
+    float * counts;                   // [n_rows, n_vocab] penalty counts
+    uint32_t * bias_ids;              // [n_rows, n_vocab] scratch: the bias list of a row, one entry per token (id n_vocab = none)
+    float * bias_values;
+    float * scratch;                  // [n_rows, n_vocab]: the biased logits
+    uint32_t * tokens;                // [n_rows][stride]
+    uint32_t * n_generated;           // [n_rows]: the row's step after this launch
+    uint32_t * passes;                // +1 for every step after which a row is active
+    int * next_tokens;                // [n_rows]: input tokens of the next pass (0 for a frozen row)
+    float * park;                     // [n_rows, n_vocab] or NULL: a row's logits are copied here when it freezes (batch contexts)
+    bool set_handles;                 // inside a conditional graph: set run_pass and keep_going
+    cudaGraphConditionalHandle run_pass, keep_going;
+    // streaming
+    uint32_t * stream_tokens;         // mapped [n_rows][GENERATE_MAX]
+    uint32_t * published;             // mapped [n_rows]: tokens published this call
+    const uint32_t * acked;           // mapped [n_rows]: 2 * tokens acknowledged + stop request
+    uint32_t * timed_out;             // mapped: set when a wait ran out
+    // constrained, logprobs and sampled
+    GenMaskRow * mask;                // [n_rows]
+    uint32_t * states_out;            // [n_rows]
+    // The logprobs kernels read the request itself; the sampled kernels read it through a device word that the call sets to the
+    // request or to NULL, so that one sampled graph serves calls with and without log-probabilities.
+    const GenLogprobRequest * lp;                 // logprobs: device
+    const GenLogprobRequest * const * lp_word;    // sampled: device word, the call's request or NULL for none
+    const GenSamplerRow * samplers;               // sampled: [n_rows] device
+    const GenBiasEntry * user_bias;               // sampled: device, the rows' entries
 };
-cudaError_t launch_generate_sampled_step(const GenSamplerParams & p, cudaStream_t s);     // the blocking kernel
-cudaError_t add_generate_sampled_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenSamplerParams & p, bool stream,
-                                           cudaGraphNode_t * node);
+// The blocking step kernel of `family`. The streaming kernels run only as graph nodes.
+cudaError_t launch_generate_step(const GenStepParams & p, GenFamily family, cudaStream_t s);
+// The step kernel of `family`, streaming or not, as a kernel node of graph g after deps (the body of the generation loop).
+cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, GenFamily family, bool stream,
+                                   cudaGraphNode_t * node);
 // After a pass of a batch context inside the generation loop: dst slice b <- src slice b (state_len floats, seq_stride apart) for
 // every frozen row, so that its state stays what it was.
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s);

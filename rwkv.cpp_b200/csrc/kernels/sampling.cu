@@ -261,7 +261,7 @@ __device__ __forceinline__ unsigned long long global_ns() {
     return t;
 }
 
-// The streaming loop's gate over the mapped words of GenStreamParams (ops.h).
+// The streaming loop's gate over the mapped words of GenStepParams (ops.h).
 struct StreamGate {
     uint32_t * tokens, * published;
     const uint32_t * acked;
@@ -296,7 +296,7 @@ struct NoMask {
     __device__ __forceinline__ void report(int) const {}
 };
 
-// The constrained loop's mask over the per-row automata of GenConstrainedParams (ops.h); a row with a NULL table is unconstrained.
+// The constrained loop's mask over the per-row automata of GenStepParams::mask (ops.h); a row with a NULL table is unconstrained.
 struct TableMask {
     GenMaskRow * rows;
     uint32_t * states_out;
@@ -384,7 +384,7 @@ struct NoSampler {
     __device__ __forceinline__ NoFilter filter(int) const { return NoFilter{}; }
 };
 
-// The per-row samplers of GenSamplerParams (ops.h).
+// The per-row samplers of GenStepParams::samplers (ops.h).
 struct RowSampler {
     const GenSamplerRow * rows;
     const GenBiasEntry * bias;
@@ -495,6 +495,16 @@ __device__ __forceinline__ void generate_step(const GenStepParams gp, const Gate
     }
 }
 
+// generate_step's parameters in the kernels with a gate or a mask: a copy with one field stored, which the compiler loads into
+// registers at entry. Passed gp itself, as generate_sample_kernel passes it, these kernels would read each field from the parameter
+// space where it is used: another schedule, with other register and spill counts than those DESIGN.md 6.4.5 lists. The store keeps
+// the compiler from folding the copy back into the parameter.
+__device__ __forceinline__ GenStepParams local_copy(const GenStepParams & gp) {
+    GenStepParams p = gp;
+    p.set_handles = gp.set_handles;
+    return p;
+}
+
 template <int PER>
 __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
@@ -504,58 +514,54 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) generate_sample_kernel(const G
 // At one CTA per SM ptxas may give every thread 64 registers: with the default bound it holds PER <= 4 to 32, and the gate's wait
 // loop then spills more than generate_sample_kernel does. Only a step of more than one row per SM pays for it, with a second wave.
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sample_kernel(const GenStreamParams sp) {
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, NoMask{});
+    generate_step<PER>(local_copy(gp), StreamGate{gp.stream_tokens, gp.published, gp.acked, gp.timed_out}, NoMask{});
 }
 
-// The constrained twins of the two step kernels (rwkv_b200_generate_constrained); the blocking one ignores cp.stream's mapped words.
-// Both are bounded at one CTA per SM: with the default bound the mask's table read makes PER = 4 spill more than
-// generate_sample_kernel<4>.
+// The constrained twins of the two step kernels (rwkv_b200_generate_constrained). Both are bounded at one CTA per SM: with the default
+// bound the mask's table read makes PER = 4 spill more than generate_sample_kernel<4>.
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_constrained_sample_kernel(const GenConstrainedParams cp) {
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_constrained_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    generate_step<PER>(cp.stream.step, NoGate{}, TableMask{cp.mask, cp.states_out});
-}
-
-template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_constrained_sample_kernel(const GenConstrainedParams cp) {
-    pdl_prologue();
-    const GenStreamParams & sp = cp.stream;
-    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, TableMask{cp.mask, cp.states_out});
-}
-
-// The constrained steps that also report log-probabilities (GenLogprobParams); a row with a NULL table is unconstrained, so these two
-// serve the logprob calls with and without automata.
-template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_logprob_sample_kernel(const GenLogprobParams lp) {
-    pdl_prologue();
-    generate_step<PER>(lp.gen.stream.step, NoGate{}, TableMask{lp.gen.mask, lp.gen.states_out}, Logprobs<PER>{lp.req, false});
+    generate_step<PER>(local_copy(gp), NoGate{}, TableMask{gp.mask, gp.states_out});
 }
 
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_logprob_sample_kernel(const GenLogprobParams lp) {
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_constrained_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    const GenStreamParams & sp = lp.gen.stream;
-    generate_step<PER>(sp.step, StreamGate{sp.tokens, sp.published, sp.acked, sp.timed_out}, TableMask{lp.gen.mask, lp.gen.states_out},
-                       Logprobs<PER>{lp.req, true});
+    generate_step<PER>(local_copy(gp), StreamGate{gp.stream_tokens, gp.published, gp.acked, gp.timed_out}, TableMask{gp.mask, gp.states_out});
 }
 
-// The constrained steps with a per-row sampler (GenSamplerParams) and, when the call's request word is set, log-probabilities; a row
-// with a NULL table is unconstrained, so these two serve every sampled call.
+// The constrained steps that also report log-probabilities; a row with a NULL table is unconstrained, so these two serve the logprob
+// calls with and without automata.
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_sampled_sample_kernel(const GenSamplerParams sp) {
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_logprob_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    generate_step<PER>(sp.gen.stream.step, NoGate{}, TableMask{sp.gen.mask, sp.gen.states_out}, RequestedLogprobs<PER>{*sp.req, false},
-                       RowSampler{sp.rows, sp.bias});
+    generate_step<PER>(local_copy(gp), NoGate{}, TableMask{gp.mask, gp.states_out}, Logprobs<PER>{gp.lp, false});
 }
 
 template <int PER>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sampled_sample_kernel(const GenSamplerParams sp) {
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_logprob_sample_kernel(const GenStepParams gp) {
     pdl_prologue();
-    const GenStreamParams & st = sp.gen.stream;
-    generate_step<PER>(st.step, StreamGate{st.tokens, st.published, st.acked, st.timed_out}, TableMask{sp.gen.mask, sp.gen.states_out},
-                       RequestedLogprobs<PER>{*sp.req, true}, RowSampler{sp.rows, sp.bias});
+    generate_step<PER>(local_copy(gp), StreamGate{gp.stream_tokens, gp.published, gp.acked, gp.timed_out}, TableMask{gp.mask, gp.states_out},
+                       Logprobs<PER>{gp.lp, true});
+}
+
+// The constrained steps with a per-row sampler and, when the call's request word is set, log-probabilities; a row with a NULL table
+// is unconstrained, so these two serve every sampled call.
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_sampled_sample_kernel(const GenStepParams gp) {
+    pdl_prologue();
+    generate_step<PER>(local_copy(gp), NoGate{}, TableMask{gp.mask, gp.states_out}, RequestedLogprobs<PER>{*gp.lp_word, false},
+                       RowSampler{gp.samplers, gp.user_bias});
+}
+
+template <int PER>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) generate_stream_sampled_sample_kernel(const GenStepParams gp) {
+    pdl_prologue();
+    generate_step<PER>(local_copy(gp), StreamGate{gp.stream_tokens, gp.published, gp.acked, gp.timed_out}, TableMask{gp.mask, gp.states_out},
+                       RequestedLogprobs<PER>{*gp.lp_word, true}, RowSampler{gp.samplers, gp.user_bias});
 }
 
 constexpr int RESTORE_THREADS = 256, RESTORE_BLOCKS_PER_ROW = 64;
@@ -568,119 +574,42 @@ __global__ void __launch_bounds__(RESTORE_THREADS) restore_frozen_kernel(const G
     for (size_t i = (size_t) blockIdx.x * RESTORE_THREADS + threadIdx.x; i < n; i += (size_t) gridDim.x * RESTORE_THREADS) dst[base + i] = src[base + i];
 }
 
-template <int PER> void * generate_step_fn(bool stream, bool constrained) {
-    if (constrained)
-        return stream ? reinterpret_cast<void *>(generate_stream_constrained_sample_kernel<PER>) : reinterpret_cast<void *>(generate_constrained_sample_kernel<PER>);
-    return stream ? reinterpret_cast<void *>(generate_stream_sample_kernel<PER>) : reinterpret_cast<void *>(generate_sample_kernel<PER>);
-}
-void * generate_step_for(int n_vocab, bool stream, bool constrained) {
-    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? generate_step_fn<1>(stream, constrained) : per <= 4 ? generate_step_fn<4>(stream, constrained)
-         : per <= 16 ? generate_step_fn<16>(stream, constrained) : per <= 50 ? generate_step_fn<50>(stream, constrained) : generate_step_fn<64>(stream, constrained);
-}
+using StepKernel = void (*)(const GenStepParams);
 
-template <int PER> void * generate_logprob_step_fn(bool stream) {
-    return stream ? reinterpret_cast<void *>(generate_stream_logprob_sample_kernel<PER>) : reinterpret_cast<void *>(generate_logprob_sample_kernel<PER>);
-}
-void * generate_logprob_step_for(int n_vocab, bool stream) {
-    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? generate_logprob_step_fn<1>(stream) : per <= 4 ? generate_logprob_step_fn<4>(stream) : per <= 16 ? generate_logprob_step_fn<16>(stream)
-         : per <= 50 ? generate_logprob_step_fn<50>(stream) : generate_logprob_step_fn<64>(stream);
-}
+// The step kernels of one PER by family and streaming.
+template <int PER>
+const StepKernel step_kernels[4][2] = {
+    {generate_sample_kernel<PER>, generate_stream_sample_kernel<PER>},
+    {generate_constrained_sample_kernel<PER>, generate_stream_constrained_sample_kernel<PER>},
+    {generate_logprob_sample_kernel<PER>, generate_stream_logprob_sample_kernel<PER>},
+    {generate_sampled_sample_kernel<PER>, generate_stream_sampled_sample_kernel<PER>},
+};
 
-template <int PER> void * generate_sampled_step_fn(bool stream) {
-    return stream ? reinterpret_cast<void *>(generate_stream_sampled_sample_kernel<PER>) : reinterpret_cast<void *>(generate_sampled_sample_kernel<PER>);
-}
-void * generate_sampled_step_for(int n_vocab, bool stream) {
-    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    return per <= 1 ? generate_sampled_step_fn<1>(stream) : per <= 4 ? generate_sampled_step_fn<4>(stream) : per <= 16 ? generate_sampled_step_fn<16>(stream)
-         : per <= 50 ? generate_sampled_step_fn<50>(stream) : generate_sampled_step_fn<64>(stream);
-}
-
-// A node of graph g after deps running step kernel `func` with the single kernel parameter `arg`.
-template <class P>
-cudaError_t add_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, const P & arg, void * func,
-                          cudaGraphNode_t * node) {
-    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    P copy = arg;
-    void * args[] = {&copy};
-    cudaKernelNodeParams kp = {};
-    kp.func = func;
-    kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
-    kp.kernelParams = args; kp.extra = nullptr;
-    return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
+// The kernel of a step, or NULL when its vocabulary or its rows are out of range.
+StepKernel step_kernel(const GenStepParams & p, GenFamily family, bool stream) {
+    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return nullptr;
+    return with_sample_per(p.n_vocab, [&](auto per) { return step_kernels<decltype(per)::value>[family][stream]; });
 }
 
 }  // namespace
 
-cudaError_t launch_generate_step(const GenStepParams & p, cudaStream_t s) {
-    if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    const dim3 grid(p.n_rows);
-    if (per <= 1) return launch_pdl(generate_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(generate_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(generate_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(generate_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(generate_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+cudaError_t launch_generate_step(const GenStepParams & p, GenFamily family, cudaStream_t s) {
+    const StepKernel k = step_kernel(p, family, false);
+    if (!k) return cudaErrorInvalidValue;
+    return launch_pdl(k, dim3(p.n_rows), dim3(SAMPLE_THREADS), 0, s, p);
 }
 
-cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p, p, generate_step_for(p.n_vocab, false, false), node);
-}
-
-cudaError_t add_generate_stream_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStreamParams & p, cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.step, p, generate_step_for(p.step.n_vocab, true, false), node);
-}
-
-cudaError_t launch_generate_constrained_step(const GenConstrainedParams & p, cudaStream_t s) {
-    const GenStepParams & gp = p.stream.step;
-    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    const dim3 grid(gp.n_rows);
-    if (per <= 1) return launch_pdl(generate_constrained_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(generate_constrained_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(generate_constrained_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(generate_constrained_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(generate_constrained_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-}
-
-cudaError_t add_generate_constrained_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenConstrainedParams & p, bool stream,
-                                               cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.stream.step, p, generate_step_for(p.stream.step.n_vocab, stream, true), node);
-}
-
-cudaError_t launch_generate_logprob_step(const GenLogprobParams & p, cudaStream_t s) {
-    const GenStepParams & gp = p.gen.stream.step;
-    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    const dim3 grid(gp.n_rows);
-    if (per <= 1) return launch_pdl(generate_logprob_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(generate_logprob_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(generate_logprob_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(generate_logprob_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(generate_logprob_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-}
-
-cudaError_t add_generate_logprob_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenLogprobParams & p, bool stream,
-                                           cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.gen.stream.step, p, generate_logprob_step_for(p.gen.stream.step.n_vocab, stream), node);
-}
-
-cudaError_t launch_generate_sampled_step(const GenSamplerParams & p, cudaStream_t s) {
-    const GenStepParams & gp = p.gen.stream.step;
-    if (gp.n_vocab <= 0 || gp.n_vocab > SAMPLE_THREADS * 64 || gp.n_rows <= 0 || gp.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    const int per = (gp.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    const dim3 grid(gp.n_rows);
-    if (per <= 1) return launch_pdl(generate_sampled_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(generate_sampled_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(generate_sampled_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(generate_sampled_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(generate_sampled_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-}
-
-cudaError_t add_generate_sampled_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenSamplerParams & p, bool stream,
-                                           cudaGraphNode_t * node) {
-    return add_step_node(g, deps, n_deps, p.gen.stream.step, p, generate_sampled_step_for(p.gen.stream.step.n_vocab, stream), node);
+cudaError_t add_generate_step_node(cudaGraph_t g, const cudaGraphNode_t * deps, size_t n_deps, const GenStepParams & p, GenFamily family, bool stream,
+                                   cudaGraphNode_t * node) {
+    const StepKernel k = step_kernel(p, family, stream);
+    if (!k) return cudaErrorInvalidValue;
+    GenStepParams copy = p;
+    void * args[] = {&copy};
+    cudaKernelNodeParams kp = {};
+    kp.func = reinterpret_cast<void *>(k);
+    kp.gridDim = dim3(p.n_rows); kp.blockDim = dim3(SAMPLE_THREADS); kp.sharedMemBytes = 0;
+    kp.kernelParams = args; kp.extra = nullptr;
+    return cudaGraphAddKernelNode(node, g, deps, n_deps, &kp);
 }
 
 cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float * src, float * dst, long long seq_stride, size_t state_len, cudaStream_t s) {
@@ -689,23 +618,14 @@ cudaError_t launch_restore_frozen(const GenRow * rows, int n_rows, const float *
 
 cudaError_t launch_sample(const SampleParams & p, cudaStream_t s) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64) return cudaErrorInvalidValue;
-    const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    if (per <= 1) return launch_pdl(sample_kernel<1>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(sample_kernel<4>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(sample_kernel<16>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(sample_kernel<50>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(sample_kernel<64>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p);
+    return with_sample_per(p.n_vocab, [&](auto per) { return launch_pdl(sample_kernel<decltype(per)::value>, dim3(1), dim3(SAMPLE_THREADS), 0, s, p); });
 }
 
 cudaError_t launch_sample_batch(const SampleBatchParams & p, cudaStream_t s) {
     if (p.n_vocab <= 0 || p.n_vocab > SAMPLE_THREADS * 64 || p.n_rows <= 0 || p.n_rows > SAMPLE_MAX_ROWS) return cudaErrorInvalidValue;
-    const int per = (p.n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
-    const dim3 grid(p.n_rows);
-    if (per <= 1) return launch_pdl(batch_sample_kernel<1>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 4) return launch_pdl(batch_sample_kernel<4>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 16) return launch_pdl(batch_sample_kernel<16>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    if (per <= 50) return launch_pdl(batch_sample_kernel<50>, grid, dim3(SAMPLE_THREADS), 0, s, p);
-    return launch_pdl(batch_sample_kernel<64>, grid, dim3(SAMPLE_THREADS), 0, s, p);
+    return with_sample_per(p.n_vocab, [&](auto per) {
+        return launch_pdl(batch_sample_kernel<decltype(per)::value>, dim3(p.n_rows), dim3(SAMPLE_THREADS), 0, s, p);
+    });
 }
 
 }  // namespace rwkv

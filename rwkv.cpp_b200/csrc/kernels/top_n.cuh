@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <type_traits>
 
 #include "ops.h"    // GEN_TOP_MAX
 
@@ -10,6 +11,18 @@ namespace rwkv {
 
 constexpr int SAMPLE_THREADS = 1024;
 constexpr int SAMPLE_WARPS = SAMPLE_THREADS / 32;
+
+// The column kernels of sampling.cu and beam.cu hold PER entries of a column per thread, PER in {1, 4, 16, 50, 64}
+// (n_vocab <= SAMPLE_THREADS * 64). Returns f(std::integral_constant<int, PER>{}) for the smallest PER that covers n_vocab.
+template <class F>
+auto with_sample_per(int n_vocab, F && f) {
+    const int per = (n_vocab + SAMPLE_THREADS - 1) / SAMPLE_THREADS;
+    if (per <= 1) return f(std::integral_constant<int, 1>{});
+    if (per <= 4) return f(std::integral_constant<int, 4>{});
+    if (per <= 16) return f(std::integral_constant<int, 16>{});
+    if (per <= 50) return f(std::integral_constant<int, 50>{});
+    return f(std::integral_constant<int, 64>{});
+}
 
 // Top-N order over (logit, id): a larger logit first, the smaller id first among equal logits. The key holds the logit's bits mapped to
 // an unsigned order in its upper half (-0 counted as +0, so that equal values differ by id alone) and ~id in its lower half, so every
